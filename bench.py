@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Learner steps/sec on synthetic (T=20, B=4096, O=24, A=4, H=256) trajectories.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Own arm (default): one process per GPU (torchrun for N > 1), global batch B=4096 sharded
 B/N per rank ("scaling": "strong"), one all-reduce of [gradient | loss scalars] per step (done by the
@@ -15,6 +15,11 @@ optimizer kernel over NVLink peer memory; NCCL with IMPALA_ALLREDUCE=nccl).
            FP32 FMA pipe for the MLP kernels - see DESIGN.md)
   cpu_baseline : the per-trajectory float64 torch port of learner.py (oracle/) on host cores
 Reference arm (--impl reference): rank 0 times that CPU port alone and prints its own line.
+--dump-outputs DIR (own arm, rank 0): after the K timed device-resident steps, what the last of them
+  computed is written (with N > 1 ranks: the per-element arrays of rank 0's batch shard) as DIR/<name>.npy - the updated parameters of both networks, the logged loss
+  scalars and gradient norms, and the per-element outputs of the step (logits, values, vs, pg_adv,
+  dlogits, the pre-clip gradient).  Inputs and initial parameters are seeded, so two builds run with
+  the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -42,7 +47,7 @@ WORKLOADS = {
 WORKLOAD = {k: v for k, v in WORKLOADS["c4"].items() if k != "name"}
 WORKLOAD_NAME = WORKLOADS["c4"]["name"]
 METRIC = "learner steps/sec on synthetic (T=20,B=4096) trajectories"
-SMS, FP32_LANES = 148, 128
+FP32_LANES = 128  # per SM (Hopper)
 
 
 _REAL_STDOUT = None
@@ -67,9 +72,10 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return dict(hbm_gbs=float(d["hbm_gbs"]), sm_max_mhz=float(d.get("sm_max_mhz", 1965.0)),
-                    bf16_tflops=float(d.get("bf16_tflops", 1590.0)), source="MEASURED_PEAKS.json (measured)")
-    return dict(hbm_gbs=6650.0, sm_max_mhz=1965.0, bf16_tflops=1590.0, source="fallback (B200_PROFILING.md)")
+        return dict(hbm_gbs=float(d["hbm_gbs"]), sm_max_mhz=float(d.get("sm_max_mhz", 1980.0)),
+                    bf16_tflops=float(d.get("bf16_tflops", 989.0)), source="MEASURED_PEAKS.json (measured)")
+    # NVIDIA H100 SXM data sheet (a card at its 700 W limit; a lower power limit lowers what is reachable)
+    return dict(hbm_gbs=3350.0, sm_max_mhz=1980.0, bf16_tflops=989.0, source="H100 SXM data sheet")
 
 
 def hparams(B):
@@ -97,7 +103,7 @@ class _TimedCounter:
 
 def time_reference_learner(sample_B: int, warm: int, timed: int, threads: int):
     """The UNMODIFIED reference `Learner._learn` (learner.py:67-275) from oracle/_ref (or
-    /root/reference), driven in-process through a list-backed queue; returns (median seconds per
+    $IMPALA_REFERENCE_DIR), driven in-process through a list-backed queue; returns (median seconds per
     update, kind).  Falls back to the float64 per-trajectory port when the reference is absent."""
     import torch
 
@@ -181,7 +187,7 @@ def run_reference_arm(args):
     if rank != 0:
         return
     os.environ["CUDA_VISIBLE_DEVICES"] = ""  # the reference picks its device at import (learner.py:13)
-    steps, warm = max(1, min(args.steps, 20)), max(1, min(args.warmup, 2))
+    steps, warm = max(1, args.steps), max(1, min(args.warmup, 2))
     cb = cpu_reference_numbers(warm, steps)
     emit(reference_line(args, cb, steps, warm))
 
@@ -417,6 +423,37 @@ def kernel_breakdown(eng, flush, iters=20, barrier=lambda: None):
     return out
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(eng, out_dir: str) -> None:
+    """What the last timed step computed, as float32 / float64 .npy files (at most 64 MiB in all:
+    if the per-element arrays would not fit, all of them keep the same fixed, seeded sample of
+    batch columns)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    small = {}
+    st, g = eng.state(dtype=torch.float32), eng.grads()
+    for grp in ("policy", "value_fn"):
+        small.update({f"{grp}.{k}": v.numpy() for k, v in st[grp].items()})
+        small.update({f"grad.{grp}.{k}": v for k, v in g[grp].items()})
+    sc = eng.read_scalars()
+    small["scalars"] = np.array([sc[k] for k in sorted(sc)], dtype=np.float64)
+    with open(os.path.join(out_dir, "scalars.names.txt"), "w") as f:
+        f.write("\n".join(sorted(sc)) + "\n")
+    per_elem = {n: getattr(eng, n).detach().cpu().numpy() for n in ("logits", "values", "vs", "pg_adv", "dlogits")}
+    budget = DUMP_LIMIT_BYTES - sum(a.nbytes for a in small.values())
+    big = sum(a.nbytes for a in per_elem.values())
+    if big > budget:  # axis 1 is the batch for every per-element array
+        B = per_elem["vs"].shape[1]
+        cols = np.sort(np.random.default_rng(12345).permutation(B)[:max(1, B * budget // big)])
+        per_elem = {n: a[:, cols] for n, a in per_elem.items()}
+    for name, a in {**small, **per_elem}.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def run_own_arm(args):
     import torch
 
@@ -458,7 +495,7 @@ def run_own_arm(args):
     eng.load_state(params0)
     for i, b in enumerate(batches):
         eng.fill_host(b, i)
-    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=eng.dev)  # 2x the 126 MB L2
+    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=eng.dev)  # 5x the 50 MB L2
 
     def flush():
         flush_buf.zero_()  # on the current (= engine) stream
@@ -504,6 +541,8 @@ def run_own_arm(args):
     dev_ms = max_over_ranks(sum(a.elapsed_time(b) for a, b in evs))
     launches = eng.launches_per_step * args.steps
     scal_dev = eng.read_scalars()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, args.dump_outputs)
 
     # ---------------- end to end through host buffers ----------------
     # software pipeline: the DMA of batch i+1 (copy stream) runs under the kernels of batch i;
@@ -557,19 +596,20 @@ def run_own_arm(args):
     with torch.cuda.stream(eng.stream):
         kern = kernel_breakdown(eng, flush, barrier=barrier)
     pk = peaks()
-    fp32_peak = SMS * FP32_LANES * 2 * pk["sm_max_mhz"] * 1e6 / 1e12  # TFLOP/s at max SM clock
-    tf32_peak = pk["bf16_tflops"] / 2.0  # tf32 UMMA rate = half the (measured) bf16 rate
+    sms = torch.cuda.get_device_properties(eng.dev).multi_processor_count
+    fp32_peak = sms * FP32_LANES * 2 * pk["sm_max_mhz"] * 1e6 / 1e12  # TFLOP/s at max SM clock
+    tf32_peak = pk["bf16_tflops"] / 2.0  # dense tf32 wgmma rate = half the bf16 rate
     H, O, A = eng.H_pi, eng.O, eng.A
     tc_on = os.environ.get("IMPALA_MLP_TC", "1") != "0" and O % 4 == 0 and A <= 4
     narrow = tc_on and 4 <= O <= 28 and H in (128, 256)                       # mlp_fwd_tc.cu / mlp_bwd_tc.cu
     wide = (tc_on and not narrow and 4 <= O <= 64 and H % 128 == 0 and H <= 4096
-            and os.environ.get("IMPALA_MLP_TCW", "1") != "0")                 # mlp_tcw.cu (c5)
+            and os.environ.get("IMPALA_MLP_TCW", "1") != "0")                 # wide shapes (c5)
     on_tc = narrow or wide
-    # tensor-core work actually issued: 3xTF32 (3 UMMAs per product).  Narrow kernels: forward and recompute
-    # K = [x | 1] padded to a multiple of 8, dW1 reduction over 32 output columns.  Wide kernels: K = O
-    # padded to 8 (the bias is added on the CUDA cores), dW1 reduction over 64 output columns.
-    kb = (O + 7) // 8 * 8
-    kf, ncol = ((O + 1 + 7) // 8 * 8, 32) if narrow else (kb, 64)
+    # tensor-core work actually issued: 3xTF32 (3 MMAs per product).  Forward and recompute: K = O padded
+    # to a multiple of 8 (the bias is added on the CUDA cores); dW1 reduction over O padded to 32 (one
+    # swizzle atom) or 64 output columns.
+    kf = (O + 7) // 8 * 8
+    ncol = 32 if O <= 32 else 64
     executed = {"mlp_forward(policy)": 2.0 * eng.M_pi * H * kf * 3, "mlp_forward(value_fn)": 2.0 * eng.M_vf * H * kf * 3,
                 "mlp_backward(policy)": 2.0 * eng.M_pi * H * (kf + ncol) * 3,
                 "mlp_backward(value_fn)": 2.0 * eng.M_vf * H * (kf + ncol) * 3}
@@ -598,19 +638,12 @@ def run_own_arm(args):
     for n in kernels:
         kernels[n]["in_step"] = n in in_step
     dom = max(in_step, key=lambda n: kernels[n]["us"])
-    traffic = None
-    # ncu dram__bytes per launch of the dominant kernel: profiles/dram_traffic.json is the c4 capture,
-    # other configs have their own file (dram_traffic_c5.json) or report null
-    prof = os.path.join(ROOT, "profiles", "dram_traffic.json" if args.config == "c4" else f"dram_traffic_{args.config}.json")
-    if os.path.exists(prof):
-        with open(prof) as f:
-            traffic = json.load(f).get(dom)
     src = {"hbm": pk["source"],
-           "tensor": f"tf32 UMMA peak = measured bf16 {pk['bf16_tflops']:.1f} TF/s / 2 ({pk['source']}); `achieved` counts "
+           "tensor": f"tf32 peak = bf16 {pk['bf16_tflops']:.1f} TF/s / 2 ({pk['source']}); `achieved` counts "
                      "ALGORITHMIC fp32 FLOPs (SURVEY 8d), `executed_tflops` the 3xTF32 / K-padded / recompute work issued",
-           "fp32": f"148 SMs x 128 FP32 lanes x 2 x {pk['sm_max_mhz']:.0f} MHz (max SM clock, {pk['source']}); "
+           "fp32": f"{sms} SMs x 128 FP32 lanes x 2 x {pk['sm_max_mhz']:.0f} MHz (max SM clock, {pk['source']}); "
                    "MEASURED_PEAKS has no FP32 figure"}[kernels[dom]["bound"]]
-    roofline = dict(kernel=dom, traffic=traffic, peak_source=src,
+    roofline = dict(kernel=dom, peak_source=src,
                     **{k: kernels[dom][k] for k in kernels[dom] if k not in ("us", "in_step")})
 
     # ---------------- weak scaling beside the strong line: B per GPU = the full workload batch
@@ -706,6 +739,9 @@ def main():
     ap.add_argument("--no-parity", action="store_true", help="skip the first-step oracle check")
     ap.add_argument("--no-weak", action="store_true", help="N > 1: skip the weak-scaling measurement")
     ap.add_argument("--no-learner", action="store_true", help="skip the run through Learner + RingQueue + actor processes")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (float32/float64, <= 64 MiB); "
+                         "with --gpus N > 1 rank 0 writes them, so the per-element arrays cover rank 0's batch shard")
     args = ap.parse_args()
     select_workload(args.config)
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * impala_b200.h - C ABI of the B200-native IMPALA learner hot path.
+ * impala_b200.h - C ABI of the GPU-native (H100, sm_90a) IMPALA learner hot path.
  *
  * Every entry point replaces a stretch of the reference learner's update
  * (threewisemonkeys-as/torched_impala, learner.py) that the reference executes as
@@ -42,7 +42,7 @@ extern "C" {
 
 #define IMPALA_PARAM_ALIGN 32 /* floats */
 
-/* Version / build info: returns the sm arch the library was compiled for (100). */
+/* Version / build info: returns the sm arch the library was compiled for (90). */
 int impala_abi_version(void);
 int impala_compiled_sm(void);
 

@@ -4,8 +4,8 @@ This is the second restatement: it keeps the reference's *execution structure*
 (python loop over trajectories, python loop over time for the V-trace recurrence,
 torch autograd, `clip_grad_norm_`, `torch.optim.Adam` + `LambdaLR`) so that, timed
 on host cores, it costs what the reference learner costs
-(`/root/reference/learner.py:75-183`).  It is what `bench.py` times as the CPU
-baseline (`cpu_baseline.kind = "port"`) on machines where `/root/reference` is not
+(`learner.py:75-183`).  It is what `bench.py` times as the CPU
+baseline (`cpu_baseline.kind = "port"`) on machines where the reference checkout is not
 present, and `tests/test_oracle_golden.py` pins it against outputs of the real
 reference.  Dropout (models.py:15,44) is the identity here: the parity setting is
 `.eval()` for both nets (SURVEY.md section 0.4).

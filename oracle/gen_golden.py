@@ -1,12 +1,12 @@
 """TEST INFRASTRUCTURE - generate tests/golden/*.npz by running the REAL reference.
 
-Run here (the authoring container), where /root/reference exists:
+Run where the reference checkout can be imported (oracle/refload.py):
 
     python -m oracle.gen_golden
 
 For every case below a seeded synthetic batch per update is converted to the
 reference wire format (lists of float64 tensors), pushed through the unmodified
-`/root/reference/learner.py::Learner._learn` via an in-process list queue, and the
+`learner.py::Learner._learn` via an in-process list queue, and the
 numbers the reference exposes are recorded: the five TensorBoard scalars of every
 update (`learner.py:217-240`) and both state_dicts after every update.  The
 per-element tensors the reference keeps in locals (`vt`, `pg_adv`, `learner.py:127-135`)

@@ -1,18 +1,18 @@
 """TEST INFRASTRUCTURE - recipe that materialises the UNMODIFIED reference under oracle/_ref/.
 
-    python -m oracle.make_ref            (needs /root/reference; run by __graft_entry__.build())
+    python -m oracle.make_ref            (needs the reference checkout; run by __graft_entry__.build())
 
 The reference is six pure-Python files with no package metadata (no setup.py / pyproject, so the
-base contract's `pip install ... /root/reference` has nothing to install) and nothing to compile.
+`pip install` has nothing to install) and nothing to compile.
 This recipe copies `learner.py models.py utils.py actor.py train.py` byte for byte from where
-they lie under /root/reference into `oracle/_ref/` - a build OUTPUT directory: git-ignored (no
-reference source ever enters the history), not gpurun-ignored (it travels to the GPU box like the
-built .so) - and writes the two stub modules the reference imports but this image lacks
+they lie in the reference checkout ($IMPALA_REFERENCE_DIR) into `oracle/_ref/` - a build OUTPUT directory: git-ignored (no
+reference source ever enters the history), shipped with the built .so to
+wherever the GPU tests run - and writes the two stub modules the reference imports but this image lacks
 (`gym` -> the in-repo old-API CartPole of oracle/cartpole_env.py, `pybullet_envs` -> empty).
 
 With oracle/_ref/ present, `bench.py --impl reference` and the `cpu_baseline` leg time the real
 `learner.Learner._learn` (`cpu_baseline.kind = "reference"`), and `tests/test_gpu_reference_train.py`
-runs the reference's own train.py / actor.py against the B200 learner.
+runs the reference's own train.py / actor.py against the GPU learner.
 """
 from __future__ import annotations
 

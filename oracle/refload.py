@@ -1,10 +1,10 @@
-"""TEST INFRASTRUCTURE - import the unmodified reference modules in this container.
+"""TEST INFRASTRUCTURE - import the unmodified reference modules.
 
-`/root/reference/utils.py:6-7` imports `gym` and `pybullet_envs`, neither of which is
+`utils.py:6-7` imports `gym` and `pybullet_envs`, neither of which is
 installed; two empty stub modules make `learner`, `models`, `utils`, `actor` import
 cleanly (SURVEY.md section 8c).  `device` is resolved at import time
-(`learner.py:13`), so CUDA is hidden first.  On the GPU box `/root/reference`
-does not exist; the modules then come from `oracle/_ref/` (see oracle/make_ref.py).
+(`learner.py:13`), so CUDA is hidden first.  Unless $IMPALA_REFERENCE_DIR names a reference
+checkout, the modules come from `oracle/_ref/` (see oracle/make_ref.py).
 """
 from __future__ import annotations
 
@@ -16,10 +16,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def reference_dir():
-    """Where the unmodified reference modules can be imported from: $IMPALA_REFERENCE_DIR, the
-    checkout under /root/reference (authoring container), or the copy oracle/make_ref.py left under
-    oracle/_ref/ (git-ignored build output that travels to the GPU box)."""
-    for d in (os.environ.get("IMPALA_REFERENCE_DIR"), "/root/reference", os.path.join(_HERE, "_ref")):
+    """Where the unmodified reference modules can be imported from: $IMPALA_REFERENCE_DIR, or the
+    copy oracle/make_ref.py left under oracle/_ref/ (git-ignored build output that travels to the
+    GPU machine)."""
+    for d in (os.environ.get("IMPALA_REFERENCE_DIR"), os.path.join(_HERE, "_ref")):
         if d and os.path.isfile(os.path.join(d, "learner.py")):
             return d
     return None
@@ -37,7 +37,7 @@ def load(env_factory=None):
     """
     ref_dir = reference_dir()
     if ref_dir is None:
-        raise RuntimeError("reference not found (no /root/reference and no oracle/_ref: run python -m oracle.make_ref)")
+        raise RuntimeError("reference not found (no $IMPALA_REFERENCE_DIR and no oracle/_ref: run python -m oracle.make_ref)")
     os.environ["CUDA_VISIBLE_DEVICES"] = ""
     if "torch" in sys.modules:
         import torch

@@ -1,4 +1,4 @@
-"""First-light check of the tcgen05 backward against the float64 oracle and the FP32 kernel."""
+"""First-light check of the wgmma backward against the float64 oracle and the FP32 kernel."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 """End to end THROUGH the product API: K synthetic actor processes -> RingQueue -> forked `Learner`
--> sm_100a kernels -> weight publication, for a BASELINE config (default c3: 32 CPU actors, one GPU).
+-> sm_90a kernels -> weight publication, for a BASELINE config (default c3: 32 CPU actors, one GPU).
 
     python scripts/learner_e2e.py [--config c3|c4] [--actors 32] [--updates 300] [--devices 1]
                                   [--payload block|trajectory] [--block 128]

@@ -1,4 +1,4 @@
-"""Wide tensor-core MLP kernels (mlp_tcw.cu) against the FP32 FFMA kernels on the same inputs:
+"""Wide tensor-core MLP kernels (two K atoms, hidden layer in passes) against the FP32 FFMA kernels on the same inputs:
 max abs difference and CUDA-event time of impala_mlp_forward / impala_mlp_backward per network.
 
     python scripts/time_mlp_wide.py [--M 819200] [--O 64] [--H 512] [--reps 5]

@@ -16,7 +16,7 @@ PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on a GPU machine)")
 
 
 def golden_names():

@@ -1,4 +1,4 @@
-"""Run the reference's OWN `train.py` + `actor.py` (unmodified, from oracle/_ref) against the B200 Learner.
+"""Run the reference's OWN `train.py` + `actor.py` (unmodified, from oracle/_ref) against the GPU Learner.
 
 BASELINE.json configs[0] (c1): CartPole, 2 CPU actors, T=20, batch=8, hidden=32.  Executed by
 test_gpu_reference_train.py in a fresh interpreter.  Nothing of the reference is edited:
@@ -31,7 +31,7 @@ def main():
     sys.path.insert(0, ROOT)
     sys.path.insert(0, REF)
     if not os.path.isfile(os.path.join(REF, "train.py")):
-        print("oracle/_ref missing: run python -m oracle.make_ref where /root/reference exists")
+        print("oracle/_ref missing: run python -m oracle.make_ref where the reference checkout exists")
         sys.exit(2)
     import torch
 

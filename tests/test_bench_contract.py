@@ -21,7 +21,7 @@ def run_bench(*args, timeout):
 
 
 def test_reference_arm_line():
-    """`--impl reference`: the unmodified reference learner (oracle/_ref or /root/reference; the
+    """`--impl reference`: the unmodified reference learner (oracle/_ref or $IMPALA_REFERENCE_DIR; the
     float64 port only where neither exists) on the same workload, here the small c3 config."""
     from oracle import refload
 

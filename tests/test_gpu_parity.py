@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a kernels (through the C ABI) against the float64 oracle.
+"""GPU parity: the sm_90a kernels (through the C ABI) against the float64 oracle.
 
 Tolerance (BASELINE.json north_star): V-trace targets, pg advantages and the three loss
 scalars within 1e-5 absolute of the reference in float32.  Gradients are compared
@@ -52,7 +52,7 @@ MLP_SHAPES = [
     (21 * 8, 4, 32, 2), (21 * 8, 4, 32, 1), (1000, 7, 40, 3), (1000, 7, 24, 1),
     (20 * 64 + 5, 24, 256, 4), (21 * 64, 24, 256, 1), (333, 64, 512, 4), (333, 64, 512, 1),
     (97, 32, 128, 16), (64, 8, 100, 5), (4097, 24, 256, 4), (86016, 24, 256, 1), (700, 28, 96, 3),
-    # wide tensor-core kernels (mlp_tcw.cu): O <= 64, H a multiple of 128, several tiles and passes per CTA
+    # wide tensor-core shapes (two K atoms, hidden layer in passes): O <= 64, H a multiple of 128, several tiles and passes per CTA
     (60001, 64, 512, 4), (60001, 64, 512, 1), (1000, 40, 384, 3), (130, 24, 512, 1), (257, 32, 128, 2),
     (5, 64, 512, 4), (129, 4, 512, 2),
 ]
@@ -61,7 +61,7 @@ MLP_SHAPES = [
 @pytest.mark.parametrize("tensor_cores", ["1", "0"])
 @pytest.mark.parametrize("M,O,H,N2", MLP_SHAPES)
 def test_mlp_forward(ops, monkeypatch, M, O, H, N2, tensor_cores):
-    """Both forward paths: tcgen05 3xTF32 (default where the layer is GEMM-shaped) and FP32 FFMA."""
+    """Both forward paths: wgmma 3xTF32 (default where the layer is GEMM-shaped) and FP32 FFMA."""
     monkeypatch.setenv("IMPALA_MLP_TC", tensor_cores)
     rng = np.random.default_rng(M + O + H + N2)
     p = synth.init_params(M, O, N2, H)["policy"]
@@ -75,7 +75,7 @@ def test_mlp_forward(ops, monkeypatch, M, O, H, N2, tensor_cores):
 @pytest.mark.parametrize("tensor_cores", ["1", "0"])
 @pytest.mark.parametrize("M,O,H,N2", MLP_SHAPES + [(96, 4, 128, 1), (4100, 8, 256, 3), (2500, 28, 128, 4)])
 def test_mlp_backward(ops, monkeypatch, M, O, H, N2, tensor_cores):
-    """Both backward paths (tcgen05 3xTF32 for H in {128,256}, O%4==0, O<=28; FP32 FFMA otherwise).
+    """Both backward paths (wgmma 3xTF32 for H in {128,256}, O%4==0, O<=28; FP32 FFMA otherwise).
 
     A ReLU unit whose pre-activation is within rounding of 0 may be switched differently than in
     float64; that moves one entry by one row's contribution, hence the tolerance term below."""

@@ -1,4 +1,4 @@
-"""GPU: the reference's unmodified train.py + actor.py (oracle/_ref) drive the B200 Learner - c1.
+"""GPU: the reference's unmodified train.py + actor.py (oracle/_ref) drive the GPU Learner - c1.
 
 BASELINE.json configs[0]: CartPole-v1, 2 CPU actors, T=20, batch=8, hidden=32.  See
 tests/reference_train_check.py for what is (not) touched."""
@@ -15,7 +15,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def test_unmodified_train_py_runs_against_the_b200_learner(tmp_path):
     if not os.path.isfile(os.path.join(ROOT, "oracle", "_ref", "train.py")):
         pytest.fail("oracle/_ref is missing: __graft_entry__.build() / python -m oracle.make_ref creates it "
-                    "where /root/reference exists, and it travels to the GPU box with the snapshot")
+                    "from the reference checkout, and it travels with the tree to the GPU machine")
     script = os.path.join(os.path.dirname(__file__), "reference_train_check.py")
     out = tmp_path / "logs"
     out.mkdir()

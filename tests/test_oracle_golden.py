@@ -1,6 +1,6 @@
 """CPU: both oracle restatements against the golden vectors of the real reference.
 
-The fixtures were produced by running the unmodified /root/reference/learner.py
+The fixtures were produced by running the unmodified reference learner.py
 (oracle/gen_golden.py); these tests pin the oracle without needing the reference.
 """
 import numpy as np

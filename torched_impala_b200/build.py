@@ -1,4 +1,4 @@
-"""In-tree build of libimpala_b200.so for sm_100a (nvcc, no torch extension machinery).
+"""In-tree build of libimpala_b200.so for sm_90a (H100) (nvcc, no torch extension machinery).
 
 `python -m torched_impala_b200.build` (or `__graft_entry__.build()`) compiles every
 translation unit under csrc/ in parallel and links them into
@@ -21,7 +21,7 @@ _LIB_DIR = os.environ.get("IMPALA_LIB_DIR", os.path.join(HERE, "lib"))
 OBJ = os.path.join(_LIB_DIR, "obj")
 LIB = os.path.join(_LIB_DIR, "libimpala_b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 MLP_WIDTHS = (8, 24, 32, 64)
 
@@ -37,7 +37,6 @@ def _units():
     units = [("mlp", "mlp.cu", []), ("vtrace_loss", "vtrace_loss.cu", []),
              ("optim", "optim.cu", []), ("abi", "abi.cu", []),
              ("mlp_fwd_tc", "mlp_fwd_tc.cu", []), ("mlp_bwd_tc", "mlp_bwd_tc.cu", []),
-             ("mlp_tcw", "mlp_tcw.cu", []),
              ("loss_terms", "loss_terms.cu", [])]
     for op in MLP_WIDTHS:
         for bwd in (0, 1):

@@ -9,7 +9,7 @@ extern "C" int impala_abi_version(void) { return 1; }
 
 extern "C" long long impala_launch_count(void) { return __atomic_load_n(&g_impala_launches, __ATOMIC_RELAXED); }
 
-extern "C" int impala_compiled_sm(void) { return 100; }
+extern "C" int impala_compiled_sm(void) { return 90; }
 
 extern "C" int impala_param_layout(int O, int H, int N2, int64_t offsets[4], int64_t* total) {
     if (O < 1 || H < 1 || N2 < 1 || !offsets || !total) return IMPALA_ERR_BAD_ARG;

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a learner kernels.
+// Shared helpers for the sm_90a learner kernels.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -84,14 +84,12 @@ __device__ __forceinline__ double warp_sum_f64(double x) {
 // anything their predecessor produces.  No kernel triggers early (no griddepcontrol.launch_dependents):
 // the trigger is the implicit one at the exit of each predecessor CTA, i.e. every write of the
 // predecessor precedes it, so the successor's CTAs are merely pre-staged - they occupy SMs as the
-// predecessor's CTAs drain and run their own prologue (barrier init, TMEM allocation, weight
-// staging, optimizer-state loads) while the last predecessor CTAs finish - and pdl_wait()
-// returns once the predecessor grid is complete and flushed.  (An early trigger at kernel start
+// predecessor's CTAs drain and run their own prologue (weight staging, optimizer-state loads) while
+// the last predecessor CTAs finish - and pdl_wait() returns once the predecessor grid is complete and flushed.  (An early trigger at kernel start
 // was measured first: the optimizer then read gradients the backward's reduction phase had not
 // written yet - tests/test_gpu_fullsize.py caught it - so the wait must not be relied on to cover
 // writes issued after a trigger.)  Inside a captured CUDA graph these launches become programmatic
-// edges.  Measured on the B200 (c4, 100 steps): 84.9 us per step with the attribute, 84.3 us without -
-// without an early trigger there is nothing left to overlap, so the attribute is OFF by default
+// edges.  Without an early trigger there is little left to overlap, so the attribute is OFF by default
 // (IMPALA_PDL=1 enables it; the waits are no-ops on plain launches).
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 

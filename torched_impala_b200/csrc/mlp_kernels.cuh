@@ -30,7 +30,7 @@ constexpr int kMaxParts = 1024;  // upper bound on persistent CTAs (= per-CTA pa
 int impala_mlp_launch(void (*kernel)(MlpArgs), const MlpArgs& a, const MlpConfig& c, size_t smem,
                       cudaStream_t st, int* grid_out);
 
-// Tensor-core (tcgen05, 3xTF32) forward for GEMM-shaped layers, defined in mlp_fwd_tc.cu.
+// Tensor-core (wgmma, 3xTF32) forward for GEMM-shaped layers, defined in mlp_fwd_tc.cu.
 bool impala_mlp_fwd_tc_eligible(const float* x, int M, int O, int H, int N2);
 int impala_mlp_fwd_tc(const float* x, const float* params, float* out, int M, int O, int H, int N2,
                       cudaStream_t st);
@@ -51,8 +51,8 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
                            int H_pi, int H_vf, int A, cudaStream_t st, const PushArgs* push = nullptr,
                            const double* extra = nullptr, int n_extra = 0);
 
-// Wide tensor-core kernels (mlp_tcw.cu): O <= 64, H a multiple of 128 (BASELINE c5: O = 64, H = 512).  The
-// forward needs no workspace; the backward leaves *nparts float32 partial rows in ws for
+// Wide tensor-core kernels (forward in mlp_fwd_tc.cu, backward in mlp_bwd_tc.cu): O <= 64, H a multiple
+// of 128 (BASELINE c5: O = 64, H = 512).  The forward needs no workspace; the backward leaves *nparts float32 partial rows in ws for
 // reduce_partials_kernel.  IMPALA_MLP_TCW=0 disables them.
 bool impala_mlp_tcw_eligible(const float* x, int M, int O, int H, int N2);
 int impala_mlp_fwd_tcw(const float* x, const float* params, float* out, int M, int O, int H, int N2,

@@ -1,9 +1,13 @@
-// Inline-PTX wrappers for the sm_100a tensor-core path: mbarrier, tcgen05 (TMEM alloc, UMMA
-// issue/commit, TMEM loads) and the shared-memory / instruction descriptors of
-// `tcgen05.mma.kind::tf32` with K-major, 128-byte-swizzled operands.
+// Inline-PTX wrappers for the sm_90a tensor-core path: warpgroup MMA (`wgmma.mma_async`, kind
+// tf32, fp32 accumulators in registers) with K-major, 128-byte-swizzled shared-memory operands,
+// and the 3xTF32 operand split.
 //
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix/instruction descriptor" tables
-// (same fields CuTe's UMMA::SmemDescriptor / UMMA::InstrDescriptor encode).
+// Descriptor bit layout follows the PTX ISA "Matrix Descriptor Format" table for wgmma (the same
+// fields CuTe's GMMA::DescriptorIterator encodes).  Fragment layouts (PTX ISA, "Register
+// Fragments" of wgmma .m64nNk8 with .tf32 inputs), for thread t of a warpgroup, warp w = t / 32,
+// g = (t % 32) / 4, q = t % 4:
+//   accumulator d[r]: row 16 w + g + 8 ((r >> 1) & 1), column 8 (r >> 2) + 2 q + (r & 1)
+//   A operand a[i]:   row 16 w + g + 8 (i & 1),        column q + 4 (i >> 1)
 #pragma once
 
 #include <cuda_runtime.h>
@@ -15,323 +19,94 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// one lane of a fully converged warp (same lane every time for the same mask)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-// ------------------------------------------------------------------ mbarrier
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_fence_init() {
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t"
-        "}" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-// producer side of a transaction barrier: one arrival + `bytes` expected from bulk copies
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
-                 "r"(bytes)
-                 : "memory");
-}
-// TMA bulk copy (no tensor map): `bytes` contiguous bytes global -> shared, completion counted on
-// `bar`.  src/dst 16-byte aligned, bytes a multiple of 16.
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes,
-                                         uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-            smem_u32(dst_smem)),
-        "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
-        : "memory");
-}
-// generic-proxy shared-memory writes -> visible to the async proxy (UMMA operand reads)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ------------------------------------------------------------------ TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(slot_in_smem)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// this thread's TMEM lane, 32 consecutive 32-bit columns starting at taddr's column
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31},"
-        "[%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-          "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-          "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+// named barrier over `nthreads` threads (multiple of 32); id 0 is __syncthreads
+__device__ __forceinline__ void named_bar(int id, int nthreads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// this thread's TMEM lane: write 32 consecutive 32-bit columns starting at taddr's column
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32"
-        "[%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16,"
-        " %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n"
-        :
-        : "r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-          "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-          "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])),
-          "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-          "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])),
-          "r"(__float_as_uint(v[15])), "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])),
-          "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])), "r"(__float_as_uint(v[20])),
-          "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-          "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])),
-          "r"(__float_as_uint(v[27])), "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])),
-          "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() {
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-
-// 16-column variants (this thread's TMEM lane, 16 consecutive 32-bit columns): finer-grained software
-// pipelining of TMEM traffic against CUDA-core math in the epilogues.  tmem_wait_ld / tmem_wait_st
-// complete ALL of the thread's outstanding loads / stores.
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32"
-        "[%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n"
-        :
-        : "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-          "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-
-// tcgen05.wait::ld that is also a compiler-visible dependency of the loaded registers: every use of
-// r[] stays behind it (a plain wait is only ordered against other volatile asm statements).
-__device__ __forceinline__ void tmem_wait_ld16(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld32(uint32_t (&r)[32]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                   "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]),
-                   "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-                 :
-                 : "memory");
-}
-
-// same without the wait, so several loads can be in flight; follow with tmem_wait_ld()
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31},"
-        "[%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-          "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-          "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait_ld() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ------------------------------------------------------------------ UMMA
+// ------------------------------------------------------------------ wgmma
 // K-major operand tile, rows of 128 bytes (32 tf32), SWIZZLE_128B, 8-row groups 1024 B apart.
-// `byte_off` selects the K step inside the 128-byte row (32 bytes per K=8 step).
+// `byte_off` selects the K step inside the 128-byte row (32 bytes per K = 8 step) or a later
+// 8-row group (multiples of 1024).  Tiles are 1024-byte aligned (base offset field 0).
 __device__ __forceinline__ uint64_t smem_desc_k_sw128(const void* tile, uint32_t byte_off) {
     const uint32_t addr = smem_u32(tile) + byte_off;
     uint64_t d = 0;
-    d |= static_cast<uint64_t>((addr >> 4) & 0x3fff);  // start address  [0,14)
-    d |= static_cast<uint64_t>(1) << 16;               // leading byte offset (unused, canonical 1)
+    d |= static_cast<uint64_t>((addr >> 4) & 0x3fff);  // start address          [0,14)
+    d |= static_cast<uint64_t>(1) << 16;               // leading byte offset (unused for swizzled K-major)
     d |= static_cast<uint64_t>(1024 >> 4) << 32;       // stride byte offset: next 8-row group
-    d |= static_cast<uint64_t>(1) << 46;               // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(2) << 61;               // SWIZZLE_128B
+    d |= static_cast<uint64_t>(1) << 62;               // SWIZZLE_128B
     return d;
 }
-// kind::tf32, fp32 accumulate, A and B K-major, M = 128, N = n (multiple of 16, <= 256).
-// (tf32 MN-major operands exist but only in the SWIZZLE_128B_BASE32B format, a different memory
-// image from the K-major tiles used here - the kernels transpose on the way into smem instead.)
-__device__ __forceinline__ uint32_t instr_desc_tf32_m128(uint32_t n) {
-    return (1u << 4)      // c_format = F32
-           | (2u << 7)    // a_format = TF32
-           | (2u << 10)   // b_format = TF32
-           | ((n >> 3) << 17) | ((128u >> 4) << 24);
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, bool accumulate) {
-    const uint32_t acc = accumulate ? 1u : 0u, zero = 0u;
+// the accumulator registers are not touched by the compiler across an in-flight wgmma
+__device__ __forceinline__ void fence_acc(float (&d)[16]) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#define IMPALA_WG_D16                                                                                   \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}"
+#define IMPALA_WG_D16_OPS(d)                                                                            \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),     \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]),        \
+        "+f"(d[15])
+
+// D[64, 32] (+)= A[64, 8] * B[32, 8]^T, both operands from shared memory (warpgroup-collective)
+__device__ __forceinline__ void wgmma_n32_ss(float (&d)[16], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc), "r"(zero)
-        : "memory");
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 " IMPALA_WG_D16 ", %16, %17, p, 1, 1;\n\t"
+        "}\n"
+        : IMPALA_WG_D16_OPS(d)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate ? 1 : 0));
 }
-// D[tmem] (+)= A[tmem] * B[smem]: A is read from TMEM (lane = row m, 8 consecutive columns =
-// the K = 8 slice), so only B costs shared-memory operand bandwidth.  Issued by ONE thread.
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                             uint32_t idesc, bool accumulate) {
-    const uint32_t acc = accumulate ? 1u : 0u, zero = 0u;
+// the same with A from registers (fragment layout in the header comment)
+__device__ __forceinline__ void wgmma_n32_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b_desc,
+                                             bool accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(acc), "r"(zero)
-        : "memory");
+        "setp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 " IMPALA_WG_D16 ", {%16, %17, %18, %19}, %20, p, 1, 1;\n\t"
+        "}\n"
+        : IMPALA_WG_D16_OPS(d)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate ? 1 : 0));
 }
-// arrive on `bar` once every UMMA issued so far by this thread has completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     smem_u32(bar))
-                 : "memory");
-}
+#undef IMPALA_WG_D16
+#undef IMPALA_WG_D16_OPS
 
 // ------------------------------------------------------------------ 3xTF32 operand split
 // hi = round-to-nearest tf32 of x (what the tensor core will see exactly), lo = x - hi (exact in
 // fp32; the tensor core truncates it to tf32, an error of 2^-21 relative to x).
-__device__ __forceinline__ float round_tf32(float x) {
-    uint32_t h;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(x));
-    return __uint_as_float(h);
-}
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
     uint32_t h;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(x));
     hi = __uint_as_float(h);
     lo = x - hi;
 }
-// Packed fp32 pairs (FFMA2 / FADD2 / FMUL2 on sm_100): one issue slot for two lanes of a
-// 64-bit register pair - the epilogues are issue-bound, so this is where their time goes.
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-    uint64_t d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;"
-        : "=l"(d)
-        : "l"(*reinterpret_cast<uint64_t*>(&a)), "l"(*reinterpret_cast<uint64_t*>(&b)),
-          "l"(*reinterpret_cast<uint64_t*>(&c)));
-    return *reinterpret_cast<float2*>(&d);
+__device__ __forceinline__ void split4(const float4& v, float4& hi, float4& lo) {
+    split_tf32(v.x, hi.x, lo.x);
+    split_tf32(v.y, hi.y, lo.y);
+    split_tf32(v.z, hi.z, lo.z);
+    split_tf32(v.w, hi.w, lo.w);
 }
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-    uint64_t d;
-    asm("add.rn.f32x2 %0, %1, %2;"
-        : "=l"(d)
-        : "l"(*reinterpret_cast<uint64_t*>(&a)), "l"(*reinterpret_cast<uint64_t*>(&b)));
-    return *reinterpret_cast<float2*>(&d);
-}
-__device__ __forceinline__ float2 fsub2(float2 a, float2 b) {
-    uint64_t d;
-    asm("sub.rn.f32x2 %0, %1, %2;"
-        : "=l"(d)
-        : "l"(*reinterpret_cast<uint64_t*>(&a)), "l"(*reinterpret_cast<uint64_t*>(&b)));
-    return *reinterpret_cast<float2*>(&d);
-}
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-    uint64_t d;
-    asm("mul.rn.f32x2 %0, %1, %2;"
-        : "=l"(d)
-        : "l"(*reinterpret_cast<uint64_t*>(&a)), "l"(*reinterpret_cast<uint64_t*>(&b)));
-    return *reinterpret_cast<float2*>(&d);
-}
+
 // byte offset of 16-byte chunk `c16` (0..7) of row `r` inside a K-major SWIZZLE_128B tile
 __device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t c16) {
     return (r >> 3) * 1024u + (r & 7u) * 128u + ((c16 ^ (r & 7u)) << 4);
-}
-
-// W1' = [W1 | b1 | 0] (H rows x 32 floats) split into tf32 hi / lo K-major SWIZZLE_128B tiles.
-// All global loads of a thread are issued before the first conversion so their latencies overlap
-// (the rows are L2-resident parameters; a load -> convert -> store loop would serialise ~8 round
-// trips).  nthreads <= 8 * 256 / MAXIT must hold for H <= 256: MAXIT = 8 covers >= 256 threads.
-__device__ __forceinline__ void stage_w1_tiles(uint8_t* w_hi, uint8_t* w_lo, const float* __restrict__ W1,
-                                               const float* __restrict__ b1, int H, int O, int tid,
-                                               int nthreads, bool bias_column = true) {
-    constexpr int MAXIT = 8;
-    const int ochunks = O >> 2;
-    float4 v[MAXIT];
-#pragma unroll
-    for (int it = 0; it < MAXIT; ++it) {
-        const int idx = tid + it * nthreads;
-        v[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (idx < H * 8) {
-            const int j = idx >> 3, c = idx & 7;
-            if (c < ochunks) v[it] = __ldg(reinterpret_cast<const float4*>(W1 + (size_t)j * O) + c);
-            else if (c == ochunks && bias_column) v[it].x = __ldg(b1 + j);
-        }
-    }
-#pragma unroll
-    for (int it = 0; it < MAXIT; ++it) {
-        const int idx = tid + it * nthreads;
-        if (idx < H * 8) {
-            float4 hi, lo;
-            split_tf32(v[it].x, hi.x, lo.x);
-            split_tf32(v[it].y, hi.y, lo.y);
-            split_tf32(v[it].z, hi.z, lo.z);
-            split_tf32(v[it].w, hi.w, lo.w);
-            const uint32_t off = sw128_offset(idx >> 3, idx & 7);
-            *reinterpret_cast<float4*>(w_hi + off) = hi;
-            *reinterpret_cast<float4*>(w_lo + off) = lo;
-        }
-    }
 }
 
 }  // namespace tc

@@ -385,11 +385,10 @@ int launch_s(const VtArgs& a, bool vec, unsigned groups, int nw, int cl, cudaStr
 constexpr int kMaxCluster = 8;  // portable cluster size
 
 // Steps per thread (S), warps per CTA (nw) and CTAs per cluster (cl); wide action sets trade S for
-// registers.  Measured on B200 (scripts/tune_vtrace.py, ncu): S = 2; up to 10 segments (T <= 20) one CTA
-// holds the whole unroll in one chunk; longer unrolls walk chunks of 8 x S steps with 8 warps per CTA
-// (T = 100, B = 8192: 17.4 us).  Spreading the segments of a long unroll over a thread-block cluster
-// (DSMEM carry exchange, cl = 4 / 8) works but measured SLOWER - 34-42 us at T = 100, B = 8192: the
-// cluster barriers cost more than the chunk loop they replace - so cl = 1 unless overridden.
+// registers.  S = 2; up to 10 segments (T <= 20) one CTA holds the whole unroll in one chunk; longer
+// unrolls walk chunks of 8 x S steps with 8 warps per CTA.  Spreading the segments of a long unroll
+// over a thread-block cluster (DSMEM carry exchange, cl = 4 / 8) works, but its cluster barriers
+// replace a cheap chunk loop, so cl = 1 unless overridden (scripts/tune_vtrace.py compares them).
 // IMPALA_VTRACE_S / IMPALA_VTRACE_NSEG (warps per CTA) / IMPALA_VTRACE_CLUSTER override the choice.
 template <bool WITH_LOSS>
 int launch(VtArgs& a, cudaStream_t st) {

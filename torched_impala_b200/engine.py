@@ -1,4 +1,4 @@
-"""Host-side step engine of the B200 learner: buffers, streams, CUDA graph, peer buffers.
+"""Host-side step engine of the GPU learner: buffers, streams, CUDA graph, peer buffers.
 
 One `LearnerEngine` lives in the learner process of one GPU.  It owns every device
 buffer of the update path and enqueues, per learner step, exactly the C-ABI calls of

@@ -1,7 +1,7 @@
-"""Drop-in `Learner` for the reference's actor/learner split, running the update on B200s.
+"""Drop-in `Learner` for the reference's actor/learner split, running the update on the GPU.
 
 Same constructor, lifecycle methods, events, checkpoint format and module-level loss
-helpers as `/root/reference/learner.py` (constructor `:18-28`, `start/terminate/join`
+helpers as `learner.py` (constructor `:18-28`, `start/terminate/join`
 `:55-65`, `_learn` `:67-275`, `save/load/policy_weights` `:277-295`, helpers `:298-321`),
 so `train.py:69` and the unmodified `actor.py` (`:68,70,118,121`) work against it:
 
@@ -18,7 +18,7 @@ path of the device (SURVEY 8f-2, 8f-4):
 
   * `_learn` packs each trajectory into a pinned, zero-padded time-major host slab (replacing the
     torch.stack calls at `:104-109,117`) and hands the batch to `engine.LearnerEngine`, i.e. to the
-    sm_100a kernels behind include/impala_b200.h; batch i+1 is collected and DMA'd while the
+    sm_90a kernels behind include/impala_b200.h; batch i+1 is collected and DMA'd while the
     kernels of batch i run;
   * weight publication: only the POLICY is published (it is all `actor.py:70` reads; `train.py:67`
     shares only the policy): after the step an in-stream device copy freezes the policy block, a
@@ -453,10 +453,8 @@ class Learner:
                 # a slab goes back to the actors when its DMA has completed.  Do not WAIT for that here
                 # unless the ring would otherwise run dry (or both device slabs' events are in use): the
                 # next batch is collected and its DMA queued right behind the running one, so the copy
-                # engine never idles for the host part of an iteration (B200 box, c4, 32 actor processes:
-                # 3 079 -> 3 273 updates/s; IMPALA_LOOP_STATS=1 then shows 169 us of the 280 us per update still
-                # spent waiting here - the 10 MB DMA out of the shared-memory ring the actors are writing into
-                # runs at ~37 GB/s where a quiet pinned buffer gives 54 GB/s - and ~110 us of host calls)
+                # engine never idles for the host part of an iteration (IMPALA_LOOP_STATS=1 shows how long
+                # an update still waits here)
                 t0 = clock()
                 while to_release:
                     ev, kk = to_release[0]

@@ -2,7 +2,7 @@
 
 The reference has no (T, B) tensor anywhere: a "batch" is `batch_size` python
 `Trajectory` objects pulled one at a time from the queue
-(`/root/reference/learner.py:89-117`).  The B200 learner's device layout is
+(`learner.py:89-117`).  The GPU learner's device layout is
 time-major and dense:
 
     obs        (T+1, B, O) f32   index T is the bootstrap observation slot

@@ -1,8 +1,8 @@
 """Boundary types of the learner hot path.
 
 These are the three containers that cross the actor -> learner boundary in the
-reference (`/root/reference/utils.py:17-45` Hyperparameters, `:48-77`
-Trajectory, `:80-92` Counter).  The B200 learner consumes the reference's own
+reference (`utils.py:17-45` Hyperparameters, `:48-77`
+Trajectory, `:80-92` Counter).  The GPU learner consumes the reference's own
 objects unchanged (it only duck-types on attribute names); the definitions
 here exist so that the package, its tests and its benchmark are self-contained
 on a machine that does not have the reference checked out.  Field names and
