@@ -1,4 +1,6 @@
-"""Device-resident learner step time for any BASELINE config (c2..c5): CUDA events, L2 flushed."""
+"""Device-resident learner step time for any BASELINE config (c2..c5) or the Atari-RAM shape: CUDA events,
+L2 flushed.  --compare-tc also times the FP32 FFMA MLP path (IMPALA_MLP_TC=0) in the same process,
+alternating step by step with the default path, so both numbers see the same clocks and neighbours."""
 import argparse
 import os
 import statistics
@@ -12,27 +14,43 @@ from torched_impala_b200.engine import LearnerEngine  # noqa: E402
 from torched_impala_b200.utils import default_hparams  # noqa: E402
 
 CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256), "c5": dict(T=100, B=8192, O=64, A=4, H=512),
-       "c3": dict(T=20, B=1024, O=24, A=4, H=256), "c2": dict(T=20, B=256, O=4, A=2, H=32)}
+       "c3": dict(T=20, B=1024, O=24, A=4, H=256), "c2": dict(T=20, B=256, O=4, A=2, H=32),
+       # Atari from RAM (128-byte observation, 18 actions): P = 70 931 parameters, 50 675 712 input bytes
+       # and 24.4 GFLOP of MLP work per step (SURVEY 8d formulas)
+       "ram": dict(T=20, B=4096, O=128, A=18, H=256)}
 ap = argparse.ArgumentParser()
 ap.add_argument("--config", default="c5")
 ap.add_argument("--steps", type=int, default=30)
+ap.add_argument("--compare-tc", action="store_true", help="alternate with IMPALA_MLP_TC=0 and report both")
 a = ap.parse_args()
 w = CFG[a.config]
 hp = default_hparams(batch_size=w["B"], max_timesteps=w["T"])
-eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp)
-eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
-eng.load_device_batch(synth.make_batch(1, w["T"], w["B"], w["O"], w["A"]))
+arms = {"default": os.environ.get("IMPALA_MLP_TC", "1")}
+if a.compare_tc:
+    arms = {"tc": "1", "fp32 (IMPALA_MLP_TC=0)": "0"}
+engines = {}
+for name, tc in arms.items():
+    os.environ["IMPALA_MLP_TC"] = tc  # read by the C library at every launch (and at graph capture)
+    eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp)
+    eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
+    eng.load_device_batch(synth.make_batch(1, w["T"], w["B"], w["O"], w["A"]))
+    engines[name] = eng
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-ts = []
-with torch.cuda.stream(eng.stream):
-    for i in range(a.steps + 5):
-        flush.zero_()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(eng.stream)
-        eng.step(0)
-        e1.record(eng.stream)
-        e1.synchronize()
-        if i >= 5:
-            ts.append(e0.elapsed_time(e1) * 1e3)
-print(f"{a.config} {w}: median {statistics.median(ts):.1f} us/step ({1e6 / statistics.median(ts):.0f} steps/s), "
-      f"loss {eng.read_scalars()['total_loss']:.5f}")
+ts = {name: [] for name in arms}
+for i in range(a.steps + 5):
+    for name, eng in engines.items():
+        os.environ["IMPALA_MLP_TC"] = arms[name]
+        with torch.cuda.stream(eng.stream):
+            flush.zero_()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(eng.stream)
+            eng.step(0)
+            e1.record(eng.stream)
+            e1.synchronize()
+            if i >= 5:
+                ts[name].append(e0.elapsed_time(e1) * 1e3)
+dev = torch.cuda.get_device_name()
+for name, eng in engines.items():
+    med = statistics.median(ts[name])
+    print(f"{a.config} {w} [{name}] on {dev}: median {med:.1f} us/step ({1e6 / med:.0f} steps/s), "
+          f"loss {eng.read_scalars()['total_loss']:.5f}")

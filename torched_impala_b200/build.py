@@ -23,7 +23,7 @@ LIB = os.path.join(_LIB_DIR, "libimpala_b200.so")
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
-MLP_WIDTHS = (8, 24, 32, 64)
+MLP_WIDTHS = (8, 24, 32, 64, 128)
 
 
 def _nvcc() -> str:

@@ -75,16 +75,26 @@ bool pick_config(int O, int H, int N2, bool bwd, MlpConfig* c) {
     else if (O <= 24) c->op = 24;
     else if (O <= 32) c->op = 32;
     else if (O <= 64) c->op = 64;
+    else if (O <= 128) c->op = 128;
     else return false;
     if (N2 <= 1) c->np = 1;
     else if (N2 <= 4) c->np = 4;
     else if (N2 <= 16) c->np = 16;
+    else if (N2 <= 32) c->np = 32;
     else return false;
-    // register budget: forward holds JPT*OP weights, backward 2*JPT*OP (weights + gradient); at OP = 64
-    // the backward splits the features of a hidden unit over a lane pair (ks = 2: 2 x 32 + 2 x 32)
-    c->ks = (bwd && c->op == 64) ? 2 : 1;
-    if (H < 128 || (bwd && c->op == 64)) c->jpt = 1, c->maxt = bwd && H >= 128 ? 256 : 128;
-    else c->jpt = 2, c->maxt = 256;
+    if (c->op == 128 || c->np == 32) {
+        // wide observations or outputs: one hidden unit per thread (the forward then holds at most 256
+        // units); the backward splits a unit's features over a lane quad from OP = 64 up (ks = 4: 2 x 32
+        // at OP = 128) and over a lane pair below it, and at NP = 32 its W2 column as well
+        c->jpt = 1, c->maxt = 256;
+        c->ks = bwd ? (c->op >= 64 ? 4 : 2) : 1;
+    } else {
+        // register budget: forward holds JPT*OP weights, backward 2*JPT*OP (weights + gradient); at OP = 64
+        // the backward splits the features of a hidden unit over a lane pair (ks = 2: 2 x 32 + 2 x 32)
+        c->ks = (bwd && c->op == 64) ? 2 : 1;
+        if (H < 128 || (bwd && c->op == 64)) c->jpt = 1, c->maxt = bwd && H >= 128 ? 256 : 128;
+        else c->jpt = 2, c->maxt = 256;
+    }
     const int want = (int)impala_round_up((int64_t)c->ks * ((H + c->jpt - 1) / c->jpt), 32);
     if (bwd) {
         c->threads = want < c->maxt ? want : c->maxt;
@@ -114,7 +124,8 @@ int dispatch(bool bwd, const MlpArgs& a, const MlpConfig& c, size_t smem, cudaSt
         case 8: return bwd ? impala_mlp_bwd_op8(a, c, smem, st, grid) : impala_mlp_fwd_op8(a, c, smem, st, grid);
         case 24: return bwd ? impala_mlp_bwd_op24(a, c, smem, st, grid) : impala_mlp_fwd_op24(a, c, smem, st, grid);
         case 32: return bwd ? impala_mlp_bwd_op32(a, c, smem, st, grid) : impala_mlp_fwd_op32(a, c, smem, st, grid);
-        default: return bwd ? impala_mlp_bwd_op64(a, c, smem, st, grid) : impala_mlp_fwd_op64(a, c, smem, st, grid);
+        case 64: return bwd ? impala_mlp_bwd_op64(a, c, smem, st, grid) : impala_mlp_fwd_op64(a, c, smem, st, grid);
+        default: return bwd ? impala_mlp_bwd_op128(a, c, smem, st, grid) : impala_mlp_fwd_op128(a, c, smem, st, grid);
     }
 }
 
@@ -167,6 +178,8 @@ extern "C" int impala_mlp_forward(const float* x, const float* params, float* ou
         return impala_mlp_fwd_tc(x, params, out, M, O, H, N2, (cudaStream_t)stream);
     if (!(tc_env && tc_env[0] == '0') && impala_mlp_tcw_eligible(x, M, O, H, N2))
         return impala_mlp_fwd_tcw(x, params, out, M, O, H, N2, (cudaStream_t)stream);
+    if (!(tc_env && tc_env[0] == '0') && impala_mlp_fwd_tcx_eligible(x, M, O, H, N2))
+        return impala_mlp_fwd_tcx(x, params, out, M, O, H, N2, (cudaStream_t)stream);
     MlpArgs a{};
     MlpConfig c{};
     size_t smem;
@@ -222,9 +235,12 @@ extern "C" int impala_mlp_backward(const float* x, const float* params, const fl
         (reinterpret_cast<uintptr_t>(grad) & 15) == 0)
         return impala_mlp_bwd_tc(x, params, dout, a.ws, grad, static_cast<unsigned int*>(workspace), M, O, H,
                                  N2, (cudaStream_t)stream);  // reduces in-kernel
-    const bool wide = !(tc_env && tc_env[0] == '0') && impala_mlp_tcw_eligible(x, M, O, H, N2);
-    const int rc = wide ? impala_mlp_bwd_tcw(x, params, dout, a.ws, M, O, H, N2, (cudaStream_t)stream, &grid)
-                        : dispatch(true, a, c, smem, (cudaStream_t)stream, &grid);
+    const bool tc_on = !(tc_env && tc_env[0] == '0');
+    const bool wide = tc_on && impala_mlp_tcw_eligible(x, M, O, H, N2);
+    const bool widex = tc_on && !wide && impala_mlp_bwd_tcx_eligible(x, M, O, H, N2);
+    const int rc = wide    ? impala_mlp_bwd_tcw(x, params, dout, a.ws, M, O, H, N2, (cudaStream_t)stream, &grid)
+                   : widex ? impala_mlp_bwd_tcx(x, params, dout, a.ws, M, O, H, N2, (cudaStream_t)stream, &grid)
+                           : dispatch(true, a, c, smem, (cudaStream_t)stream, &grid);
     if (rc != IMPALA_OK) return rc;
     const int64_t total = a.lay.total;
     reduce_partials_kernel<<<(unsigned)((total + 31) / 32), kRedWarps * 32, 0,

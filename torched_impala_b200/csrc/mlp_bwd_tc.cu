@@ -10,7 +10,8 @@
 //                          db1 += DP
 //   GEMM2 (RS, reduction)  dW1_blk[64 hid, K] += DP[64 hid, 64 rows] * X[64 rows, K]
 //
-// K = the observation width padded to 32 (one 128-byte swizzle atom) or 64 (two atoms, BASELINE c5).
+// K = the observation width padded to 32 (one 128-byte swizzle atom), 64 (two atoms, BASELINE c5) or
+// 128 (four atoms, Atari RAM; see bwd_tc_body).
 // DP never leaves the registers: the GEMM1 accumulator layout of a thread (two hidden units, 16 batch
 // columns) becomes the A operand of GEMM2 directly, by reordering the batch rows INSIDE each group of
 // 8 in the B operand of GEMM2 (K is a sum, so any order does, as long as A and B agree): A fragment
@@ -58,10 +59,13 @@ struct BwdTcArgs {
 };
 
 __host__ __device__ constexpr size_t bwd_smem_bytes(int ka, int np) {
-    // W1 block hi / lo [KA][128 hidden][128 B] + x hi / lo [KA][64][128 B] + x^T hi / lo
-    // [2 K atoms][32 KA features][128 B] + dz [64][NP] + db2 exchange
-    return 1024 + (size_t)2 * ka * kHB * 128 + (size_t)2 * ka * kXAtomBytes + (size_t)2 * 2 * 32 * ka * 128 +
-           (size_t)kRowsT * np * sizeof(float) + 4 * sizeof(float);
+    // W1 block hi / lo [KA][128 hidden][128 B] + x hi / lo [KA][RT rows][128 B] + x^T hi / lo
+    // [RT / 32 K atoms][32 KA features][128 B] + dz [RT][NPS] + db2 exchange; NP = 32 (layer 2 through
+    // shared memory): + W2 block [128 hidden][NPS] + db2 exchange [8 warps][32]
+    return 1024 + (size_t)2 * ka * kHB * 128 + (size_t)2 * ka * (ka == 4 ? 32 : kRowsT) * 128 +
+           (size_t)2 * ((ka == 4 ? 32 : kRowsT) / 32) * 32 * ka * 128 +
+           (size_t)(ka == 4 ? 32 : kRowsT) * (np > 4 ? np + 4 : np) * sizeof(float) +
+           (np > 4 ? (size_t)kHB * (np + 4) * sizeof(float) + 8 * 32 * sizeof(float) : 4 * sizeof(float));
 }
 
 // component e of a float4 (e known at compile time)
@@ -70,21 +74,39 @@ __device__ __forceinline__ float f4(const float4& v, int e) { return e == 0 ? v.
 // One persistent CTA's share of a network's backward: CTA `cta` of `ncta` takes tiles cta,
 // cta + ncta, ... and leaves its float32 partial gradient in row `cta` of a.ws.  Returns a shared
 // memory region of >= 16 KiB the caller may use as scratch once every thread is past it.
+//
+// KA = 4 (observations up to 128): the dW1 accumulators of all four feature atoms would be 128
+// registers per thread, so a pass holds one 64-feature half of dW1 (two atoms) and the hidden blocks
+// are walked once per half, GEMM1 re-run for each (x is re-read once per pass).  Tiles are 32 batch rows
+// so that W1 hi / lo of 128 hidden units, the tile and its transpose fit in shared memory.
+// NP = 32 (17..32 outputs): layer 2 goes through shared memory - the pass's W2 block [128][NP + 4]
+// (rows padded so the lanes of a quad, two batch rows or hidden units apart, hit different banks) -
+// and dW2 is formed per tile in chunks of 8 outputs, summed over the quad and kept by lane q for
+// outputs [8 q, 8 q + 8).  dW2 / db1 are accumulated in the first feature half only.
 template <int NP, int KA>
 __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int cta, const int ncta) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+    constexpr bool X4 = KA == 4;
+    constexpr bool L2S = NP > 4;                      // layer 2 through shared memory
+    constexpr int RT = X4 ? 32 : kRowsT;             // batch rows per tile
+    constexpr int NB = RT / 32;                       // N = 32 halves of GEMM1 / K atoms of GEMM2
+    constexpr int FA = X4 ? 2 : KA;                   // feature atoms of dW1 per pass
+    constexpr int NPS = L2S ? NP + 4 : NP;            // row stride of dz (and W2) in shared memory
+    constexpr int NPR = L2S ? 1 : NP;                 // layer-2 values held in registers
+    constexpr int kXA = RT * 128;                     // one x atom: RT rows x 128 B
     constexpr int kWBytes = KA * kHB * 128;          // one of hi / lo, [KA][128 rows][128 B]
-    constexpr int kXBytes = KA * kXAtomBytes;        // one of hi / lo, [KA][64 rows][128 B]
+    constexpr int kXBytes = KA * kXA;                // one of hi / lo, [KA][RT rows][128 B]
     constexpr int kXtAtomBytes = 32 * KA * 128;      // 32 batch rows of K x 32 KA feature rows
     uint8_t* w_hi = smem;
     uint8_t* w_lo = w_hi + kWBytes;
     uint8_t* x_hi = w_lo + kWBytes;
     uint8_t* x_lo = x_hi + kXBytes;
-    uint8_t* xt_hi = x_lo + kXBytes;                 // [2 K atoms][32 KA rows][128 B]
-    uint8_t* xt_lo = xt_hi + 2 * kXtAtomBytes;
-    float* dzs = reinterpret_cast<float*>(xt_lo + 2 * kXtAtomBytes);  // [64 rows][NP]
-    float* gb2x = dzs + kRowsT * NP;                                   // [4]
+    uint8_t* xt_hi = x_lo + kXBytes;                 // [NB K atoms][32 KA rows][128 B]
+    uint8_t* xt_lo = xt_hi + NB * kXtAtomBytes;
+    float* dzs = reinterpret_cast<float*>(xt_lo + NB * kXtAtomBytes);  // [RT rows][NPS]
+    float* gb2x = dzs + RT * NPS;                                      // [4] | [8 warps][32]
+    float* w2s = gb2x + (L2S ? 8 * 32 : 4);                            // L2S: [128 hidden][NPS]
 
     const int tid = threadIdx.x, wg = tid >> 7, lt = tid & 127, warp = lt >> 5, lane = tid & 31;
     const int g = lane >> 2, q = lane & 3;
@@ -95,27 +117,36 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
     float* wsb = a.ws + (size_t)cta * a.lay.total;  // this CTA's partial gradient row
 
     // x rows of a tile -> registers (chunk idx = tid + kThreads k is (row idx / (8 KA), 16-byte chunk
-    // idx % (8 KA))); dz row `tid` for tid < 64
-    constexpr int kLd = kRowsT * 8 * KA / kThreads;
+    // idx % (8 KA))); dz row `tid` for tid < RT (L2S: dz row tid / 8, outputs 4 (tid % 8) .. + 3)
+    constexpr int kLd = RT * 8 * KA / kThreads;
+    constexpr int NZ = L2S ? 4 : NP;
     float4 v[kLd];
-    float z[NP];
+    float z[NZ];
     auto load = [&](int tile) {
 #pragma unroll
         for (int k = 0; k < kLd; ++k) {
             const int idx = tid + kThreads * k, r = idx / (8 * KA), c = idx % (8 * KA);
-            const int row = tile * kRowsT + r;
+            const int row = tile * RT + r;
             v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (tile < a.num_tiles && row < a.M && c < ochunks)
                 v[k] = __ldg(reinterpret_cast<const float4*>(a.x + (size_t)row * O) + c);
         }
-        const int row = tile * kRowsT + tid;
+        if constexpr (L2S) {
+            static_assert(RT * NP == 4 * kThreads, "one float4 of dz per thread");
+            const int row = tile * RT + (tid >> 3), n0 = 4 * (tid & 7);
 #pragma unroll
-        for (int n = 0; n < NP; ++n)
-            z[n] = (tid < kRowsT && tile < a.num_tiles && row < a.M && n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
+            for (int n = 0; n < 4; ++n)
+                z[n] = (tile < a.num_tiles && row < a.M && n0 + n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n0 + n) : 0.f;
+        } else {
+            const int row = tile * RT + tid;
+#pragma unroll
+            for (int n = 0; n < NP; ++n)
+                z[n] = (tid < RT && tile < a.num_tiles && row < a.M && n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
+        }
     };
-    float gb2[NP];  // db2 = column sums of dout: this thread's rows (tid < 64), first pass only
+    float gb2[NZ];  // db2 = column sums of dout: this thread's dz values, first pass only
 #pragma unroll
-    for (int n = 0; n < NP; ++n) gb2[n] = 0.f;
+    for (int n = 0; n < NZ; ++n) gb2[n] = 0.f;
 
     // pads of the partial row
     {
@@ -128,38 +159,54 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
 
     // dz of the tile is the output of the kernel before this one (PDL, common.cuh)
     pdl_wait();
-    const int npass = H / kHB;
+    const int nfh = X4 ? (O + 63) / 64 : 1;  // feature halves of dW1
+    const int npass = H / kHB * nfh;
     for (int p = 0; p < npass; ++p) {
+        const int blk = X4 ? p / nfh : p, fh = X4 ? p % nfh : 0;
+        const bool l2 = X4 ? fh == 0 : true;  // this pass forms db1 / dW2 (and, first of all, db2)
+        const int fa0 = X4 ? 2 * fh : 0;      // first feature atom of this pass's dW1
         // ---- this pass's W1 rows -> hi / lo swizzled tiles (warpgroup w: rows [64 w, 64 w + 64))
         __syncthreads();  // the previous pass is done with the weights
         for (int idx = tid; idx < kHB * 8 * KA; idx += kThreads) {
             const int r = idx / (8 * KA), c = idx % (8 * KA);
             float4 w = make_float4(0.f, 0.f, 0.f, 0.f), hi, lo;
-            if (c < ochunks) w = __ldg(reinterpret_cast<const float4*>(W1 + (size_t)(p * kHB + r) * O) + c);
+            if (c < ochunks) w = __ldg(reinterpret_cast<const float4*>(W1 + (size_t)(blk * kHB + r) * O) + c);
             tc::split4(w, hi, lo);
             const uint32_t off = (r >> 6) * (KA * 64 * 128) + (c >> 3) * (64 * 128) + tc::sw128_offset(r & 63, c & 7);
             *reinterpret_cast<float4*>(w_hi + off) = hi;
             *reinterpret_cast<float4*>(w_lo + off) = lo;
         }
+        if constexpr (L2S) {
+            for (int idx = tid; idx < kHB * NP; idx += kThreads) {
+                const int j = idx / NP, n = idx - j * NP;
+                w2s[j * NPS + n] = n < a.N2 ? __ldg(W2 + (size_t)n * H + blk * kHB + j) : 0.f;
+            }
+        }
         uint8_t* wa_hi = w_hi + wg * (KA * 64 * 128);  // this warpgroup's A operand of GEMM1
         uint8_t* wa_lo = w_lo + wg * (KA * 64 * 128);
         // the thread's two hidden units
-        const int j0 = p * kHB + 64 * wg + 16 * warp + g, j1 = j0 + 8;
+        const int j0 = blk * kHB + 64 * wg + 16 * warp + g, j1 = j0 + 8;
         const float bj0 = __ldg(b1 + j0), bj1 = __ldg(b1 + j1);
-        float w2r0[NP], w2r1[NP], gw0[NP], gw1[NP], gb10 = 0.f, gb11 = 0.f;
+        float w2r0[NPR], w2r1[NPR], gw0[NPR], gw1[NPR], gb10 = 0.f, gb11 = 0.f;
+        float gq0[L2S ? 8 : 1], gq1[L2S ? 8 : 1];  // L2S: dW2 of outputs [8 q, 8 q + 8)
+        if constexpr (L2S) {
 #pragma unroll
-        for (int n = 0; n < NP; ++n) {
-            w2r0[n] = n < a.N2 ? __ldg(W2 + (size_t)n * H + j0) : 0.f;
-            w2r1[n] = n < a.N2 ? __ldg(W2 + (size_t)n * H + j1) : 0.f;
-            gw0[n] = gw1[n] = 0.f;
+            for (int k = 0; k < 8; ++k) gq0[k] = gq1[k] = 0.f;
+        } else {
+#pragma unroll
+            for (int n = 0; n < NP; ++n) {
+                w2r0[n] = n < a.N2 ? __ldg(W2 + (size_t)n * H + j0) : 0.f;
+                w2r1[n] = n < a.N2 ? __ldg(W2 + (size_t)n * H + j1) : 0.f;
+                gw0[n] = gw1[n] = 0.f;
+            }
         }
-        float acc_hh[KA][16], acc_c[KA][16];  // dW1: dp_hi * x_hi | dp_hi * x_lo + dp_lo * x_hi
+        float acc_hh[FA][16], acc_c[FA][16];  // dW1: dp_hi * x_hi | dp_hi * x_lo + dp_lo * x_hi
 #pragma unroll
-        for (int fa = 0; fa < KA; ++fa)
+        for (int fa = 0; fa < FA; ++fa)
 #pragma unroll
             for (int i = 0; i < 16; ++i) acc_hh[fa][i] = acc_c[fa][i] = 0.f;
 #pragma unroll
-        for (int fa = 0; fa < KA; ++fa) tc::fence_acc(acc_hh[fa]), tc::fence_acc(acc_c[fa]);
+        for (int fa = 0; fa < FA; ++fa) tc::fence_acc(acc_hh[fa]), tc::fence_acc(acc_c[fa]);
 
         load(cta);
         for (int tile = cta, it = 0; tile < a.num_tiles; tile += ncta, ++it) {
@@ -170,7 +217,7 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
                 const int idx = tid + kThreads * k, r = idx / (8 * KA), c = idx % (8 * KA);
                 float4 hi, lo;
                 tc::split4(v[k], hi, lo);
-                const uint32_t off = (c >> 3) * kXAtomBytes + tc::sw128_offset(r, c & 7);
+                const uint32_t off = (c >> 3) * kXA + tc::sw128_offset(r, c & 7);
                 *reinterpret_cast<float4*>(x_hi + off) = hi;
                 *reinterpret_cast<float4*>(x_lo + off) = lo;
                 // batch row r -> K atom r / 32, position 8 kk + (qq >> 1) + 4 (qq & 1) with r % 32 = 8 kk + qq
@@ -184,7 +231,13 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
                     *reinterpret_cast<float*>(xt_lo + toff) = f4(lo, e);
                 }
             }
-            if (tid < kRowsT) {
+            if constexpr (L2S) {
+                *reinterpret_cast<float4*>(dzs + (tid >> 3) * NPS + 4 * (tid & 7)) = make_float4(z[0], z[1], z[2], z[3]);
+                if (p == 0) {
+#pragma unroll
+                    for (int n = 0; n < 4; ++n) gb2[n] += z[n];
+                }
+            } else if (tid < RT) {
 #pragma unroll
                 for (int n = 0; n < NP; ++n) {
                     dzs[tid * NP + n] = z[n];
@@ -195,24 +248,24 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
             __syncthreads();
             load(tile + ncta);  // in flight during this tile's MMAs and epilogue
 
-            // ---- GEMM1: PRE = W1_blk * X^T (two N = 32 halves of the tile's batch rows)
-            float d[2][16];
+            // ---- GEMM1: PRE = W1_blk * X^T (N = 32 halves of the tile's batch rows)
+            float d[NB][16];
 #pragma unroll
-            for (int nb = 0; nb < 2; ++nb)
+            for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
                 for (int i = 0; i < 16; ++i) d[nb][i] = 0.f;
             // the zeroed accumulators are defined HERE, before the warpgroup fence: left alone, the compiler
             // sinks the moves behind the K-step guards, past the fence, and ptxas then serializes every wgmma
-            tc::fence_acc(d[0]);
-            tc::fence_acc(d[1]);
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb) tc::fence_acc(d[nb]);
             tc::wgmma_fence();
 #pragma unroll
-            for (int nb = 0; nb < 2; ++nb) {
+            for (int nb = 0; nb < NB; ++nb) {
 #pragma unroll
                 for (int kk = 0; kk < 4 * KA; ++kk) {
                     if (kk < ksteps) {
                         const uint32_t wo = (kk >> 2) * (64 * 128) + (kk & 3) * 32;
-                        const uint32_t xo = (kk >> 2) * kXAtomBytes + nb * 32 * 128 + (kk & 3) * 32;
+                        const uint32_t xo = (kk >> 2) * kXA + nb * 32 * 128 + (kk & 3) * 32;
                         tc::wgmma_n32_ss(d[nb], tc::smem_desc_k_sw128(wa_lo, wo), tc::smem_desc_k_sw128(x_hi, xo), kk > 0);
                         tc::wgmma_n32_ss(d[nb], tc::smem_desc_k_sw128(wa_hi, wo), tc::smem_desc_k_sw128(x_lo, xo), true);
                     }
@@ -221,67 +274,143 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
                 for (int kk = 0; kk < 4 * KA; ++kk) {
                     if (kk < ksteps) {
                         const uint32_t wo = (kk >> 2) * (64 * 128) + (kk & 3) * 32;
-                        const uint32_t xo = (kk >> 2) * kXAtomBytes + nb * 32 * 128 + (kk & 3) * 32;
+                        const uint32_t xo = (kk >> 2) * kXA + nb * 32 * 128 + (kk & 3) * 32;
                         tc::wgmma_n32_ss(d[nb], tc::smem_desc_k_sw128(wa_hi, wo), tc::smem_desc_k_sw128(x_hi, xo), true);
                     }
                 }
             }
             tc::wgmma_commit();
             tc::wgmma_wait<0>();
-            tc::fence_acc(d[0]);
-            tc::fence_acc(d[1]);
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb) tc::fence_acc(d[nb]);
 
             // ---- epilogue: d <- DP in place (thread: hidden units j0 / j1, batch columns 8 i + 2 q + e)
+            if constexpr (L2S) {
+                const float* w2a = w2s + (64 * wg + 16 * warp + g) * NPS;  // unit j0 of the block
+                const float* w2b = w2a + 8 * NPS;
+                if (l2) {
+                    // dW2 in chunks of 8 outputs: the quad's partial sums meet, lane q keeps chunk q
 #pragma unroll
-            for (int nb = 0; nb < 2; ++nb) {
+                    for (int cc = 0; cc < 4; ++cc) {
+                        float s0[8], s1[8];
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
+                        for (int k = 0; k < 8; ++k) s0[k] = s1[k] = 0.f;
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int m = 32 * nb + 8 * i + 2 * q + e;
-                        float dz[NP];
-                        if constexpr (NP == 4) {
-                            const float4 t = *reinterpret_cast<const float4*>(dzs + 4 * m);
-                            dz[0] = t.x, dz[1] = t.y, dz[2] = t.z, dz[3] = t.w;
-                        } else {
-                            dz[0] = dzs[m];
+                        for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+                            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    const int m = 32 * nb + 8 * i + 2 * q + e;
+                                    const float h0 = fmaxf(d[nb][4 * i + e] + bj0, 0.f);
+                                    const float h1 = fmaxf(d[nb][4 * i + 2 + e] + bj1, 0.f);
+                                    const float4 za = *reinterpret_cast<const float4*>(dzs + m * NPS + 8 * cc);
+                                    const float4 zb = *reinterpret_cast<const float4*>(dzs + m * NPS + 8 * cc + 4);
+#pragma unroll
+                                    for (int k = 0; k < 8; ++k) {
+                                        const float zk = k < 4 ? f4(za, k) : f4(zb, k - 4);
+                                        s0[k] = fmaf(zk, h0, s0[k]), s1[k] = fmaf(zk, h1, s1[k]);
+                                    }
+                                }
+#pragma unroll
+                        for (int k = 0; k < 8; ++k) {
+                            s0[k] += __shfl_xor_sync(IMPALA_FULL_MASK, s0[k], 1);
+                            s1[k] += __shfl_xor_sync(IMPALA_FULL_MASK, s1[k], 1);
+                            s0[k] += __shfl_xor_sync(IMPALA_FULL_MASK, s0[k], 2);
+                            s1[k] += __shfl_xor_sync(IMPALA_FULL_MASK, s1[k], 2);
                         }
-                        // relu'(0) = 0 as in torch
-                        const float pre0 = d[nb][4 * i + e] + bj0, pre1 = d[nb][4 * i + 2 + e] + bj1;
-                        const float h0 = fmaxf(pre0, 0.f), h1 = fmaxf(pre1, 0.f);
-                        float dh0 = dz[0] * w2r0[0], dh1 = dz[0] * w2r1[0];
+                        if (q == cc) {
 #pragma unroll
-                        for (int n = 1; n < NP; ++n) dh0 = fmaf(dz[n], w2r0[n], dh0), dh1 = fmaf(dz[n], w2r1[n], dh1);
+                            for (int k = 0; k < 8; ++k) gq0[k] += s0[k], gq1[k] += s1[k];
+                        }
+                    }
+                }
 #pragma unroll
-                        for (int n = 0; n < NP; ++n) gw0[n] = fmaf(dz[n], h0, gw0[n]), gw1[n] = fmaf(dz[n], h1, gw1[n]);
-                        const float dp0 = pre0 > 0.f ? dh0 : 0.f, dp1 = pre1 > 0.f ? dh1 : 0.f;
-                        gb10 += dp0, gb11 += dp1;
-                        d[nb][4 * i + e] = dp0, d[nb][4 * i + 2 + e] = dp1;
+                for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int m = 32 * nb + 8 * i + 2 * q + e;
+                            const float pre0 = d[nb][4 * i + e] + bj0, pre1 = d[nb][4 * i + 2 + e] + bj1;
+                            float dh0 = 0.f, dh1 = 0.f;
+#pragma unroll
+                            for (int n = 0; n < NP; n += 4) {
+                                const float4 zv = *reinterpret_cast<const float4*>(dzs + m * NPS + n);
+                                const float4 wa = *reinterpret_cast<const float4*>(w2a + n);
+                                const float4 wb = *reinterpret_cast<const float4*>(w2b + n);
+                                dh0 = fmaf(zv.x, wa.x, dh0), dh0 = fmaf(zv.y, wa.y, dh0);
+                                dh0 = fmaf(zv.z, wa.z, dh0), dh0 = fmaf(zv.w, wa.w, dh0);
+                                dh1 = fmaf(zv.x, wb.x, dh1), dh1 = fmaf(zv.y, wb.y, dh1);
+                                dh1 = fmaf(zv.z, wb.z, dh1), dh1 = fmaf(zv.w, wb.w, dh1);
+                            }
+                            const float dp0 = pre0 > 0.f ? dh0 : 0.f, dp1 = pre1 > 0.f ? dh1 : 0.f;
+                            gb10 += dp0, gb11 += dp1;
+                            d[nb][4 * i + e] = dp0, d[nb][4 * i + 2 + e] = dp1;
+                        }
+            } else {
+#pragma unroll
+                for (int nb = 0; nb < NB; ++nb) {
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int m = 32 * nb + 8 * i + 2 * q + e;
+                            float dz[NP];
+                            if constexpr (NP == 4) {
+                                const float4 t = *reinterpret_cast<const float4*>(dzs + 4 * m);
+                                dz[0] = t.x, dz[1] = t.y, dz[2] = t.z, dz[3] = t.w;
+                            } else {
+                                dz[0] = dzs[m];
+                            }
+                            // relu'(0) = 0 as in torch
+                            const float pre0 = d[nb][4 * i + e] + bj0, pre1 = d[nb][4 * i + 2 + e] + bj1;
+                            const float h0 = fmaxf(pre0, 0.f), h1 = fmaxf(pre1, 0.f);
+                            float dh0 = dz[0] * w2r0[0], dh1 = dz[0] * w2r1[0];
+#pragma unroll
+                            for (int n = 1; n < NP; ++n) dh0 = fmaf(dz[n], w2r0[n], dh0), dh1 = fmaf(dz[n], w2r1[n], dh1);
+                            if (!X4 || l2) {
+#pragma unroll
+                                for (int n = 0; n < NP; ++n) gw0[n] = fmaf(dz[n], h0, gw0[n]), gw1[n] = fmaf(dz[n], h1, gw1[n]);
+                            }
+                            const float dp0 = pre0 > 0.f ? dh0 : 0.f, dp1 = pre1 > 0.f ? dh1 : 0.f;
+                            gb10 += dp0, gb11 += dp1;
+                            d[nb][4 * i + e] = dp0, d[nb][4 * i + 2 + e] = dp1;
+                        }
                     }
                 }
             }
 
             // ---- GEMM2: dW1 += DP * X (A = DP from registers).  Phase 1: dp_lo * x_hi; phase 2 (DP
             // overwritten by dp_hi in place): dp_hi * x_lo, then dp_hi * x_hi into its own accumulator.
-            uint32_t lo[2][16];
+            // X4: round-to-nearest split (lo of either sign), so the tensor core's truncation of lo does not
+            // pull every product of the longer K = 128 reductions towards zero
+            uint32_t lo[NB][16];
 #pragma unroll
-            for (int nb = 0; nb < 2; ++nb)
+            for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
                 for (int i = 0; i < 16; ++i) {
-                    const float hi = __uint_as_float(__float_as_uint(d[nb][i]) & 0xffffe000u);
-                    lo[nb][i] = __float_as_uint(d[nb][i] - hi);
-                    d[nb][i] = hi;
+                    if constexpr (X4) {
+                        float hi, lof;
+                        tc::split_tf32(d[nb][i], hi, lof);
+                        lo[nb][i] = __float_as_uint(lof);
+                        d[nb][i] = hi;
+                    } else {
+                        const float hi = __uint_as_float(__float_as_uint(d[nb][i]) & 0xffffe000u);
+                        lo[nb][i] = __float_as_uint(d[nb][i] - hi);
+                        d[nb][i] = hi;
+                    }
                 }
             tc::wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < 8; ++kk) {
+            for (int kk = 0; kk < 4 * NB; ++kk) {
                 const int nb = kk >> 2, i = kk & 3;
                 const uint32_t al[4] = {lo[nb][4 * i], lo[nb][4 * i + 2], lo[nb][4 * i + 1], lo[nb][4 * i + 3]};
                 const uint32_t ah[4] = {__float_as_uint(d[nb][4 * i]), __float_as_uint(d[nb][4 * i + 2]),
                                         __float_as_uint(d[nb][4 * i + 1]), __float_as_uint(d[nb][4 * i + 3])};
 #pragma unroll
-                for (int fa = 0; fa < KA; ++fa) {
-                    const uint32_t xo = nb * kXtAtomBytes + fa * 32 * 128 + i * 32;
+                for (int fa = 0; fa < FA; ++fa) {
+                    const uint32_t xo = nb * kXtAtomBytes + (fa0 + fa) * 32 * 128 + i * 32;
                     tc::wgmma_n32_rs(acc_c[fa], al, tc::smem_desc_k_sw128(xt_hi, xo), true);
                     tc::wgmma_n32_rs(acc_c[fa], ah, tc::smem_desc_k_sw128(xt_lo, xo), true);
                     tc::wgmma_n32_rs(acc_hh[fa], ah, tc::smem_desc_k_sw128(xt_hi, xo), true);
@@ -291,38 +420,51 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
             tc::wgmma_wait<0>();
             // the A registers are read asynchronously: keep them (and the accumulators) untouched until here
 #pragma unroll
-            for (int nb = 0; nb < 2; ++nb) {
+            for (int nb = 0; nb < NB; ++nb) {
                 tc::fence_acc(d[nb]);
 #pragma unroll
                 for (int i = 0; i < 16; ++i) asm volatile("" : "+r"(lo[nb][i])::"memory");
             }
 #pragma unroll
-            for (int fa = 0; fa < KA; ++fa) tc::fence_acc(acc_hh[fa]), tc::fence_acc(acc_c[fa]);
+            for (int fa = 0; fa < FA; ++fa) tc::fence_acc(acc_hh[fa]), tc::fence_acc(acc_c[fa]);
         }
 
         // ---- end of the pass: the quad's column sets meet (fixed order); dW1 / db1 / dW2 of the block
+        if (!X4 || l2) {
 #pragma unroll
-        for (int s = 1; s <= 2; s <<= 1) {
-            gb10 += __shfl_xor_sync(IMPALA_FULL_MASK, gb10, s);
-            gb11 += __shfl_xor_sync(IMPALA_FULL_MASK, gb11, s);
+            for (int s = 1; s <= 2; s <<= 1) {
+                gb10 += __shfl_xor_sync(IMPALA_FULL_MASK, gb10, s);
+                gb11 += __shfl_xor_sync(IMPALA_FULL_MASK, gb11, s);
 #pragma unroll
-            for (int n = 0; n < NP; ++n) {
-                gw0[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gw0[n], s);
-                gw1[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gw1[n], s);
+                for (int n = 0; n < NPR; ++n) {
+                    if constexpr (!L2S) {
+                        gw0[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gw0[n], s);
+                        gw1[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gw1[n], s);
+                    }
+                }
+            }
+            if (q == 0) {
+                wsb[a.lay.ob1 + j0] = gb10;
+                wsb[a.lay.ob1 + j1] = gb11;
+                if constexpr (!L2S) {
+#pragma unroll
+                    for (int n = 0; n < NP; ++n)
+                        if (n < a.N2) wsb[a.lay.oW2 + (size_t)n * H + j0] = gw0[n], wsb[a.lay.oW2 + (size_t)n * H + j1] = gw1[n];
+                }
+            }
+            if constexpr (L2S) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) {
+                    const int n = 8 * q + k;
+                    if (n < a.N2) wsb[a.lay.oW2 + (size_t)n * H + j0] = gq0[k], wsb[a.lay.oW2 + (size_t)n * H + j1] = gq1[k];
+                }
             }
         }
-        if (q == 0) {
-            wsb[a.lay.ob1 + j0] = gb10;
-            wsb[a.lay.ob1 + j1] = gb11;
 #pragma unroll
-            for (int n = 0; n < NP; ++n)
-                if (n < a.N2) wsb[a.lay.oW2 + (size_t)n * H + j0] = gw0[n], wsb[a.lay.oW2 + (size_t)n * H + j1] = gw1[n];
-        }
-#pragma unroll
-        for (int fa = 0; fa < KA; ++fa) {
+        for (int fa = 0; fa < FA; ++fa) {
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                const int f = 32 * fa + 8 * i + 2 * q;  // features f, f + 1 (O % 4 == 0: both or neither valid)
+                const int f = 32 * (fa0 + fa) + 8 * i + 2 * q;  // features f, f + 1 (O % 4 == 0: both or neither valid)
                 if (f < O) {
                     *reinterpret_cast<float2*>(wsb + a.lay.oW1 + (size_t)j0 * O + f) =
                         make_float2(acc_hh[fa][4 * i] + acc_c[fa][4 * i], acc_hh[fa][4 * i + 1] + acc_c[fa][4 * i + 1]);
@@ -333,21 +475,42 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
         }
     }
 
-    // db2: fixed-order tree over the 64 threads that loaded dz rows
+    if constexpr (L2S) {
+        // db2: thread t holds outputs 4 (t % 8) .. + 3 of rows t / 8 (+ 32 k); lanes l, l ^ 8, l ^ 16, l ^ 24
+        // hold the same outputs, then the 8 warps meet through shared memory (fixed order)
 #pragma unroll
-    for (int n = 0; n < NP; ++n) {
+        for (int n = 0; n < 4; ++n) {
+            gb2[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gb2[n], 8);
+            gb2[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gb2[n], 16);
+        }
+        if (lane < 8) {
 #pragma unroll
-        for (int off = 16; off > 0; off >>= 1) gb2[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gb2[n], off);
-    }
-    if (tid == 32) {
+            for (int n = 0; n < 4; ++n) gb2x[(tid >> 5) * 32 + 4 * lane + n] = gb2[n];
+        }
+        __syncthreads();
+        if (tid < a.N2) {
+            float s = 0.f;
 #pragma unroll
-        for (int n = 0; n < NP; ++n) gb2x[n] = gb2[n];
-    }
-    __syncthreads();
-    if (tid == 0) {
+            for (int w = 0; w < kWarps; ++w) s += gb2x[w * 32 + tid];
+            wsb[a.lay.ob2 + tid] = s;
+        }
+    } else {
+        // db2: fixed-order tree over the 64 threads that loaded dz rows
 #pragma unroll
-        for (int n = 0; n < NP; ++n)
-            if (n < a.N2) wsb[a.lay.ob2 + n] = gb2[n] + gb2x[n];
+        for (int n = 0; n < NP; ++n) {
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) gb2[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gb2[n], off);
+        }
+        if (tid == 32) {
+#pragma unroll
+            for (int n = 0; n < NP; ++n) gb2x[n] = gb2[n];
+        }
+        __syncthreads();
+        if (tid == 0) {
+#pragma unroll
+            for (int n = 0; n < NP; ++n)
+                if (n < a.N2) wsb[a.lay.ob2 + n] = gb2[n] + gb2x[n];
+        }
     }
     __threadfence();  // this thread's partial-row stores are visible device-wide
     __syncthreads();
@@ -576,6 +739,35 @@ int impala_mlp_bwd_tcw(const float* x, const float* params, const float* dout, f
     const size_t smem = bwd_smem_bytes(ka, N2 == 1 ? 1 : 4);
     auto kernel = ka == 1 ? (N2 == 1 ? mlp_bwd_tcw_kernel<1, 1> : mlp_bwd_tcw_kernel<4, 1>)
                           : (N2 == 1 ? mlp_bwd_tcw_kernel<1, 2> : mlp_bwd_tcw_kernel<4, 2>);
+    cudaError_t e;
+    int sms = 0, per_sm = 0;
+    if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
+    if ((e = opt_in(kernel, smem)) != cudaSuccess) return (int)e;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem)) != cudaSuccess) return (int)e;
+    if (per_sm < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    int grid = per_sm * sms;
+    if (grid > a.num_tiles) grid = a.num_tiles;
+    if (grid > kMaxParts) grid = kMaxParts;
+    if ((e = impala_launch(kernel, grid, kThreads, smem, st, true, a)) != cudaSuccess) return (int)e;
+    *nparts = grid;
+    return impala_launch_status();
+}
+
+// Beyond the wide kernels' limits (impala_mlp_bwd_tcx_eligible): four K atoms, GEMM2 in 64-feature halves,
+// 32-row tiles; 17..32 outputs through shared memory.  Partial rows as impala_mlp_bwd_tcw.
+bool impala_mlp_bwd_tcx_eligible(const float* x, int M, int O, int H, int N2) {
+    return M >= 1 && O >= 4 && O <= 128 && (O & 3) == 0 && H >= 128 && H % 128 == 0 && H <= 4096 && N2 >= 1 &&
+           N2 <= 32 && (O > 64 || N2 > 16) && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
+           impala_env_int("IMPALA_MLP_TCW", 1) != 0;
+}
+
+int impala_mlp_bwd_tcx(const float* x, const float* params, const float* dout, float* ws, int M, int O, int H,
+                       int N2, cudaStream_t st, int* nparts) {
+    BwdTcArgs a = make_bwd_args(x, params, dout, ws, nullptr, nullptr, M, O, H, N2);
+    a.num_tiles = (M + 31) / 32;  // 32-row tiles at four K atoms
+    const int np = N2 == 1 ? 1 : (N2 <= 4 ? 4 : 32);
+    const size_t smem = bwd_smem_bytes(4, np);
+    auto kernel = np == 1 ? mlp_bwd_tcw_kernel<1, 4> : (np == 4 ? mlp_bwd_tcw_kernel<4, 4> : mlp_bwd_tcw_kernel<32, 4>);
     cudaError_t e;
     int sms = 0, per_sm = 0;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;

@@ -12,7 +12,7 @@
 //
 // The accumulator of a 32-unit slice of the hidden layer is 16 registers per thread, so the CUDA
 // cores see each hidden activation exactly once, in the registers wgmma left it in: bias, ReLU and
-// the tiny second layer (<= 4 outputs) run on the thread's two rows and eight columns, and the four
+// the small second layer (<= 32 outputs) run on the thread's two rows and eight columns, and the four
 // threads of a quad that share a row combine their partial sums with two shuffles (fixed order).
 //
 // One CTA = kWG independent warpgroups, each owning its own 64-row tiles and x stage; the weights
@@ -45,9 +45,13 @@ struct FwdTcArgs {
     MlpLayout lay;
 };
 
+// W2 rows in shared memory are padded to NP + 4 at NP = 32: the lanes of a quad read hidden units two
+// apart, and with 128-byte rows their 16-byte loads would fall into one bank group
+__host__ __device__ constexpr int w2s_stride(int np) { return np > 4 ? np + 4 : np; }
+
 __host__ __device__ constexpr size_t fwd_smem_bytes(int hb, int ka, int np) {
     return 1024 /*alignment slack*/ + (size_t)2 * ka * hb * 128 + (size_t)kWG * 2 * ka * kXAtomBytes +
-           (size_t)hb * (np + 1) * sizeof(float);
+           (size_t)hb * (w2s_stride(np) + 1) * sizeof(float);
 }
 
 // One CTA's share of a network: CTA `cta` of `ncta`; warpgroup w takes tiles u, u + ncta * kWG, ...
@@ -64,7 +68,8 @@ __device__ __forceinline__ void fwd_tc_body(const FwdTcArgs& a, const int cta, c
     uint8_t* x_hi = w_lo + KA * HB * 128 + wg * 2 * KA * kXAtomBytes;  // this warpgroup's [KA][64 rows][128 B]
     uint8_t* x_lo = x_hi + KA * kXAtomBytes;
     float* b1s = reinterpret_cast<float*>(smem + 2 * KA * HB * 128 + kWG * 2 * KA * kXAtomBytes);  // [HB]
-    float* w2s = b1s + HB;                                                                         // [HB][NP]
+    float* w2s = b1s + HB;                                                                         // [HB][NPS]
+    constexpr int NPS = w2s_stride(NP);
 
     const int O = a.O, ochunks = O >> 2, ksteps = (O + 7) >> 3;
     const float* __restrict__ W1 = a.params + a.lay.oW1;
@@ -104,7 +109,7 @@ __device__ __forceinline__ void fwd_tc_body(const FwdTcArgs& a, const int cta, c
         for (int idx = tid; idx < HB; idx += kThreads) b1s[idx] = __ldg(b1 + p * HB + idx);
         for (int idx = tid; idx < HB * NP; idx += kThreads) {
             const int j = idx / NP, n = idx - j * NP;
-            w2s[idx] = n < a.N2 ? __ldg(W2 + (size_t)n * a.H + p * HB + j) : 0.f;
+            w2s[j * NPS + n] = n < a.N2 ? __ldg(W2 + (size_t)n * a.H + p * HB + j) : 0.f;
         }
         tc::fence_proxy_async();
         __syncthreads();
@@ -164,12 +169,15 @@ __device__ __forceinline__ void fwd_tc_body(const FwdTcArgs& a, const int cta, c
                         const float bj = b1s[j];
                         const float h0 = fmaxf(d[4 * i + e] + bj, 0.f);
                         const float h1 = fmaxf(d[4 * i + 2 + e] + bj, 0.f);
-                        if constexpr (NP == 4) {
-                            const float4 w = *reinterpret_cast<const float4*>(w2s + 4 * j);
-                            p0[0] = fmaf(h0, w.x, p0[0]), p0[1] = fmaf(h0, w.y, p0[1]);
-                            p0[2] = fmaf(h0, w.z, p0[2]), p0[3] = fmaf(h0, w.w, p0[3]);
-                            p1[0] = fmaf(h1, w.x, p1[0]), p1[1] = fmaf(h1, w.y, p1[1]);
-                            p1[2] = fmaf(h1, w.z, p1[2]), p1[3] = fmaf(h1, w.w, p1[3]);
+                        if constexpr (NP % 4 == 0) {
+#pragma unroll
+                            for (int n = 0; n < NP; n += 4) {
+                                const float4 w = *reinterpret_cast<const float4*>(w2s + NPS * j + n);
+                                p0[n] = fmaf(h0, w.x, p0[n]), p0[n + 1] = fmaf(h0, w.y, p0[n + 1]);
+                                p0[n + 2] = fmaf(h0, w.z, p0[n + 2]), p0[n + 3] = fmaf(h0, w.w, p0[n + 3]);
+                                p1[n] = fmaf(h1, w.x, p1[n]), p1[n + 1] = fmaf(h1, w.y, p1[n + 1]);
+                                p1[n + 2] = fmaf(h1, w.z, p1[n + 2]), p1[n + 3] = fmaf(h1, w.w, p1[n + 3]);
+                            }
                         } else {
                             const float w = w2s[j];
                             p0[0] = fmaf(h0, w, p0[0]), p1[0] = fmaf(h1, w, p1[0]);
@@ -313,4 +321,28 @@ int impala_mlp_fwd_tcw(const float* x, const float* params, float* out, int M, i
     const FwdTcArgs a = make_fwd_args(x, params, out, M, O, H, N2);
     if (O <= 32) return N2 == 1 ? launch_fwd<1, 1>(a, st) : launch_fwd<4, 1>(a, st);
     return N2 == 1 ? launch_fwd<1, 2>(a, st) : launch_fwd<4, 2>(a, st);
+}
+
+// Beyond the wide kernels' limits: observations up to 128 (four K atoms) or 17..32 outputs (the
+// epilogue keeps 2 x 32 partial sums per thread).  Shapes that the kernels above take never get here.
+bool impala_mlp_fwd_tcx_eligible(const float* x, int M, int O, int H, int N2) {
+    return M >= 1 && O >= 4 && O <= 128 && (O & 3) == 0 && H >= 128 && H % 128 == 0 && H <= 4096 && N2 >= 1 &&
+           N2 <= 32 && (O > 64 || N2 > 16) && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
+           impala_env_int("IMPALA_MLP_TCW", 1) != 0;
+}
+
+int impala_mlp_fwd_tcx(const float* x, const float* params, float* out, int M, int O, int H, int N2,
+                       cudaStream_t st) {
+    FwdTcArgs a = make_fwd_args(x, params, out, M, O, H, N2);
+    if (N2 > 16) {
+        if (O <= 32) return launch_fwd<32, 1>(a, st);
+        if (O <= 64) {
+            a.hb = 128;  // 256 units would need 235 520 B with the padded W2 rows
+            return launch_fwd<32, 2>(a, st);
+        }
+    }
+    // four K atoms: 64 hidden units per pass keep W1 hi / lo + both warpgroups' x stages in 227 KB
+    a.hb = 64;
+    if (N2 > 16) return launch_fwd<32, 4>(a, st);
+    return N2 == 1 ? launch_fwd<1, 4>(a, st) : launch_fwd<4, 4>(a, st);
 }

@@ -3,7 +3,7 @@
 #include "mlp_kernels.cuh"
 
 #ifndef IMPALA_OP
-#error "compile with -DIMPALA_OP=<8|24|32|64> -DIMPALA_BWD=<0|1>"
+#error "compile with -DIMPALA_OP=<8|24|32|64|128> -DIMPALA_BWD=<0|1>"
 #endif
 
 #define CAT_(a, b) a##b
@@ -12,9 +12,11 @@
 #if IMPALA_BWD
 #define KERNEL impala_mlp::mlp_bwd_kernel
 #define ENTRY CAT(impala_mlp_bwd_op, IMPALA_OP)
+#define KS_WIDE , (IMPALA_OP >= 64 ? 4 : 2)  // lanes per hidden unit of the wide shapes (mlp.cu pick_config)
 #else
 #define KERNEL impala_mlp::mlp_fwd_kernel
 #define ENTRY CAT(impala_mlp_fwd_op, IMPALA_OP)
+#define KS_WIDE
 #endif
 
 #define BY_NP(JPT, MAXT)                                                                      \
@@ -32,6 +34,17 @@
     }
 
 int ENTRY(const MlpArgs& a, const MlpConfig& c, size_t smem, cudaStream_t st, int* grid) {
+#if IMPALA_OP == 128
+    // only shapes beyond the O <= 64 limit get here: one hidden unit per thread (per lane quad backward)
+    switch (c.np) {
+        case 1: return impala_mlp_launch(KERNEL<1, 128, 1, 256 KS_WIDE>, a, c, smem, st, grid);
+        case 4: return impala_mlp_launch(KERNEL<1, 128, 4, 256 KS_WIDE>, a, c, smem, st, grid);
+        case 16: return impala_mlp_launch(KERNEL<1, 128, 16, 256 KS_WIDE>, a, c, smem, st, grid);
+        default: return impala_mlp_launch(KERNEL<1, 128, 32, 256 KS_WIDE>, a, c, smem, st, grid);
+    }
+#else
+    // 17..32 outputs: one hidden unit per thread (per lane group backward)
+    if (c.np == 32) return impala_mlp_launch(KERNEL<1, IMPALA_OP, 32, 256 KS_WIDE>, a, c, smem, st, grid);
 #if IMPALA_BWD && IMPALA_OP == 64
     // wide observations: a lane pair per hidden unit (KS = 2), see mlp_kernels.cuh
     if (c.maxt == 128) { BY_NP_KS2(128) }
@@ -39,5 +52,6 @@ int ENTRY(const MlpArgs& a, const MlpConfig& c, size_t smem, cudaStream_t st, in
 #else
     if (c.jpt == 1) { BY_NP(1, 128) }
     BY_NP(2, 256)
+#endif
 #endif
 }

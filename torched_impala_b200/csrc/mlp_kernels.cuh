@@ -18,7 +18,7 @@ struct MlpArgs {
 
 struct MlpConfig {
     int jpt, maxt, op, np, threads, slices;
-    int ks;  // backward: threads per hidden unit (2 = the observation features are split over a lane pair)
+    int ks;  // backward: threads per hidden unit (2 / 4 = the observation features are split over a lane pair / quad)
 };
 
 constexpr int kRows = 32;        // rows per staged tile
@@ -60,6 +60,16 @@ int impala_mlp_fwd_tcw(const float* x, const float* params, float* out, int M, i
 int impala_mlp_bwd_tcw(const float* x, const float* params, const float* dout, float* ws, int M, int O, int H,
                        int N2, cudaStream_t st, int* nparts);
 
+// Wide tensor-core forward of the shapes beyond the limits above (O in 65..128 = four K atoms, or N2 in
+// 17..32): O % 4 == 0, H a multiple of 128 up to 4096.  IMPALA_MLP_TCW=0 disables them too.
+bool impala_mlp_fwd_tcx_eligible(const float* x, int M, int O, int H, int N2);
+int impala_mlp_fwd_tcx(const float* x, const float* params, float* out, int M, int O, int H, int N2,
+                       cudaStream_t st);
+// ... and its backward (mlp_bwd_tc.cu): per-CTA float32 partial rows in ws, *nparts of them.
+bool impala_mlp_bwd_tcx_eligible(const float* x, int M, int O, int H, int N2);
+int impala_mlp_bwd_tcx(const float* x, const float* params, const float* dout, float* ws, int M, int O, int H,
+                       int N2, cudaStream_t st, int* nparts);
+
 // One per padded observation width / direction, defined in mlp_inst.cu.
 #define IMPALA_DECL_DISPATCH(OPV)                                                             \
     int impala_mlp_fwd_op##OPV(const MlpArgs&, const MlpConfig&, size_t, cudaStream_t, int*); \
@@ -68,6 +78,7 @@ IMPALA_DECL_DISPATCH(8)
 IMPALA_DECL_DISPATCH(24)
 IMPALA_DECL_DISPATCH(32)
 IMPALA_DECL_DISPATCH(64)
+IMPALA_DECL_DISPATCH(128)
 
 namespace impala_mlp {
 
@@ -117,9 +128,34 @@ __device__ __forceinline__ void layer1(float (&acc)[JPT][kGroup], const float (&
     }
 }
 
+// p ? x : y as an opaque selp: the plain select of two elements of the butterfly's value array is turned
+// into a dynamically indexed load by the compiler, which sends the array to local memory.
+__device__ __forceinline__ float selp_f32(bool p, float x, float y) {
+    float d;
+    asm("{\n\t.reg .pred q;\n\tsetp.ne.s32 q, %3, 0;\n\tselp.f32 %0, %1, %2, q;\n\t}" : "=f"(d) : "f"(x), "f"(y), "r"((int)p));
+    return d;
+}
+
+// One step of the transposing butterfly with compile-time indices: lanes exchange HALF values with the
+// lane HALF away and keep the half of the set their lane bit selects.
+template <int HALF>
+__device__ __forceinline__ void bfly_step(float (&vals)[32], int lane) {
+    const bool hi = (lane & HALF) != 0;
+#pragma unroll
+    for (int i = 0; i < HALF; ++i) {
+        const float send = selp_f32(hi, vals[i], vals[i + HALF]);
+        const float keep = selp_f32(hi, vals[i + HALF], vals[i]);
+        vals[i] = keep + __shfl_xor_sync(IMPALA_FULL_MASK, send, HALF);
+    }
+}
+
+// The wide-shape instantiations ask for one resident CTA per SM: without it ptxas caps the OP = 64,
+// NP = 32 kernel at 128 registers and spills.
 template <int JPT, int OP, int NP, int MAXT>
-__global__ void __launch_bounds__(MAXT) mlp_fwd_kernel(MlpArgs a) {
+__global__ void __launch_bounds__(MAXT, (OP == 128 || NP == 32) ? 1 : 0) mlp_fwd_kernel(MlpArgs a) {
     static_assert(kGroup * NP == 32 || NP != 4, "butterfly chunk must be 32 values");
+    // the instantiations of the wide shapes (O > 64 or N2 > 16) keep the butterfly in registers
+    constexpr bool kSelp = OP == 128 || NP == 32;
     extern __shared__ __align__(16) float smem[];
     const int nt = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nwarps = nt >> 5;
@@ -166,15 +202,20 @@ __global__ void __launch_bounds__(MAXT) mlp_fwd_kernel(MlpArgs a) {
                         vals[i] = s;
                     }
                     // transposing butterfly: 32 values x 32 lanes -> lane i holds warp-sum of value i
+                    if constexpr (kSelp) {
+                        bfly_step<16>(vals, lane), bfly_step<8>(vals, lane), bfly_step<4>(vals, lane);
+                        bfly_step<2>(vals, lane), bfly_step<1>(vals, lane);
+                    } else {
 #pragma unroll
-                    for (int s = 0; s < 5; ++s) {
-                        const int half = 16 >> s;
-                        const bool hi = (lane & half) != 0;
+                        for (int s = 0; s < 5; ++s) {
+                            const int half = 16 >> s;
+                            const bool hi = (lane & half) != 0;
 #pragma unroll
-                        for (int i = 0; i < half; ++i) {
-                            const float send = hi ? vals[i] : vals[i + half];
-                            const float keep = hi ? vals[i + half] : vals[i];
-                            vals[i] = keep + __shfl_xor_sync(IMPALA_FULL_MASK, send, half);
+                            for (int i = 0; i < half; ++i) {
+                                const float send = hi ? vals[i] : vals[i + half];
+                                const float keep = hi ? vals[i + half] : vals[i];
+                                vals[i] = keep + __shfl_xor_sync(IMPALA_FULL_MASK, send, half);
+                            }
                         }
                     }
                     part[warp * (kRows * NP) + g * VALS + c * 32 + lane] = vals[0];
@@ -231,33 +272,46 @@ __device__ __forceinline__ void zero_range(float* p, int64_t lo, int64_t hi) {
 // form spilled ~1.5 KB per thread at this width); the two partial dot products of the recompute
 // meet through one shuffle per row, everything downstream of the pre-activation is computed by
 // both lanes and stored by the even one.
+// KS = 4 (wide shapes, OP = 64 / 128): the same over a lane quad, OP / 4 features per lane; the quad's
+// features are interleaved in 16-byte chunks (lane `half` holds chunks half, half + 4, ...) so that the
+// four broadcast loads of a row hit four different bank groups.
+// NP = 32 (and NP = 16 at KS = 4): the W2 column of a unit and its gradient are split over the KS lanes
+// as well (NP / KS outputs per lane); the partial dh of the lanes meet through log2(KS) shuffles per row.
 template <int JPT, int OP, int NP, int MAXT, int KS = 1>
 __global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgs a) {
     extern __shared__ __align__(16) float smem[];
     constexpr int OPH = OP / KS;  // features held by this thread
+    constexpr bool SPLITN = NP > 16 || (KS == 4 && NP == 16);
+    constexpr int NPL = SPLITN ? NP / KS : NP;  // W2 outputs held by this thread
+    static_assert(!SPLITN || KS > 1, "the NP = 32 backward splits W2 over a lane group");
+    constexpr int XSTEP = KS == 4 ? 4 * KS : 4;  // feature distance of this thread's 16-byte chunks
     const int nt = blockDim.x, tid = threadIdx.x;
-    const int half = KS == 2 ? (tid & 1) : 0, ju = KS == 2 ? (tid >> 1) : tid, nu = nt / KS;
+    const int half = KS == 2 ? (tid & 1) : (KS == 4 ? (tid & 3) : 0);
+    const int ju = KS == 2 ? (tid >> 1) : (KS == 4 ? (tid >> 2) : tid), nu = nt / KS;
     const int j0 = blockIdx.y * nu * JPT + ju;
-    const int koff = half * OPH;
+    const int koff = KS == 4 ? 4 * half : half * OPH;  // first feature of this thread
+    const int n0 = SPLITN ? half * NPL : 0;             // first W2 output of this thread
     float* xs = smem;               // [kRows][OP]
     float* dzs = xs + kRows * OP;   // [kRows][NP]
     const float* __restrict__ W1 = a.params + a.lay.oW1;
     const float* __restrict__ b1 = a.params + a.lay.ob1;
     const float* __restrict__ W2 = a.params + a.lay.oW2;
 
-    float w[JPT][OPH], b1r[JPT], w2r[JPT][NP];
-    float gw1[JPT][OPH], gb1[JPT], gw2[JPT][NP], gb2 = 0.f;
+    float w[JPT][OPH], b1r[JPT], w2r[JPT][NPL];
+    float gw1[JPT][OPH], gb1[JPT], gw2[JPT][NPL], gb2 = 0.f;
 #pragma unroll
     for (int q = 0; q < JPT; ++q) {
         const int j = j0 + q * nu;
 #pragma unroll
-        for (int k = 0; k < OPH; ++k)
-            w[q][k] = (j < a.H && koff + k < a.O) ? __ldg(W1 + (size_t)j * a.O + koff + k) : 0.f;
+        for (int k = 0; k < OPH; ++k) {
+            const int f = KS == 4 ? koff + XSTEP * (k >> 2) + (k & 3) : koff + k;  // feature of w[q][k]
+            w[q][k] = (j < a.H && f < a.O) ? __ldg(W1 + (size_t)j * a.O + f) : 0.f;
+        }
         b1r[q] = (j < a.H && half == 0) ? __ldg(b1 + j) : 0.f;  // added once per unit
         gb1[q] = 0.f;
 #pragma unroll
-        for (int n = 0; n < NP; ++n) {
-            w2r[q][n] = (j < a.H && n < a.N2) ? __ldg(W2 + (size_t)n * a.H + j) : 0.f;
+        for (int n = 0; n < NPL; ++n) {
+            w2r[q][n] = (j < a.H && n0 + n < a.N2) ? __ldg(W2 + (size_t)(n0 + n) * a.H + j) : 0.f;
             gw2[q][n] = 0.f;
         }
 #pragma unroll
@@ -288,7 +342,7 @@ __global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgs a) {
             for (int k4 = 0; k4 < OPH / 4; ++k4) {
 #pragma unroll
                 for (int r = 0; r < kGroup; ++r) {
-                    const float4 xv = *reinterpret_cast<const float4*>(xg + r * OP + 4 * k4);
+                    const float4 xv = *reinterpret_cast<const float4*>(xg + r * OP + XSTEP * k4);
 #pragma unroll
                     for (int q = 0; q < JPT; ++q) {
                         acc[q][r] = fmaf(w[q][4 * k4 + 0], xv.x, acc[q][r]);
@@ -298,24 +352,25 @@ __global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgs a) {
                     }
                 }
             }
-            if constexpr (KS == 2) {
+#pragma unroll
+            for (int m = 1; m < KS; m <<= 1)
 #pragma unroll
                 for (int q = 0; q < JPT; ++q)
 #pragma unroll
-                    for (int r = 0; r < kGroup; ++r) acc[q][r] += __shfl_xor_sync(IMPALA_FULL_MASK, acc[q][r], 1);
-            }
+                    for (int r = 0; r < kGroup; ++r) acc[q][r] += __shfl_xor_sync(IMPALA_FULL_MASK, acc[q][r], m);
 #pragma unroll
             for (int r = 0; r < kGroup; ++r) {
-                float dz[NP];
-                if constexpr (NP % 4 == 0) {
+                float dz[NPL];
+                const float* dzr = dzg + r * NP + n0;
+                if constexpr (NPL % 4 == 0) {
 #pragma unroll
-                    for (int n4 = 0; n4 < NP / 4; ++n4) {
-                        const float4 t = *reinterpret_cast<const float4*>(dzg + r * NP + 4 * n4);
+                    for (int n4 = 0; n4 < NPL / 4; ++n4) {
+                        const float4 t = *reinterpret_cast<const float4*>(dzr + 4 * n4);
                         dz[4 * n4] = t.x, dz[4 * n4 + 1] = t.y, dz[4 * n4 + 2] = t.z, dz[4 * n4 + 3] = t.w;
                     }
                 } else {
 #pragma unroll
-                    for (int n = 0; n < NP; ++n) dz[n] = dzg[r * NP + n];
+                    for (int n = 0; n < NPL; ++n) dz[n] = dzr[n];
                 }
 #pragma unroll
                 for (int q = 0; q < JPT; ++q) {
@@ -323,9 +378,13 @@ __global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgs a) {
                     const float h = fmaxf(pre, 0.f);
                     float dh = 0.f;
 #pragma unroll
-                    for (int n = 0; n < NP; ++n) {
+                    for (int n = 0; n < NPL; ++n) {
                         dh = fmaf(dz[n], w2r[q][n], dh);
                         gw2[q][n] = fmaf(dz[n], h, gw2[q][n]);
+                    }
+                    if constexpr (SPLITN) {
+#pragma unroll
+                        for (int m = 1; m < KS; m <<= 1) dh += __shfl_xor_sync(IMPALA_FULL_MASK, dh, m);
                     }
                     const float dp = pre > 0.f ? dh : 0.f;  // relu'(0) = 0 as in torch
                     acc[q][r] = dp;
@@ -336,7 +395,7 @@ __global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgs a) {
             for (int k4 = 0; k4 < OPH / 4; ++k4) {
 #pragma unroll
                 for (int r = 0; r < kGroup; ++r) {
-                    const float4 xv = *reinterpret_cast<const float4*>(xg + r * OP + 4 * k4);
+                    const float4 xv = *reinterpret_cast<const float4*>(xg + r * OP + XSTEP * k4);
 #pragma unroll
                     for (int q = 0; q < JPT; ++q) {
                         gw1[q][4 * k4 + 0] = fmaf(acc[q][r], xv.x, gw1[q][4 * k4 + 0]);
@@ -359,13 +418,22 @@ __global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgs a) {
         const int j = j0 + q * nu;
         if (j < a.H) {
 #pragma unroll
-            for (int k = 0; k < OPH; ++k)
-                if (koff + k < a.O) wsb[a.lay.oW1 + (size_t)j * a.O + koff + k] = gw1[q][k];
+            for (int k = 0; k < OPH; ++k) {
+                const int f = KS == 4 ? koff + XSTEP * (k >> 2) + (k & 3) : koff + k;
+                if (f < a.O) wsb[a.lay.oW1 + (size_t)j * a.O + f] = gw1[q][k];
+            }
             if (half == 0) {
                 wsb[a.lay.ob1 + j] = gb1[q];
+                if constexpr (!SPLITN) {
 #pragma unroll
-                for (int n = 0; n < NP; ++n)
-                    if (n < a.N2) wsb[a.lay.oW2 + (size_t)n * a.H + j] = gw2[q][n];
+                    for (int n = 0; n < NP; ++n)
+                        if (n < a.N2) wsb[a.lay.oW2 + (size_t)n * a.H + j] = gw2[q][n];
+                }
+            }
+            if constexpr (SPLITN) {
+#pragma unroll
+                for (int n = 0; n < NPL; ++n)
+                    if (n0 + n < a.N2) wsb[a.lay.oW2 + (size_t)(n0 + n) * a.H + j] = gw2[q][n];
             }
         }
     }

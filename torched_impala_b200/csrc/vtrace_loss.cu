@@ -105,6 +105,30 @@ __device__ __forceinline__ void store_logits(float* __restrict__ p, unsigned ele
     }
 }
 
+// Streaming log-softmax of one (T, B, A) row for the wide action sets (AP > 16), where the
+// whole-row register arrays of the other instantiations no longer fit: the row is loaded, reduced
+// and dropped.  Returns the base-2 shift -max * log2(e) and lse2 = log2 sum_k 2^(z_k log2(e) - max
+// log2(e)), so log2 pi(k) = fmaf(z_k, log2(e), shift) - lse2; *za is the shifted logit of `act`.
+template <int AP, bool VEC>
+__device__ __forceinline__ void row_lse2(const float* __restrict__ p, unsigned elem, int A, int act, float* shift,
+                                         float* lse2, float* za) {
+    float z[AP];
+    load_logits<AP, VEC>(p, elem, A, z);
+    float mx = z[0];
+#pragma unroll
+    for (int k = 1; k < AP; ++k)
+        if (k < A) mx = fmaxf(mx, z[k]);
+    const float sh = -mx * kLog2e;
+    float se = 0.f, z_a = fmaf(z[0], kLog2e, sh);
+#pragma unroll
+    for (int k = 0; k < AP; ++k) {
+        const float zs = fmaf(z[k], kLog2e, sh);
+        if (k < A) se += ex2f(zs);
+        if (k > 0) z_a = selp_f32(k == act, zs, z_a);
+    }
+    *shift = sh, *lse2 = lg2f(se), *za = z_a;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Lane = trajectory, warp = time segment.
 //
@@ -124,9 +148,16 @@ __device__ __forceinline__ void store_logits(float* __restrict__ p, unsigned ele
 //      loss terms and closed-form gradients) and stores them row-contiguously.
 // Total threads = B * NSEG, so the small benchmark batch (T = 20, B = 4096) still spreads over
 // 1280 warps and the long unroll (T = 100, B = 8192) keeps ~2 500 warps x S rows of loads in flight.
+// Wide action sets (AP = 32, STREAM): the logit rows are not prefetched into registers (two row sets
+// of both logit vectors would be ~130 registers on their own); step 2 reduces each row as it loads
+// (row_lse2) and keeps the two taken-action logits, and step 4 re-reads the current row (an L1 / L2
+// hit) for the entropy and the logit gradient.
 // ------------------------------------------------------------------------------------------------
 template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool VEC>
 __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a) {
+    constexpr bool STREAM = AP > 16;
+    constexpr int SR = STREAM ? 1 : S, AR = STREAM ? 1 : AP;  // extent of the held logit rows
+    static_assert(!STREAM || S == 1, "the streaming rows keep one step per thread");
     __shared__ float2 s_map[2][kMaxSeg][32];
     __shared__ float2 s_cta[2][32];  // this CTA's segments composed into one map (read by the cluster)
     __shared__ double s_red[kMaxSeg][4];
@@ -155,7 +186,7 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
     // (last chunk only) re-read step T - 1 and dead lanes read trajectory B - 1; both are masked
     // by `valid` below (rho = c = disc = 0).
     struct Rows {
-        float zc[S][AP], zb[S][AP], r[S], vv[S + 1];
+        float zc[SR][AR], zb[SR][AR], r[S], vv[S + 1];
         int act[S];
         unsigned char dn[S];  // raw: compared where it is used, so the load is not waited for at issue
     };
@@ -164,8 +195,10 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
 #pragma unroll
         for (int i = 0; i < S; ++i) {
             const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
-            load_logits<AP, VEC>(a.cur_logits, e, A, R.zc[i]);
-            load_logits<AP, VEC>(a.beh_logits, e, A, R.zb[i]);
+            if constexpr (!STREAM) {
+                load_logits<AP, VEC>(a.cur_logits, e, A, R.zc[i]);
+                load_logits<AP, VEC>(a.beh_logits, e, A, R.zb[i]);
+            }
             R.r[i] = __ldg(a.rewards + e);
             R.act[i] = __ldg(a.actions + e);
             R.dn[i] = __ldg(a.done + e);
@@ -177,31 +210,41 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
         const int tb = c * rows + seg * S;  // first step of this thread's segment
         // ---- 2. per-step terms and the zero-carry scan of this segment
         float rho[S], disc[S], fa[S], g[S], lp2a[S];
+        float shc[SR], lsec[SR];  // STREAM: log2 pi(k) = fmaf(z_k, log2(e), shc) - lsec
 #pragma unroll
         for (int i = 0; i < S; ++i) {
             const bool valid = tb + i < L;
             // log-softmax of both logit vectors in the base-2 domain (learner.py:298-303)
-            float mx = R.zc[i][0], mxb = R.zb[i][0];
+            float z_a, zb_a, lse, lseb;
+            if constexpr (STREAM) {
+                const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
+                float shb;
+                row_lse2<AP, VEC>(a.cur_logits, e, A, R.act[i], &shc[i], &lsec[i], &z_a);
+                row_lse2<AP, VEC>(a.beh_logits, e, A, R.act[i], &shb, &lseb, &zb_a);
+                lse = lsec[i];
+            } else {
+                float mx = R.zc[i][0], mxb = R.zb[i][0];
 #pragma unroll
-            for (int k = 1; k < AP; ++k)
-                if (k < A) mx = fmaxf(mx, R.zc[i][k]), mxb = fmaxf(mxb, R.zb[i][k]);
-            float se = 0.f, seb = 0.f;
-            const float mxl = -mx * kLog2e, mxbl = -mxb * kLog2e;
+                for (int k = 1; k < AP; ++k)
+                    if (k < A) mx = fmaxf(mx, R.zc[i][k]), mxb = fmaxf(mxb, R.zb[i][k]);
+                float se = 0.f, seb = 0.f;
+                const float mxl = -mx * kLog2e, mxbl = -mxb * kLog2e;
 #pragma unroll
-            for (int k = 0; k < AP; ++k) {
-                R.zc[i][k] = fmaf(R.zc[i][k], kLog2e, mxl);   // (z - max) log2(e), one rounding
-                R.zb[i][k] = fmaf(R.zb[i][k], kLog2e, mxbl);
-                if (k < A) se += ex2f(R.zc[i][k]), seb += ex2f(R.zb[i][k]);
+                for (int k = 0; k < AP; ++k) {
+                    R.zc[i][k] = fmaf(R.zc[i][k], kLog2e, mxl);   // (z - max) log2(e), one rounding
+                    R.zb[i][k] = fmaf(R.zb[i][k], kLog2e, mxbl);
+                    if (k < A) se += ex2f(R.zc[i][k]), seb += ex2f(R.zb[i][k]);
+                }
+                lse = lg2f(se), lseb = lg2f(seb);
+                z_a = R.zc[i][0], zb_a = R.zb[i][0];
+#pragma unroll
+                for (int k = 1; k < AP; ++k) {
+                    const bool hit = k == R.act[i];
+                    z_a = selp_f32(hit, R.zc[i][k], z_a), zb_a = selp_f32(hit, R.zb[i][k], zb_a);
+                }
+#pragma unroll
+                for (int k = 0; k < AP; ++k) R.zc[i][k] -= lse;  // log2 pi(k)
             }
-            const float lse = lg2f(se), lseb = lg2f(seb);
-            float z_a = R.zc[i][0], zb_a = R.zb[i][0];
-#pragma unroll
-            for (int k = 1; k < AP; ++k) {
-                const bool hit = k == R.act[i];
-                z_a = selp_f32(hit, R.zc[i][k], z_a), zb_a = selp_f32(hit, R.zb[i][k], zb_a);
-            }
-#pragma unroll
-            for (int k = 0; k < AP; ++k) R.zc[i][k] -= lse;  // log2 pi(k)
             lp2a[i] = z_a - lse;                                               // log2 pi(a)
             const float ratio = ex2f(lp2a[i] - (zb_a - lseb));                 // :121-123
             rho[i] = valid ? fminf(ratio, a.rho_bar) : 0.f;                    // :124
@@ -272,19 +315,38 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
             }
             if constexpr (WITH_LOSS) {
                 // d total / d v = v_loss_c (v - vs) / B = -v_loss_c acc / B  (:149, :306-307)
-                float ent = 0.f, pk[AP], lz[AP], dz[AP];
+                float ent = 0.f, dz[AP];
+                if constexpr (STREAM) {
+                    // re-read the row; dz holds log2 pi(k), then the gradient (one row of registers)
+                    load_logits<AP, VEC>(a.cur_logits, (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl, A, dz);
 #pragma unroll
-                for (int k = 0; k < AP; ++k) {
-                    lz[k] = R.zc[i][k] * kLn2;
-                    pk[k] = (k < A) ? ex2f(R.zc[i][k]) : 0.f;
-                    if (k < A) ent -= pk[k] * lz[k];                           // :310-314, :153
-                }
+                    for (int k = 0; k < AP; ++k) {
+                        dz[k] = fmaf(dz[k], kLog2e, shc[i]) - lsec[i];
+                        if (k < A) ent -= ex2f(dz[k]) * (dz[k] * kLn2);
+                    }
 #pragma unroll
-                for (int k = 0; k < AP; ++k) {
-                    const float onehot = (k == R.act[i]) ? 1.f : 0.f;
-                    const float d = a.inv_batch * (a.policy_loss_c * pg * (pk[k] - onehot) +
-                                                   a.entropy_c * pk[k] * (lz[k] + ent));
-                    dz[k] = (valid && k < A) ? d : 0.f;
+                    for (int k = 0; k < AP; ++k) {
+                        const float lz = dz[k] * kLn2, pk = (k < A) ? ex2f(dz[k]) : 0.f;
+                        const float onehot = (k == R.act[i]) ? 1.f : 0.f;
+                        const float d = a.inv_batch * (a.policy_loss_c * pg * (pk - onehot) +
+                                                       a.entropy_c * pk * (lz + ent));
+                        dz[k] = (valid && k < A) ? d : 0.f;
+                    }
+                } else {
+                    float pk[AP], lz[AP];
+#pragma unroll
+                    for (int k = 0; k < AP; ++k) {
+                        lz[k] = R.zc[i][k] * kLn2;
+                        pk[k] = (k < A) ? ex2f(R.zc[i][k]) : 0.f;
+                        if (k < A) ent -= pk[k] * lz[k];                           // :310-314, :153
+                    }
+#pragma unroll
+                    for (int k = 0; k < AP; ++k) {
+                        const float onehot = (k == R.act[i]) ? 1.f : 0.f;
+                        const float d = a.inv_batch * (a.policy_loss_c * pg * (pk[k] - onehot) +
+                                                       a.entropy_c * pk[k] * (lz[k] + ent));
+                        dz[k] = (valid && k < A) ? d : 0.f;
+                    }
                 }
                 if (live && t < T) {
                     a.dv[e] = valid ? -a.v_loss_c * a.inv_batch * acc[i] : 0.f;
@@ -368,6 +430,7 @@ int pick_ap(int A) {
     if (A <= 4) return 4;
     if (A <= 8) return 8;
     if (A <= 16) return 16;
+    if (A <= 32) return 32;
     return 0;
 }
 
@@ -400,7 +463,7 @@ int launch(VtArgs& a, cudaStream_t st) {
     const unsigned groups = (unsigned)((a.B + 31) / 32);
     const bool vec = a.A == AP && aligned16(a.cur_logits) && aligned16(a.beh_logits) &&
                      (!WITH_LOSS || aligned16(a.dlogits));
-    int S = AP == 16 ? 1 : 2;
+    int S = AP >= 16 ? 1 : 2;
     const int s_env = impala_env_int("IMPALA_VTRACE_S", 0);
     if (AP <= 4 && (s_env == 1 || s_env == 2 || s_env == 5)) S = s_env;
     const int max_w = S == 5 ? 10 : (AP <= 4 && S == 1 ? kMaxSeg : 16);
@@ -422,7 +485,8 @@ int launch(VtArgs& a, cudaStream_t st) {
     VT_AP(4)
 #undef VT_AP
     if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);
-    return launch_s<16, 1, 512, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);
+    if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);
+    return launch_s<32, 1, 512, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);
 }
 
 }  // namespace
