@@ -5,7 +5,7 @@
 // Transposed formulation so that a thread owns HIDDEN units (accumulator rows = hidden units), per
 // tile of 64 batch rows and warpgroup (64 hidden units):
 //
-//   GEMM1 (SS, recompute)  PRE[64 hid, 64 rows] = W1_blk[64, K] * X[64 rows, K]^T
+//   GEMM1 (recompute)      PRE[64 hid, 64 rows] = W1_blk[64, K] * X[64 rows, K]^T
 //   CUDA cores             h = relu(PRE + b1); dh = W2^T dz; dW2 += dz h; DP = (PRE + b1 > 0) ? dh : 0;
 //                          db1 += DP
 //   GEMM2 (RS, reduction)  dW1_blk[64 hid, K] += DP[64 hid, 64 rows] * X[64 rows, K]
@@ -24,13 +24,22 @@
 // hi = round-to-nearest tf32; DP: hi = dp with the low 13 mantissa bits cleared, lo = the exact
 // remainder); the small terms go into their own accumulator (dW1) or first (PRE), so that the
 // full-magnitude hi*hi additions are the only ones that round at full size.  dW1 accumulates in
-// registers over every tile of the persistent CTA and is written out once per pass.
+// registers over every tile of the persistent CTA (or warpgroup) and is written out once per pass.
 //
-// One CTA = 2 warpgroups = 128 hidden units per pass; wider layers are walked in passes (x is
-// re-read once per pass).  Every gradient entry of W1 / b1 / W2 belongs to exactly one hidden unit,
-// so each CTA writes a float32 partial gradient row (same layout as the FP32 kernels) and the rows
-// are summed in float64 in a fixed order: in-kernel after a grid barrier (narrow shapes, paired
-// launch, optional peer push), or by reduce_partials_kernel (wide shapes).
+// Every gradient entry of W1 / b1 / W2 belongs to exactly one hidden unit, so each CTA writes a float32
+// partial gradient row (same layout as the FP32 kernels) and the rows are summed in float64 in a fixed
+// order.
+//
+// Narrow shapes (impala_mlp_bwd_tc_eligible: one K atom, <= 4 outputs; bwd_blk_body): a CTA owns ONE
+// 64-unit hidden block of one network for the whole launch, so W1 of the block is loaded once and held
+// in registers as GEMM1's A operand (only the x tile is read from shared memory).  Its two warpgroups
+// are independent - each takes alternate tiles of the CTA's share, with its own x stage and named
+// barrier - so one warpgroup's MMAs overlap the other's CUDA-core epilogue.  The warpgroups meet once,
+// at the end (fixed order), and the rows are summed in-kernel after a grid barrier (paired launch,
+// optional peer push).
+//
+// Wide shapes (bwd_tc_body): one CTA = 2 warpgroups = 128 hidden units per pass, wider layers walked
+// in passes (x is re-read once per pass); reduce_partials_kernel sums the rows.
 #include <map>
 #include <mutex>
 #include <tuple>
@@ -517,6 +526,306 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
     return x_hi;
 }
 
+// ---- narrow shapes: one 64-unit hidden block per CTA, independent warpgroups
+constexpr int kXtBytes = 2 * 32 * 128;  // x^T: 2 K atoms of 32 batch rows, 32 feature rows of 128 B
+// one warpgroup's stage: x hi / lo, x^T hi / lo (1024-byte aligned), dz [64 rows][<= 4]
+constexpr int kStageBytes = 2 * kXAtomBytes + 2 * kXtBytes + kRowsT * 4 * (int)sizeof(float);
+// + the db2 exchange [4 dz-loading warps][4]
+constexpr size_t kBlkSmemBytes = 1024 + (size_t)kWG * kStageBytes + 16 * sizeof(float);
+static_assert(kStageBytes % 1024 == 0, "stages stay 1024-byte aligned");
+
+// CTA `cta` of the `ncta` that take one network (a multiple of its H / 64 hidden blocks) belongs to
+// group cta / (ncta / (H / 64)) - the group of a hidden block - and is CTA `r` = cta % (ncta / (H / 64))
+// of it: it takes the tiles r, r + ncta / (H / 64), ... (warpgroups alternating) for its block and writes
+// the block's entries of partial row r (dW1 rows, db1, dW2 columns; group 0 also db2 and the pads), so
+// that the rows hold every entry exactly once each.  Returns >= 16 KiB of shared memory the caller may
+// use as scratch.
+template <int NP>
+__device__ __forceinline__ uint8_t* bwd_blk_body(const BwdTcArgs& a, const int cta, const int ncta) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+    // the warpgroup index broadcast from lane 0: known warp-uniform, so the stage addresses and the
+    // wgmma descriptors built from them stay in uniform registers
+    const int wg = __shfl_sync(IMPALA_FULL_MASK, (int)threadIdx.x >> 7, 0);
+    const int tid = threadIdx.x, lt = tid & 127, warp = lt >> 5, lane = tid & 31;
+    const int g = lane >> 2, q = lane & 3;
+    const int O = a.O, H = a.H, ochunks = O >> 2, ksteps = (O + 7) >> 3;
+    const int cpg = ncta / (H / 64), grp = cta / cpg, r = cta - grp * cpg;
+    uint8_t* x_hi = smem + wg * kStageBytes;
+    uint8_t* x_lo = x_hi + kXAtomBytes;
+    uint8_t* xt_hi = x_lo + kXAtomBytes;  // [2 K atoms][32 feature rows][128 B]
+    uint8_t* xt_lo = xt_hi + kXtBytes;
+    float* dzs = reinterpret_cast<float*>(xt_lo + kXtBytes);         // [64 rows][NP]
+    float* gb2x = reinterpret_cast<float*>(smem + kWG * kStageBytes);  // [4 warps][4]
+    const float* __restrict__ W1 = a.params + a.lay.oW1;
+    const float* __restrict__ b1 = a.params + a.lay.ob1;
+    const float* __restrict__ W2 = a.params + a.lay.oW2;
+    float* wsb = a.ws + (size_t)r * a.lay.total;
+
+    if (grp == 0) {  // pads of the partial row
+        const int64_t lo4[4] = {a.lay.oW1 + (int64_t)H * O, a.lay.ob1 + H, a.lay.oW2 + (int64_t)a.N2 * H,
+                                a.lay.ob2 + a.N2};
+        const int64_t hi4[4] = {a.lay.ob1, a.lay.oW2, a.lay.ob2, a.lay.total};
+        for (int sgm = 0; sgm < 4; ++sgm)
+            for (int64_t p = lo4[sgm] + tid; p < hi4[sgm]; p += kThreads) wsb[p] = 0.f;
+    }
+
+    // x rows of a tile -> registers: thread (warp, lane) holds row 16 warp + lane % 16, 16-byte chunks
+    // 2 k + lane / 16 (a warp's transposed stores then hit 32 different banks, and chunk pairs GEMM1
+    // never reads, k >= ksteps, are skipped by whole warps); dz row lt for lt < 64
+    constexpr int kLd = kRowsT * 8 / 128;
+    const int rr = 16 * warp + (lane & 15);
+    float4 v[kLd];
+    float z[NP];
+    auto load = [&](int tile) {
+#pragma unroll
+        for (int k = 0; k < kLd; ++k) {
+            const int c = 2 * k + (lane >> 4), row = tile * kRowsT + rr;
+            v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (k < ksteps && tile < a.num_tiles && row < a.M && c < ochunks)
+                v[k] = __ldg(reinterpret_cast<const float4*>(a.x + (size_t)row * O) + c);
+        }
+        const int row = tile * kRowsT + lt;
+#pragma unroll
+        for (int n = 0; n < NP; ++n)
+            z[n] = (lt < kRowsT && tile < a.num_tiles && row < a.M && n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
+    };
+    float gb2[NP];  // db2 = column sums of dout: this thread's dz values
+#pragma unroll
+    for (int n = 0; n < NP; ++n) gb2[n] = 0.f;
+
+    // dz of the tile is the output of the kernel before this one (PDL, common.cuh)
+    pdl_wait();
+    // the thread's two hidden units; W1 hi / lo of both as GEMM1's A fragments (K step kk: feature
+    // 8 kk + q + 4 (i >> 1) of unit i & 1 ? j1 : j0), for the whole launch
+    const int j0 = 64 * grp + 16 * warp + g, j1 = j0 + 8;
+    uint32_t wh[4][4], wl[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int f = 8 * kk + q + 4 * (i >> 1);
+            float hi, lo;
+            tc::split_tf32(f < O ? __ldg(W1 + (size_t)(i & 1 ? j1 : j0) * O + f) : 0.f, hi, lo);
+            wh[kk][i] = __float_as_uint(hi), wl[kk][i] = __float_as_uint(lo);
+        }
+    const float bj0 = __ldg(b1 + j0), bj1 = __ldg(b1 + j1);
+    float w2r0[NP], w2r1[NP], gw0[NP], gw1[NP], gb10 = 0.f, gb11 = 0.f;
+#pragma unroll
+    for (int n = 0; n < NP; ++n) {
+        w2r0[n] = n < a.N2 ? __ldg(W2 + (size_t)n * H + j0) : 0.f;
+        w2r1[n] = n < a.N2 ? __ldg(W2 + (size_t)n * H + j1) : 0.f;
+        gw0[n] = gw1[n] = 0.f;
+    }
+    float acc_hh[16], acc_c[16];  // dW1: dp_hi * x_hi | dp_hi * x_lo + dp_lo * x_hi
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc_hh[i] = acc_c[i] = 0.f;
+    tc::fence_acc(acc_hh), tc::fence_acc(acc_c);
+    const uint64_t dx_hi = tc::smem_desc_k_sw128(x_hi, 0), dx_lo = tc::smem_desc_k_sw128(x_lo, 0);
+    const uint64_t dxt_hi = tc::smem_desc_k_sw128(xt_hi, 0), dxt_lo = tc::smem_desc_k_sw128(xt_lo, 0);
+
+    const int bar = 1 + wg, tstride = 2 * cpg;  // this warpgroup's named barrier and tile stride
+    load(r + cpg * wg);
+    for (int tile = r + cpg * wg; tile < a.num_tiles; tile += tstride) {
+        // ---- stage the tile: x row-major (B of GEMM1) and transposed (B of GEMM2), hi / lo; dz
+        tc::named_bar(bar, 128);  // every MMA of the warpgroup that read the previous tile has retired
+#pragma unroll
+        for (int k = 0; k < kLd; ++k) {
+            if (k >= ksteps) continue;  // features GEMM1 does not read; GEMM2's columns of them are dropped
+            const int c = 2 * k + (lane >> 4);
+            float4 hi, lo;
+            tc::split4(v[k], hi, lo);
+            const uint32_t off = tc::sw128_offset(rr, c);
+            *reinterpret_cast<float4*>(x_hi + off) = hi;
+            *reinterpret_cast<float4*>(x_lo + off) = lo;
+            // batch row rr -> K atom rr / 32, position 8 kk + (qq >> 1) + 4 (qq & 1) with rr % 32 = 8 kk + qq
+            const int r32 = rr & 31, pos = (r32 & ~7) + ((r32 & 7) >> 1) + 4 * (r32 & 1);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int f = 4 * c + e;
+                const uint32_t toff = (rr >> 5) * (32 * 128) + (f >> 3) * 1024 + (f & 7) * 128 +
+                                      (((pos >> 2) ^ (f & 7)) << 4) + (pos & 3) * 4;
+                *reinterpret_cast<float*>(xt_hi + toff) = f4(hi, e);
+                *reinterpret_cast<float*>(xt_lo + toff) = f4(lo, e);
+            }
+        }
+        if (lt < kRowsT) {
+#pragma unroll
+            for (int n = 0; n < NP; ++n) dzs[lt * NP + n] = z[n], gb2[n] += z[n];
+        }
+        tc::fence_proxy_async();
+        tc::named_bar(bar, 128);
+        load(tile + tstride);  // in flight during this tile's MMAs and epilogue
+
+        // ---- GEMM1: PRE = W1_blk * X^T (N = 32 halves of the tile's batch rows), A from registers;
+        // descriptors = the stage's plus the operand's offset in 16-byte units (start address field)
+        // (bases opaque per tile: hoisted out of the loop, every descriptor would hold two registers)
+        uint64_t bx_hi = dx_hi, bx_lo = dx_lo;
+        asm volatile("" : "+l"(bx_hi), "+l"(bx_lo));
+        float d[2][16];
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb)
+#pragma unroll
+            for (int i = 0; i < 16; ++i) d[nb][i] = 0.f;
+        // zeroed accumulators defined before the warpgroup fence (see bwd_tc_body)
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb) tc::fence_acc(d[nb]);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb) {
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                if (kk < ksteps) {
+                    const uint32_t xo = (nb * 32 * 128 + kk * 32) >> 4;
+                    tc::wgmma_n32_rs(d[nb], wl[kk], bx_hi + xo, kk > 0);
+                    tc::wgmma_n32_rs(d[nb], wh[kk], bx_lo + xo, true);
+                }
+            }
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                if (kk < ksteps) tc::wgmma_n32_rs(d[nb], wh[kk], bx_hi + ((nb * 32 * 128 + kk * 32) >> 4), true);
+            }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb) tc::fence_acc(d[nb]);
+
+        // ---- epilogue: d <- DP in place (thread: hidden units j0 / j1, batch columns 8 i + 2 q + e)
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int m = 32 * nb + 8 * i + 2 * q + e;
+                    float dz[NP];
+                    if constexpr (NP == 4) {
+                        const float4 t = *reinterpret_cast<const float4*>(dzs + 4 * m);
+                        dz[0] = t.x, dz[1] = t.y, dz[2] = t.z, dz[3] = t.w;
+                    } else {
+                        dz[0] = dzs[m];
+                    }
+                    // relu'(0) = 0 as in torch
+                    const float pre0 = d[nb][4 * i + e] + bj0, pre1 = d[nb][4 * i + 2 + e] + bj1;
+                    const float h0 = fmaxf(pre0, 0.f), h1 = fmaxf(pre1, 0.f);
+                    float dh0 = dz[0] * w2r0[0], dh1 = dz[0] * w2r1[0];
+#pragma unroll
+                    for (int n = 1; n < NP; ++n) dh0 = fmaf(dz[n], w2r0[n], dh0), dh1 = fmaf(dz[n], w2r1[n], dh1);
+#pragma unroll
+                    for (int n = 0; n < NP; ++n) gw0[n] = fmaf(dz[n], h0, gw0[n]), gw1[n] = fmaf(dz[n], h1, gw1[n]);
+                    const float dp0 = pre0 > 0.f ? dh0 : 0.f, dp1 = pre1 > 0.f ? dh1 : 0.f;
+                    gb10 += dp0, gb11 += dp1;
+                    d[nb][4 * i + e] = dp0, d[nb][4 * i + 2 + e] = dp1;
+                }
+            }
+        }
+
+        // ---- GEMM2: dW1 += DP * X (A = DP from registers).  Phase 1: dp_lo * x_hi; phase 2 (DP
+        // overwritten by dp_hi in place): dp_hi * x_lo, then dp_hi * x_hi into its own accumulator
+        uint32_t lo[2][16];
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb)
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const float hi = __uint_as_float(__float_as_uint(d[nb][i]) & 0xffffe000u);
+                lo[nb][i] = __float_as_uint(d[nb][i] - hi);
+                d[nb][i] = hi;
+            }
+        uint64_t bxt_hi = dxt_hi, bxt_lo = dxt_lo;
+        asm volatile("" : "+l"(bxt_hi), "+l"(bxt_lo));
+        tc::wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+            const int nb = kk >> 2, i = kk & 3;
+            const uint32_t al[4] = {lo[nb][4 * i], lo[nb][4 * i + 2], lo[nb][4 * i + 1], lo[nb][4 * i + 3]};
+            const uint32_t ah[4] = {__float_as_uint(d[nb][4 * i]), __float_as_uint(d[nb][4 * i + 2]),
+                                    __float_as_uint(d[nb][4 * i + 1]), __float_as_uint(d[nb][4 * i + 3])};
+            const uint32_t xo = (nb * 32 * 128 + i * 32) >> 4;
+            tc::wgmma_n32_rs(acc_c, al, bxt_hi + xo, true);
+            tc::wgmma_n32_rs(acc_c, ah, bxt_lo + xo, true);
+            tc::wgmma_n32_rs(acc_hh, ah, bxt_hi + xo, true);
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        // the A registers are read asynchronously: keep them (and the accumulators) untouched until here
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb) {
+            tc::fence_acc(d[nb]);
+#pragma unroll
+            for (int i = 0; i < 16; ++i) asm volatile("" : "+r"(lo[nb][i])::"memory");
+        }
+        tc::fence_acc(acc_hh), tc::fence_acc(acc_c);
+    }
+
+    // ---- end of the launch: the quad's column sets meet, then warpgroup 0 + warpgroup 1 (fixed order)
+#pragma unroll
+    for (int s = 1; s <= 2; s <<= 1) {
+        gb10 += __shfl_xor_sync(IMPALA_FULL_MASK, gb10, s);
+        gb11 += __shfl_xor_sync(IMPALA_FULL_MASK, gb11, s);
+#pragma unroll
+        for (int n = 0; n < NP; ++n) {
+            gw0[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gw0[n], s);
+            gw1[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gw1[n], s);
+        }
+    }
+    float gwt[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) gwt[i] = acc_hh[i] + acc_c[i];
+    // db2: fixed-order tree over each warp that loaded dz rows, then the 4 warps (below)
+#pragma unroll
+    for (int n = 0; n < NP; ++n) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) gb2[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gb2[n], off);
+    }
+    if (lt < kRowsT && lane == 0) {
+#pragma unroll
+        for (int n = 0; n < NP; ++n) gb2x[(2 * wg + warp) * 4 + n] = gb2[n];
+    }
+    // warpgroup 1's values -> its stage, laid out by thread (both warpgroups hold the same entries)
+    float* xch = reinterpret_cast<float*>(smem + kStageBytes);
+    __syncthreads();  // warpgroup 1's last MMAs have retired
+    if (wg == 1) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) xch[i * 128 + lt] = gwt[i];
+        xch[16 * 128 + lt] = gb10, xch[17 * 128 + lt] = gb11;
+#pragma unroll
+        for (int n = 0; n < NP; ++n) xch[(18 + n) * 128 + lt] = gw0[n], xch[(18 + NP + n) * 128 + lt] = gw1[n];
+    }
+    __syncthreads();
+    if (wg == 0) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) gwt[i] += xch[i * 128 + lt];
+        gb10 += xch[16 * 128 + lt], gb11 += xch[17 * 128 + lt];
+#pragma unroll
+        for (int n = 0; n < NP; ++n) gw0[n] += xch[(18 + n) * 128 + lt], gw1[n] += xch[(18 + NP + n) * 128 + lt];
+        if (q == 0) {
+            wsb[a.lay.ob1 + j0] = gb10;
+            wsb[a.lay.ob1 + j1] = gb11;
+#pragma unroll
+            for (int n = 0; n < NP; ++n)
+                if (n < a.N2) wsb[a.lay.oW2 + (size_t)n * H + j0] = gw0[n], wsb[a.lay.oW2 + (size_t)n * H + j1] = gw1[n];
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int f = 8 * i + 2 * q;  // features f, f + 1 (O % 4 == 0: both or neither valid)
+            if (f < O) {
+                *reinterpret_cast<float2*>(wsb + a.lay.oW1 + (size_t)j0 * O + f) = make_float2(gwt[4 * i], gwt[4 * i + 1]);
+                *reinterpret_cast<float2*>(wsb + a.lay.oW1 + (size_t)j1 * O + f) = make_float2(gwt[4 * i + 2], gwt[4 * i + 3]);
+            }
+        }
+        // db2 from group 0 only: its CTAs see every tile once
+        if (grp == 0 && tid == 0) {
+#pragma unroll
+            for (int n = 0; n < NP; ++n)
+                if (n < a.N2) wsb[a.lay.ob2 + n] = (gb2x[n] + gb2x[4 + n]) + (gb2x[8 + n] + gb2x[12 + n]);
+        }
+    }
+    __threadfence();  // this thread's partial-row stores are visible device-wide
+    __syncthreads();
+    return smem;
+}
+
 // Grid barrier: every CTA of the launch is resident (grid <= SM count, COOPERATIVE launch - it
 // fails instead of hanging where co-residency cannot be had).  ctl[0] counts arrivals; a workspace
 // that was not zero-filled once traps instead of hanging.
@@ -599,17 +908,18 @@ __device__ __forceinline__ void reduce_rows(const BwdTcArgs& a, const int nparts
     }
 }
 
+// grid = a multiple of the H / 64 hidden blocks; partial rows = CTAs per block
 template <int NP>
 __global__ void __launch_bounds__(kThreads, 1) mlp_bwd_tc_kernel(const __grid_constant__ BwdTcArgs a) {
-    uint8_t* scratch = bwd_tc_body<NP, 1>(a, blockIdx.x, gridDim.x);
+    uint8_t* scratch = bwd_blk_body<NP>(a, blockIdx.x, gridDim.x);
     grid_arrive_and_wait(a.ctl);
-    reduce_rows(a, gridDim.x, blockIdx.x, gridDim.x, reinterpret_cast<double*>(scratch));
+    reduce_rows(a, gridDim.x / (a.H / 64), blockIdx.x, gridDim.x, reinterpret_cast<double*>(scratch));
     grid_depart(a.ctl);
 }
 
 // Policy and value network of one learner step in ONE launch: CTAs [0, n_pi) take the policy's
-// tiles (partial rows 0 .. n_pi of its workspace), the rest the value function's.  After the grid
-// barrier every CTA helps reduce both sets of rows (the value function's chunks are dealt from
+// tiles (partial rows 0 .. n_pi / (H_pi / 64) of its workspace), the rest the value function's.  After
+// the grid barrier every CTA helps reduce both sets of rows (the value function's chunks are dealt from
 // the far end so that no CTA gets two chunks of each).  Uses the policy workspace's control words.
 // PUSH: data-parallel learner - the reduced gradient [policy | value fn] and `n_extra` local
 // scalars (the loss sums the V-trace kernel left at `extra`) go straight into every rank's gather
@@ -621,13 +931,13 @@ mlp_bwd_tc_pair_kernel(const __grid_constant__ BwdTcArgs a_pi, const __grid_cons
                        const int n_extra) {
     const int n_vf = (int)gridDim.x - n_pi;
     uint8_t* scratch;
-    if ((int)blockIdx.x < n_pi) scratch = bwd_tc_body<4, 1>(a_pi, blockIdx.x, n_pi);
-    else scratch = bwd_tc_body<1, 1>(a_vf, (int)blockIdx.x - n_pi, n_vf);
+    if ((int)blockIdx.x < n_pi) scratch = bwd_blk_body<4>(a_pi, blockIdx.x, n_pi);
+    else scratch = bwd_blk_body<1>(a_vf, (int)blockIdx.x - n_pi, n_vf);
     grid_arrive_and_wait(a_pi.ctl);
     const PushArgs* pp = PUSH ? &push : nullptr;
-    reduce_rows(a_pi, n_pi, blockIdx.x, gridDim.x, reinterpret_cast<double*>(scratch), pp, 0);
-    reduce_rows(a_vf, n_vf, (int)gridDim.x - 1 - (int)blockIdx.x, gridDim.x, reinterpret_cast<double*>(scratch), pp,
-                a_pi.lay.total);
+    reduce_rows(a_pi, n_pi / (a_pi.H / 64), blockIdx.x, gridDim.x, reinterpret_cast<double*>(scratch), pp, 0);
+    reduce_rows(a_vf, n_vf / (a_vf.H / 64), (int)gridDim.x - 1 - (int)blockIdx.x, gridDim.x,
+                reinterpret_cast<double*>(scratch), pp, a_pi.lay.total);
     if (PUSH && blockIdx.x == gridDim.x / 2 && (int)threadIdx.x < n_extra) {
         const long long step = *push.seq + 1;
         const int64_t off = (step & 1) * push.buf_stride + (int64_t)push.rank * push.slot_stride + a_pi.lay.total +
@@ -674,6 +984,21 @@ BwdTcArgs make_bwd_args(const float* x, const float* params, const float* dout, 
     return a;
 }
 
+// impala_pair_split for networks that take whole sets of CTAs (one per hidden block: ga / gb CTAs):
+// *na policy sets and *nb value-function sets, at most `grid` CTAs and no more sets than tiles, so
+// that the slower side finishes earliest at per-tile cost wa / wb.  Needs ga + gb <= grid.
+void split_sets(int tiles_a, int tiles_b, int grid, int ga, int gb, int64_t wa, int64_t wb, int* na, int* nb) {
+    int64_t best_cost = INT64_MAX, best_sum = INT64_MAX;
+    *na = *nb = 1;
+    for (int sa = 1; sa <= tiles_a && sa * ga + gb <= grid; ++sa) {
+        int sb = (grid - sa * ga) / gb;
+        if (sb > tiles_b) sb = tiles_b;
+        const int64_t ca = (int64_t)((tiles_a + sa - 1) / sa) * wa, cb = (int64_t)((tiles_b + sb - 1) / sb) * wb;
+        const int64_t cost = ca > cb ? ca : cb, sum = ca + cb;
+        if (cost < best_cost || (cost == best_cost && sum < best_sum)) *na = sa, *nb = sb, best_cost = cost, best_sum = sum;
+    }
+}
+
 }  // namespace
 
 bool impala_mlp_bwd_tc_eligible(const float* x, const float* dout, int M, int O, int H, int N2) {
@@ -687,15 +1012,19 @@ bool impala_mlp_bwd_tc_eligible(const float* x, const float* dout, int M, int O,
 int impala_mlp_bwd_tc(const float* x, const float* params, const float* dout, float* ws,
                       double* grad, unsigned int* ctl, int M, int O, int H, int N2, cudaStream_t st) {
     const BwdTcArgs a = make_bwd_args(x, params, dout, ws, grad, ctl, M, O, H, N2);
-    const size_t smem = bwd_smem_bytes(1, 4);
+    const size_t smem = kBlkSmemBytes;
     cudaError_t e;
     int sms = 0;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
     auto kernel = N2 == 1 ? mlp_bwd_tc_kernel<1> : mlp_bwd_tc_kernel<4>;
     if ((e = opt_in(kernel, smem)) != cudaSuccess) return (int)e;
-    int grid = a.num_tiles < sms ? a.num_tiles : sms;  // <= SM count: the grid barrier needs residency
-    if (grid > kMaxParts) grid = kMaxParts;
-    if ((e = impala_launch_ex(kernel, grid, kThreads, smem, st, true, true, a)) != cudaSuccess) return (int)e;
+    // every hidden block gets the same number of CTAs, no more than there are tiles (= partial rows the
+    // workspace holds); grid <= SM count: the grid barrier needs residency
+    const int nblk = H / 64;
+    int cpg = (sms < kMaxParts ? sms : kMaxParts) / nblk;
+    if (cpg > a.num_tiles) cpg = a.num_tiles;
+    if (cpg < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    if ((e = impala_launch_ex(kernel, nblk * cpg, kThreads, smem, st, true, true, a)) != cudaSuccess) return (int)e;
     return impala_launch_status();
 }
 
@@ -708,19 +1037,20 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
                            int n_extra) {
     const BwdTcArgs a_pi = make_bwd_args(x, params_pi, dlogits, ws_pi, grad_pi, ctl, M_pi, O, H_pi, A);
     const BwdTcArgs a_vf = make_bwd_args(x, params_vf, dv, ws_vf, grad_vf, ctl, M_vf, O, H_vf, 1);
-    const size_t smem = bwd_smem_bytes(1, 4);
+    const size_t smem = kBlkSmemBytes;
     cudaError_t e;
     int sms = 0;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
     e = push ? opt_in(mlp_bwd_tc_pair_kernel<true>, smem) : opt_in(mlp_bwd_tc_pair_kernel<false>, smem);
     if (e != cudaSuccess) return (int)e;
-    const int total_tiles = a_pi.num_tiles + a_vf.num_tiles;
-    int grid = total_tiles < sms ? total_tiles : sms;
-    if (grid > kMaxParts) grid = kMaxParts;
-    if (grid < 2) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    const int n_pi = impala_pair_split(a_pi.num_tiles, a_vf.num_tiles, grid,
-                                       impala_env_int("IMPALA_PAIR_W_BWD", 105) * (H_pi / 128),
-                                       100 * (H_vf / 128));
+    // a CTA does one hidden block of a tile whatever H is: the per-tile weights do not scale with H
+    const int gp = H_pi / 64, gv = H_vf / 64;
+    int grid = sms < kMaxParts ? sms : kMaxParts;  // <= SM count: the grid barrier needs residency
+    if (grid < gp + gv) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    int sp = 1, sv = 1;
+    split_sets(a_pi.num_tiles, a_vf.num_tiles, grid, gp, gv, impala_env_int("IMPALA_PAIR_W_BWD", 105), 100, &sp, &sv);
+    grid = gp * sp + gv * sv;
+    const int n_pi = gp * sp;
     // cooperative launch: the in-kernel grid barrier needs every CTA resident
     e = push ? impala_launch_ex(mlp_bwd_tc_pair_kernel<true>, grid, kThreads, smem, st, true, true, a_pi, a_vf, n_pi,
                                 *push, extra, n_extra)
