@@ -15,16 +15,21 @@
 // the small second layer (<= 32 outputs) run on the thread's two rows and eight columns, and the four
 // threads of a quad that share a row combine their partial sums with two shuffles (fixed order).
 //
-// One CTA = kWG independent warpgroups, each owning its own 64-row tiles and x stage; the weights
-// W1 hi / lo of up to 256 hidden units (a "block") sit in shared memory and are shared.  While one
-// warpgroup runs its epilogue the other's MMAs keep the tensor cores busy, and every warpgroup has
-// the next tile's x rows in flight in registers while it computes the current one.  Wider hidden
+// One CTA = kWG independent warpgroups, each owning its own 64-row tiles; the weights W1 hi / lo of
+// up to 256 hidden units (a "block") sit in shared memory and are shared.  At one K atom (O <= 32)
+// the x tile is wgmma's A operand straight from registers: each thread loads the x elements of its
+// own fragment slots from global memory and splits them, so nothing is staged and the tile loop has
+// no barrier (fwd_rs_body).  With two or four K atoms the tile is split into per-warpgroup hi / lo
+// stages in shared memory instead (fwd_ss_body).  While one
+// warpgroup runs its epilogue the other warpgroups' MMAs keep the tensor cores busy, and every
+// warpgroup has the next tile's x in flight in registers while it computes the current one.  Wider hidden
 // layers walk their blocks in passes: out[row] = ((b2 + z_0) + z_1) + ...  where the thread that
 // owns a row adds the block's partial second-layer sum to what the SAME thread wrote in the
 // previous pass (fixed order, bitwise reproducible, no workspace).
 #include <map>
 #include <mutex>
 #include <tuple>
+#include <type_traits>
 
 #include "mlp_kernels.cuh"
 #include "tc_common.cuh"
@@ -49,15 +54,253 @@ struct FwdTcArgs {
 // apart, and with 128-byte rows their 16-byte loads would fall into one bank group
 __host__ __device__ constexpr int w2s_stride(int np) { return np > 4 ? np + 4 : np; }
 
+// At one K atom the x tile is the wgmma A operand straight from registers; with more atoms the tile is
+// staged in shared memory (at two atoms the register path held 185 registers and took 12 % longer at
+// BASELINE c5; at four the fragments alone would take 128 registers).
+__host__ __device__ constexpr bool x_in_regs(int ka) { return ka == 1; }
+
 __host__ __device__ constexpr size_t fwd_smem_bytes(int hb, int ka, int np) {
-    return 1024 /*alignment slack*/ + (size_t)2 * ka * hb * 128 + (size_t)kWG * 2 * ka * kXAtomBytes +
-           (size_t)hb * (w2s_stride(np) + 1) * sizeof(float);
+    return 1024 /*alignment slack*/ + (size_t)2 * ka * hb * 128 +
+           (x_in_regs(ka) ? 0 : (size_t)kWG * 2 * ka * kXAtomBytes) + (size_t)hb * (w2s_stride(np) + 1) * sizeof(float);
+}
+
+// Stage one pass's W1 rows (hi / lo swizzled K-major tiles), b1 and W2 (transposed, rows padded to NPS).
+// The weights are read L2-cold at the start of a step, so each thread keeps kStageLd loads in flight
+// before it stores any of them (one dependent load per loop trip would put every one of them on the
+// launch's critical path).
+constexpr int kStageLd = 8;
+
+template <int NP, int KA>
+__device__ __forceinline__ void stage_weights(const FwdTcArgs& a, int p, uint8_t* w_hi, uint8_t* w_lo, float* b1s,
+                                              float* w2s) {
+    constexpr int NPS = w2s_stride(NP);
+    const int HB = a.hb, ochunks = a.O >> 2, tid = threadIdx.x;
+    const float* __restrict__ W1 = a.params + a.lay.oW1;
+    const float* __restrict__ b1 = a.params + a.lay.ob1;
+    const float* __restrict__ W2 = a.params + a.lay.oW2;
+    const int n_w1 = HB * 8 * KA, n_w2 = HB * NP;
+    for (int base = tid; base < n_w1; base += kStageLd * kThreads) {
+        float4 w[kStageLd];
+#pragma unroll
+        for (int u = 0; u < kStageLd; ++u) {
+            const int idx = base + u * kThreads, r = idx / (8 * KA), c = idx % (8 * KA);
+            w[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (idx < n_w1 && c < ochunks) w[u] = __ldg(reinterpret_cast<const float4*>(W1 + (size_t)(p * HB + r) * a.O) + c);
+        }
+#pragma unroll
+        for (int u = 0; u < kStageLd; ++u) {
+            const int idx = base + u * kThreads, r = idx / (8 * KA), c = idx % (8 * KA);
+            if (idx < n_w1) {
+                float4 hi, lo;
+                tc::split4(w[u], hi, lo);
+                const uint32_t off = (c >> 3) * (HB * 128) + tc::sw128_offset(r, c & 7);
+                *reinterpret_cast<float4*>(w_hi + off) = hi;
+                *reinterpret_cast<float4*>(w_lo + off) = lo;
+            }
+        }
+    }
+    for (int idx = tid; idx < HB; idx += kThreads) b1s[idx] = __ldg(b1 + p * HB + idx);
+    for (int base = tid; base < n_w2; base += kStageLd * kThreads) {
+        float w[kStageLd];
+#pragma unroll
+        for (int u = 0; u < kStageLd; ++u) {
+            const int idx = base + u * kThreads, j = idx / NP, n = idx - j * NP;
+            w[u] = idx < n_w2 && n < a.N2 ? __ldg(W2 + (size_t)n * a.H + p * HB + j) : 0.f;
+        }
+#pragma unroll
+        for (int u = 0; u < kStageLd; ++u) {
+            const int idx = base + u * kThreads, j = idx / NP, n = idx - j * NP;
+            if (idx < n_w2) w2s[j * NPS + n] = w[u];
+        }
+    }
+}
+
+// Epilogue of one 32-unit slice: bias, ReLU, second layer on this thread's 2 rows x 8 units of the
+// accumulator, added into the partial sums p0 / p1 of rows 16 warp + g and + 8
+template <int NP>
+__device__ __forceinline__ void slice_epilogue(const float (&d)[16], int nc, int q, const float* b1s, const float* w2s,
+                                               float (&p0)[NP], float (&p1)[NP]) {
+    constexpr int NPS = w2s_stride(NP);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int j = nc * 32 + 8 * i + 2 * q + e;
+            const float bj = b1s[j];
+            const float h0 = fmaxf(d[4 * i + e] + bj, 0.f);
+            const float h1 = fmaxf(d[4 * i + 2 + e] + bj, 0.f);
+            if constexpr (NP % 4 == 0) {
+#pragma unroll
+                for (int n = 0; n < NP; n += 4) {
+                    const float4 w = *reinterpret_cast<const float4*>(w2s + NPS * j + n);
+                    p0[n] = fmaf(h0, w.x, p0[n]), p0[n + 1] = fmaf(h0, w.y, p0[n + 1]);
+                    p0[n + 2] = fmaf(h0, w.z, p0[n + 2]), p0[n + 3] = fmaf(h0, w.w, p0[n + 3]);
+                    p1[n] = fmaf(h1, w.x, p1[n]), p1[n + 1] = fmaf(h1, w.y, p1[n + 1]);
+                    p1[n + 2] = fmaf(h1, w.z, p1[n + 2]), p1[n + 3] = fmaf(h1, w.w, p1[n + 3]);
+                }
+            } else {
+                const float w = w2s[j];
+                p0[0] = fmaf(h0, w, p0[0]), p1[0] = fmaf(h1, w, p1[0]);
+            }
+        }
+    }
+}
+
+// The quad's four column sets meet (fixed order), lane q == 0 writes (pass 0: b2 + z_0) or adds to
+// what it wrote in the previous pass the two rows of this tile
+template <int NP>
+__device__ __forceinline__ void write_rows(const FwdTcArgs& a, int p, int tile, int warp, int g, int q, float (&p0)[NP],
+                                           float (&p1)[NP]) {
+    const float* __restrict__ b2 = a.params + a.lay.ob2;
+#pragma unroll
+    for (int n = 0; n < NP; ++n) {
+        p0[n] += __shfl_xor_sync(IMPALA_FULL_MASK, p0[n], 1);
+        p1[n] += __shfl_xor_sync(IMPALA_FULL_MASK, p1[n], 1);
+        p0[n] += __shfl_xor_sync(IMPALA_FULL_MASK, p0[n], 2);
+        p1[n] += __shfl_xor_sync(IMPALA_FULL_MASK, p1[n], 2);
+    }
+    if (q == 0) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = tile * kTileM + 16 * warp + g + 8 * h;
+            if (row < a.M) {
+                float* o = a.out + (size_t)row * a.N2;
+#pragma unroll
+                for (int n = 0; n < NP; ++n)
+                    if (n < a.N2) o[n] = (p == 0 ? __ldg(b2 + n) : o[n]) + (h ? p1[n] : p0[n]);
+            }
+        }
+    }
 }
 
 // One CTA's share of a network: CTA `cta` of `ncta`; warpgroup w takes tiles u, u + ncta * kWG, ...
 // with u = cta * kWG + w (a launch may give different CTA ranges to different networks).
+//
+// x fragments in registers (one K atom).  Thread (warp, g, q) owns rows 16 warp + g and + 8
+// of the tile in both the A fragment and the accumulator, so it loads its own features 8 kk + q and
+// 8 kk + q + 4 of those two rows straight from global memory: nothing is staged, and a warpgroup
+// never waits for another thread.  The next tile's raw values are in flight in xr while the current
+// tile computes; they are split into hi / lo after the tile's last MMA batch has retired.  Only W1
+// is read from shared memory (1 KB per MMA instead of 3 KB), and the tile loop has no barrier.
+// The 32-unit slices go to the tensor cores two at a time, in one batch with two accumulators (see
+// `issue`): a tile waits on 4 MMA chains instead of 8.
 template <int NP, int KA>
-__device__ __forceinline__ void fwd_tc_body(const FwdTcArgs& a, const int cta, const int ncta) {
+__device__ __forceinline__ void fwd_rs_body(const FwdTcArgs& a, const int cta, const int ncta) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+    const int HB = a.hb;
+    uint8_t* w_hi = smem;  // [KA atoms][HB rows][128 B]
+    uint8_t* w_lo = w_hi + KA * HB * 128;
+    float* b1s = reinterpret_cast<float*>(smem + 2 * KA * HB * 128);  // [HB]
+    float* w2s = b1s + HB;                                             // [HB][NPS]
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int g = lane >> 2, q = lane & 3;
+    const int O = a.O, ksteps = (O + 7) >> 3, nslices = HB / 32;
+    const int unit = cta * kWG + wg, nunits = ncta * kWG;
+
+    constexpr int KS = 4 * KA;  // K steps of 8 features
+    float xr[KS][4];            // next tile, raw: A fragment slot i = row + 8 (i & 1), feature 8 kk + q + 4 (i >> 1)
+    uint32_t xh[KS][4], xl[KS][4];
+    auto load = [&](int tile) {
+#pragma unroll
+        for (int kk = 0; kk < KS; ++kk) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int row = tile * kTileM + 16 * warp + g + 8 * (i & 1), f = 8 * kk + q + 4 * (i >> 1);
+                xr[kk][i] = 0.f;
+                if (kk < ksteps && tile < a.num_tiles && row < a.M && f < O) xr[kk][i] = __ldg(a.x + (size_t)row * O + f);
+            }
+        }
+    };
+    // One MMA batch for S = 1 or 2 slices (nc, nc + 1), each into its own accumulator: per slice
+    // lo * hi + hi * lo over all K steps first, hi * hi last (see the header).  The MMAs into one
+    // accumulator form a dependent chain; with two slices the two chains interleave, so a batch takes
+    // about as long as one chain.  Descriptors = W1 hi / lo's plus the operand's offset in 16-byte
+    // units (start address field); the bases are opaque per batch, or every descriptor is hoisted
+    // into a register pair of its own.
+    const uint64_t dw_hi = tc::smem_desc_k_sw128(w_hi, 0), dw_lo = tc::smem_desc_k_sw128(w_lo, 0);
+    auto issue = [&](float (&d0)[16], float (&d1)[16], int nc, auto nslc) {
+        constexpr int S = decltype(nslc)::value;
+        uint64_t bw_hi = dw_hi, bw_lo = dw_lo;
+        asm volatile("" : "+l"(bw_hi), "+l"(bw_lo));
+        auto wo = [&](int kk, int s) -> uint32_t {
+            return ((kk >> 2) * (HB * 128) + (nc + s) * 32 * 128 + (kk & 3) * 32) >> 4;
+        };
+#pragma unroll
+        for (int i = 0; i < 16; ++i) d0[i] = 0.f, d1[i] = 0.f;
+        tc::fence_acc(d0);  // zeroed before the warpgroup fence (see mlp_bwd_tc.cu)
+        if constexpr (S == 2) tc::fence_acc(d1);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < KS; ++kk) {
+            if (kk < ksteps) {
+                tc::wgmma_n32_rs(d0, xl[kk], bw_hi + wo(kk, 0), kk > 0);
+                if constexpr (S == 2) tc::wgmma_n32_rs(d1, xl[kk], bw_hi + wo(kk, 1), kk > 0);
+                tc::wgmma_n32_rs(d0, xh[kk], bw_lo + wo(kk, 0), true);
+                if constexpr (S == 2) tc::wgmma_n32_rs(d1, xh[kk], bw_lo + wo(kk, 1), true);
+            }
+        }
+#pragma unroll
+        for (int kk = 0; kk < KS; ++kk) {
+            if (kk < ksteps) {
+                tc::wgmma_n32_rs(d0, xh[kk], bw_hi + wo(kk, 0), true);
+                if constexpr (S == 2) tc::wgmma_n32_rs(d1, xh[kk], bw_hi + wo(kk, 1), true);
+            }
+        }
+        tc::wgmma_commit();
+    };
+
+    const int npass = a.H / HB;
+    for (int p = 0; p < npass; ++p) {
+        load(unit);       // in flight during the weight staging
+        __syncthreads();  // the previous pass is done with the weights
+        stage_weights<NP, KA>(a, p, w_hi, w_lo, b1s, w2s);
+        tc::fence_proxy_async();
+        __syncthreads();
+
+        for (int tile = unit; tile < a.num_tiles; tile += nunits) {
+            // the previous tile's MMAs have all retired: its fragments may be overwritten
+#pragma unroll
+            for (int kk = 0; kk < KS; ++kk) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    float hi, lo;
+                    tc::split_tf32(xr[kk][i], hi, lo);
+                    xh[kk][i] = __float_as_uint(hi), xl[kk][i] = __float_as_uint(lo);
+                }
+                tc::fence_frag(xh[kk]);
+                tc::fence_frag(xl[kk]);
+            }
+            load(tile + nunits);  // in flight during this tile's MMAs and epilogue
+
+            float p0[NP], p1[NP];
+#pragma unroll
+            for (int n = 0; n < NP; ++n) p0[n] = 0.f, p1[n] = 0.f;
+            int nc = 0;
+            for (; nc + 2 <= nslices; nc += 2) {
+                float d0[16], d1[16];
+                issue(d0, d1, nc, std::integral_constant<int, 2>{});
+                tc::wgmma_wait<0>();
+                tc::fence_acc(d0), tc::fence_acc(d1);
+                slice_epilogue<NP>(d0, nc, q, b1s, w2s, p0, p1);
+                slice_epilogue<NP>(d1, nc + 1, q, b1s, w2s, p0, p1);
+            }
+            if (nc < nslices) {  // odd number of slices (H = 32, 96, 160, 224)
+                float d0[16], d1[16];
+                issue(d0, d1, nc, std::integral_constant<int, 1>{});
+                tc::wgmma_wait<0>();
+                tc::fence_acc(d0);
+                slice_epilogue<NP>(d0, nc, q, b1s, w2s, p0, p1);
+            }
+            write_rows<NP>(a, p, tile, warp, g, q, p0, p1);
+        }
+    }
+}
+
+// x tile staged in shared memory (four K atoms): each warpgroup splits it into its own hi / lo
+// swizzled tiles, and every slice waits for its MMAs before its epilogue.
+template <int NP, int KA>
+__device__ __forceinline__ void fwd_ss_body(const FwdTcArgs& a, const int cta, const int ncta) {
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment (SWIZZLE_128B atoms) by OFFSETTING the __shared__ array
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -69,13 +312,8 @@ __device__ __forceinline__ void fwd_tc_body(const FwdTcArgs& a, const int cta, c
     uint8_t* x_lo = x_hi + KA * kXAtomBytes;
     float* b1s = reinterpret_cast<float*>(smem + 2 * KA * HB * 128 + kWG * 2 * KA * kXAtomBytes);  // [HB]
     float* w2s = b1s + HB;                                                                         // [HB][NPS]
-    constexpr int NPS = w2s_stride(NP);
 
     const int O = a.O, ochunks = O >> 2, ksteps = (O + 7) >> 3;
-    const float* __restrict__ W1 = a.params + a.lay.oW1;
-    const float* __restrict__ b1 = a.params + a.lay.ob1;
-    const float* __restrict__ W2 = a.params + a.lay.oW2;
-    const float* __restrict__ b2 = a.params + a.lay.ob2;
     const int unit = cta * kWG + wg, nunits = ncta * kWG;
     const int g = lane >> 2, q = lane & 3;
 
@@ -95,26 +333,12 @@ __device__ __forceinline__ void fwd_tc_body(const FwdTcArgs& a, const int cta, c
 
     const int npass = a.H / HB;
     for (int p = 0; p < npass; ++p) {
-        // ---- stage this block's W1 rows (hi / lo swizzled tiles), b1 and W2 (transposed)
+        load(unit);       // in flight during the weight staging
         __syncthreads();  // the previous pass is done with the weights
-        for (int idx = tid; idx < HB * 8 * KA; idx += kThreads) {
-            const int r = idx / (8 * KA), c = idx % (8 * KA);
-            float4 w = make_float4(0.f, 0.f, 0.f, 0.f), hi, lo;
-            if (c < ochunks) w = __ldg(reinterpret_cast<const float4*>(W1 + (size_t)(p * HB + r) * O) + c);
-            tc::split4(w, hi, lo);
-            const uint32_t off = (c >> 3) * (HB * 128) + tc::sw128_offset(r, c & 7);
-            *reinterpret_cast<float4*>(w_hi + off) = hi;
-            *reinterpret_cast<float4*>(w_lo + off) = lo;
-        }
-        for (int idx = tid; idx < HB; idx += kThreads) b1s[idx] = __ldg(b1 + p * HB + idx);
-        for (int idx = tid; idx < HB * NP; idx += kThreads) {
-            const int j = idx / NP, n = idx - j * NP;
-            w2s[j * NPS + n] = n < a.N2 ? __ldg(W2 + (size_t)n * a.H + p * HB + j) : 0.f;
-        }
+        stage_weights<NP, KA>(a, p, w_hi, w_lo, b1s, w2s);
         tc::fence_proxy_async();
         __syncthreads();
 
-        load(unit);
         for (int tile = unit; tile < a.num_tiles; tile += nunits) {
             // ---- x tile -> hi / lo swizzled tiles (the warpgroup's previous MMAs have all retired)
             tc::named_bar(1 + wg, 128);
@@ -160,68 +384,38 @@ __device__ __forceinline__ void fwd_tc_body(const FwdTcArgs& a, const int cta, c
                 tc::wgmma_commit();
                 tc::wgmma_wait<0>();
                 tc::fence_acc(d);
-                // ---- epilogue of the slice: bias, ReLU, second layer (this thread's 2 rows x 8 units)
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int j = nc * 32 + 8 * i + 2 * q + e;
-                        const float bj = b1s[j];
-                        const float h0 = fmaxf(d[4 * i + e] + bj, 0.f);
-                        const float h1 = fmaxf(d[4 * i + 2 + e] + bj, 0.f);
-                        if constexpr (NP % 4 == 0) {
-#pragma unroll
-                            for (int n = 0; n < NP; n += 4) {
-                                const float4 w = *reinterpret_cast<const float4*>(w2s + NPS * j + n);
-                                p0[n] = fmaf(h0, w.x, p0[n]), p0[n + 1] = fmaf(h0, w.y, p0[n + 1]);
-                                p0[n + 2] = fmaf(h0, w.z, p0[n + 2]), p0[n + 3] = fmaf(h0, w.w, p0[n + 3]);
-                                p1[n] = fmaf(h1, w.x, p1[n]), p1[n + 1] = fmaf(h1, w.y, p1[n + 1]);
-                                p1[n + 2] = fmaf(h1, w.z, p1[n + 2]), p1[n + 3] = fmaf(h1, w.w, p1[n + 3]);
-                            }
-                        } else {
-                            const float w = w2s[j];
-                            p0[0] = fmaf(h0, w, p0[0]), p1[0] = fmaf(h1, w, p1[0]);
-                        }
-                    }
-                }
+                slice_epilogue<NP>(d, nc, q, b1s, w2s, p0, p1);
             }
-            // the quad's four column sets meet (fixed order), lane q == 0 writes the two rows
-#pragma unroll
-            for (int n = 0; n < NP; ++n) {
-                p0[n] += __shfl_xor_sync(IMPALA_FULL_MASK, p0[n], 1);
-                p1[n] += __shfl_xor_sync(IMPALA_FULL_MASK, p1[n], 1);
-                p0[n] += __shfl_xor_sync(IMPALA_FULL_MASK, p0[n], 2);
-                p1[n] += __shfl_xor_sync(IMPALA_FULL_MASK, p1[n], 2);
-            }
-            if (q == 0) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int row = tile * kTileM + 16 * warp + g + 8 * h;
-                    if (row < a.M) {
-                        float* o = a.out + (size_t)row * a.N2;
-#pragma unroll
-                        for (int n = 0; n < NP; ++n)
-                            if (n < a.N2) o[n] = (p == 0 ? __ldg(b2 + n) : o[n]) + (h ? p1[n] : p0[n]);
-                    }
-                }
-            }
+            write_rows<NP>(a, p, tile, warp, g, q, p0, p1);
         }
     }
 }
 
 template <int NP, int KA>
 __global__ void __launch_bounds__(kThreads) mlp_fwd_tc_kernel(const __grid_constant__ FwdTcArgs a) {
-    fwd_tc_body<NP, KA>(a, blockIdx.x, gridDim.x);
+    if constexpr (x_in_regs(KA)) fwd_rs_body<NP, KA>(a, blockIdx.x, gridDim.x);
+    else fwd_ss_body<NP, KA>(a, blockIdx.x, gridDim.x);
 }
 
 // Policy and value network of one learner step in ONE launch: CTAs [0, n_pi) run the policy
 // tiles, the rest the value-function tiles.  Both read the same observations; one launch means
-// one weight staging per CTA and a finer tile quantisation than two launches.
+// one weight staging per CTA and a finer tile quantisation than two launches.  Both networks run
+// through ONE body instantiation (NP = 4; the value function's W2 rows are zero-padded to 4 outputs,
+// and its output 0 takes exactly the FMAs, in the same order, of the one-output epilogue): with a
+// branch on the network around two instantiations, or around the epilogue form, ptxas serializes
+// every wgmma of the kernel (C7520, a compiler-inserted warpgroup arrive in a divergent path).  The
+// arguments are selected field by field for the same reason.
 __global__ void __launch_bounds__(kThreads)
 mlp_fwd_tc_pair_kernel(const __grid_constant__ FwdTcArgs a_pi, const __grid_constant__ FwdTcArgs a_vf,
                        const int n_pi) {
-    if ((int)blockIdx.x < n_pi) fwd_tc_body<4, 1>(a_pi, blockIdx.x, n_pi);
-    else fwd_tc_body<1, 1>(a_vf, (int)blockIdx.x - n_pi, (int)gridDim.x - n_pi);
+    const bool pi = (int)blockIdx.x < n_pi;
+    FwdTcArgs a = a_pi;
+    a.params = pi ? a_pi.params : a_vf.params, a.out = pi ? a_pi.out : a_vf.out;
+    a.M = pi ? a_pi.M : a_vf.M, a.H = pi ? a_pi.H : a_vf.H, a.N2 = pi ? a_pi.N2 : a_vf.N2;
+    a.num_tiles = pi ? a_pi.num_tiles : a_vf.num_tiles, a.hb = pi ? a_pi.hb : a_vf.hb;
+    a.lay.oW1 = pi ? a_pi.lay.oW1 : a_vf.lay.oW1, a.lay.ob1 = pi ? a_pi.lay.ob1 : a_vf.lay.ob1;
+    a.lay.oW2 = pi ? a_pi.lay.oW2 : a_vf.lay.oW2, a.lay.ob2 = pi ? a_pi.lay.ob2 : a_vf.lay.ob2;
+    fwd_rs_body<4, 1>(a, pi ? (int)blockIdx.x : (int)blockIdx.x - n_pi, pi ? n_pi : (int)gridDim.x - n_pi);
 }
 
 FwdTcArgs make_fwd_args(const float* x, const float* params, float* out, int M, int O, int H, int N2) {
@@ -288,14 +482,16 @@ int impala_mlp_fwd_tc(const float* x, const float* params, float* out, int M, in
 }
 
 // Both networks in one launch (policy: 2..4 outputs, value fn: 1 output); the caller has checked
-// impala_mlp_fwd_tc_eligible for each.  Per-tile cost weights (policy epilogue does 4 FMA per
-// hidden unit, the value fn 1) split the CTAs between the two tile lists.
+// impala_mlp_fwd_tc_eligible for each.  Per-tile cost weights split the CTAs between the two tile
+// lists; both networks run the same MMAs and the same 4-output epilogue per tile, so the default
+// weighs a policy tile as one value-function tile.
 int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* params_vf, float* logits,
                            float* values, int M_pi, int M_vf, int O, int H_pi, int H_vf, int A,
                            cudaStream_t st) {
     const FwdTcArgs a_pi = make_fwd_args(x, params_pi, logits, M_pi, O, H_pi, A);
     const FwdTcArgs a_vf = make_fwd_args(x, params_vf, values, M_vf, O, H_vf, 1);
-    const size_t s_pi = fwd_smem_bytes(a_pi.hb, 1, 4), s_vf = fwd_smem_bytes(a_vf.hb, 1, 1);
+    // both networks stage W2 in the 4-output layout (one body instantiation, see the kernel)
+    const size_t s_pi = fwd_smem_bytes(a_pi.hb, 1, 4), s_vf = fwd_smem_bytes(a_vf.hb, 1, 4);
     const size_t smem = s_pi > s_vf ? s_pi : s_vf;
     int grid = 0;
     const int rc = resident_grid(mlp_fwd_tc_pair_kernel, smem, &grid);
@@ -303,7 +499,7 @@ int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* 
     const int units_pi = (a_pi.num_tiles + kWG - 1) / kWG, units_vf = (a_vf.num_tiles + kWG - 1) / kWG;
     if (grid > units_pi + units_vf) grid = units_pi + units_vf;
     const int n_pi = impala_pair_split(units_pi, units_vf, grid,
-                                       impala_env_int("IMPALA_PAIR_W_FWD", 160) * (H_pi / 32),
+                                       impala_env_int("IMPALA_PAIR_W_FWD", 100) * (H_pi / 32),
                                        100 * (H_vf / 32));
     mlp_fwd_tc_pair_kernel<<<grid, kThreads, smem, st>>>(a_pi, a_vf, n_pi);
     return impala_launch_status();

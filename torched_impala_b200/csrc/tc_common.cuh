@@ -54,6 +54,11 @@ __device__ __forceinline__ void fence_acc(float (&d)[16]) {
 #pragma unroll
     for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// the same for an A fragment held in registers: defined before the warpgroup fence, untouched after
+__device__ __forceinline__ void fence_frag(uint32_t (&a)[4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
 
 #define IMPALA_WG_D16                                                                                   \
     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}"
