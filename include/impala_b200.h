@@ -76,7 +76,10 @@ int impala_ingest_shard(void* dev_slab, const void* host_slab, int T, int B, int
 /* out[m, :] = relu(x[m, :] W1^T + b1) W2^T + b2 for m < M.
  * Replaces MlpPolicy.forward / MlpValueFn.forward in eval mode
  * (models.py:23-25, :51-52) as called at learner.py:112-113 on the flattened
- * (T*B, O) / ((T+1)*B, O) batch.  x row-major (M,O); out row-major (M,N2). */
+ * (T*B, O) / ((T+1)*B, O) batch.  x row-major (M,O); out row-major (M,N2).
+ * Shapes: O <= 128 with N2 <= 32 (tensor cores or FP32 kernels), and 128 < O <= 1024 with O % 4 == 0,
+ * H = 128 k <= 1024, N2 <= 32 (tensor cores only: refused under IMPALA_MLP_TC=0 / IMPALA_MLP_TCW=0);
+ * anything else returns IMPALA_ERR_UNSUPPORTED_SHAPE. */
 int impala_mlp_forward(const float* x, const float* params, float* out, int M, int O, int H,
                        int N2, void* stream);
 
@@ -92,7 +95,9 @@ int impala_mlp_forward_pair(const float* x, const float* params_pi, const float*
 /* Bytes of scratch impala_mlp_backward needs for these dimensions.  The caller zero-fills
  * it ONCE after allocation; every call leaves its control words zeroed again (the tensor-core
  * kernel meets at a self-re-arming grid barrier before its in-kernel reduction; on a workspace
- * that was never zeroed it traps - a launch failure, not a hang). */
+ * that was never zeroed it traps - a launch failure, not a hang).  For O > 128 it holds DP^T (H x M
+ * floats, the bulk of it) and two bounded sets of partial gradient rows.  Shape limits as
+ * impala_mlp_forward; IMPALA_ERR_UNSUPPORTED_SHAPE (-2) outside them. */
 int64_t impala_mlp_backward_workspace(int M, int O, int H, int N2);
 
 /* Gradient of sum_m <dout[m,:], mlp(x[m,:])> w.r.t. the parameter block, written

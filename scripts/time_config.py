@@ -1,4 +1,4 @@
-"""Device-resident learner step time for any BASELINE config (c2..c5) or the Atari-RAM shape: CUDA events,
+"""Device-resident learner step time for any BASELINE config (c2..c5) or the Atari-RAM / MinAtar shapes: CUDA events,
 L2 flushed.  --compare-tc also times the FP32 FFMA MLP path (IMPALA_MLP_TC=0) in the same process,
 alternating step by step with the default path, so both numbers see the same clocks and neighbours."""
 import argparse
@@ -17,7 +17,13 @@ CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256), "c5": dict(T=100, B=8192, O=6
        "c3": dict(T=20, B=1024, O=24, A=4, H=256), "c2": dict(T=20, B=256, O=4, A=2, H=32),
        # Atari from RAM (128-byte observation, 18 actions): P = 70 931 parameters, 50 675 712 input bytes
        # and 24.4 GFLOP of MLP work per step (SURVEY 8d formulas)
-       "ram": dict(T=20, B=4096, O=128, A=18, H=256)}
+       "ram": dict(T=20, B=4096, O=128, A=18, H=256),
+       # 4 stacked Atari RAM frames: P = 267 539 parameters, 4x the layer-1 work of "ram": 88 GFLOP per step
+       # (forward + dW1 of both networks), ~400 GFLOP executed on the tensor cores (3xTF32, the backward's
+       # recompute), 176 MB of observations
+       "ram4": dict(T=20, B=4096, O=512, A=18, H=256),
+       # MinAtar Breakout / Asterix, flattened 10x10x4 binary grids: P = 207 111 parameters
+       "minatar": dict(T=20, B=4096, O=400, A=6, H=256)}
 ap = argparse.ArgumentParser()
 ap.add_argument("--config", default="c5")
 ap.add_argument("--steps", type=int, default=30)

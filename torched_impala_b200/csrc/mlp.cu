@@ -180,6 +180,8 @@ extern "C" int impala_mlp_forward(const float* x, const float* params, float* ou
         return impala_mlp_fwd_tcw(x, params, out, M, O, H, N2, (cudaStream_t)stream);
     if (!(tc_env && tc_env[0] == '0') && impala_mlp_fwd_tcx_eligible(x, M, O, H, N2))
         return impala_mlp_fwd_tcx(x, params, out, M, O, H, N2, (cudaStream_t)stream);
+    if (O > 128 && impala_mlp_obs_shape_ok(M, O, H, N2))  // wide observations: K-streamed kernels
+        return impala_mlp_fwd_obs(x, params, out, M, O, H, N2, (cudaStream_t)stream);
     MlpArgs a{};
     MlpConfig c{};
     size_t smem;
@@ -209,6 +211,10 @@ extern "C" int impala_mlp_forward_pair(const float* x, const float* params_pi, c
 }
 
 extern "C" int64_t impala_mlp_backward_workspace(int M, int O, int H, int N2) {
+    if (O > 128) {
+        ObsBwdLayout L;
+        return impala_mlp_obs_bwd_layout(M, O, H, N2, &L) ? kWsHeader + L.bytes : IMPALA_ERR_UNSUPPORTED_SHAPE;
+    }
     MlpConfig c{};
     if (M < 1 || !pick_config(O, H, N2, true, &c)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
     int64_t tiles = (M + kRows - 1) / kRows;
@@ -220,6 +226,23 @@ extern "C" int impala_mlp_backward(const float* x, const float* params, const fl
                                    double* grad, void* workspace, int64_t workspace_bytes, int M,
                                    int O, int H, int N2, void* stream) {
     if (!x || !params || !dout || !grad || !workspace) return IMPALA_ERR_BAD_ARG;
+    if (O > 128) {
+        // wide observations: DP^T and two sets of partial rows in the workspace, each summed in float64
+        ObsBwdLayout L;
+        if (!impala_mlp_obs_bwd_layout(M, O, H, N2, &L)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+        if (workspace_bytes < kWsHeader + L.bytes) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
+        char* ws = static_cast<char*>(workspace) + kWsHeader;
+        const int rc = impala_mlp_bwd_obs(x, params, dout, ws, L, M, O, H, N2, (cudaStream_t)stream);
+        if (rc != IMPALA_OK) return rc;
+        const MlpLayout lay = impala_make_layout(O, H, N2);
+        const int64_t nr = lay.total - lay.ob1;
+        reduce_partials_kernel<<<(unsigned)((nr + 31) / 32), kRedWarps * 32, 0, (cudaStream_t)stream>>>(
+            reinterpret_cast<const float*>(ws + L.rest_off), grad + lay.ob1, L.r1, nr);
+        if (const int e = impala_launch_status(); e != IMPALA_OK) return e;
+        reduce_partials_kernel<<<(unsigned)((lay.ob1 + 31) / 32), kRedWarps * 32, 0, (cudaStream_t)stream>>>(
+            reinterpret_cast<const float*>(ws + L.w1_off), grad, L.p2, lay.ob1);
+        return impala_launch_status();
+    }
     MlpArgs a{};
     MlpConfig c{};
     size_t smem;

@@ -70,6 +70,20 @@ bool impala_mlp_bwd_tcx_eligible(const float* x, int M, int O, int H, int N2);
 int impala_mlp_bwd_tcx(const float* x, const float* params, const float* dout, float* ws, int M, int O, int H,
                        int N2, cudaStream_t st, int* nparts);
 
+// Wide observations (mlp_obs_tc.cu): 128 < O <= 1024, O % 4 == 0, H a multiple of 128 up to 1024, N2 <= 32,
+// K streamed; false under IMPALA_MLP_TC=0 / IMPALA_MLP_TCW=0 (there is no FP32 kernel for these widths).
+bool impala_mlp_obs_shape_ok(int M, int O, int H, int N2);
+int impala_mlp_fwd_obs(const float* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st);
+// Backward workspace past the control header: byte offsets of DP^T and of the two sets of float32 partial
+// rows (r1 rows of layout entries [ob1, total), p2 rows of [0, ob1)) for reduce_partials_kernel.
+struct ObsBwdLayout {
+    int64_t dpt_off, rest_off, w1_off, bytes;
+    int mp, r1, p2;
+};
+bool impala_mlp_obs_bwd_layout(int M, int O, int H, int N2, ObsBwdLayout* L);
+int impala_mlp_bwd_obs(const float* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L, int M,
+                       int O, int H, int N2, cudaStream_t st);
+
 // One per padded observation width / direction, defined in mlp_inst.cu.
 #define IMPALA_DECL_DISPATCH(OPV)                                                             \
     int impala_mlp_fwd_op##OPV(const MlpArgs&, const MlpConfig&, size_t, cudaStream_t, int*); \
