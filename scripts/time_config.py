@@ -15,6 +15,8 @@ from torched_impala_b200.utils import default_hparams  # noqa: E402
 
 CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256), "c5": dict(T=100, B=8192, O=64, A=4, H=512),
        "c3": dict(T=20, B=1024, O=24, A=4, H=256), "c2": dict(T=20, B=256, O=4, A=2, H=32),
+       # c4 with 512 hidden units: the wide forward at one K atom (two passes of 256) and the wide backward
+       "c4h512": dict(T=20, B=4096, O=24, A=4, H=512),
        # Atari from RAM (128-byte observation, 18 actions): P = 70 931 parameters, 50 675 712 input bytes
        # and 24.4 GFLOP of MLP work per step (SURVEY 8d formulas)
        "ram": dict(T=20, B=4096, O=128, A=18, H=256),

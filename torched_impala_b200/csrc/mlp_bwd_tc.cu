@@ -36,7 +36,9 @@
 // are independent - each takes alternate tiles of the CTA's share, with its own x stage and named
 // barrier - so one warpgroup's MMAs overlap the other's CUDA-core epilogue.  The warpgroups meet once,
 // at the end (fixed order), and the rows are summed in-kernel after a grid barrier (paired launch,
-// optional peer push).
+// optional peer push).  GEMM1 covers the tile's 64 batch rows with one m64n64 MMA per product (the
+// accumulator is the two 32-row halves side by side, so every entry takes the same products in the same
+// order as with two m64n32 chains); GEMM2 (N = 32 features) stays m64n32.
 //
 // Wide shapes (bwd_tc_body): one CTA = 2 warpgroups = 128 hidden units per pass, wider layers walked
 // in passes (x is re-read once per pass); reduce_partials_kernel sums the rows.
@@ -657,91 +659,79 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdTcArgs& a, const int c
         tc::named_bar(bar, 128);
         load(tile + tstride);  // in flight during this tile's MMAs and epilogue
 
-        // ---- GEMM1: PRE = W1_blk * X^T (N = 32 halves of the tile's batch rows), A from registers;
-        // descriptors = the stage's plus the operand's offset in 16-byte units (start address field)
-        // (bases opaque per tile: hoisted out of the loop, every descriptor would hold two registers)
+        // ---- GEMM1: PRE = W1_blk * X^T (one m64n64 MMA per product over the tile's 64 batch rows), A
+        // from registers; descriptors = the stage's plus the operand's offset in 16-byte units (start
+        // address field) (bases opaque per tile: hoisted out of the loop, every descriptor would hold two
+        // registers)
         uint64_t bx_hi = dx_hi, bx_lo = dx_lo;
         asm volatile("" : "+l"(bx_hi), "+l"(bx_lo));
-        float d[2][16];
+        float d[32];
 #pragma unroll
-        for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) d[nb][i] = 0.f;
+        for (int i = 0; i < 32; ++i) d[i] = 0.f;
         // zeroed accumulators defined before the warpgroup fence (see bwd_tc_body)
-#pragma unroll
-        for (int nb = 0; nb < 2; ++nb) tc::fence_acc(d[nb]);
+        tc::fence_acc(d);
         tc::wgmma_fence();
 #pragma unroll
-        for (int nb = 0; nb < 2; ++nb) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                if (kk < ksteps) {
-                    const uint32_t xo = (nb * 32 * 128 + kk * 32) >> 4;
-                    tc::wgmma_n32_rs(d[nb], wl[kk], bx_hi + xo, kk > 0);
-                    tc::wgmma_n32_rs(d[nb], wh[kk], bx_lo + xo, true);
-                }
+        for (int kk = 0; kk < 4; ++kk) {
+            if (kk < ksteps) {
+                const uint32_t xo = (kk * 32) >> 4;
+                tc::wgmma_n64_rs(d, wl[kk], bx_hi + xo, kk > 0);
+                tc::wgmma_n64_rs(d, wh[kk], bx_lo + xo, true);
             }
+        }
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                if (kk < ksteps) tc::wgmma_n32_rs(d[nb], wh[kk], bx_hi + ((nb * 32 * 128 + kk * 32) >> 4), true);
-            }
+        for (int kk = 0; kk < 4; ++kk) {
+            if (kk < ksteps) tc::wgmma_n64_rs(d, wh[kk], bx_hi + ((kk * 32) >> 4), true);
         }
         tc::wgmma_commit();
         tc::wgmma_wait<0>();
-#pragma unroll
-        for (int nb = 0; nb < 2; ++nb) tc::fence_acc(d[nb]);
+        tc::fence_acc(d);
 
         // ---- epilogue: d <- DP in place (thread: hidden units j0 / j1, batch columns 8 i + 2 q + e)
 #pragma unroll
-        for (int nb = 0; nb < 2; ++nb) {
+        for (int i = 0; i < 8; ++i) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int m = 32 * nb + 8 * i + 2 * q + e;
-                    float dz[NP];
-                    if constexpr (NP == 4) {
-                        const float4 t = *reinterpret_cast<const float4*>(dzs + 4 * m);
-                        dz[0] = t.x, dz[1] = t.y, dz[2] = t.z, dz[3] = t.w;
-                    } else {
-                        dz[0] = dzs[m];
-                    }
-                    // relu'(0) = 0 as in torch
-                    const float pre0 = d[nb][4 * i + e] + bj0, pre1 = d[nb][4 * i + 2 + e] + bj1;
-                    const float h0 = fmaxf(pre0, 0.f), h1 = fmaxf(pre1, 0.f);
-                    float dh0 = dz[0] * w2r0[0], dh1 = dz[0] * w2r1[0];
-#pragma unroll
-                    for (int n = 1; n < NP; ++n) dh0 = fmaf(dz[n], w2r0[n], dh0), dh1 = fmaf(dz[n], w2r1[n], dh1);
-#pragma unroll
-                    for (int n = 0; n < NP; ++n) gw0[n] = fmaf(dz[n], h0, gw0[n]), gw1[n] = fmaf(dz[n], h1, gw1[n]);
-                    const float dp0 = pre0 > 0.f ? dh0 : 0.f, dp1 = pre1 > 0.f ? dh1 : 0.f;
-                    gb10 += dp0, gb11 += dp1;
-                    d[nb][4 * i + e] = dp0, d[nb][4 * i + 2 + e] = dp1;
+            for (int e = 0; e < 2; ++e) {
+                const int m = 8 * i + 2 * q + e;
+                float dz[NP];
+                if constexpr (NP == 4) {
+                    const float4 t = *reinterpret_cast<const float4*>(dzs + 4 * m);
+                    dz[0] = t.x, dz[1] = t.y, dz[2] = t.z, dz[3] = t.w;
+                } else {
+                    dz[0] = dzs[m];
                 }
+                // relu'(0) = 0 as in torch
+                const float pre0 = d[4 * i + e] + bj0, pre1 = d[4 * i + 2 + e] + bj1;
+                const float h0 = fmaxf(pre0, 0.f), h1 = fmaxf(pre1, 0.f);
+                float dh0 = dz[0] * w2r0[0], dh1 = dz[0] * w2r1[0];
+#pragma unroll
+                for (int n = 1; n < NP; ++n) dh0 = fmaf(dz[n], w2r0[n], dh0), dh1 = fmaf(dz[n], w2r1[n], dh1);
+#pragma unroll
+                for (int n = 0; n < NP; ++n) gw0[n] = fmaf(dz[n], h0, gw0[n]), gw1[n] = fmaf(dz[n], h1, gw1[n]);
+                const float dp0 = pre0 > 0.f ? dh0 : 0.f, dp1 = pre1 > 0.f ? dh1 : 0.f;
+                gb10 += dp0, gb11 += dp1;
+                d[4 * i + e] = dp0, d[4 * i + 2 + e] = dp1;
             }
         }
 
         // ---- GEMM2: dW1 += DP * X (A = DP from registers).  Phase 1: dp_lo * x_hi; phase 2 (DP
         // overwritten by dp_hi in place): dp_hi * x_lo, then dp_hi * x_hi into its own accumulator
-        uint32_t lo[2][16];
+        uint32_t lo[32];
 #pragma unroll
-        for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const float hi = __uint_as_float(__float_as_uint(d[nb][i]) & 0xffffe000u);
-                lo[nb][i] = __float_as_uint(d[nb][i] - hi);
-                d[nb][i] = hi;
-            }
+        for (int i = 0; i < 32; ++i) {
+            const float hi = __uint_as_float(__float_as_uint(d[i]) & 0xffffe000u);
+            lo[i] = __float_as_uint(d[i] - hi);
+            d[i] = hi;
+        }
         uint64_t bxt_hi = dxt_hi, bxt_lo = dxt_lo;
         asm volatile("" : "+l"(bxt_hi), "+l"(bxt_lo));
         tc::wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < 8; ++kk) {
-            const int nb = kk >> 2, i = kk & 3;
-            const uint32_t al[4] = {lo[nb][4 * i], lo[nb][4 * i + 2], lo[nb][4 * i + 1], lo[nb][4 * i + 3]};
-            const uint32_t ah[4] = {__float_as_uint(d[nb][4 * i]), __float_as_uint(d[nb][4 * i + 2]),
-                                    __float_as_uint(d[nb][4 * i + 1]), __float_as_uint(d[nb][4 * i + 3])};
-            const uint32_t xo = (nb * 32 * 128 + i * 32) >> 4;
+            const uint32_t al[4] = {lo[4 * kk], lo[4 * kk + 2], lo[4 * kk + 1], lo[4 * kk + 3]};
+            const uint32_t ah[4] = {__float_as_uint(d[4 * kk]), __float_as_uint(d[4 * kk + 2]),
+                                    __float_as_uint(d[4 * kk + 1]), __float_as_uint(d[4 * kk + 3])};
+            const uint32_t xo = ((kk >> 2) * 32 * 128 + (kk & 3) * 32) >> 4;
             tc::wgmma_n32_rs(acc_c, al, bxt_hi + xo, true);
             tc::wgmma_n32_rs(acc_c, ah, bxt_lo + xo, true);
             tc::wgmma_n32_rs(acc_hh, ah, bxt_hi + xo, true);
@@ -749,12 +739,9 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdTcArgs& a, const int c
         tc::wgmma_commit();
         tc::wgmma_wait<0>();
         // the A registers are read asynchronously: keep them (and the accumulators) untouched until here
+        tc::fence_acc(d);
 #pragma unroll
-        for (int nb = 0; nb < 2; ++nb) {
-            tc::fence_acc(d[nb]);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) asm volatile("" : "+r"(lo[nb][i])::"memory");
-        }
+        for (int i = 0; i < 32; ++i) asm volatile("" : "+r"(lo[i])::"memory");
         tc::fence_acc(acc_hh), tc::fence_acc(acc_c);
     }
 
@@ -1043,12 +1030,13 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
     e = push ? opt_in(mlp_bwd_tc_pair_kernel<true>, smem) : opt_in(mlp_bwd_tc_pair_kernel<false>, smem);
     if (e != cudaSuccess) return (int)e;
-    // a CTA does one hidden block of a tile whatever H is: the per-tile weights do not scale with H
+    // a CTA does one hidden block of a tile whatever H is: the per-tile weights do not scale with H.  A
+    // policy tile (4-output epilogue) costs about 1.25 value-function tiles (scripts/tune_pair_split.py)
     const int gp = H_pi / 64, gv = H_vf / 64;
     int grid = sms < kMaxParts ? sms : kMaxParts;  // <= SM count: the grid barrier needs residency
     if (grid < gp + gv) return IMPALA_ERR_UNSUPPORTED_SHAPE;
     int sp = 1, sv = 1;
-    split_sets(a_pi.num_tiles, a_vf.num_tiles, grid, gp, gv, impala_env_int("IMPALA_PAIR_W_BWD", 105), 100, &sp, &sv);
+    split_sets(a_pi.num_tiles, a_vf.num_tiles, grid, gp, gv, impala_env_int("IMPALA_PAIR_W_BWD", 125), 100, &sp, &sv);
     grid = gp * sp + gv * sv;
     const int n_pi = gp * sp;
     // cooperative launch: the in-kernel grid barrier needs every CTA resident

@@ -29,7 +29,6 @@
 #include <map>
 #include <mutex>
 #include <tuple>
-#include <type_traits>
 
 #include "mlp_fwd_tc.cuh"
 #include "tc_common.cuh"
@@ -110,8 +109,9 @@ __device__ __forceinline__ void stage_weights(const FwdTcArgs& a, int p, uint8_t
 // never waits for another thread.  The next tile's raw values are in flight in xr while the current
 // tile computes; they are split into hi / lo after the tile's last MMA batch has retired.  Only W1
 // is read from shared memory (1 KB per MMA instead of 3 KB), and the tile loop has no barrier.
-// The 32-unit slices go to the tensor cores two at a time, in one batch with two accumulators (see
-// `issue`): a tile waits on 4 MMA chains instead of 8.
+// The 32-unit slices go to the tensor cores two at a time, as one m64n64 MMA chain into one
+// 32-register accumulator (see `issue`): a tile waits on 4 batches instead of 8, and issues 9 MMAs per
+// batch instead of 18.
 template <int NP, int KA>
 __device__ __forceinline__ void fwd_rs_body(const FwdTcArgs& a, const int cta, const int ncta) {
     extern __shared__ uint8_t smem_raw[];
@@ -140,40 +140,36 @@ __device__ __forceinline__ void fwd_rs_body(const FwdTcArgs& a, const int cta, c
             }
         }
     };
-    // One MMA batch for S = 1 or 2 slices (nc, nc + 1), each into its own accumulator: per slice
-    // lo * hi + hi * lo over all K steps first, hi * hi last (see the header).  The MMAs into one
-    // accumulator form a dependent chain; with two slices the two chains interleave, so a batch takes
-    // about as long as one chain.  Descriptors = W1 hi / lo's plus the operand's offset in 16-byte
+    // One MMA batch over the slices from nc on that the accumulator holds: two (32 registers, one
+    // m64n64 MMA per product, B = W1 rows [32 nc, 32 nc + 64), contiguous in the swizzled tile) or one
+    // (the odd slice, m64n32); lo * hi + hi * lo over all K steps first, hi * hi last (see the header).
+    // The MMAs form one dependent chain.  Descriptors = W1 hi / lo's plus the operand's offset in 16-byte
     // units (start address field); the bases are opaque per batch, or every descriptor is hoisted
     // into a register pair of its own.
     const uint64_t dw_hi = tc::smem_desc_k_sw128(w_hi, 0), dw_lo = tc::smem_desc_k_sw128(w_lo, 0);
-    auto issue = [&](float (&d0)[16], float (&d1)[16], int nc, auto nslc) {
-        constexpr int S = decltype(nslc)::value;
+    auto issue = [&](auto& d, int nc) {
+        constexpr int ND = sizeof(d) / sizeof(float);
+        auto mma = [&](const uint32_t(&x)[4], uint64_t bw, bool acc) {
+            if constexpr (ND == 32) tc::wgmma_n64_rs(d, x, bw, acc);
+            else tc::wgmma_n32_rs(d, x, bw, acc);
+        };
         uint64_t bw_hi = dw_hi, bw_lo = dw_lo;
         asm volatile("" : "+l"(bw_hi), "+l"(bw_lo));
-        auto wo = [&](int kk, int s) -> uint32_t {
-            return ((kk >> 2) * (HB * 128) + (nc + s) * 32 * 128 + (kk & 3) * 32) >> 4;
-        };
+        auto wo = [&](int kk) -> uint32_t { return ((kk >> 2) * (HB * 128) + nc * 32 * 128 + (kk & 3) * 32) >> 4; };
 #pragma unroll
-        for (int i = 0; i < 16; ++i) d0[i] = 0.f, d1[i] = 0.f;
-        tc::fence_acc(d0);  // zeroed before the warpgroup fence (see mlp_bwd_tc.cu)
-        if constexpr (S == 2) tc::fence_acc(d1);
+        for (int i = 0; i < ND; ++i) d[i] = 0.f;
+        tc::fence_acc(d);  // zeroed before the warpgroup fence (see mlp_bwd_tc.cu)
         tc::wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < KS; ++kk) {
             if (kk < ksteps) {
-                tc::wgmma_n32_rs(d0, xl[kk], bw_hi + wo(kk, 0), kk > 0);
-                if constexpr (S == 2) tc::wgmma_n32_rs(d1, xl[kk], bw_hi + wo(kk, 1), kk > 0);
-                tc::wgmma_n32_rs(d0, xh[kk], bw_lo + wo(kk, 0), true);
-                if constexpr (S == 2) tc::wgmma_n32_rs(d1, xh[kk], bw_lo + wo(kk, 1), true);
+                mma(xl[kk], bw_hi + wo(kk), kk > 0);
+                mma(xh[kk], bw_lo + wo(kk), true);
             }
         }
 #pragma unroll
         for (int kk = 0; kk < KS; ++kk) {
-            if (kk < ksteps) {
-                tc::wgmma_n32_rs(d0, xh[kk], bw_hi + wo(kk, 0), true);
-                if constexpr (S == 2) tc::wgmma_n32_rs(d1, xh[kk], bw_hi + wo(kk, 1), true);
-            }
+            if (kk < ksteps) mma(xh[kk], bw_hi + wo(kk), true);
         }
         tc::wgmma_commit();
     };
@@ -206,19 +202,18 @@ __device__ __forceinline__ void fwd_rs_body(const FwdTcArgs& a, const int cta, c
             for (int n = 0; n < NP; ++n) p0[n] = 0.f, p1[n] = 0.f;
             int nc = 0;
             for (; nc + 2 <= nslices; nc += 2) {
-                float d0[16], d1[16];
-                issue(d0, d1, nc, std::integral_constant<int, 2>{});
+                float d[32];
+                issue(d, nc);
                 tc::wgmma_wait<0>();
-                tc::fence_acc(d0), tc::fence_acc(d1);
-                slice_epilogue<NP>(d0, nc, q, b1s, w2s, p0, p1);
-                slice_epilogue<NP>(d1, nc + 1, q, b1s, w2s, p0, p1);
+                tc::fence_acc(d);
+                slice_epilogue<NP>(d, nc, q, b1s, w2s, p0, p1);
             }
             if (nc < nslices) {  // odd number of slices (H = 32, 96, 160, 224)
-                float d0[16], d1[16];
-                issue(d0, d1, nc, std::integral_constant<int, 1>{});
+                float d[16];
+                issue(d, nc);
                 tc::wgmma_wait<0>();
-                tc::fence_acc(d0);
-                slice_epilogue<NP>(d0, nc, q, b1s, w2s, p0, p1);
+                tc::fence_acc(d);
+                slice_epilogue<NP>(d, nc, q, b1s, w2s, p0, p1);
             }
             write_rows<NP>(a, p, tile, warp, g, q, p0, p1);
         }

@@ -21,14 +21,16 @@ struct FwdTcArgs {
 // apart, and with 128-byte rows their 16-byte loads would fall into one bank group
 __host__ __device__ constexpr int w2s_stride(int np) { return np > 4 ? np + 4 : np; }
 
-// Epilogue of one 32-unit slice: bias, ReLU, second layer on this thread's 2 rows x 8 units of the
-// accumulator, added into the partial sums p0 / p1 of rows 16 warp + g and + 8
-template <int NP>
-__device__ __forceinline__ void slice_epilogue(const float (&d)[16], int nc, int q, const float* b1s, const float* w2s,
+// Epilogue of the 32-unit slices nc, nc + 1, ... held in one accumulator (16 registers per slice: an
+// m64n32 accumulator, or the halves of an m64n64 one), slice by slice: bias, ReLU, second layer on this
+// thread's 2 rows x 8 units of the slice, added into the partial sums p0 / p1 of rows 16 warp + g and + 8
+template <int NP, int ND>
+__device__ __forceinline__ void slice_epilogue(const float (&d)[ND], int nc, int q, const float* b1s, const float* w2s,
                                                float (&p0)[NP], float (&p1)[NP]) {
     constexpr int NPS = w2s_stride(NP);
+    static_assert(ND % 16 == 0, "whole 32-unit slices");
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < ND / 4; ++i) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             const int j = nc * 32 + 8 * i + 2 * q + e;

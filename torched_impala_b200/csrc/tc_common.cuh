@@ -50,9 +50,10 @@ __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 // the accumulator registers are not touched by the compiler across an in-flight wgmma
-__device__ __forceinline__ void fence_acc(float (&d)[16]) {
+template <int N>
+__device__ __forceinline__ void fence_acc(float (&d)[N]) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 // the same for an A fragment held in registers: defined before the warpgroup fence, untouched after
 __device__ __forceinline__ void fence_frag(uint32_t (&a)[4]) {
@@ -90,8 +91,33 @@ __device__ __forceinline__ void wgmma_n32_rs(float (&d)[16], const uint32_t (&a)
         : IMPALA_WG_D16_OPS(d)
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate ? 1 : 0));
 }
+
+// m64n64k8: 32 accumulators, columns 8 (r >> 2) + 2 q + (r & 1) as above, so d[0, 16) are the
+// accumulators of an m64n32 MMA on B rows [0, 32) and d[16, 32) those of one on B rows [32, 64)
+#define IMPALA_WG_D32                                                                                   \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "  \
+    "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define IMPALA_WG_D32_OPS(d)                                                                            \
+    IMPALA_WG_D16_OPS(d), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]),  \
+        "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]),       \
+        "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+
+// D[64, 64] (+)= A[64, 8] * B[64, 8]^T, A from registers (warpgroup-collective)
+__device__ __forceinline__ void wgmma_n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc,
+                                             bool accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " IMPALA_WG_D32 ", {%32, %33, %34, %35}, %36, p, 1, 1;\n\t"
+        "}\n"
+        : IMPALA_WG_D32_OPS(d)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate ? 1 : 0));
+}
 #undef IMPALA_WG_D16
 #undef IMPALA_WG_D16_OPS
+#undef IMPALA_WG_D32
+#undef IMPALA_WG_D32_OPS
 
 // ------------------------------------------------------------------ 3xTF32 operand split
 // hi = round-to-nearest tf32 of x (what the tensor core will see exactly), lo = x - hi (exact in
