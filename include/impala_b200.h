@@ -16,7 +16,7 @@
  *     <0 = IMPALA_ERR_* (argument / unsupported-shape errors).  No exceptions.
  *
  * Batch layout in HBM (time-major, dense, zero padded; `lens[b]` valid steps):
- *   obs (T+1,B,O) f32 | beh_logits (T,B,A) f32 | actions (T,B) i32 |
+ *   obs (T+1,B,O) f32 (or u8, impala_batch_layout_obs) | beh_logits (T,B,A) f32 | actions (T,B) i32 |
  *   rewards (T,B) f32 | done (T,B) u8 | lens (B) i32
  * Parameter block of one MLP (Linear(O,H) -> ReLU -> Linear(H,N2)), f32, every
  * tensor starting on a 32-float boundary:  W1 (H,O) | b1 (H) | W2 (N2,H) | b2 (N2)
@@ -63,6 +63,16 @@ int impala_param_layout(int O, int H, int N2, int64_t offsets[4], int64_t* total
  * Replaces the five torch.stack calls at learner.py:104-109,117. */
 int impala_batch_layout(int T, int B, int O, int A, int64_t offsets[6], int64_t* total_bytes);
 
+/* Observation element types of a batch slab.  IMPALA_OBS_U8: byte observations (Atari RAM, MinAtar
+ * planes), values 0..255 entering the network as they are - a quarter of the slab bytes of float32. */
+#define IMPALA_OBS_F32 0
+#define IMPALA_OBS_U8 1
+
+/* impala_batch_layout with the obs tensor of type obs_dtype ((T+1)*B*O bytes for IMPALA_OBS_U8);
+ * every other tensor as above.  impala_batch_layout is its IMPALA_OBS_F32 case.  An unknown obs_dtype
+ * returns IMPALA_ERR_BAD_ARG. */
+int impala_batch_layout_obs(int T, int B, int O, int A, int obs_dtype, int64_t offsets[6], int64_t* total_bytes);
+
 /* Host slab -> device slab, async on `stream` (host memory should be pinned). */
 int impala_ingest(void* dev_slab, const void* host_slab, int64_t bytes, void* stream);
 
@@ -72,6 +82,14 @@ int impala_ingest(void* dev_slab, const void* host_slab, int64_t bytes, void* st
  * pulls its own shard of the actors' shared-memory slab over its own PCIe link. */
 int impala_ingest_shard(void* dev_slab, const void* host_slab, int T, int B, int O, int A, int b0,
                         int B_local, void* stream);
+/* The same for slabs laid out by impala_batch_layout_obs(..., obs_dtype) (obs rows of O bytes for
+ * IMPALA_OBS_U8); impala_ingest_shard is its IMPALA_OBS_F32 case. */
+int impala_ingest_shard_obs(void* dev_slab, const void* host_slab, int T, int B, int O, int A, int obs_dtype,
+                            int b0, int B_local, void* stream);
+
+/* out[i] = (float)x[i] for i < n: exact widening of byte observations, for the MLP shapes that read
+ * float32 rows only (O <= 128). */
+int impala_obs_u8_to_f32(const uint8_t* x, float* out, int64_t n, void* stream);
 
 /* out[m, :] = relu(x[m, :] W1^T + b1) W2^T + b2 for m < M.
  * Replaces MlpPolicy.forward / MlpValueFn.forward in eval mode
@@ -107,6 +125,17 @@ int64_t impala_mlp_backward_workspace(int M, int O, int H, int N2);
 int impala_mlp_backward(const float* x, const float* params, const float* dout, double* grad,
                         void* workspace, int64_t workspace_bytes, int M, int O, int H, int N2,
                         void* stream);
+
+/* impala_mlp_forward / impala_mlp_backward on byte observations (x row-major (M,O) uint8, 4-byte
+ * aligned; values 0..255 enter the network unscaled).  Results are identical to the float entry points
+ * on the same values converted to float32; the workspace is sized by impala_mlp_backward_workspace.
+ * Shapes: 128 < O <= 1024 under the limits of impala_mlp_forward (K-streamed tensor-core kernels that
+ * read the bytes directly).  O <= 128 returns IMPALA_ERR_UNSUPPORTED_SHAPE: callers widen those rows
+ * once with impala_obs_u8_to_f32 and call the float entry points. */
+int impala_mlp_forward_u8(const uint8_t* x, const float* params, float* out, int M, int O, int H, int N2,
+                          void* stream);
+int impala_mlp_backward_u8(const uint8_t* x, const float* params, const float* dout, double* grad,
+                           void* workspace, int64_t workspace_bytes, int M, int O, int H, int N2, void* stream);
 
 /* The MLP part of the single loss.backward() at learner.py:175 for both networks in one launch:
  * same results as impala_mlp_backward(policy; dout = dlogits) followed by

@@ -1,9 +1,14 @@
 """Device-resident learner step time for any BASELINE config (c2..c5) or the Atari-RAM / MinAtar shapes: CUDA events,
 L2 flushed.  --compare-tc also times the FP32 FFMA MLP path (IMPALA_MLP_TC=0) in the same process,
-alternating step by step with the default path, so both numbers see the same clocks and neighbours."""
+alternating step by step with the default path, so both numbers see the same clocks and neighbours.
+--compare-obs alternates a float32-slab engine and a uint8-slab engine (byte observations 0..255) the same way
+and reports, for both, the device-resident step time and the pinned-slab end-to-end step time (the DMA of
+slab i+1 runs under step i; a step's window also waits for that DMA), with the GPU name, power limit and
+maximum SM clock read in the same run."""
 import argparse
 import os
 import statistics
+import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -30,18 +35,29 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--config", default="c5")
 ap.add_argument("--steps", type=int, default=30)
 ap.add_argument("--compare-tc", action="store_true", help="alternate with IMPALA_MLP_TC=0 and report both")
+ap.add_argument("--compare-obs", action="store_true", help="alternate float32 and uint8 observation slabs")
 a = ap.parse_args()
 w = CFG[a.config]
 hp = default_hparams(batch_size=w["B"], max_timesteps=w["T"])
 arms = {"default": os.environ.get("IMPALA_MLP_TC", "1")}
+obs_dt = {"default": "float32"}
 if a.compare_tc:
     arms = {"tc": "1", "fp32 (IMPALA_MLP_TC=0)": "0"}
+if a.compare_obs:
+    arms = {"obs float32": arms["default"], "obs uint8": arms["default"]}
+    obs_dt = {"obs float32": "float32", "obs uint8": "uint8"}
 engines = {}
 for name, tc in arms.items():
     os.environ["IMPALA_MLP_TC"] = tc  # read by the C library at every launch (and at graph capture)
-    eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp)
+    dt = obs_dt.get(name, "float32")
+    eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt)
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
-    eng.load_device_batch(synth.make_batch(1, w["T"], w["B"], w["O"], w["A"]))
+    batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if a.compare_obs else "normal")
+    if dt == "float32":
+        batch["obs"] = batch["obs"].astype("float32")
+    eng.load_device_batch(batch)
+    if a.compare_obs:
+        eng.load_device_batch(batch, 1)
     engines[name] = eng
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 ts = {name: [] for name in arms}
@@ -57,8 +73,30 @@ for i in range(a.steps + 5):
             e1.synchronize()
             if i >= 5:
                 ts[name].append(e0.elapsed_time(e1) * 1e3)
+te = {name: [] for name in arms}
+if a.compare_obs:  # pinned-slab end to end: ingest(slab i+1) on the copy stream under step(slab i)
+    for i in range(a.steps + 5):
+        for name, eng in engines.items():
+            with torch.cuda.stream(eng.stream):
+                flush.zero_()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(eng.stream)
+                eng.copy_stream.wait_event(e0)
+                eng.ingest((i + 1) % 2)
+                eng.step(i % 2)
+                eng.stream.wait_event(eng.slab_ready[(i + 1) % 2])
+                e1.record(eng.stream)
+                e1.synchronize()
+                if i >= 5:
+                    te[name].append(e0.elapsed_time(e1) * 1e3)
 dev = torch.cuda.get_device_name()
+if a.compare_obs:
+    q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
+                        "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"GPU (nvidia-smi): {q}")
 for name, eng in engines.items():
     med = statistics.median(ts[name])
-    print(f"{a.config} {w} [{name}] on {dev}: median {med:.1f} us/step ({1e6 / med:.0f} steps/s), "
+    e2e = f", pinned-slab end to end {statistics.median(te[name]):.1f} us/step, slab {eng.slab_bytes / 1e6:.1f} MB" \
+        if te[name] else ""
+    print(f"{a.config} {w} [{name}] on {dev}: median {med:.1f} us/step ({1e6 / med:.0f} steps/s){e2e}, "
           f"loss {eng.read_scalars()['total_loss']:.5f}")

@@ -5,7 +5,8 @@ backward through the C ABI with L2 flushed before each call; torch.profiler (CUD
 every kernel.  Each kernel is reported against the H100 SXM data-sheet peak that bounds it: 495 TFLOP/s dense
 TF32 for the tensor-core kernels (algorithmic = the fp32 FLOPs of the math, executed = what the tensor cores
 issue: x3 for 3xTF32, K padded to whole chunks, the backward's recompute); the float64 reduction of the
-partial rows is a memory / latency kernel.  Run on the GPU: there is no CPU path.
+partial rows is a memory / latency kernel.  --obs-dtype uint8 runs the byte form (impala_mlp_{forward,backward}_u8
+on 0..255 observations: 2 of the 3 products per GEMM remain).  Run on the GPU: there is no CPU path.
 """
 import argparse
 import collections
@@ -24,12 +25,20 @@ PEAK_TF32 = 495e12
 ap = argparse.ArgumentParser()
 ap.add_argument("--config", default="ram4", choices=sorted(CFG))
 ap.add_argument("--iters", type=int, default=20)
+ap.add_argument("--obs-dtype", default="float32", choices=["float32", "uint8"])
 a = ap.parse_args()
 w = CFG[a.config]
 T, B, O, A, H = w["T"], w["B"], w["O"], w["A"], w["H"]
 lib = _cabi.lib()
 rng = np.random.default_rng(0)
-obs = torch.from_numpy(rng.random(((T + 1) * B, O), dtype=np.float32)).cuda()
+U8 = a.obs_dtype == "uint8"
+if U8:
+    obs = torch.from_numpy(rng.integers(0, 256, ((T + 1) * B, O), dtype=np.uint8)).cuda()
+else:
+    obs = torch.from_numpy(rng.random(((T + 1) * B, O), dtype=np.float32)).cuda()
+fwd_fn = lib.impala_mlp_forward_u8 if U8 else lib.impala_mlp_forward
+bwd_fn = lib.impala_mlp_backward_u8 if U8 else lib.impala_mlp_backward
+SPLIT = 2 if U8 else 3  # products per GEMM: x_lo = 0 drops one for byte observations
 nets = []
 for M, N2 in ((T * B, A), ((T + 1) * B, 1)):
     params = ops.pack_params(synth.init_params(1, O, N2, H)["policy"])
@@ -47,10 +56,10 @@ flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 def run_once():
     for M, N2, params, out, dout, ws, grad in nets:
         flush.zero_()
-        _cabi.check(lib.impala_mlp_forward(ops._p(obs), ops._p(params), ops._p(out), M, O, H, N2, ops._st()), "fwd")
+        _cabi.check(fwd_fn(ops._p(obs), ops._p(params), ops._p(out), M, O, H, N2, ops._st()), "fwd")
         flush.zero_()
-        _cabi.check(lib.impala_mlp_backward(ops._p(obs), ops._p(params), ops._p(dout), ops._p(grad), ops._p(ws),
-                                            ws.numel(), M, O, H, N2, ops._st()), "bwd")
+        _cabi.check(bwd_fn(ops._p(obs), ops._p(params), ops._p(dout), ops._p(grad), ops._p(ws),
+                           ws.numel(), M, O, H, N2, ops._st()), "bwd")
 
 
 for _ in range(3):
@@ -71,7 +80,7 @@ def up(x, m):
 
 
 def is_vf(name):  # the one-output instantiation (value function)
-    return "<1>" in name or "ILi1E" in name
+    return re.search(r"<1[,>]", name) is not None or "ILi1E" in name
 
 
 def work(name):
@@ -81,23 +90,23 @@ def work(name):
         Mp = up(M, 64)
         if "fwd_obs" in name and is_vf(name) == (N2 == 1):
             alg += 2 * M * O * H + 2 * M * H * N2
-            exe += 3 * 2 * Mp * up(O, 32) * H
+            exe += SPLIT * 2 * Mp * up(O, 32) * H
         elif "pre_kernel" in name and is_vf(name) == (N2 == 1):
             alg += 4 * M * H * N2  # dh and dW2; the recompute is not algorithmic
-            exe += 3 * 2 * Mp * up(O, 32) * H
+            exe += SPLIT * 2 * Mp * up(O, 32) * H
         elif "dw1_kernel" in name:
             alg += 2 * M * O * H
-            exe += 3 * 2 * Mp * up(O, 64) * H
+            exe += SPLIT * 2 * Mp * up(O, 64) * H
     return alg, exe
 
 
 dev = torch.cuda.get_device_name()
-print(f"{a.config} {w} on {dev}, L2 flushed before each C-ABI call, {a.iters} iterations")
+print(f"{a.config} {w} obs {a.obs_dtype} on {dev}, L2 flushed before each C-ABI call, {a.iters} iterations")
 for name, ts in sorted(times.items()):
     n_launch = len(ts) / a.iters  # launches of this kernel per iteration (one per network where both use it)
     us = float(np.mean(ts)) * n_launch  # per iteration
     alg, exe = work(name)
-    short = re.search(r"(mlp_\w+|reduce_partials_kernel)(<\d+>)?", name).group(0)
+    short = re.search(r"(mlp_\w+|reduce_partials_kernel)(<[^>]*>)?", name).group(0)
     if exe:
         print(f"  {short:40s} {us:9.1f} us/step  algorithmic {alg / us / 1e6:6.1f} TFLOP/s  executed {exe / us / 1e6:6.1f}"
               f" TFLOP/s = {exe / us / 1e6 / (PEAK_TF32 / 1e12):.2f} of the TF32 peak (bound: tensor)")

@@ -15,6 +15,16 @@ MODE_REFERENCE = 0
 MODE_PAPER = 1
 MODES = {"reference": MODE_REFERENCE, "paper": MODE_PAPER}
 
+OBS_F32 = 0
+OBS_U8 = 1
+OBS_DTYPES = {"float32": OBS_F32, "uint8": OBS_U8}  # batch-slab observation types (impala_batch_layout_obs)
+
+
+def obs_dtype_code(obs_dtype: str) -> int:
+    if obs_dtype not in OBS_DTYPES:
+        raise ValueError(f"obs_dtype must be one of {sorted(OBS_DTYPES)}, got {obs_dtype!r}")
+    return OBS_DTYPES[obs_dtype]
+
 _ERRORS = {-1: "IMPALA_ERR_BAD_ARG", -2: "IMPALA_ERR_UNSUPPORTED_SHAPE",
            -3: "IMPALA_ERR_WORKSPACE_TOO_SMALL"}
 
@@ -29,9 +39,14 @@ SIGNATURES = {
     "impala_compiled_sm": (_i, []),
     "impala_param_layout": (_i, [_i, _i, _i, C.POINTER(_i64), C.POINTER(_i64)]),
     "impala_batch_layout": (_i, [_i, _i, _i, _i, C.POINTER(_i64), C.POINTER(_i64)]),
+    "impala_batch_layout_obs": (_i, [_i, _i, _i, _i, _i, C.POINTER(_i64), C.POINTER(_i64)]),
     "impala_ingest": (_i, [_p, _p, _i64, _p]),
     "impala_ingest_shard": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _p]),
+    "impala_ingest_shard_obs": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _i, _p]),
+    "impala_obs_u8_to_f32": (_i, [_p, _p, _i64, _p]),
     "impala_mlp_forward": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
+    "impala_mlp_forward_u8": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
+    "impala_mlp_backward_u8": (_i, [_p, _p, _p, _p, _p, _i64, _i, _i, _i, _i, _p]),
     "impala_launch_count": (C.c_longlong, []),
     "impala_mlp_forward_pair": (_i, [_p] * 5 + [_i] * 6 + [_p]),
     "impala_mlp_backward_workspace": (_i64, [_i, _i, _i, _i]),
@@ -94,8 +109,9 @@ def param_layout(O: int, H: int, N2: int):
     return list(offs), total.value
 
 
-def batch_layout(T: int, B: int, O: int, A: int):
+def batch_layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32"):
     offs = (_i64 * 6)()
     total = _i64()
-    check(lib().impala_batch_layout(T, B, O, A, offs, C.byref(total)), "impala_batch_layout")
+    check(lib().impala_batch_layout_obs(T, B, O, A, obs_dtype_code(obs_dtype), offs, C.byref(total)),
+          "impala_batch_layout_obs")
     return list(offs), total.value

@@ -15,6 +15,7 @@
 //
 // This file: host-side configuration, occupancy cache, the partial reduction and the
 // C-ABI entry points.  Kernel templates: mlp_kernels.cuh; instantiations: mlp_inst.cu.
+#include <algorithm>
 #include <cstdlib>
 #include <map>
 #include <mutex>
@@ -222,27 +223,33 @@ extern "C" int64_t impala_mlp_backward_workspace(int M, int O, int H, int N2) {
     return kWsHeader + tiles * impala_make_layout(O, H, N2).total * (int64_t)sizeof(float);
 }
 
+// Wide observations (O > 128, float or byte rows): DP^T and two sets of partial rows in the workspace,
+// each summed in float64.
+template <typename XT>
+static int backward_obs(const XT* x, const float* params, const float* dout, double* grad, void* workspace,
+                        int64_t workspace_bytes, int M, int O, int H, int N2, cudaStream_t st) {
+    ObsBwdLayout L;
+    if (!impala_mlp_obs_bwd_layout(M, O, H, N2, &L)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    if (workspace_bytes < kWsHeader + L.bytes) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
+    char* ws = static_cast<char*>(workspace) + kWsHeader;
+    const int rc = impala_mlp_bwd_obs(x, params, dout, ws, L, M, O, H, N2, st);
+    if (rc != IMPALA_OK) return rc;
+    const MlpLayout lay = impala_make_layout(O, H, N2);
+    const int64_t nr = lay.total - lay.ob1;
+    reduce_partials_kernel<<<(unsigned)((nr + 31) / 32), kRedWarps * 32, 0, st>>>(
+        reinterpret_cast<const float*>(ws + L.rest_off), grad + lay.ob1, L.r1, nr);
+    if (const int e = impala_launch_status(); e != IMPALA_OK) return e;
+    reduce_partials_kernel<<<(unsigned)((lay.ob1 + 31) / 32), kRedWarps * 32, 0, st>>>(
+        reinterpret_cast<const float*>(ws + L.w1_off), grad, L.p2, lay.ob1);
+    return impala_launch_status();
+}
+
 extern "C" int impala_mlp_backward(const float* x, const float* params, const float* dout,
                                    double* grad, void* workspace, int64_t workspace_bytes, int M,
                                    int O, int H, int N2, void* stream) {
     if (!x || !params || !dout || !grad || !workspace) return IMPALA_ERR_BAD_ARG;
-    if (O > 128) {
-        // wide observations: DP^T and two sets of partial rows in the workspace, each summed in float64
-        ObsBwdLayout L;
-        if (!impala_mlp_obs_bwd_layout(M, O, H, N2, &L)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-        if (workspace_bytes < kWsHeader + L.bytes) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
-        char* ws = static_cast<char*>(workspace) + kWsHeader;
-        const int rc = impala_mlp_bwd_obs(x, params, dout, ws, L, M, O, H, N2, (cudaStream_t)stream);
-        if (rc != IMPALA_OK) return rc;
-        const MlpLayout lay = impala_make_layout(O, H, N2);
-        const int64_t nr = lay.total - lay.ob1;
-        reduce_partials_kernel<<<(unsigned)((nr + 31) / 32), kRedWarps * 32, 0, (cudaStream_t)stream>>>(
-            reinterpret_cast<const float*>(ws + L.rest_off), grad + lay.ob1, L.r1, nr);
-        if (const int e = impala_launch_status(); e != IMPALA_OK) return e;
-        reduce_partials_kernel<<<(unsigned)((lay.ob1 + 31) / 32), kRedWarps * 32, 0, (cudaStream_t)stream>>>(
-            reinterpret_cast<const float*>(ws + L.w1_off), grad, L.p2, lay.ob1);
-        return impala_launch_status();
-    }
+    if (O > 128)
+        return backward_obs(x, params, dout, grad, workspace, workspace_bytes, M, O, H, N2, (cudaStream_t)stream);
     MlpArgs a{};
     MlpConfig c{};
     size_t smem;
@@ -268,6 +275,56 @@ extern "C" int impala_mlp_backward(const float* x, const float* params, const fl
     const int64_t total = a.lay.total;
     reduce_partials_kernel<<<(unsigned)((total + 31) / 32), kRedWarps * 32, 0,
                              (cudaStream_t)stream>>>(a.ws, grad, grid, total);
+    return impala_launch_status();
+}
+
+// ---- byte observations: the K-streamed kernels read uint8 rows (O > 128); narrower shapes are refused,
+// their callers widen the rows once with impala_obs_u8_to_f32
+extern "C" int impala_mlp_forward_u8(const uint8_t* x, const float* params, float* out, int M, int O, int H, int N2,
+                                     void* stream) {
+    if (!x || !params || !out) return IMPALA_ERR_BAD_ARG;
+    if (O <= 128 || !impala_mlp_obs_shape_ok(M, O, H, N2)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    return impala_mlp_fwd_obs(x, params, out, M, O, H, N2, (cudaStream_t)stream);
+}
+
+extern "C" int impala_mlp_backward_u8(const uint8_t* x, const float* params, const float* dout, double* grad,
+                                      void* workspace, int64_t workspace_bytes, int M, int O, int H, int N2,
+                                      void* stream) {
+    if (!x || !params || !dout || !grad || !workspace) return IMPALA_ERR_BAD_ARG;
+    if (O <= 128) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    return backward_obs(x, params, dout, grad, workspace, workspace_bytes, M, O, H, N2, (cudaStream_t)stream);
+}
+
+// out[i] = x[i] (exact): 4 bytes -> one float4 per thread and iteration when both pointers allow it
+template <bool kVec>
+__global__ void __launch_bounds__(256) obs_u8_to_f32_kernel(const uint8_t* __restrict__ x, float* __restrict__ out,
+                                                            int64_t n) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x, t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t done = 0;
+    if constexpr (kVec) {
+        const int64_t n4 = n >> 2;
+        for (int64_t i = t; i < n4; i += stride) {
+            const uint32_t w = __ldg(reinterpret_cast<const unsigned int*>(x) + i);
+            reinterpret_cast<float4*>(out)[i] = make_float4((float)(w & 255u), (float)((w >> 8) & 255u),
+                                                            (float)((w >> 16) & 255u), (float)(w >> 24));
+        }
+        done = n4 << 2;
+    }
+    for (int64_t i = done + t; i < n; i += stride) out[i] = (float)x[i];
+}
+
+extern "C" int impala_obs_u8_to_f32(const uint8_t* x, float* out, int64_t n, void* stream) {
+    if (!x || !out || n < 0) return IMPALA_ERR_BAD_ARG;
+    if (n == 0) return IMPALA_OK;
+    int sms = 0;
+    if (const cudaError_t e = impala_sm_count(&sms); e != cudaSuccess) return (int)e;
+    const bool vec = ((reinterpret_cast<uintptr_t>(x) & 3) | (reinterpret_cast<uintptr_t>(out) & 15)) == 0;
+    const int64_t work = vec ? (n + 3) / 4 : n;
+    const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((work + 255) / 256, (int64_t)sms * 16));
+    if (vec)
+        obs_u8_to_f32_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(x, out, n);
+    else
+        obs_u8_to_f32_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, out, n);
     return impala_launch_status();
 }
 

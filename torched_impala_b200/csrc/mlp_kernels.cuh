@@ -74,6 +74,8 @@ int impala_mlp_bwd_tcx(const float* x, const float* params, const float* dout, f
 // K streamed; false under IMPALA_MLP_TC=0 / IMPALA_MLP_TCW=0 (there is no FP32 kernel for these widths).
 bool impala_mlp_obs_shape_ok(int M, int O, int H, int N2);
 int impala_mlp_fwd_obs(const float* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st);
+// The same with byte observations (values 0..255 enter the network as they are); x 4-byte aligned.
+int impala_mlp_fwd_obs(const uint8_t* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st);
 // Backward workspace past the control header: byte offsets of DP^T and of the two sets of float32 partial
 // rows (r1 rows of layout entries [ob1, total), p2 rows of [0, ob1)) for reduce_partials_kernel.
 struct ObsBwdLayout {
@@ -83,6 +85,8 @@ struct ObsBwdLayout {
 bool impala_mlp_obs_bwd_layout(int M, int O, int H, int N2, ObsBwdLayout* L);
 int impala_mlp_bwd_obs(const float* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L, int M,
                        int O, int H, int N2, cudaStream_t st);
+int impala_mlp_bwd_obs(const uint8_t* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L,
+                       int M, int O, int H, int N2, cudaStream_t st);
 
 // One per padded observation width / direction, defined in mlp_inst.cu.
 #define IMPALA_DECL_DISPATCH(OPV)                                                             \

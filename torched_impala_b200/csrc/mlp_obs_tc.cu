@@ -28,6 +28,13 @@
 // workspace and per-CTA partial rows of db1 / dW2 / db2; backward 2 reads DP^T and writes per-CTA partial
 // rows of dW1.  Each set of partial rows is summed in float64 in fixed order by reduce_partials_kernel
 // (mlp.cu), so results are bitwise reproducible.  Every partial entry is written by every launch.
+//
+// Byte observations (uint8 x, Atari RAM / MinAtar planes).  Every kernel also exists with x as bytes
+// (trailing template parameter XT = uint8_t).  An integer in 0..255 is exact in tf32: its split has lo = 0,
+// so the MMAs with x_lo as an operand add nothing and are not issued (16 instead of 24 per chunk), x is
+// loaded 4 features per 32-bit word and the lo buffer of an x stage is never filled.  The remaining MMAs
+// keep their order and the first of a chunk takes over scale-d = 0, so each accumulator sees the same
+// non-zero additions in the same order as the float kernels on the same values converted to float.
 #include <algorithm>
 #include <cstdlib>
 #include <map>
@@ -45,10 +52,34 @@ constexpr int kHBlk = 64;            // hidden units per CTA (A rows in the back
 constexpr int kFBlk = 64;            // features per CTA in backward 2
 
 // A K-contiguous matrix [rows][ld]; entries with row >= rows are zero.
+template <typename T>
 struct Mat {
-    const float* p;
+    const T* p;
     int64_t ld;
     int rows;
+};
+
+// Operand element types.  Raw = 4 consecutive entries as loaded (kept raw while the load is in flight);
+// kExact: every value is exact in tf32 (the split's lo is zero).
+template <typename T>
+struct Elem;
+template <>
+struct Elem<float> {
+    using Raw = float4;
+    static constexpr bool kExact = false;
+    __device__ static __forceinline__ Raw zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+    __device__ static __forceinline__ Raw load(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+    __device__ static __forceinline__ float4 widen(const Raw& r) { return r; }
+};
+template <>
+struct Elem<uint8_t> {
+    using Raw = uint32_t;
+    static constexpr bool kExact = true;
+    __device__ static __forceinline__ Raw zero() { return 0u; }
+    __device__ static __forceinline__ Raw load(const uint8_t* p) { return __ldg(reinterpret_cast<const unsigned int*>(p)); }
+    __device__ static __forceinline__ float4 widen(const Raw& r) {
+        return make_float4((float)(r & 255u), (float)((r >> 8) & 255u), (float)((r >> 16) & 255u), (float)(r >> 24));
+    }
 };
 
 // position of feature k (0..31) of a chunk inside the chunk's 32 K positions (see the header)
@@ -63,41 +94,48 @@ __device__ __forceinline__ float f4(const float4& v, int e) { return e == 0 ? v.
 // + (r & 1).  A entries with k >= ke are zero.  B: BT = false - Bm[b0 + n][k] (k >= ke zero); BT = true -
 // Bm[k][b0 + n] (transposed: rows of Bm are K; n >= ncols zero).  kb is a multiple of 32.  The caller
 // has a barrier between any earlier use of `stage` and this call; the call ends with one.
-template <bool BT>
-__device__ __forceinline__ void kstream(const Mat& A, int a0, const Mat& Bm, int b0, int ncols, int kb, int ke,
-                                        uint8_t* stage, float (&run)[2][16]) {
+// TA / TB: element types of A and B.  An exact operand (bytes) has no lo part: the MMAs that would take
+// it are not issued, and for B its lo buffer is left unwritten.
+template <bool BT, typename TA, typename TB>
+__device__ __forceinline__ void kstream(const Mat<TA>& A, int a0, const Mat<TB>& Bm, int b0, int ncols, int kb,
+                                        int ke, uint8_t* stage, float (&run)[2][16]) {
+    using EA = Elem<TA>;
+    using EB = Elem<TB>;
+    constexpr bool kLoA = !EA::kExact, kLoB = !EB::kExact;
+    static_assert(kLoA || kLoB, "at most one operand is exact");
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
-    float4 ra[4], rb[4];              // raw A (row half h, 16-feature group j: ra[2 h + j]) and B of the next chunk
-    uint32_t xh[4][4], xl[4][4];      // A fragments of the current chunk: [K step][slot]
+    typename EA::Raw ra[4];           // raw A (row half h, 16-feature group j: ra[2 h + j]) of the next chunk
+    typename EB::Raw rb[4];           // raw B of the next chunk
+    uint32_t xh[4][4], xl[4][4];      // A fragments of the current chunk: [K step][slot] (xl unused if A is exact)
     auto load = [&](int kc) {
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
                 const int row = a0 + 16 * warp + g + 8 * h, k = kc + 16 * j + 4 * q;
-                ra[2 * h + j] = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (row < A.rows && k < ke) ra[2 * h + j] = __ldg(reinterpret_cast<const float4*>(A.p + row * A.ld + k));
+                ra[2 * h + j] = EA::zero();
+                if (row < A.rows && k < ke) ra[2 * h + j] = EA::load(A.p + row * A.ld + k);
             }
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
-            rb[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+            rb[t] = EB::zero();
             if constexpr (!BT) {
-                // thread -> (row n, 16-byte chunk u): a warp stores 4 rows x 8 chunks, conflict-free
+                // thread -> (row n, 4-feature chunk u): a warp stores 4 rows x 8 chunks, conflict-free
                 const int idx = tid + kT * t, n = idx >> 3, k = kc + 4 * (idx & 7);
-                if (b0 + n < Bm.rows && k < ke) rb[t] = __ldg(reinterpret_cast<const float4*>(Bm.p + (b0 + n) * Bm.ld + k));
+                if (b0 + n < Bm.rows && k < ke) rb[t] = EB::load(Bm.p + (b0 + n) * Bm.ld + k);
             } else {
                 // lane -> K position (batch row), warp -> 4 of the 64 columns: the transposed stores of a
                 // warp hit 32 different banks
                 const int col = b0 + 4 * (warp + 4 * t), k = kc + lane;
-                if (k < Bm.rows && col < ncols) rb[t] = __ldg(reinterpret_cast<const float4*>(Bm.p + k * Bm.ld + col));
+                if (k < Bm.rows && col < ncols) rb[t] = EB::load(Bm.p + k * Bm.ld + col);
             }
         }
     };
     auto stage_b = [&](uint8_t* hi, uint8_t* lo) {
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
-            float4 vh, vl;
-            tc::split4(rb[t], vh, vl);
+            float4 vh = EB::widen(rb[t]), vl;
+            if constexpr (kLoB) tc::split4(EB::widen(rb[t]), vh, vl);
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 uint32_t off;
@@ -108,7 +146,7 @@ __device__ __forceinline__ void kstream(const Mat& A, int a0, const Mat& Bm, int
                     off = stage_off(4 * (warp + 4 * t) + e, kpos(lane));
                 }
                 *reinterpret_cast<float*>(hi + off) = f4(vh, e);
-                *reinterpret_cast<float*>(lo + off) = f4(vl, e);
+                if constexpr (kLoB) *reinterpret_cast<float*>(lo + off) = f4(vl, e);
             }
         }
     };
@@ -116,16 +154,21 @@ __device__ __forceinline__ void kstream(const Mat& A, int a0, const Mat& Bm, int
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int j = 0; j < 2; ++j)
+            for (int j = 0; j < 2; ++j) {
+                const float4 v = EA::widen(ra[2 * h + j]);
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                    float hi, lo;
-                    tc::split_tf32(f4(ra[2 * h + j], e), hi, lo);
+                    float hi = f4(v, e), lo;
+                    if constexpr (kLoA) tc::split_tf32(f4(v, e), hi, lo);
                     xh[2 * j + (e >> 1)][h + 2 * (e & 1)] = __float_as_uint(hi);
-                    xl[2 * j + (e >> 1)][h + 2 * (e & 1)] = __float_as_uint(lo);
+                    if constexpr (kLoA) xl[2 * j + (e >> 1)][h + 2 * (e & 1)] = __float_as_uint(lo);
                 }
+            }
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) tc::fence_frag(xh[kk]), tc::fence_frag(xl[kk]);
+        for (int kk = 0; kk < 4; ++kk) {
+            tc::fence_frag(xh[kk]);
+            if constexpr (kLoA) tc::fence_frag(xl[kk]);
+        }
     };
 
     const int nch = (ke - kb + 31) >> 5;
@@ -147,10 +190,14 @@ __device__ __forceinline__ void kstream(const Mat& A, int a0, const Mat& Bm, int
         tc::wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
-            tc::wgmma_n32_rs(d0, xl[kk], dh + ((kk * 32) >> 4), kk > 0);
-            tc::wgmma_n32_rs(d1, xl[kk], dh + ((32 * 128 + kk * 32) >> 4), kk > 0);
-            tc::wgmma_n32_rs(d0, xh[kk], dl + ((kk * 32) >> 4), true);
-            tc::wgmma_n32_rs(d1, xh[kk], dl + ((32 * 128 + kk * 32) >> 4), true);
+            if constexpr (kLoA) {
+                tc::wgmma_n32_rs(d0, xl[kk], dh + ((kk * 32) >> 4), kk > 0);
+                tc::wgmma_n32_rs(d1, xl[kk], dh + ((32 * 128 + kk * 32) >> 4), kk > 0);
+            }
+            if constexpr (kLoB) {  // the first MMA of the chunk when A is exact
+                tc::wgmma_n32_rs(d0, xh[kk], dl + ((kk * 32) >> 4), kLoA || kk > 0);
+                tc::wgmma_n32_rs(d1, xh[kk], dl + ((32 * 128 + kk * 32) >> 4), kLoA || kk > 0);
+            }
         }
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
@@ -181,15 +228,17 @@ __device__ __forceinline__ uint8_t* aligned_smem() {
 // ------------------------------------------------------------------ forward
 // CTA = one 64-row tile; the hidden layer is walked in 64-unit passes, out[row] = ((b2 + z_0) + z_1) + ...
 // written by the thread that wrote the previous pass (write_rows).
-template <int NP>
-__global__ void __launch_bounds__(kT) mlp_fwd_obs_kernel(const __grid_constant__ FwdTcArgs a) {
+// x: the observation rows (a.x is not read; it is the same address for XT = float).
+template <int NP, typename XT>
+__global__ void __launch_bounds__(kT) mlp_fwd_obs_kernel(const __grid_constant__ FwdTcArgs a, const XT* __restrict__ x) {
     constexpr int NPS = w2s_stride(NP);
     uint8_t* stage = aligned_smem();
     float* b1s = reinterpret_cast<float*>(stage + kStageBytes);  // [64]
     float* w2s = b1s + kHBlk;                                     // [64][NPS]
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
     const int tile = blockIdx.x;
-    const Mat X{a.x, a.O, a.M}, W1{a.params + a.lay.oW1, a.O, a.H};
+    const Mat<XT> X{x, a.O, a.M};
+    const Mat<float> W1{a.params + a.lay.oW1, a.O, a.H};
     for (int p = 0; p < a.H / kHBlk; ++p) {
         __syncthreads();  // the previous pass's epilogue is done with b1s / w2s
         for (int j = tid; j < kHBlk; j += kT) b1s[j] = __ldg(a.params + a.lay.ob1 + p * kHBlk + j);
@@ -210,7 +259,7 @@ __global__ void __launch_bounds__(kT) mlp_fwd_obs_kernel(const __grid_constant__
 
 // ------------------------------------------------------------------ backward
 struct ObsBwdArgs {
-    const float* x;
+    const void* x;  // float or uint8_t rows (the kernels' XT)
     const float* params;
     const float* dout;
     float* dpt;     // DP^T [H][mp]
@@ -225,7 +274,7 @@ struct ObsBwdArgs {
 // block, 16 batch rows): h = relu(PRE + b1), dh = W2^T dz, dW2 += dz h, DP = PRE + b1 > 0 ? dh : 0,
 // db1 += DP; DP goes to DP^T.  dW2 / db1 of the block (and db2 and the pads: blk 0) go to partial row r.
 // NP = 32: dW2 in chunks of 8 outputs that the quad sums and lane q keeps (as bwd_tc_body).
-template <int NP>
+template <int NP, typename XT>
 __global__ void __launch_bounds__(kT) mlp_bwd_obs_pre_kernel(const __grid_constant__ ObsBwdArgs a) {
     constexpr bool L2S = NP > 4;
     constexpr int NPS = w2s_stride(NP);
@@ -259,7 +308,8 @@ __global__ void __launch_bounds__(kT) mlp_bwd_obs_pre_kernel(const __grid_consta
 #pragma unroll
     for (int n = 0; n < NG; ++n) gw0[n] = gw1[n] = 0.f;
 
-    const Mat W1{a.params + a.lay.oW1, a.O, H}, X{a.x, a.O, a.M};
+    const Mat<float> W1{a.params + a.lay.oW1, a.O, H};
+    const Mat<XT> X{static_cast<const XT*>(a.x), a.O, a.M};
     for (int tile = r; tile < a.num_tiles; tile += a.r1) {
         __syncthreads();  // the previous tile's epilogue is done with dzs
         for (int idx = tid; idx < kTileM * NP; idx += kT) {
@@ -395,6 +445,7 @@ __global__ void __launch_bounds__(kT) mlp_bwd_obs_pre_kernel(const __grid_consta
 // Backward 2: CTA (r, fb, hb) forms dW1 of hidden block hb x feature block fb over the batch-row chunks
 // [r nc / p2, (r + 1) nc / p2) (nc = mp / 32) and writes it (and, CTA (r, 0, 0), the W1 pads) to
 // partial row r.
+template <typename XT>
 __global__ void __launch_bounds__(kT) mlp_bwd_obs_dw1_kernel(const __grid_constant__ ObsBwdArgs a) {
     uint8_t* stage = aligned_smem();
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
@@ -404,7 +455,8 @@ __global__ void __launch_bounds__(kT) mlp_bwd_obs_dw1_kernel(const __grid_consta
         for (int64_t e = (int64_t)a.H * O + tid; e < a.lay.ob1; e += kT) wsb[e] = 0.f;
     const int nc = a.mp / 32;
     const int c0 = (int)((int64_t)r * nc / a.p2), c1 = (int)((int64_t)(r + 1) * nc / a.p2);
-    const Mat DPt{a.dpt, a.mp, a.H}, X{a.x, O, a.M};
+    const Mat<float> DPt{a.dpt, a.mp, a.H};
+    const Mat<XT> X{static_cast<const XT*>(a.x), O, a.M};
     float run[2][16] = {};
     kstream<true>(DPt, hb * kHBlk, X, fb * kFBlk, O, 32 * c0, 32 * c1, stage, run);
     const int j0 = hb * kHBlk + 16 * warp + g, j1 = j0 + 8;
@@ -449,6 +501,53 @@ int launch(void (*kernel)(KArgs...), dim3 grid, size_t smem, cudaStream_t st, Ar
 
 int np_of(int N2) { return N2 == 1 ? 1 : (N2 <= 4 ? 4 : 32); }
 
+// x alignment the loads need: 16 bytes for float rows, 4 for byte rows (O % 4 == 0 keeps every row aligned)
+template <typename XT>
+bool x_aligned(const XT* x) {
+    return (reinterpret_cast<uintptr_t>(x) & (sizeof(XT) == 4 ? 15 : 3)) == 0;
+}
+
+template <typename XT>
+int fwd_obs(const XT* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st) {
+    if (!impala_mlp_obs_shape_ok(M, O, H, N2) || !x_aligned(x)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    FwdTcArgs a{};
+    a.x = sizeof(XT) == 4 ? reinterpret_cast<const float*>(x) : nullptr, a.params = params, a.out = out;
+    a.M = M, a.O = O, a.H = H, a.N2 = N2;
+    a.num_tiles = (M + kTileM - 1) / kTileM;
+    a.hb = kHBlk;
+    a.lay = impala_make_layout(O, H, N2);
+    const dim3 grid(a.num_tiles);
+    switch (np_of(N2)) {
+        case 1: return launch(mlp_fwd_obs_kernel<1, XT>, grid, kFwdSmem(1), st, a, x);
+        case 4: return launch(mlp_fwd_obs_kernel<4, XT>, grid, kFwdSmem(4), st, a, x);
+        default: return launch(mlp_fwd_obs_kernel<32, XT>, grid, kFwdSmem(32), st, a, x);
+    }
+}
+
+template <typename XT>
+int bwd_obs(const XT* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L, int M, int O,
+            int H, int N2, cudaStream_t st) {
+    if (!x_aligned(x)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    ObsBwdArgs a{};
+    a.x = x, a.params = params, a.dout = dout;
+    a.dpt = reinterpret_cast<float*>(static_cast<char*>(ws) + L.dpt_off);
+    a.ws_r = reinterpret_cast<float*>(static_cast<char*>(ws) + L.rest_off);
+    a.ws_w = reinterpret_cast<float*>(static_cast<char*>(ws) + L.w1_off);
+    a.M = M, a.O = O, a.H = H, a.N2 = N2;
+    a.num_tiles = (M + kTileM - 1) / kTileM;
+    a.mp = L.mp, a.r1 = L.r1, a.p2 = L.p2;
+    a.lay = impala_make_layout(O, H, N2);
+    const dim3 g1(L.r1, H / kHBlk);
+    int rc;
+    switch (np_of(N2)) {
+        case 1: rc = launch(mlp_bwd_obs_pre_kernel<1, XT>, g1, kPreSmem(1), st, a); break;
+        case 4: rc = launch(mlp_bwd_obs_pre_kernel<4, XT>, g1, kPreSmem(4), st, a); break;
+        default: rc = launch(mlp_bwd_obs_pre_kernel<32, XT>, g1, kPreSmem(32), st, a); break;
+    }
+    if (rc != IMPALA_OK) return rc;
+    return launch(mlp_bwd_obs_dw1_kernel<XT>, dim3(L.p2, (O + kFBlk - 1) / kFBlk, H / kHBlk), kDw1Smem, st, a);
+}
+
 }  // namespace
 
 bool impala_mlp_obs_shape_ok(int M, int O, int H, int N2) {
@@ -458,20 +557,10 @@ bool impala_mlp_obs_shape_ok(int M, int O, int H, int N2) {
 }
 
 int impala_mlp_fwd_obs(const float* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st) {
-    if (!impala_mlp_obs_shape_ok(M, O, H, N2) || (reinterpret_cast<uintptr_t>(x) & 15) != 0)
-        return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    FwdTcArgs a{};
-    a.x = x, a.params = params, a.out = out;
-    a.M = M, a.O = O, a.H = H, a.N2 = N2;
-    a.num_tiles = (M + kTileM - 1) / kTileM;
-    a.hb = kHBlk;
-    a.lay = impala_make_layout(O, H, N2);
-    const dim3 grid(a.num_tiles);
-    switch (np_of(N2)) {
-        case 1: return launch(mlp_fwd_obs_kernel<1>, grid, kFwdSmem(1), st, a);
-        case 4: return launch(mlp_fwd_obs_kernel<4>, grid, kFwdSmem(4), st, a);
-        default: return launch(mlp_fwd_obs_kernel<32>, grid, kFwdSmem(32), st, a);
-    }
+    return fwd_obs(x, params, out, M, O, H, N2, st);
+}
+int impala_mlp_fwd_obs(const uint8_t* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st) {
+    return fwd_obs(x, params, out, M, O, H, N2, st);
 }
 
 // Workspace past the control header: DP^T [H][mp] | r1 partial rows of [ob1, total) | p2 partial rows of
@@ -495,23 +584,9 @@ bool impala_mlp_obs_bwd_layout(int M, int O, int H, int N2, ObsBwdLayout* L) {
 
 int impala_mlp_bwd_obs(const float* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L, int M,
                        int O, int H, int N2, cudaStream_t st) {
-    if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    ObsBwdArgs a{};
-    a.x = x, a.params = params, a.dout = dout;
-    a.dpt = reinterpret_cast<float*>(static_cast<char*>(ws) + L.dpt_off);
-    a.ws_r = reinterpret_cast<float*>(static_cast<char*>(ws) + L.rest_off);
-    a.ws_w = reinterpret_cast<float*>(static_cast<char*>(ws) + L.w1_off);
-    a.M = M, a.O = O, a.H = H, a.N2 = N2;
-    a.num_tiles = (M + kTileM - 1) / kTileM;
-    a.mp = L.mp, a.r1 = L.r1, a.p2 = L.p2;
-    a.lay = impala_make_layout(O, H, N2);
-    const dim3 g1(L.r1, H / kHBlk);
-    int rc;
-    switch (np_of(N2)) {
-        case 1: rc = launch(mlp_bwd_obs_pre_kernel<1>, g1, kPreSmem(1), st, a); break;
-        case 4: rc = launch(mlp_bwd_obs_pre_kernel<4>, g1, kPreSmem(4), st, a); break;
-        default: rc = launch(mlp_bwd_obs_pre_kernel<32>, g1, kPreSmem(32), st, a); break;
-    }
-    if (rc != IMPALA_OK) return rc;
-    return launch(mlp_bwd_obs_dw1_kernel, dim3(L.p2, (O + kFBlk - 1) / kFBlk, H / kHBlk), kDw1Smem, st, a);
+    return bwd_obs(x, params, dout, ws, L, M, O, H, N2, st);
+}
+int impala_mlp_bwd_obs(const uint8_t* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L,
+                       int M, int O, int H, int N2, cudaStream_t st) {
+    return bwd_obs(x, params, dout, ws, L, M, O, H, N2, st);
 }

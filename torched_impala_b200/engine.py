@@ -17,6 +17,11 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       order and applies the update.  IMPALA_ALLREDUCE=nccl: torch.distributed all-reduce between the
       backward and impala_clip_adam instead.
 
+obs_dtype="uint8" (byte observations): the slabs hold obs as uint8 (impala_batch_layout_obs).  For
+O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one after the other as the
+pair entry points do at those widths.  For O <= 128 impala_obs_u8_to_f32 widens the obs into a float32
+device buffer first (one more launch) and the pair entry points read that.
+
 With `use_graph=True` the whole launch sequence of a step is captured once per slab into ONE CUDA
 graph and replayed (two graphs around the collective in the NCCL scheme).
 Ingest is double buffered: two pinned host slabs, two device slabs and
@@ -60,10 +65,13 @@ class LearnerEngine:
     def __init__(self, T: int, B_local: int, O: int, A: int, H_pi: int, H_v: int, hp,
                  global_batch: int | None = None, device: str | torch.device = "cuda:0",
                  mode: str = "reference", process_group=None, use_graph: bool = True,
-                 slabs: int = 2):
+                 slabs: int = 2, obs_dtype: str = "float32"):
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
+        # "uint8": byte observations in the slabs (Atari RAM, MinAtar), entering the networks unscaled
+        self.obs_code = _cabi.obs_dtype_code(obs_dtype)
+        self.obs_dtype = obs_dtype
         self.dev = torch.device(device)
         torch.cuda.set_device(self.dev)
         self.T, self.B, self.O, self.A, self.H_pi, self.H_v = T, B_local, O, A, H_pi, H_v
@@ -96,7 +104,8 @@ class LearnerEngine:
         self.norms = torch.zeros(2, dtype=torch.float64, device=self.dev)
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts
-        self.slab_off, self.slab_bytes = _cabi.batch_layout(T, B_local, O, A)
+        self.slab_off, self.slab_bytes = _cabi.batch_layout(T, B_local, O, A, obs_dtype)
+        self.fields = ((("obs", np.uint8 if obs_dtype == "uint8" else np.float32),) + _BATCH_FIELDS[1:])
         self.n_slabs = slabs
         self.d_slabs = [torch.zeros(self.slab_bytes, dtype=torch.uint8, device=self.dev)
                         for _ in range(slabs)]
@@ -110,7 +119,7 @@ class LearnerEngine:
         for dslab, hslab in zip(self.d_slabs, self.h_slabs):
             arr = hslab.numpy()
             dv, hv = {}, {}
-            for (name, dt), off in zip(_BATCH_FIELDS, self.slab_off):
+            for (name, dt), off in zip(self.fields, self.slab_off):
                 n = int(np.prod(shapes[name])) * np.dtype(dt).itemsize
                 dv[name] = dslab[off:off + n].view(_TORCH_DT[dt]).view(shapes[name])
                 hv[name] = arr[off:off + n].view(dt).reshape(shapes[name])
@@ -133,6 +142,11 @@ class LearnerEngine:
         self.ws_vf_bytes = self._ws_bytes(self.M_vf, O, H_v, 1)
         self.ws_pi = torch.zeros(self.ws_pi_bytes, dtype=torch.uint8, device=self.dev)
         self.ws_vf = torch.zeros(self.ws_vf_bytes, dtype=torch.uint8, device=self.dev)
+        # byte observations: O > 128 runs the networks on the bytes (impala_mlp_{forward,backward}_u8); narrower
+        # observations are widened once per step into this float32 copy for the float kernels
+        self.obs_u8_native = obs_dtype == "uint8" and O > 128
+        self.obs_f32 = (torch.zeros((T + 1) * B_local * O, **f32) if obs_dtype == "uint8" and not self.obs_u8_native
+                        else None)
         self.ws_vt_bytes = int(self.lib.impala_vtrace_loss_workspace(T, B_local, A))
         self.ws_vt = torch.zeros(self.ws_vt_bytes, dtype=torch.uint8, device=self.dev)  # zeroed once
         self.h_scalars = torch.zeros(4, 8, dtype=torch.float64).pin_memory()  # ring of 4 tickets
@@ -262,7 +276,9 @@ class LearnerEngine:
         return self.h_views[slot]
 
     def fill_host(self, batch: dict, slot: int = 0) -> None:
-        for name, _ in _BATCH_FIELDS:
+        for name, _ in self.fields:
+            if name == "obs" and self.obs_dtype == "uint8" and np.asarray(batch["obs"]).dtype != np.uint8:
+                raise ValueError("a uint8-observation engine takes uint8 obs arrays")
             np.copyto(self.h_views[slot][name], batch[name])
 
     def ingest(self, slot: int = 0) -> None:
@@ -298,9 +314,10 @@ class LearnerEngine:
         cs = self.copy_stream
         if self._slab_used[slot]:
             cs.wait_event(self.slab_free[slot])
-        _cabi.check(self.lib.impala_ingest_shard(_ptr(self.d_slabs[slot]), C.c_void_p(host_address), self.T, B_total,
-                                                 self.O, self.A, b0, self.B, C.c_void_p(cs.cuda_stream)),
-                    "impala_ingest_shard")
+        _cabi.check(self.lib.impala_ingest_shard_obs(_ptr(self.d_slabs[slot]), C.c_void_p(host_address), self.T,
+                                                     B_total, self.O, self.A, self.obs_code, b0, self.B,
+                                                     C.c_void_p(cs.cuda_stream)),
+                    "impala_ingest_shard_obs")
         self.slab_ready[slot].record(cs)
 
     def load_device_batch(self, batch: dict, slot: int = 0) -> None:
@@ -325,9 +342,19 @@ class LearnerEngine:
         g_vf = C.c_void_p(gbase + 8 * self.n_pi)
         scal = C.c_void_p(gbase + 8 * self.n_total)
         obs = _ptr(d["obs"])
-        _cabi.check(lib.impala_mlp_forward_pair(obs, p_pi, p_vf, _ptr(self.logits), _ptr(self.values),
-                                                self.M_pi, self.M_vf, O, self.H_pi, self.H_v, A, st),
-                    "impala_mlp_forward_pair")
+        if self.obs_f32 is not None:  # byte observations, O <= 128: one widening launch, then the float path
+            _cabi.check(lib.impala_obs_u8_to_f32(obs, _ptr(self.obs_f32), self.obs_f32.numel(), st),
+                        "impala_obs_u8_to_f32")
+            obs = _ptr(self.obs_f32)
+        if self.obs_u8_native:
+            # the pair entry point runs the two networks one after the other at these widths: same launches
+            for p, out, M, H, N2 in ((p_pi, self.logits, self.M_pi, self.H_pi, A),
+                                     (p_vf, self.values, self.M_vf, self.H_v, 1)):
+                _cabi.check(lib.impala_mlp_forward_u8(obs, p, _ptr(out), M, O, H, N2, st), "impala_mlp_forward_u8")
+        else:
+            _cabi.check(lib.impala_mlp_forward_pair(obs, p_pi, p_vf, _ptr(self.logits), _ptr(self.values),
+                                                    self.M_pi, self.M_vf, O, self.H_pi, self.H_v, A, st),
+                        "impala_mlp_forward_pair")
         _cabi.check(lib.impala_vtrace_loss(
             _ptr(self.logits), _ptr(d["beh_logits"]), _ptr(d["actions"]),
             _ptr(d["rewards"]), _ptr(d["done"]), _ptr(d["lens"]), _ptr(self.values),
@@ -344,10 +371,17 @@ class LearnerEngine:
                 _ptr(pr["gather_ptrs"]), _ptr(pr["seq"]), pr["slot"], pr["buf"], pr["rank"], self.world, st),
                 "impala_mlp_backward_pair_push")
         else:
-            _cabi.check(lib.impala_mlp_backward_pair(
-                obs, p_pi, p_vf, _ptr(self.dlogits), _ptr(self.dv), g_pi, g_vf, _ptr(self.ws_pi), self.ws_pi_bytes,
-                _ptr(self.ws_vf), self.ws_vf_bytes, self.M_pi, self.M_vf, O, self.H_pi, self.H_v, A, st),
-                "impala_mlp_backward_pair")
+            if self.obs_u8_native:
+                for p, dout, g, ws, nbytes, M, H, N2 in (
+                        (p_pi, self.dlogits, g_pi, self.ws_pi, self.ws_pi_bytes, self.M_pi, self.H_pi, A),
+                        (p_vf, self.dv, g_vf, self.ws_vf, self.ws_vf_bytes, self.M_vf, self.H_v, 1)):
+                    _cabi.check(lib.impala_mlp_backward_u8(obs, p, _ptr(dout), g, _ptr(ws), nbytes, M, O, H, N2, st),
+                                "impala_mlp_backward_u8")
+            else:
+                _cabi.check(lib.impala_mlp_backward_pair(
+                    obs, p_pi, p_vf, _ptr(self.dlogits), _ptr(self.dv), g_pi, g_vf, _ptr(self.ws_pi),
+                    self.ws_pi_bytes, _ptr(self.ws_vf), self.ws_vf_bytes, self.M_pi, self.M_vf, O, self.H_pi,
+                    self.H_v, A, st), "impala_mlp_backward_pair")
             if pr:  # stand-alone producer: comm[0 : n_total + 8) -> every rank's gather buffer
                 _cabi.check(lib.impala_peer_push(_ptr(self.comm), self.n_total + 8, _ptr(pr["gather_ptrs"]),
                                                  _ptr(pr["seq"]), pr["slot"], pr["buf"], pr["rank"], self.world, st),

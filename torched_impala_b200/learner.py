@@ -73,14 +73,30 @@ def check_trajectory(traj, T: int) -> int:
     return L
 
 
-def pack_trajectory(views: dict, b: int, traj, T: int) -> float:
+def obs_array(traj, obs_dtype) -> np.ndarray:
+    """The trajectory's stacked observations in the slab's observation type.  "uint8" takes them only
+    when every value is an integer in [0, 255] (Atari RAM bytes, MinAtar planes) and raises ValueError
+    otherwise: nothing is truncated or rescaled."""
+    if np.dtype(obs_dtype) != np.uint8:
+        return _np(torch.stack(traj.obs), torch.float32)
+    v = torch.stack(traj.obs).detach().cpu()
+    if v.dtype != torch.uint8:
+        v = v.to(torch.float64)
+        if not bool(((v >= 0) & (v <= 255) & (v == torch.floor(v))).all()):
+            raise ValueError(f"trajectory {getattr(traj, 'id', '?')}: uint8 observations must be integers in "
+                             "[0, 255] (the values enter the network as they are)")
+    return v.to(torch.uint8).numpy()
+
+
+def pack_trajectory(views: dict, b: int, traj, T: int, obs=None) -> float:
     """Write one reference-format trajectory into column `b` of a host batch slab.
 
-    Replaces learner.py:104-109,117 (five torch.stack calls + `disc`): float64 -> float32,
-    int64 -> int32, bool -> u8, zero padding past the trajectory's length.  Returns the
+    Replaces learner.py:104-109,117 (five torch.stack calls + `disc`): float64 -> float32 (or the
+    checked uint8 of obs_array for a byte-observation slab), int64 -> int32, bool -> u8, zero padding
+    past the trajectory's length.  `obs`: obs_array's result if the caller already has it.  Returns the
     trajectory's reward sum (learner.py:108)."""
     L = check_trajectory(traj, T)
-    views["obs"][:L + 1, b] = _np(torch.stack(traj.obs), torch.float32)
+    views["obs"][:L + 1, b] = obs_array(traj, views["obs"].dtype) if obs is None else obs
     views["obs"][L + 1:, b] = 0
     views["beh_logits"][:L, b] = _np(torch.stack(traj.logits), torch.float32)
     views["beh_logits"][L:, b] = 0
@@ -200,8 +216,14 @@ class _Publisher:
 class Learner:
     def __init__(self, id, hparams, policy, value_fn, q, update_counter, log_path=None,
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
-                 evaluator=None):
+                 evaluator=None, obs_dtype="float32"):
         self.id = id
+        if obs_dtype not in ("float32", "uint8"):
+            raise ValueError(f"obs_dtype must be 'float32' or 'uint8', got {obs_dtype!r}")
+        if hasattr(q, "collect_batch") and getattr(q, "obs_dtype", "float32") != obs_dtype:
+            raise ValueError(f"the RingQueue holds {getattr(q, 'obs_dtype', 'float32')} observations, "
+                             f"the learner was built for {obs_dtype}")
+        self.obs_dtype = obs_dtype  # "uint8": byte observations end to end (ring / slabs / MLP kernels)
         self.hp = hparams
         self.policy = policy
         self.value_fn = value_fn
@@ -241,7 +263,8 @@ class Learner:
             from .ring import RingQueue
 
             O, A, _, _ = _dims(self.policy, self.value_fn)
-            self._stage_ring = RingQueue(self.hp.max_timesteps, self.hp.batch_size, O, A, slabs=2)
+            self._stage_ring = RingQueue(self.hp.max_timesteps, self.hp.batch_size, O, A, slabs=2,
+                                         obs_dtype=self.obs_dtype)
         self.p.start()
         print(f"[main] Started learner_{self.id} with pid {self.p.pid}")
 
@@ -260,7 +283,8 @@ class Learner:
         O, A, H_pi, H_v = _dims(self.policy, self.value_fn)
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
-        return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp)
+        return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
+                    obs_dtype=self.obs_dtype)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -269,7 +293,8 @@ class Learner:
         if c["B"] % world:
             raise ValueError(f"batch_size {c['B']} does not divide over {world} devices")
         eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], self.hp,
-                            global_batch=c["B"], device=self.device, mode=self.mode, process_group=process_group)
+                            global_batch=c["B"], device=self.device, mode=self.mode, process_group=process_group,
+                            obs_dtype=c["obs_dtype"])
         eng.load_state(self._init_state())
         return eng
 

@@ -76,6 +76,46 @@ def mlp_backward(x, params, dout, O: int, H: int, N2: int):
     return grad
 
 
+def mlp_forward_u8(x, params, O: int, H: int, N2: int):
+    """impala_mlp_forward_u8: byte observations x (uint8, values unscaled), 128 < O <= 1024."""
+    _need_cuda(x, params)
+    if x.dtype != torch.uint8:
+        raise _cabi.ImpalaCudaError(f"mlp_forward_u8 takes uint8 observations, got {x.dtype}")
+    M = x.numel() // O
+    out = torch.empty(M, N2, dtype=torch.float32, device=x.device)
+    _cabi.check(_cabi.lib().impala_mlp_forward_u8(_p(x), _p(params), _p(out), M, O, H, N2, _st()),
+                "impala_mlp_forward_u8")
+    return out
+
+
+def mlp_backward_u8(x, params, dout, O: int, H: int, N2: int):
+    """impala_mlp_backward_u8 (workspace as for mlp_backward)."""
+    _need_cuda(x, params, dout)
+    if x.dtype != torch.uint8:
+        raise _cabi.ImpalaCudaError(f"mlp_backward_u8 takes uint8 observations, got {x.dtype}")
+    lib = _cabi.lib()
+    M = x.numel() // O
+    _, total = _cabi.param_layout(O, H, N2)
+    nbytes = lib.impala_mlp_backward_workspace(M, O, H, N2)
+    if nbytes < 0:
+        _cabi.check(int(nbytes), "impala_mlp_backward_workspace")
+    ws = torch.zeros(int(nbytes), dtype=torch.uint8, device=x.device)
+    grad = torch.empty(total, dtype=torch.float64, device=x.device)
+    _cabi.check(lib.impala_mlp_backward_u8(_p(x), _p(params), _p(dout), _p(grad), _p(ws), int(nbytes),
+                                           M, O, H, N2, _st()), "impala_mlp_backward_u8")
+    return grad
+
+
+def obs_u8_to_f32(x):
+    """Exact float32 copy of a uint8 tensor (impala_obs_u8_to_f32)."""
+    _need_cuda(x)
+    if x.dtype != torch.uint8:
+        raise _cabi.ImpalaCudaError(f"obs_u8_to_f32 takes uint8, got {x.dtype}")
+    out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    _cabi.check(_cabi.lib().impala_obs_u8_to_f32(_p(x), _p(out), x.numel(), _st()), "impala_obs_u8_to_f32")
+    return out
+
+
 def mlp_forward_pair(x, params_pi, params_vf, M_pi: int, M_vf: int, O: int, H_pi: int, H_vf: int, A: int):
     """Policy logits on the first M_pi rows of x and values on the first M_vf rows, one call."""
     _need_cuda(x, params_pi, params_vf)

@@ -46,10 +46,15 @@ def _pause(t_start: float) -> None:
         time.sleep(_POLL_S)
 
 
-def _layout(T: int, B: int, O: int, A: int):
-    """Same 256-byte aligned layout as include/impala_b200.h::impala_batch_layout (pure python so
+_OBS_BYTES = {"float32": 4, "uint8": 1}
+
+
+def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32"):
+    """Same 256-byte aligned layout as include/impala_b200.h::impala_batch_layout_obs (pure python so
     actor processes do not need the CUDA library)."""
-    sizes = ((T + 1) * B * O * 4, T * B * A * 4, T * B * 4, T * B * 4, T * B, B * 4)
+    if obs_dtype not in _OBS_BYTES:
+        raise ValueError(f"obs_dtype must be one of {sorted(_OBS_BYTES)}, got {obs_dtype!r}")
+    sizes = ((T + 1) * B * O * _OBS_BYTES[obs_dtype], T * B * A * 4, T * B * 4, T * B * 4, T * B, B * 4)
     offs, off = [], 0
     for s in sizes:
         offs.append(off)
@@ -60,11 +65,14 @@ def _layout(T: int, B: int, O: int, A: int):
 class RingQueue:
     """Drop-in for the `mp.Queue` between actors and learner, backed by shared-memory batch slabs."""
 
-    def __init__(self, T: int, B: int, O: int, A: int, slabs: int = 3):
+    def __init__(self, T: int, B: int, O: int, A: int, slabs: int = 3, obs_dtype: str = "float32"):
         if slabs < 2:
             raise ValueError("need at least two slabs (one filling while one is consumed)")
         self.T, self.B, self.O, self.A, self.K = T, B, O, A, slabs
-        self.offsets, self.slab_bytes = _layout(T, B, O, A)
+        # "uint8": byte observations (Atari RAM, MinAtar planes), a quarter of the float32 slab bytes
+        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype)
+        self.obs_dtype = obs_dtype
+        self._fields = (("obs", np.dtype(obs_dtype).type),) + _FIELDS[1:]
         # control block after the slabs: filled u8[K][B] | rsum f64[K][B] | tid i64[K][B] |
         # released i64[K] | next_ticket i64[1]   (8-byte aligned pieces)
         kb = slabs * B
@@ -119,7 +127,7 @@ class RingQueue:
             for kk in range(self.K):
                 base = kk * self.slab_bytes
                 self._views.append({name: np.ndarray(shapes[name], dtype=dt, buffer=self.shm.buf, offset=base + off)
-                                    for (name, dt), off in zip(_FIELDS, self.offsets)})
+                                    for (name, dt), off in zip(self._fields, self.offsets)})
         return self._views[k]
 
     def slab_address(self, k: int) -> int:
@@ -132,9 +140,10 @@ class RingQueue:
 
     # ---- actor side (same call shape as mp.Queue.put used at actor.py:118)
     def put(self, traj, block: bool = True, timeout: float | None = None):
-        from .learner import check_trajectory, pack_trajectory
+        from .learner import check_trajectory, obs_array, pack_trajectory
 
         check_trajectory(traj, self.T)  # BEFORE a column is taken: a malformed trajectory must not leave a hole
+        obs = obs_array(traj, self.obs_dtype)  # the same: raises on obs a uint8 ring cannot hold
         c = self._control()
         end = None if (timeout is None or not block) else time.monotonic() + timeout
         t_wait = time.monotonic()
@@ -149,7 +158,7 @@ class RingQueue:
                 raise queue.Full  # like mp.Queue.put on a full queue; actor.py:120 retries
             _pause(t_wait)
         try:
-            rsum = pack_trajectory(self.views(k), b, traj, self.T)
+            rsum = pack_trajectory(self.views(k), b, traj, self.T, obs=obs)
         except BaseException:
             # never leave the column unfilled (the learner would stall on it until its timeout):
             # publish it as an empty trajectory - neutral padding for the update - and re-raise
@@ -178,6 +187,8 @@ class RingQueue:
         n = int(block["lens"].shape[0])
         if n < 1 or self.B % n:
             raise ValueError(f"block of {n} trajectories: n must divide the batch size {self.B}")
+        if self.obs_dtype == "uint8" and np.asarray(block["obs"]).dtype != np.uint8:
+            raise ValueError(f"a uint8-observation ring takes uint8 obs blocks, got {np.asarray(block['obs']).dtype}")
         c = self._control()
         end = None if timeout is None else time.monotonic() + timeout
         t_wait = time.monotonic()

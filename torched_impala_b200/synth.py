@@ -5,7 +5,7 @@ The reference has no (T, B) tensor anywhere: a "batch" is `batch_size` python
 (`learner.py:89-117`).  The GPU learner's device layout is
 time-major and dense:
 
-    obs        (T+1, B, O) f32   index T is the bootstrap observation slot
+    obs        (T+1, B, O) f32   index T is the bootstrap observation slot (u8 for byte observations)
     beh_logits (T,   B, A) f32   behaviour-policy logits shipped by the actor
     actions    (T,   B)    i32
     rewards    (T,   B)    f32
@@ -27,9 +27,20 @@ PARAM_ALIGN = 32  # floats; every parameter tensor starts on a 128-byte boundary
 
 
 def make_batch(seed: int, T: int, B: int, O: int, A: int, ragged: bool = False,
-               unit_reward: bool = False, done_last: bool = True) -> dict:
+               unit_reward: bool = False, done_last: bool = True, obs_kind: str = "normal") -> dict:
+    """obs_kind: "normal" - float32 N(0, 1); "bytes" - uint8 0..255 (Atari RAM); "planes" - uint8 0/1
+    (MinAtar).  The integer kinds draw from a stream of their own, so every other field equals the
+    "normal" batch of the same seed."""
     rng = np.random.default_rng(seed)
     obs = rng.standard_normal((T + 1, B, O), dtype=np.float32)
+    if obs_kind != "normal":
+        irng = np.random.default_rng(seed + 104729)
+        if obs_kind == "bytes":
+            obs = irng.integers(0, 256, (T + 1, B, O), dtype=np.uint8)
+        elif obs_kind == "planes":
+            obs = (irng.random((T + 1, B, O)) < 0.3).astype(np.uint8)
+        else:
+            raise ValueError(f"obs_kind must be 'normal', 'bytes' or 'planes', got {obs_kind!r}")
     beh = rng.standard_normal((T, B, A), dtype=np.float32)
     # Categorical(softmax(beh)) by inverse-CDF on a float64 copy.
     z = beh.astype(np.float64)
