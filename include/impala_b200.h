@@ -73,6 +73,15 @@ int impala_batch_layout(int T, int B, int O, int A, int64_t offsets[6], int64_t*
  * returns IMPALA_ERR_BAD_ARG. */
 int impala_batch_layout_obs(int T, int B, int O, int A, int obs_dtype, int64_t offsets[6], int64_t* total_bytes);
 
+/* Frame-stacked observations stored once per frame.  With `frames` = k stacked frames of F values
+ * each (the network sees O = k F features), the obs tensor of the slab is  frames (T+k, B, F)  of
+ * type obs_dtype: observation row (t, b) is frames[t .. t+k-1, b, :] concatenated, oldest first (the
+ * gym FrameStack order, flattened); frames s >= lens[b] + k are zero.  Every other tensor as in
+ * impala_batch_layout_obs, whose layout is the frames = 1 case (F = O).  Bad arguments (frames < 1
+ * included) return IMPALA_ERR_BAD_ARG. */
+int impala_batch_layout_frames(int T, int B, int F, int frames, int A, int obs_dtype, int64_t offsets[6],
+                               int64_t* total_bytes);
+
 /* Host slab -> device slab, async on `stream` (host memory should be pinned). */
 int impala_ingest(void* dev_slab, const void* host_slab, int64_t bytes, void* stream);
 
@@ -86,6 +95,19 @@ int impala_ingest_shard(void* dev_slab, const void* host_slab, int T, int B, int
  * IMPALA_OBS_U8); impala_ingest_shard is its IMPALA_OBS_F32 case. */
 int impala_ingest_shard_obs(void* dev_slab, const void* host_slab, int T, int B, int O, int A, int obs_dtype,
                             int b0, int B_local, void* stream);
+/* The same for slabs laid out by impala_batch_layout_frames (T+frames frame rows of F values);
+ * impala_ingest_shard_obs is its frames = 1 case. */
+int impala_ingest_shard_frames(void* dev_slab, const void* host_slab, int T, int B, int F, int frames, int A,
+                               int obs_dtype, int b0, int B_local, void* stream);
+
+/* Dense observation rows from frames (pure data movement, one launch):
+ *   out[(t B + b) k F + j F + f] = frames[((t + j) B + b) F + f]   for t < R, b < B, j < k, f < F.
+ * in_dtype -> out_dtype: IMPALA_OBS_U8 -> IMPALA_OBS_U8, IMPALA_OBS_U8 -> IMPALA_OBS_F32 (exact) or
+ * IMPALA_OBS_F32 -> IMPALA_OBS_F32; any other pair, a NULL pointer or R, B, F, k < 1 returns
+ * IMPALA_ERR_BAD_ARG.  16-byte loads and stores when F is a multiple of 16 bytes of frame data and both
+ * pointers are 16-byte aligned, element copies otherwise. */
+int impala_obs_unstack(const void* frames, int in_dtype, void* out, int out_dtype, int R, int B, int F, int k,
+                       void* stream);
 
 /* out[i] = (float)x[i] for i < n: exact widening of byte observations, for the MLP shapes that read
  * float32 rows only (O <= 128). */

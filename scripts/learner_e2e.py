@@ -10,6 +10,8 @@ fork start method as in reference train.py:42).  payload=block: actors push pre-
 (T, n, .) blocks (`RingQueue.put_block`, SURVEY section 7); payload=trajectory: the reference wire
 format, one `utils.Trajectory` of ~5T tiny tensors per put (what an unmodified actor.py sends).
 --obs-dtype uint8: byte observations (0..255, as Atari RAM) in the ring, the slabs and the MLP kernels.
+--frames k: the observations are k stacked frames, stored once per frame in the ring and the slabs (block
+actors push (T+k, n, O/k) frame blocks, trajectory actors the stacked observations).
 Run in a fresh interpreter (bench.py spawns it as a subprocess)."""
 import argparse
 import json
@@ -36,13 +38,14 @@ CFG = {"c3": dict(T=20, B=1024, O=24, A=4, H=256), "c4": dict(T=20, B=4096, O=24
        "minatar": dict(T=20, B=4096, O=400, A=6, H=256)}
 
 
-def actor_main(aid, ring, learner_done, w, payload, block, seed, obs_kind="normal"):
+def actor_main(aid, ring, learner_done, w, payload, block, seed, obs_kind="normal", frames=1):
     """Synthetic actor: a pool of pre-generated trajectories pushed as fast as the ring takes them.
     It reads the published policy version like actor.py:70 reads the weights (once per put)."""
     torch.set_num_threads(1)
     n = block if payload == "block" else 8
-    pool = synth.make_batch(seed, w["T"], n, w["O"], w["A"], obs_kind=obs_kind)
-    trajs = synth.to_trajectories(pool) if payload == "trajectory" else None
+    pool = synth.make_batch(seed, w["T"], n, w["O"], w["A"], obs_kind=obs_kind, frames=frames)
+    trajs = synth.to_trajectories(synth.stack_frames(pool, frames) if frames > 1 else pool) \
+        if payload == "trajectory" else None
     rsum = pool["rewards"].sum(0, dtype=np.float64)
     i = 0
     while not learner_done.is_set():
@@ -68,6 +71,7 @@ def main():
     ap.add_argument("--publish-every", type=int, default=1)
     ap.add_argument("--deadline", type=float, default=120.0)
     ap.add_argument("--obs-dtype", default="float32", choices=["float32", "uint8"])
+    ap.add_argument("--frames", type=int, default=1)
     a = ap.parse_args()
     w = CFG[a.config]
     mp.set_start_method("fork", force=True)
@@ -79,13 +83,13 @@ def main():
     block = min(a.block, w["B"])
     while w["B"] % block:
         block //= 2
-    ring = RingQueue(w["T"], w["B"], w["O"], w["A"], slabs=3, obs_dtype=a.obs_dtype)
+    ring = RingQueue(w["T"], w["B"], w["O"], w["A"], slabs=3, obs_dtype=a.obs_dtype, frames=a.frames)
     counter = Counter(0)
     devices = [f"cuda:{i}" for i in range(a.devices)]
     lrn = Learner(1, hp, policy, value_fn, ring, counter, log_path=None, timeout=120, devices=devices,
-                  publish_every=a.publish_every, obs_dtype=a.obs_dtype)
+                  publish_every=a.publish_every, obs_dtype=a.obs_dtype, frames=a.frames)
     obs_kind = "bytes" if a.obs_dtype == "uint8" else "normal"
-    actors = [mp.Process(target=actor_main, args=(i, ring, lrn.completion, w, a.payload, block, 100 + i, obs_kind),
+    actors = [mp.Process(target=actor_main, args=(i, ring, lrn.completion, w, a.payload, block, 100 + i, obs_kind, a.frames),
                          daemon=True) for i in range(a.actors)]
     for p in actors:
         p.start()
@@ -123,7 +127,8 @@ def main():
     print(json.dumps(dict(
         what="steps/s through Learner + RingQueue + synthetic actor processes (wall clock on the shared update counter)",
         config=a.config, **w, actors=a.actors, payload=a.payload, block=block if a.payload == "block" else 1,
-        devices=a.devices, **({"obs_dtype": a.obs_dtype} if a.obs_dtype != "float32" else {}), updates_timed=c_end - c_w, steps_per_s=sps, trajectories_per_s=sps * w["B"],
+        devices=a.devices, **({"obs_dtype": a.obs_dtype} if a.obs_dtype != "float32" else {}),
+        **({"frames": a.frames} if a.frames != 1 else {}), updates_timed=c_end - c_w, steps_per_s=sps, trajectories_per_s=sps * w["B"],
         h2d_bytes_per_step=int(ring.slab_bytes), weight_publications=(lrn.policy_version - (v0 or 0)) // 2,
         publish_every=a.publish_every, host_cores=os.cpu_count())))
 

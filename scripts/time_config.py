@@ -4,7 +4,10 @@ alternating step by step with the default path, so both numbers see the same clo
 --compare-obs alternates a float32-slab engine and a uint8-slab engine (byte observations 0..255) the same way
 and reports, for both, the device-resident step time and the pinned-slab end-to-end step time (the DMA of
 slab i+1 runs under step i; a step's window also waits for that DMA), with the GPU name, power limit and
-maximum SM clock read in the same run."""
+maximum SM clock read in the same run.
+--compare-frames alternates the dense engine and a frame engine (--frames k stacked frames stored once per frame,
+--obs-dtype) on the same values the same way, and times the unstacking launch alone (median of 200 launches,
+L2 flushed before each) against its HBM floor (frame bytes read + dense bytes written at 3.35 TB/s)."""
 import argparse
 import os
 import statistics
@@ -30,12 +33,17 @@ CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256), "c5": dict(T=100, B=8192, O=6
        # recompute), 176 MB of observations
        "ram4": dict(T=20, B=4096, O=512, A=18, H=256),
        # MinAtar Breakout / Asterix, flattened 10x10x4 binary grids: P = 207 111 parameters
-       "minatar": dict(T=20, B=4096, O=400, A=6, H=256)}
+       "minatar": dict(T=20, B=4096, O=400, A=6, H=256),
+       # 8 stacked Atari RAM frames
+       "ram8": dict(T=20, B=4096, O=1024, A=18, H=256)}
 ap = argparse.ArgumentParser()
 ap.add_argument("--config", default="c5")
 ap.add_argument("--steps", type=int, default=30)
 ap.add_argument("--compare-tc", action="store_true", help="alternate with IMPALA_MLP_TC=0 and report both")
 ap.add_argument("--compare-obs", action="store_true", help="alternate float32 and uint8 observation slabs")
+ap.add_argument("--compare-frames", action="store_true", help="alternate dense and frame-stacked observation slabs")
+ap.add_argument("--frames", type=int, default=4, help="stacked frames of --compare-frames")
+ap.add_argument("--obs-dtype", default="float32", choices=["float32", "uint8"], help="slab obs type of --compare-frames")
 a = ap.parse_args()
 w = CFG[a.config]
 hp = default_hparams(batch_size=w["B"], max_timesteps=w["T"])
@@ -46,17 +54,30 @@ if a.compare_tc:
 if a.compare_obs:
     arms = {"obs float32": arms["default"], "obs uint8": arms["default"]}
     obs_dt = {"obs float32": "float32", "obs uint8": "uint8"}
+n_frames = {}
+if a.compare_frames:
+    arms = {f"dense {a.obs_dtype}": arms["default"], f"frames={a.frames} {a.obs_dtype}": arms["default"]}
+    obs_dt = {name: a.obs_dtype for name in arms}
+    n_frames = {f"frames={a.frames} {a.obs_dtype}": a.frames}
 engines = {}
 for name, tc in arms.items():
     os.environ["IMPALA_MLP_TC"] = tc  # read by the C library at every launch (and at graph capture)
     dt = obs_dt.get(name, "float32")
-    eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt)
+    k = n_frames.get(name, 1)
+    eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k)
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
-    batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if a.compare_obs else "normal")
+    byte_obs = a.compare_obs or (a.compare_frames and dt == "uint8")
+    if a.compare_frames:  # the same observation values in both arms: the dense arm gets the stacked frames
+        batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if byte_obs else "normal",
+                                 frames=a.frames)
+        if k == 1:
+            batch = synth.stack_frames(batch, a.frames)
+    else:
+        batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if byte_obs else "normal")
     if dt == "float32":
         batch["obs"] = batch["obs"].astype("float32")
     eng.load_device_batch(batch)
-    if a.compare_obs:
+    if a.compare_obs or a.compare_frames:
         eng.load_device_batch(batch, 1)
     engines[name] = eng
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
@@ -74,7 +95,7 @@ for i in range(a.steps + 5):
             if i >= 5:
                 ts[name].append(e0.elapsed_time(e1) * 1e3)
 te = {name: [] for name in arms}
-if a.compare_obs:  # pinned-slab end to end: ingest(slab i+1) on the copy stream under step(slab i)
+if a.compare_obs or a.compare_frames:  # pinned-slab end to end: ingest(slab i+1) on the copy stream under step(slab i)
     for i in range(a.steps + 5):
         for name, eng in engines.items():
             with torch.cuda.stream(eng.stream):
@@ -90,7 +111,33 @@ if a.compare_obs:  # pinned-slab end to end: ingest(slab i+1) on the copy stream
                 if i >= 5:
                     te[name].append(e0.elapsed_time(e1) * 1e3)
 dev = torch.cuda.get_device_name()
-if a.compare_obs:
+if a.compare_frames:  # the unstacking launch alone, back to back
+    import ctypes
+
+    from torched_impala_b200 import _cabi
+
+    eng = engines[f"frames={a.frames} {a.obs_dtype}"]
+    out_code = _cabi.OBS_U8 if eng.obs_dense.dtype == torch.uint8 else _cabi.OBS_F32
+    args = (ctypes.c_void_p(eng.d["obs"].data_ptr()), eng.obs_code, ctypes.c_void_p(eng.obs_dense.data_ptr()),
+            out_code, w["T"] + 1, w["B"], eng.F, a.frames)
+    with torch.cuda.stream(eng.stream):
+        st = ctypes.c_void_p(eng.stream.cuda_stream)
+        tu = []
+        for i in range(220):
+            flush.zero_()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(eng.stream)
+            _cabi.check(eng.lib.impala_obs_unstack(*args, st), "impala_obs_unstack")
+            e1.record(eng.stream)
+            e1.synchronize()
+            if i >= 20:
+                tu.append(e0.elapsed_time(e1) * 1e3)
+    us = statistics.median(tu)
+    nbytes = eng.d["obs"].numel() * eng.d["obs"].element_size() + eng.obs_dense.numel() * eng.obs_dense.element_size()
+    print(f"impala_obs_unstack {a.config} frames={a.frames} {a.obs_dtype} -> {eng.obs_dense.dtype}: {us:.1f} us, "
+          f"{nbytes / 1e6:.1f} MB moved, HBM floor {nbytes / 3.35e12 * 1e6:.1f} us at 3.35 TB/s "
+          f"({nbytes / 3.35e12 * 1e6 / us:.0%} of it)")
+if a.compare_obs or a.compare_frames:
     q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
                         "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     print(f"GPU (nvidia-smi): {q}")

@@ -43,6 +43,9 @@ SIGNATURES = {
     "impala_ingest": (_i, [_p, _p, _i64, _p]),
     "impala_ingest_shard": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _p]),
     "impala_ingest_shard_obs": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _i, _p]),
+    "impala_batch_layout_frames": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_i64), C.POINTER(_i64)]),
+    "impala_ingest_shard_frames": (_i, [_p, _p] + [_i] * 8 + [_p]),
+    "impala_obs_unstack": (_i, [_p, _i, _p, _i, _i, _i, _i, _i, _p]),
     "impala_obs_u8_to_f32": (_i, [_p, _p, _i64, _p]),
     "impala_mlp_forward": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
     "impala_mlp_forward_u8": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
@@ -109,9 +112,17 @@ def param_layout(O: int, H: int, N2: int):
     return list(offs), total.value
 
 
-def batch_layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32"):
+def batch_layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1):
+    """Slab layout for networks of O observation features; frames > 1 stores the O / frames features of
+    each stacked frame once (impala_batch_layout_frames)."""
     offs = (_i64 * 6)()
     total = _i64()
-    check(lib().impala_batch_layout_obs(T, B, O, A, obs_dtype_code(obs_dtype), offs, C.byref(total)),
-          "impala_batch_layout_obs")
+    if frames == 1:
+        check(lib().impala_batch_layout_obs(T, B, O, A, obs_dtype_code(obs_dtype), offs, C.byref(total)),
+              "impala_batch_layout_obs")
+    else:
+        if frames < 1 or O % frames:
+            raise ValueError(f"{O} observation features do not split into {frames} frames")
+        check(lib().impala_batch_layout_frames(T, B, O // frames, frames, A, obs_dtype_code(obs_dtype), offs,
+                                               C.byref(total)), "impala_batch_layout_frames")
     return list(offs), total.value

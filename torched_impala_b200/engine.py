@@ -22,6 +22,11 @@ O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one 
 pair entry points do at those widths.  For O <= 128 impala_obs_u8_to_f32 widens the obs into a float32
 device buffer first (one more launch) and the pair entry points read that.
 
+frames=k > 1 (frame-stacked observations, O = k F): the slabs hold each frame once, obs (T+k, B, F)
+(impala_batch_layout_frames), and the step's first launch, impala_obs_unstack, rebuilds the dense (T+1, B, O)
+rows into a device buffer the unchanged kernels read: uint8 for the byte kernels (O > 128), the float32 buffer
+of the widened path (O <= 128 bytes: it replaces the widening launch), float32 for float32 frames.
+
 With `use_graph=True` the whole launch sequence of a step is captured once per slab into ONE CUDA
 graph and replayed (two graphs around the collective in the NCCL scheme).
 Ingest is double buffered: two pinned host slabs, two device slabs and
@@ -65,13 +70,16 @@ class LearnerEngine:
     def __init__(self, T: int, B_local: int, O: int, A: int, H_pi: int, H_v: int, hp,
                  global_batch: int | None = None, device: str | torch.device = "cuda:0",
                  mode: str = "reference", process_group=None, use_graph: bool = True,
-                 slabs: int = 2, obs_dtype: str = "float32"):
+                 slabs: int = 2, obs_dtype: str = "float32", frames: int = 1):
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
         # "uint8": byte observations in the slabs (Atari RAM, MinAtar), entering the networks unscaled
         self.obs_code = _cabi.obs_dtype_code(obs_dtype)
         self.obs_dtype = obs_dtype
+        if frames < 1 or O % frames:
+            raise ValueError(f"{O} observation features do not split into {frames} stacked frames")
+        self.frames, self.F = frames, O // frames
         self.dev = torch.device(device)
         torch.cuda.set_device(self.dev)
         self.T, self.B, self.O, self.A, self.H_pi, self.H_v = T, B_local, O, A, H_pi, H_v
@@ -104,14 +112,14 @@ class LearnerEngine:
         self.norms = torch.zeros(2, dtype=torch.float64, device=self.dev)
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts
-        self.slab_off, self.slab_bytes = _cabi.batch_layout(T, B_local, O, A, obs_dtype)
+        self.slab_off, self.slab_bytes = _cabi.batch_layout(T, B_local, O, A, obs_dtype, frames)
         self.fields = ((("obs", np.uint8 if obs_dtype == "uint8" else np.float32),) + _BATCH_FIELDS[1:])
         self.n_slabs = slabs
         self.d_slabs = [torch.zeros(self.slab_bytes, dtype=torch.uint8, device=self.dev)
                         for _ in range(slabs)]
         self.h_slabs = [torch.zeros(self.slab_bytes, dtype=torch.uint8).pin_memory()
                         for _ in range(slabs)]
-        shapes = {"obs": (T + 1, B_local, O), "beh_logits": (T, B_local, A),
+        shapes = {"obs": (T + frames, B_local, self.F), "beh_logits": (T, B_local, A),
                   "actions": (T, B_local), "rewards": (T, B_local), "done": (T, B_local),
                   "lens": (B_local,)}
         self.shapes = shapes
@@ -147,6 +155,11 @@ class LearnerEngine:
         self.obs_u8_native = obs_dtype == "uint8" and O > 128
         self.obs_f32 = (torch.zeros((T + 1) * B_local * O, **f32) if obs_dtype == "uint8" and not self.obs_u8_native
                         else None)
+        # frames > 1: the dense rows the kernels read, rebuilt from the slab's frames once per step
+        self.obs_dense = None
+        if frames > 1:
+            self.obs_dense = self.obs_f32 if self.obs_f32 is not None else torch.zeros(
+                (T + 1) * B_local * O, dtype=torch.uint8 if self.obs_u8_native else torch.float32, device=self.dev)
         self.ws_vt_bytes = int(self.lib.impala_vtrace_loss_workspace(T, B_local, A))
         self.ws_vt = torch.zeros(self.ws_vt_bytes, dtype=torch.uint8, device=self.dev)  # zeroed once
         self.h_scalars = torch.zeros(4, 8, dtype=torch.float64).pin_memory()  # ring of 4 tickets
@@ -314,10 +327,10 @@ class LearnerEngine:
         cs = self.copy_stream
         if self._slab_used[slot]:
             cs.wait_event(self.slab_free[slot])
-        _cabi.check(self.lib.impala_ingest_shard_obs(_ptr(self.d_slabs[slot]), C.c_void_p(host_address), self.T,
-                                                     B_total, self.O, self.A, self.obs_code, b0, self.B,
-                                                     C.c_void_p(cs.cuda_stream)),
-                    "impala_ingest_shard_obs")
+        _cabi.check(self.lib.impala_ingest_shard_frames(_ptr(self.d_slabs[slot]), C.c_void_p(host_address), self.T,
+                                                        B_total, self.F, self.frames, self.A, self.obs_code, b0,
+                                                        self.B, C.c_void_p(cs.cuda_stream)),
+                    "impala_ingest_shard_frames")
         self.slab_ready[slot].record(cs)
 
     def load_device_batch(self, batch: dict, slot: int = 0) -> None:
@@ -342,7 +355,12 @@ class LearnerEngine:
         g_vf = C.c_void_p(gbase + 8 * self.n_pi)
         scal = C.c_void_p(gbase + 8 * self.n_total)
         obs = _ptr(d["obs"])
-        if self.obs_f32 is not None:  # byte observations, O <= 128: one widening launch, then the float path
+        if self.obs_dense is not None:  # frames: one unstacking launch (widening bytes for O <= 128)
+            out_code = _cabi.OBS_U8 if self.obs_dense.dtype == torch.uint8 else _cabi.OBS_F32
+            _cabi.check(lib.impala_obs_unstack(obs, self.obs_code, _ptr(self.obs_dense), out_code, T + 1, B, self.F,
+                                               self.frames, st), "impala_obs_unstack")
+            obs = _ptr(self.obs_dense)
+        elif self.obs_f32 is not None:  # byte observations, O <= 128: one widening launch, then the float path
             _cabi.check(lib.impala_obs_u8_to_f32(obs, _ptr(self.obs_f32), self.obs_f32.numel(), st),
                         "impala_obs_u8_to_f32")
             obs = _ptr(self.obs_f32)

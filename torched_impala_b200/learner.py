@@ -88,16 +88,36 @@ def obs_array(traj, obs_dtype) -> np.ndarray:
     return v.to(torch.uint8).numpy()
 
 
+def obs_frames(obs: np.ndarray, k: int, traj=None) -> np.ndarray:
+    """Stacked observations (L+1, k F), oldest frame first -> the trajectory's frames (L+k, F): obs[0] split
+    into its k frames, then the newest frame of each obs[t].  Raises ValueError, naming the trajectory and
+    the step, where obs[t] does not continue obs[t-1] (obs[t][:(k-1)F] != obs[t-1][F:]): such a trajectory
+    cannot be stored once per frame and is refused rather than misaligned."""
+    n, O = obs.shape
+    F = O // k
+    if k > 1 and n > 1:
+        bad = np.flatnonzero((obs[1:, :(k - 1) * F] != obs[:-1, F:]).any(axis=1))
+        if bad.size:
+            raise ValueError(f"trajectory {getattr(traj, 'id', '?')}: observation {int(bad[0]) + 1} does not continue "
+                             f"observation {int(bad[0])} as {k} stacked frames (flattened, oldest frame first)")
+    return np.concatenate([obs[0].reshape(k, F), obs[1:, (k - 1) * F:]], axis=0)
+
+
 def pack_trajectory(views: dict, b: int, traj, T: int, obs=None) -> float:
     """Write one reference-format trajectory into column `b` of a host batch slab.
 
     Replaces learner.py:104-109,117 (five torch.stack calls + `disc`): float64 -> float32 (or the
     checked uint8 of obs_array for a byte-observation slab), int64 -> int32, bool -> u8, zero padding
-    past the trajectory's length.  `obs`: obs_array's result if the caller already has it.  Returns the
-    trajectory's reward sum (learner.py:108)."""
+    past the trajectory's length.  `obs`: obs_array's result if the caller already has it.  A frame slab
+    (obs (T+k, B, F), k > 1) receives obs_frames' L+k frames.  Returns the trajectory's reward sum
+    (learner.py:108)."""
     L = check_trajectory(traj, T)
-    views["obs"][:L + 1, b] = obs_array(traj, views["obs"].dtype) if obs is None else obs
-    views["obs"][L + 1:, b] = 0
+    obs = obs_array(traj, views["obs"].dtype) if obs is None else obs
+    k = views["obs"].shape[0] - T
+    if k > 1:
+        obs = obs_frames(obs, k, traj)
+    views["obs"][:L + k, b] = obs
+    views["obs"][L + k:, b] = 0
     views["beh_logits"][:L, b] = _np(torch.stack(traj.logits), torch.float32)
     views["beh_logits"][L:, b] = 0
     views["actions"][:L, b] = _np(torch.stack(traj.a).reshape(L), torch.int32)
@@ -216,14 +236,21 @@ class _Publisher:
 class Learner:
     def __init__(self, id, hparams, policy, value_fn, q, update_counter, log_path=None,
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
-                 evaluator=None, obs_dtype="float32"):
+                 evaluator=None, obs_dtype="float32", frames=1):
         self.id = id
         if obs_dtype not in ("float32", "uint8"):
             raise ValueError(f"obs_dtype must be 'float32' or 'uint8', got {obs_dtype!r}")
         if hasattr(q, "collect_batch") and getattr(q, "obs_dtype", "float32") != obs_dtype:
             raise ValueError(f"the RingQueue holds {getattr(q, 'obs_dtype', 'float32')} observations, "
                              f"the learner was built for {obs_dtype}")
+        if frames != 1 and (frames < 1 or _dims(policy, value_fn)[0] % frames):
+            raise ValueError(f"{_dims(policy, value_fn)[0]} observation features do not split into {frames} "
+                             "stacked frames")
+        if hasattr(q, "collect_batch") and getattr(q, "frames", 1) != frames:
+            raise ValueError(f"the RingQueue stores observations as {getattr(q, 'frames', 1)} frames, "
+                             f"the learner was built for frames={frames}")
         self.obs_dtype = obs_dtype  # "uint8": byte observations end to end (ring / slabs / MLP kernels)
+        self.frames = frames  # > 1: each of the stacked frames stored once (ring / slabs), unstacked on the device
         self.hp = hparams
         self.policy = policy
         self.value_fn = value_fn
@@ -264,7 +291,7 @@ class Learner:
 
             O, A, _, _ = _dims(self.policy, self.value_fn)
             self._stage_ring = RingQueue(self.hp.max_timesteps, self.hp.batch_size, O, A, slabs=2,
-                                         obs_dtype=self.obs_dtype)
+                                         obs_dtype=self.obs_dtype, frames=self.frames)
         self.p.start()
         print(f"[main] Started learner_{self.id} with pid {self.p.pid}")
 
@@ -284,7 +311,7 @@ class Learner:
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
-                    obs_dtype=self.obs_dtype)
+                    obs_dtype=self.obs_dtype, frames=self.frames)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -294,7 +321,7 @@ class Learner:
             raise ValueError(f"batch_size {c['B']} does not divide over {world} devices")
         eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], self.hp,
                             global_batch=c["B"], device=self.device, mode=self.mode, process_group=process_group,
-                            obs_dtype=c["obs_dtype"])
+                            obs_dtype=c["obs_dtype"], frames=c["frames"])
         eng.load_state(self._init_state())
         return eng
 

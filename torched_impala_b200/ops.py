@@ -116,6 +116,23 @@ def obs_u8_to_f32(x):
     return out
 
 
+def obs_unstack(frames, k: int, out_dtype=None):
+    """Dense stacked observations (R, B, k F) from frames (R + k - 1, B, F) (impala_obs_unstack): row (t, b) is
+    frames t .. t+k-1 of column b, oldest first.  uint8 -> uint8 | float32, float32 -> float32."""
+    _need_cuda(frames)
+    codes = {torch.uint8: _cabi.OBS_U8, torch.float32: _cabi.OBS_F32}
+    out_dtype = frames.dtype if out_dtype is None else out_dtype
+    if frames.dim() != 3 or frames.dtype not in codes or out_dtype not in codes:
+        raise _cabi.ImpalaCudaError(f"obs_unstack takes (R+k-1, B, F) uint8 / float32 frames, got {tuple(frames.shape)} "
+                                    f"{frames.dtype} -> {out_dtype}")
+    n, B, F = frames.shape
+    R = n - k + 1
+    out = torch.empty(max(R, 0), B, k * F, dtype=out_dtype, device=frames.device)
+    _cabi.check(_cabi.lib().impala_obs_unstack(_p(frames), codes[frames.dtype], _p(out), codes[out_dtype], R, B, F, k,
+                                               _st()), "impala_obs_unstack")
+    return out
+
+
 def mlp_forward_pair(x, params_pi, params_vf, M_pi: int, M_vf: int, O: int, H_pi: int, H_vf: int, A: int):
     """Policy logits on the first M_pi rows of x and values on the first M_vf rows, one call."""
     _need_cuda(x, params_pi, params_vf)

@@ -49,12 +49,15 @@ def _pause(t_start: float) -> None:
 _OBS_BYTES = {"float32": 4, "uint8": 1}
 
 
-def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32"):
-    """Same 256-byte aligned layout as include/impala_b200.h::impala_batch_layout_obs (pure python so
-    actor processes do not need the CUDA library)."""
+def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1):
+    """Same 256-byte aligned layout as include/impala_b200.h::impala_batch_layout_frames with F = O / frames
+    (impala_batch_layout_obs at frames = 1; pure python so actor processes do not need the CUDA library)."""
     if obs_dtype not in _OBS_BYTES:
         raise ValueError(f"obs_dtype must be one of {sorted(_OBS_BYTES)}, got {obs_dtype!r}")
-    sizes = ((T + 1) * B * O * _OBS_BYTES[obs_dtype], T * B * A * 4, T * B * 4, T * B * 4, T * B, B * 4)
+    if frames < 1 or O % frames:
+        raise ValueError(f"{O} observation features do not split into {frames} frames")
+    sizes = ((T + frames) * B * (O // frames) * _OBS_BYTES[obs_dtype], T * B * A * 4, T * B * 4, T * B * 4, T * B,
+             B * 4)
     offs, off = [], 0
     for s in sizes:
         offs.append(off)
@@ -65,13 +68,16 @@ def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32"):
 class RingQueue:
     """Drop-in for the `mp.Queue` between actors and learner, backed by shared-memory batch slabs."""
 
-    def __init__(self, T: int, B: int, O: int, A: int, slabs: int = 3, obs_dtype: str = "float32"):
+    def __init__(self, T: int, B: int, O: int, A: int, slabs: int = 3, obs_dtype: str = "float32", frames: int = 1):
         if slabs < 2:
             raise ValueError("need at least two slabs (one filling while one is consumed)")
         self.T, self.B, self.O, self.A, self.K = T, B, O, A, slabs
         # "uint8": byte observations (Atari RAM, MinAtar planes), a quarter of the float32 slab bytes
-        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype)
+        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype, frames)
         self.obs_dtype = obs_dtype
+        # frames > 1: observations are `frames` stacked frames of O / frames features, each frame stored once
+        # per column, (T + frames, B, O / frames); the learner rebuilds the stacked rows on the device
+        self.frames = frames
         self._fields = (("obs", np.dtype(obs_dtype).type),) + _FIELDS[1:]
         # control block after the slabs: filled u8[K][B] | rsum f64[K][B] | tid i64[K][B] |
         # released i64[K] | next_ticket i64[1]   (8-byte aligned pieces)
@@ -120,7 +126,7 @@ class RingQueue:
     def views(self, k: int) -> dict:
         """Numpy views of slab k (the six batch tensors, learner layout)."""
         if self._views is None:
-            shapes = {"obs": (self.T + 1, self.B, self.O), "beh_logits": (self.T, self.B, self.A),
+            shapes = {"obs": (self.T + self.frames, self.B, self.O // self.frames), "beh_logits": (self.T, self.B, self.A),
                       "actions": (self.T, self.B), "rewards": (self.T, self.B), "done": (self.T, self.B),
                       "lens": (self.B,)}
             self._views = []
@@ -179,7 +185,8 @@ class RingQueue:
 
     def put_block(self, block: dict, block_rsum=None, timeout: float | None = None) -> None:
         """Pre-stacked payload (SURVEY section 7: synthetic actors push stacked arrays through the same
-        queue): `block` holds n trajectories in the learner layout - obs (T+1, n, O) f32, beh_logits
+        queue): `block` holds n trajectories in the learner layout - obs (T+1, n, O) f32 (frames
+        (T+frames, n, O/frames) on a frame ring), beh_logits
         (T, n, A) f32, actions (T, n) i32, rewards (T, n) f32, done (T, n) u8, lens (n,) i32 - and is
         copied into n consecutive columns of the slab being filled (n must divide B, so a block never
         straddles two slabs).  One lock round trip and five strided copies per block instead of
@@ -189,6 +196,9 @@ class RingQueue:
             raise ValueError(f"block of {n} trajectories: n must divide the batch size {self.B}")
         if self.obs_dtype == "uint8" and np.asarray(block["obs"]).dtype != np.uint8:
             raise ValueError(f"a uint8-observation ring takes uint8 obs blocks, got {np.asarray(block['obs']).dtype}")
+        want = (self.T + self.frames, n, self.O // self.frames)
+        if self.frames > 1 and tuple(np.shape(block["obs"])) != want:
+            raise ValueError(f"obs block of shape {tuple(np.shape(block['obs']))}; this ring takes {want}")
         c = self._control()
         end = None if timeout is None else time.monotonic() + timeout
         t_wait = time.monotonic()

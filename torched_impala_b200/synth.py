@@ -27,10 +27,12 @@ PARAM_ALIGN = 32  # floats; every parameter tensor starts on a 128-byte boundary
 
 
 def make_batch(seed: int, T: int, B: int, O: int, A: int, ragged: bool = False,
-               unit_reward: bool = False, done_last: bool = True, obs_kind: str = "normal") -> dict:
+               unit_reward: bool = False, done_last: bool = True, obs_kind: str = "normal", frames: int = 1) -> dict:
     """obs_kind: "normal" - float32 N(0, 1); "bytes" - uint8 0..255 (Atari RAM); "planes" - uint8 0/1
     (MinAtar).  The integer kinds draw from a stream of their own, so every other field equals the
-    "normal" batch of the same seed."""
+    "normal" batch of the same seed.  frames=k > 1: obs are the (T+k, B, O/k) frames of k-frame stacked
+    observations (the layout of impala_batch_layout_frames), drawn from a stream of their own, zero from
+    frame lens[b] + k on; `stack_frames` gives the dense batch."""
     rng = np.random.default_rng(seed)
     obs = rng.standard_normal((T + 1, B, O), dtype=np.float32)
     if obs_kind != "normal":
@@ -69,8 +71,29 @@ def make_batch(seed: int, T: int, B: int, O: int, A: int, ragged: bool = False,
     done[pad] = 0
     pad_obs = np.arange(T + 1)[:, None] > lens[None, :]
     obs[pad_obs] = 0
+    if frames > 1:
+        if O % frames:
+            raise ValueError(f"{O} observation features do not split into {frames} frames")
+        frng = np.random.default_rng(seed + 15485863)
+        shape = (T + frames, B, O // frames)
+        if obs_kind == "normal":
+            obs = frng.standard_normal(shape, dtype=np.float32)
+        elif obs_kind == "bytes":
+            obs = frng.integers(0, 256, shape, dtype=np.uint8)
+        else:
+            obs = (frng.random(shape) < 0.3).astype(np.uint8)
+        obs[np.arange(T + frames)[:, None] >= lens[None, :] + frames] = 0
     return dict(obs=obs, beh_logits=beh, actions=actions, rewards=rewards, done=done,
                 lens=lens)
+
+
+def stack_frames(batch: dict, k: int) -> dict:
+    """A frame batch (obs (T+k, B, F)) as the dense batch (obs (T+1, B, k F)) the frames stand for: row (t, b)
+    is frames t .. t+k-1 of column b, oldest first.  Padded rows past lens[b] keep the frames they share with
+    valid rows, as the device unstacking produces them."""
+    fr = batch["obs"]
+    T1 = fr.shape[0] - k + 1
+    return {**batch, "obs": np.concatenate([fr[j:j + T1] for j in range(k)], axis=-1)}
 
 
 def shard_batch(batch: dict, rank: int, world: int) -> dict:
