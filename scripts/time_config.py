@@ -1,5 +1,5 @@
 """Device-resident learner step time for any BASELINE config (c2..c5) or the Atari-RAM / MinAtar shapes: CUDA events,
-L2 flushed.  --compare-tc also times the FP32 FFMA MLP path (IMPALA_MLP_TC=0) in the same process,
+L2 flushed, with the GPU name, power limit and maximum SM clock read in the same run.  --compare-tc also times the FP32 FFMA MLP path (IMPALA_MLP_TC=0) in the same process,
 alternating step by step with the default path, so both numbers see the same clocks and neighbours.
 --compare-obs alternates a float32-slab engine and a uint8-slab engine (byte observations 0..255) the same way
 and reports, for both, the device-resident step time and the pinned-slab end-to-end step time (the DMA of
@@ -35,7 +35,12 @@ CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256), "c5": dict(T=100, B=8192, O=6
        # MinAtar Breakout / Asterix, flattened 10x10x4 binary grids: P = 207 111 parameters
        "minatar": dict(T=20, B=4096, O=400, A=6, H=256),
        # 8 stacked Atari RAM frames
-       "ram8": dict(T=20, B=4096, O=1024, A=18, H=256)}
+       "ram8": dict(T=20, B=4096, O=1024, A=18, H=256),
+       # minimal Atari action sets (Pong, Space Invaders, Q*bert: 6; Ms. Pac-Man, Enduro, Beam Rider: 9): the
+       # 16-output tensor-core epilogue.  ram_a9h512 has no FP32 arm (that forward refuses H > 256 at O > 64)
+       "ram_a6": dict(T=20, B=4096, O=128, A=6, H=256),
+       "c4a6": dict(T=20, B=4096, O=24, A=6, H=256),
+       "ram_a9h512": dict(T=20, B=4096, O=128, A=9, H=512)}
 ap = argparse.ArgumentParser()
 ap.add_argument("--config", default="c5")
 ap.add_argument("--steps", type=int, default=30)
@@ -137,10 +142,9 @@ if a.compare_frames:  # the unstacking launch alone, back to back
     print(f"impala_obs_unstack {a.config} frames={a.frames} {a.obs_dtype} -> {eng.obs_dense.dtype}: {us:.1f} us, "
           f"{nbytes / 1e6:.1f} MB moved, HBM floor {nbytes / 3.35e12 * 1e6:.1f} us at 3.35 TB/s "
           f"({nbytes / 3.35e12 * 1e6 / us:.0%} of it)")
-if a.compare_obs or a.compare_frames:
-    q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
-                        "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print(f"GPU (nvidia-smi): {q}")
+q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
+                    "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+print(f"GPU (nvidia-smi): {q}")
 for name, eng in engines.items():
     med = statistics.median(ts[name])
     e2e = f", pinned-slab end to end {statistics.median(te[name]):.1f} us/step, slab {eng.slab_bytes / 1e6:.1f} MB" \

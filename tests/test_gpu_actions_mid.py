@@ -1,0 +1,220 @@
+"""GPU: policies with 5..16 actions (Atari minimal action sets: 6 for Pong, 9 for Ms. Pac-Man) on the
+tensor-core MLP kernels.
+
+The forward runs the 16-output epilogue at one, two or four K atoms and the backward the 16-output
+layer-2-through-shared-memory kernel at one or two (at four it keeps the 32-output padded kernel).  Both
+are held to the float64 oracle with every logit written (the output starts as NaN), the launches are
+checked by name in a profiler trace, and the whole learner step - eager engine, byte observations,
+forked Learner behind a RingQueue - is checked at A = 6 and A = 9.
+"""
+import ctypes
+import json
+import os
+import re
+import subprocess
+import sys
+
+import numpy as np
+import pytest
+import torch
+
+from conftest import PKEYS
+from oracle import impala_oracle as orc
+from oracle.check import first_step_parity
+from torched_impala_b200 import _cabi, synth
+from torched_impala_b200.utils import default_hparams
+
+pytestmark = pytest.mark.gpu
+
+ATOL = 1e-5
+SHAPES = [
+    # (M, O, H, N2): four K atoms (the 16-output forward replaces one that wrote 4 logits) ...
+    (20 * 1024, 128, 256, 6), (5000, 100, 512, 9), (5, 128, 128, 16),
+    # ... one K atom, including observation widths the narrow kernels take at <= 4 outputs ...
+    (3001, 24, 256, 6), (60001, 28, 128, 5), (1000, 32, 1024, 8), (4097, 4, 128, 7),
+    # ... and two
+    (777, 64, 512, 16),
+]
+
+
+@pytest.fixture(scope="module")
+def ops():
+    if not torch.cuda.is_available():
+        pytest.fail("GPU test selected but no CUDA device is visible")
+    from torched_impala_b200 import ops as _ops
+
+    return _ops
+
+
+def dev(a):
+    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+
+def _p(t):
+    return ctypes.c_void_p(t.data_ptr())
+
+
+def _st():
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def forward_into_nan(x, params, M, O, H, N2):
+    out = torch.full((M, N2), float("nan"), dtype=torch.float32, device="cuda")
+    _cabi.check(_cabi.lib().impala_mlp_forward(_p(x), _p(params), _p(out), M, O, H, N2, _st()), "impala_mlp_forward")
+    return out
+
+
+def backward_into_nan(x, params, dout, M, O, H, N2):
+    lib = _cabi.lib()
+    nbytes = int(lib.impala_mlp_backward_workspace(M, O, H, N2))
+    assert nbytes > 0, nbytes
+    ws = torch.zeros(nbytes, dtype=torch.uint8, device="cuda")
+    grad = torch.full((_cabi.param_layout(O, H, N2)[1],), float("nan"), dtype=torch.float64, device="cuda")
+    _cabi.check(lib.impala_mlp_backward(_p(x), _p(params), _p(dout), _p(grad), _p(ws), nbytes, M, O, H, N2, _st()),
+                "impala_mlp_backward")
+    return grad
+
+
+@pytest.mark.parametrize("M,O,H,N2", SHAPES)
+def test_forward_matches_oracle(ops, M, O, H, N2):
+    rng = np.random.default_rng(M + O + H + N2)
+    p = synth.init_params(M, O, N2, H)["policy"]
+    x = rng.standard_normal((M, O), dtype=np.float32)
+    want, _ = orc.mlp_forward(x.astype(np.float64), *[p[k].astype(np.float64) for k in PKEYS])
+    got = forward_into_nan(dev(x), ops.pack_params(p), M, O, H, N2).cpu().numpy()
+    assert np.isfinite(got).all(), np.argwhere(~np.isfinite(got))[:4]
+    assert np.abs(got - want).max() < ATOL
+
+
+@pytest.mark.parametrize("M,O,H,N2", SHAPES)
+def test_backward_matches_oracle(ops, M, O, H, N2):
+    """5e-5 of the largest entry; W1 / b1 also get the ReLU-tie allowance of test_gpu_wide_shapes.py (one
+    batch row's contribution, three times)."""
+    rng = np.random.default_rng(7 * M + O + H + N2)
+    p = synth.init_params(M + 1, O, N2, H)["policy"]
+    x = rng.standard_normal((M, O), dtype=np.float32)
+    dout = (rng.standard_normal((M, N2), dtype=np.float32) / M).astype(np.float32)
+    p64 = [p[k].astype(np.float64) for k in PKEYS]
+    _, pre = orc.mlp_forward(x.astype(np.float64), *p64)
+    want = orc.mlp_backward(x.astype(np.float64), pre, p64[2], dout.astype(np.float64))
+    flat = backward_into_nan(dev(x), ops.pack_params(p), dev(dout), M, O, H, N2)
+    assert bool(torch.isfinite(flat).all())
+    got = ops.unpack_grad(flat, O, H, N2)
+    one_row = float(np.abs(dout).max() * np.abs(p[PKEYS[2]]).max() * max(1.0, np.abs(x).max()))
+    for k, w in zip(PKEYS, want):
+        assert got[k].shape == w.shape
+        tol = 5e-5 * np.abs(w).max() + (3 * one_row if k in PKEYS[:2] else 0.0)
+        assert np.abs(got[k] - w).max() < tol, (k, float(np.abs(got[k] - w).max()), float(np.abs(w).max()))
+
+
+def _kernel_names(fn):
+    fn()  # first launches (occupancy queries, shared-memory opt-in) stay out of the trace
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    return {ev.name for ev in prof.events() if ev.device_type == torch.autograd.DeviceType.CUDA}
+
+
+def _has(names, kernel, *targs):
+    """A launch of `kernel<targs>` (demangled or mangled name)."""
+    demangled = re.escape(kernel) + "<" + r",\s*".join(map(str, targs)) + ">"
+    mangled = re.escape(kernel) + "I" + "".join(f"Li{t}E" for t in targs) + "E"
+    return any(re.search(demangled, n) or re.search(mangled, n) for n in names)
+
+
+# O -> (forward, backward) instantiations at A = 6, H = 256
+ROUTES = {24: (("mlp_fwd_tc_kernel", 16, 1), ("mlp_bwd_tcw_kernel", 16, 1)),
+          128: (("mlp_fwd_tc_kernel", 16, 4), ("mlp_bwd_tcw_kernel", 32, 4))}
+
+
+@pytest.mark.parametrize("tensor_cores", ["1", "0"])
+@pytest.mark.parametrize("O", sorted(ROUTES))
+def test_launches_take_the_16_output_kernels(ops, monkeypatch, O, tensor_cores):
+    monkeypatch.setenv("IMPALA_MLP_TC", tensor_cores)
+    M, H, N2 = 4096, 256, 6
+    rng = np.random.default_rng(O)
+    p = ops.pack_params(synth.init_params(1, O, N2, H)["policy"])
+    x = dev(rng.standard_normal((M, O), dtype=np.float32))
+    dout = dev(rng.standard_normal((M, N2), dtype=np.float32))
+    fwd = _kernel_names(lambda: ops.mlp_forward(x, p, O, H, N2))
+    bwd = _kernel_names(lambda: ops.mlp_backward(x, p, dout, O, H, N2))
+    print(O, tensor_cores, sorted(fwd), sorted(bwd))
+    fp32_fwd = any("mlp_fwd_kernel" in n for n in fwd)
+    fp32_bwd = any("mlp_bwd_kernel" in n for n in bwd)
+    if tensor_cores == "1":
+        assert _has(fwd, *ROUTES[O][0]) and not fp32_fwd, fwd
+        assert _has(bwd, *ROUTES[O][1]) and not fp32_bwd, bwd
+    else:
+        assert fp32_fwd and not any("_tc" in n for n in fwd), fwd
+        assert fp32_bwd and not any("_tc" in n for n in bwd), bwd
+
+
+# name: (T, B, O, A, H, ragged)
+CASES = {
+    "ram_a6": (20, 4096, 128, 6, 256, False),
+    "c4a6": (20, 4096, 24, 6, 256, False),
+    "ram_a9h512_ragged_B1024": (20, 1024, 128, 9, 512, True),
+}
+
+
+@pytest.mark.parametrize("name", list(CASES))
+def test_first_step_matches_oracle(ops, name):
+    from test_gpu_wide_shapes import _check_grad_with_relu_ties
+    from torched_impala_b200.engine import LearnerEngine
+
+    T, B, O, A, H, ragged = CASES[name]
+    hp = default_hparams(batch_size=B, max_timesteps=T, policy_hidden_dims=H, value_fn_hidden_dims=H)
+    params = synth.init_params(11, O, A, H)
+    batch = synth.make_batch(17, T, B, O, A, ragged=ragged)
+    eng = LearnerEngine(T, B, O, A, H, H, hp, use_graph=False)
+    par = first_step_parity(eng, params, batch)
+    print(name, json.dumps(par))
+    assert par["max_abs_vs"] < 1e-5, par
+    assert par["max_abs_pg"] < 1e-5, par
+    for k, v in par["scalars"].items():
+        assert v["abs_err"] < 1e-5, (k, v)
+    if par["max_rel_grad"] >= 5e-5:
+        _check_grad_with_relu_ties(eng, params, batch, hp)
+    assert par["max_abs_param_after_1_update"] < 5e-5, par
+    assert par["frac_params_off"] < 1e-3, par
+    for k in ("norm_policy", "norm_value"):
+        assert abs(par[k]["got"] - par[k]["ref"]) < 5e-5 * max(1.0, par[k]["ref"]), par
+
+
+def _run_engine(obs_dtype, T, B, O, A, H, hp, params, batches):
+    from torched_impala_b200.engine import LearnerEngine
+
+    eng = LearnerEngine(T, B, O, A, H, H, hp, use_graph=True, obs_dtype=obs_dtype)
+    eng.load_state(params)
+    scal = []
+    for u in range(4):
+        b = batches[u % 2]
+        eng.fill_host(b if obs_dtype == "uint8" else {**b, "obs": b["obs"].astype(np.float32)}, u % 2)
+        eng.ingest(u % 2)
+        eng.step(u % 2)
+        scal.append(eng.read_scalars())
+    eng.synchronize()
+    return eng.params.clone(), scal
+
+
+def test_byte_observations_equal_float_at_ram_a6(ops):
+    T, B, O, A, H, _ = CASES["ram_a6"]
+    hp = default_hparams(batch_size=B, max_timesteps=T, policy_hidden_dims=H, value_fn_hidden_dims=H)
+    params = synth.init_params(31, O, A, H)
+    batches = [synth.make_batch(50 + i, T, B, O, A, obs_kind="bytes") for i in range(2)]
+    p8, s8 = _run_engine("uint8", T, B, O, A, H, hp, params, batches)
+    pf, sf = _run_engine("float32", T, B, O, A, H, hp, params, batches)
+    assert torch.equal(p8, pf), float((p8 - pf).abs().max())
+    assert s8 == sf
+
+
+def test_learner_process_ring_a6():
+    """MlpPolicy(128, 6, 256) / MlpValueFn(128, 256) in a forked Learner behind a RingQueue: the check of
+    wide_learner_process_check.py (3 updates on ragged trajectories, policy within 5e-5 of the oracle's) at
+    A = 6, in a fresh interpreter (the parent of a forked CUDA process must never have initialised CUDA)."""
+    here = os.path.dirname(os.path.abspath(__file__))
+    code = f"import sys; sys.path.insert(0, {here!r}); import wide_learner_process_check as w; w.A = 6; w.main()"
+    res = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
+    assert res.returncode == 0, res.stdout[-3000:] + res.stderr[-3000:]
+    assert "WIDE_LEARNER_OK" in res.stdout

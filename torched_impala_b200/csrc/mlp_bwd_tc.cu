@@ -90,10 +90,11 @@ __device__ __forceinline__ float f4(const float4& v, int e) { return e == 0 ? v.
 // registers per thread, so a pass holds one 64-feature half of dW1 (two atoms) and the hidden blocks
 // are walked once per half, GEMM1 re-run for each (x is re-read once per pass).  Tiles are 32 batch rows
 // so that W1 hi / lo of 128 hidden units, the tile and its transpose fit in shared memory.
-// NP = 32 (17..32 outputs): layer 2 goes through shared memory - the pass's W2 block [128][NP + 4]
-// (rows padded so the lanes of a quad, two batch rows or hidden units apart, hit different banks) -
-// and dW2 is formed per tile in chunks of 8 outputs, summed over the quad and kept by lane q for
-// outputs [8 q, 8 q + 8).  dW2 / db1 are accumulated in the first feature half only.
+// NP = 16 / 32 (5..16 outputs at one or two K atoms, 17..32 outputs at four): layer 2 goes through shared
+// memory - the pass's W2 block [128][NP + 4] (rows padded so the lanes of a quad, two batch rows or hidden
+// units apart, hit different banks) - and dW2 is formed per tile in chunks of NP / 4 outputs, summed over
+// the quad and kept by lane q for outputs [NP / 4 q, NP / 4 (q + 1)).  dW2 / db1 are accumulated in the
+// first feature half only.
 template <int NP, int KA>
 __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int cta, const int ncta) {
     extern __shared__ uint8_t smem_raw[];
@@ -128,9 +129,11 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
     float* wsb = a.ws + (size_t)cta * a.lay.total;  // this CTA's partial gradient row
 
     // x rows of a tile -> registers (chunk idx = tid + kThreads k is (row idx / (8 KA), 16-byte chunk
-    // idx % (8 KA))); dz row `tid` for tid < RT (L2S: dz row tid / 8, outputs 4 (tid % 8) .. + 3)
+    // idx % (8 KA))); dz row `tid` for tid < RT (L2S: dz row tid / NQ, outputs 4 (tid % NQ) .. + 3)
     constexpr int kLd = RT * 8 * KA / kThreads;
     constexpr int NZ = L2S ? 4 : NP;
+    constexpr int NQ = L2S ? NP / 4 : 1;  // L2S: float4s of a dz row
+    constexpr int CW = L2S ? NP / 4 : 1;  // L2S: outputs of a dW2 chunk (lane q keeps chunk q)
     float4 v[kLd];
     float z[NZ];
     auto load = [&](int tile) {
@@ -143,8 +146,9 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
                 v[k] = __ldg(reinterpret_cast<const float4*>(a.x + (size_t)row * O) + c);
         }
         if constexpr (L2S) {
+            // NP = 32 at RT = 32 (four K atoms) or NP = 16 at RT = 64
             static_assert(RT * NP == 4 * kThreads, "one float4 of dz per thread");
-            const int row = tile * RT + (tid >> 3), n0 = 4 * (tid & 7);
+            const int row = tile * RT + tid / NQ, n0 = 4 * (tid % NQ);
 #pragma unroll
             for (int n = 0; n < 4; ++n)
                 z[n] = (tile < a.num_tiles && row < a.M && n0 + n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n0 + n) : 0.f;
@@ -199,10 +203,10 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
         const int j0 = blk * kHB + 64 * wg + 16 * warp + g, j1 = j0 + 8;
         const float bj0 = __ldg(b1 + j0), bj1 = __ldg(b1 + j1);
         float w2r0[NPR], w2r1[NPR], gw0[NPR], gw1[NPR], gb10 = 0.f, gb11 = 0.f;
-        float gq0[L2S ? 8 : 1], gq1[L2S ? 8 : 1];  // L2S: dW2 of outputs [8 q, 8 q + 8)
+        float gq0[CW], gq1[CW];  // L2S: dW2 of outputs [CW q, CW q + CW)
         if constexpr (L2S) {
 #pragma unroll
-            for (int k = 0; k < 8; ++k) gq0[k] = gq1[k] = 0.f;
+            for (int k = 0; k < CW; ++k) gq0[k] = gq1[k] = 0.f;
         } else {
 #pragma unroll
             for (int n = 0; n < NP; ++n) {
@@ -243,7 +247,7 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
                 }
             }
             if constexpr (L2S) {
-                *reinterpret_cast<float4*>(dzs + (tid >> 3) * NPS + 4 * (tid & 7)) = make_float4(z[0], z[1], z[2], z[3]);
+                *reinterpret_cast<float4*>(dzs + (tid / NQ) * NPS + 4 * (tid % NQ)) = make_float4(z[0], z[1], z[2], z[3]);
                 if (p == 0) {
 #pragma unroll
                     for (int n = 0; n < 4; ++n) gb2[n] += z[n];
@@ -299,13 +303,19 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
             if constexpr (L2S) {
                 const float* w2a = w2s + (64 * wg + 16 * warp + g) * NPS;  // unit j0 of the block
                 const float* w2b = w2a + 8 * NPS;
+                // d <- h in place: h > 0 exactly where the pre-activation is (relu'(0) = 0 as in torch), and
+                // the dW2 chunks read h without holding a second copy of it
+#pragma unroll
+                for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) d[nb][i] = fmaxf(d[nb][i] + ((i & 2) ? bj1 : bj0), 0.f);
                 if (l2) {
-                    // dW2 in chunks of 8 outputs: the quad's partial sums meet, lane q keeps chunk q
+                    // dW2 in chunks of CW outputs: the quad's partial sums meet, lane q keeps chunk q
 #pragma unroll
                     for (int cc = 0; cc < 4; ++cc) {
-                        float s0[8], s1[8];
+                        float s0[CW], s1[CW];
 #pragma unroll
-                        for (int k = 0; k < 8; ++k) s0[k] = s1[k] = 0.f;
+                        for (int k = 0; k < CW; ++k) s0[k] = s1[k] = 0.f;
 #pragma unroll
                         for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
@@ -313,18 +323,19 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
 #pragma unroll
                                 for (int e = 0; e < 2; ++e) {
                                     const int m = 32 * nb + 8 * i + 2 * q + e;
-                                    const float h0 = fmaxf(d[nb][4 * i + e] + bj0, 0.f);
-                                    const float h1 = fmaxf(d[nb][4 * i + 2 + e] + bj1, 0.f);
-                                    const float4 za = *reinterpret_cast<const float4*>(dzs + m * NPS + 8 * cc);
-                                    const float4 zb = *reinterpret_cast<const float4*>(dzs + m * NPS + 8 * cc + 4);
+                                    const float h0 = d[nb][4 * i + e], h1 = d[nb][4 * i + 2 + e];
+                                    float4 zc[CW / 4];
 #pragma unroll
-                                    for (int k = 0; k < 8; ++k) {
-                                        const float zk = k < 4 ? f4(za, k) : f4(zb, k - 4);
+                                    for (int u = 0; u < CW / 4; ++u)
+                                        zc[u] = *reinterpret_cast<const float4*>(dzs + m * NPS + CW * cc + 4 * u);
+#pragma unroll
+                                    for (int k = 0; k < CW; ++k) {
+                                        const float zk = f4(zc[k >> 2], k & 3);
                                         s0[k] = fmaf(zk, h0, s0[k]), s1[k] = fmaf(zk, h1, s1[k]);
                                     }
                                 }
 #pragma unroll
-                        for (int k = 0; k < 8; ++k) {
+                        for (int k = 0; k < CW; ++k) {
                             s0[k] += __shfl_xor_sync(IMPALA_FULL_MASK, s0[k], 1);
                             s1[k] += __shfl_xor_sync(IMPALA_FULL_MASK, s1[k], 1);
                             s0[k] += __shfl_xor_sync(IMPALA_FULL_MASK, s0[k], 2);
@@ -332,7 +343,7 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
                         }
                         if (q == cc) {
 #pragma unroll
-                            for (int k = 0; k < 8; ++k) gq0[k] += s0[k], gq1[k] += s1[k];
+                            for (int k = 0; k < CW; ++k) gq0[k] += s0[k], gq1[k] += s1[k];
                         }
                     }
                 }
@@ -343,7 +354,7 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int m = 32 * nb + 8 * i + 2 * q + e;
-                            const float pre0 = d[nb][4 * i + e] + bj0, pre1 = d[nb][4 * i + 2 + e] + bj1;
+                            const float h0 = d[nb][4 * i + e], h1 = d[nb][4 * i + 2 + e];
                             float dh0 = 0.f, dh1 = 0.f;
 #pragma unroll
                             for (int n = 0; n < NP; n += 4) {
@@ -355,7 +366,7 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
                                 dh1 = fmaf(zv.x, wb.x, dh1), dh1 = fmaf(zv.y, wb.y, dh1);
                                 dh1 = fmaf(zv.z, wb.z, dh1), dh1 = fmaf(zv.w, wb.w, dh1);
                             }
-                            const float dp0 = pre0 > 0.f ? dh0 : 0.f, dp1 = pre1 > 0.f ? dh1 : 0.f;
+                            const float dp0 = h0 > 0.f ? dh0 : 0.f, dp1 = h1 > 0.f ? dh1 : 0.f;
                             gb10 += dp0, gb11 += dp1;
                             d[nb][4 * i + e] = dp0, d[nb][4 * i + 2 + e] = dp1;
                         }
@@ -465,8 +476,8 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
             }
             if constexpr (L2S) {
 #pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const int n = 8 * q + k;
+                for (int k = 0; k < CW; ++k) {
+                    const int n = CW * q + k;
                     if (n < a.N2) wsb[a.lay.oW2 + (size_t)n * H + j0] = gq0[k], wsb[a.lay.oW2 + (size_t)n * H + j1] = gq1[k];
                 }
             }
@@ -487,14 +498,14 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
     }
 
     if constexpr (L2S) {
-        // db2: thread t holds outputs 4 (t % 8) .. + 3 of rows t / 8 (+ 32 k); lanes l, l ^ 8, l ^ 16, l ^ 24
-        // hold the same outputs, then the 8 warps meet through shared memory (fixed order)
+        // db2: thread t holds outputs 4 (t % NQ) .. + 3 of rows t / NQ (+ RT k); the lanes l ^ NQ,
+        // l ^ 2 NQ, ... hold the same outputs, then the 8 warps meet through shared memory (fixed order)
 #pragma unroll
         for (int n = 0; n < 4; ++n) {
-            gb2[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gb2[n], 8);
-            gb2[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gb2[n], 16);
+#pragma unroll
+            for (int off = NQ; off < 32; off <<= 1) gb2[n] += __shfl_xor_sync(IMPALA_FULL_MASK, gb2[n], off);
         }
-        if (lane < 8) {
+        if (lane < NQ) {
 #pragma unroll
             for (int n = 0; n < 4; ++n) gb2x[(tid >> 5) * 32 + 4 * lane + n] = gb2[n];
         }
@@ -1054,9 +1065,10 @@ int impala_mlp_bwd_tcw(const float* x, const float* params, const float* dout, f
                        int N2, cudaStream_t st, int* nparts) {
     const BwdTcArgs a = make_bwd_args(x, params, dout, ws, nullptr, nullptr, M, O, H, N2);
     const int ka = O <= 32 ? 1 : 2;
-    const size_t smem = bwd_smem_bytes(ka, N2 == 1 ? 1 : 4);
-    auto kernel = ka == 1 ? (N2 == 1 ? mlp_bwd_tcw_kernel<1, 1> : mlp_bwd_tcw_kernel<4, 1>)
-                          : (N2 == 1 ? mlp_bwd_tcw_kernel<1, 2> : mlp_bwd_tcw_kernel<4, 2>);
+    const int np = N2 == 1 ? 1 : (N2 <= 4 ? 4 : 16);
+    const size_t smem = bwd_smem_bytes(ka, np);
+    auto kernel = ka == 1 ? (np == 1 ? mlp_bwd_tcw_kernel<1, 1> : np == 4 ? mlp_bwd_tcw_kernel<4, 1> : mlp_bwd_tcw_kernel<16, 1>)
+                          : (np == 1 ? mlp_bwd_tcw_kernel<1, 2> : np == 4 ? mlp_bwd_tcw_kernel<4, 2> : mlp_bwd_tcw_kernel<16, 2>);
     cudaError_t e;
     int sms = 0, per_sm = 0;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
@@ -1072,7 +1084,7 @@ int impala_mlp_bwd_tcw(const float* x, const float* params, const float* dout, f
 }
 
 // Beyond the wide kernels' limits (impala_mlp_bwd_tcx_eligible): four K atoms, GEMM2 in 64-feature halves,
-// 32-row tiles; 17..32 outputs through shared memory.  Partial rows as impala_mlp_bwd_tcw.
+// 32-row tiles; 5..32 outputs through shared memory, padded to 32.  Partial rows as impala_mlp_bwd_tcw.
 bool impala_mlp_bwd_tcx_eligible(const float* x, int M, int O, int H, int N2) {
     return M >= 1 && O >= 4 && O <= 128 && (O & 3) == 0 && H >= 128 && H % 128 == 0 && H <= 4096 && N2 >= 1 &&
            N2 <= 32 && (O > 64 || N2 > 16) && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&

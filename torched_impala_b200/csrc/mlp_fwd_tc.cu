@@ -429,17 +429,20 @@ int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* 
 }
 
 // Wide shapes (observation width up to 64 = two K atoms, hidden layers a multiple of 128 of any
-// size, walked in passes): BASELINE config c5 (obs = 64, hidden = 512).  IMPALA_MLP_TCW=0 disables.
+// size, walked in passes, up to 16 outputs): BASELINE config c5 (obs = 64, hidden = 512), and policies
+// with an Atari minimal action set (5..16 actions; epilogue padded to 16 outputs).  IMPALA_MLP_TCW=0
+// disables.
 bool impala_mlp_tcw_eligible(const float* x, int M, int O, int H, int N2) {
     return M >= 1 && O >= 4 && O <= 64 && (O & 3) == 0 && H >= 128 && H % 128 == 0 && H <= 4096 && N2 >= 1 &&
-           N2 <= 4 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && impala_env_int("IMPALA_MLP_TCW", 1) != 0;
+           N2 <= 16 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && impala_env_int("IMPALA_MLP_TCW", 1) != 0;
 }
 
 int impala_mlp_fwd_tcw(const float* x, const float* params, float* out, int M, int O, int H, int N2,
                        cudaStream_t st) {
+    // 256 hidden units per pass fit at 16 outputs too: 88 064 B at one K atom, 219 136 B at two
     const FwdTcArgs a = make_fwd_args(x, params, out, M, O, H, N2);
-    if (O <= 32) return N2 == 1 ? launch_fwd<1, 1>(a, st) : launch_fwd<4, 1>(a, st);
-    return N2 == 1 ? launch_fwd<1, 2>(a, st) : launch_fwd<4, 2>(a, st);
+    if (O <= 32) return N2 == 1 ? launch_fwd<1, 1>(a, st) : N2 <= 4 ? launch_fwd<4, 1>(a, st) : launch_fwd<16, 1>(a, st);
+    return N2 == 1 ? launch_fwd<1, 2>(a, st) : N2 <= 4 ? launch_fwd<4, 2>(a, st) : launch_fwd<16, 2>(a, st);
 }
 
 // Beyond the wide kernels' limits: observations up to 128 (four K atoms) or 17..32 outputs (the
@@ -463,5 +466,6 @@ int impala_mlp_fwd_tcx(const float* x, const float* params, float* out, int M, i
     // four K atoms: 64 hidden units per pass keep W1 hi / lo + both warpgroups' x stages in 227 KB
     a.hb = 64;
     if (N2 > 16) return launch_fwd<32, 4>(a, st);
+    if (N2 > 4) return launch_fwd<16, 4>(a, st);
     return N2 == 1 ? launch_fwd<1, 4>(a, st) : launch_fwd<4, 4>(a, st);
 }

@@ -17,8 +17,8 @@ struct FwdTcArgs {
     MlpLayout lay;
 };
 
-// W2 rows in shared memory are padded to NP + 4 at NP = 32: the lanes of a quad read hidden units two
-// apart, and with 128-byte rows their 16-byte loads would fall into one bank group
+// W2 rows in shared memory are padded to NP + 4 at NP = 16 and 32: the lanes of a quad read hidden units
+// two apart, and with 64- or 128-byte rows their 16-byte loads would fall into one bank group
 __host__ __device__ constexpr int w2s_stride(int np) { return np > 4 ? np + 4 : np; }
 
 // Epilogue of the 32-unit slices nc, nc + 1, ... held in one accumulator (16 registers per slice: an

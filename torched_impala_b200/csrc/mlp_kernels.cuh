@@ -52,7 +52,7 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
                            const double* extra = nullptr, int n_extra = 0);
 
 // Wide tensor-core kernels (forward in mlp_fwd_tc.cu, backward in mlp_bwd_tc.cu): O <= 64, H a multiple
-// of 128 (BASELINE c5: O = 64, H = 512).  The forward needs no workspace; the backward leaves *nparts float32 partial rows in ws for
+// of 128, N2 <= 16 (BASELINE c5: O = 64, H = 512).  The forward needs no workspace; the backward leaves *nparts float32 partial rows in ws for
 // reduce_partials_kernel.  IMPALA_MLP_TCW=0 disables them.
 bool impala_mlp_tcw_eligible(const float* x, int M, int O, int H, int N2);
 int impala_mlp_fwd_tcw(const float* x, const float* params, float* out, int M, int O, int H, int N2,
@@ -61,7 +61,8 @@ int impala_mlp_bwd_tcw(const float* x, const float* params, const float* dout, f
                        int N2, cudaStream_t st, int* nparts);
 
 // Wide tensor-core forward of the shapes beyond the limits above (O in 65..128 = four K atoms, or N2 in
-// 17..32): O % 4 == 0, H a multiple of 128 up to 4096.  IMPALA_MLP_TCW=0 disables them too.
+// 17..32; O in 65..128 takes N2 in 5..16 as well): O % 4 == 0, H a multiple of 128 up to 4096.
+// IMPALA_MLP_TCW=0 disables them too.
 bool impala_mlp_fwd_tcx_eligible(const float* x, int M, int O, int H, int N2);
 int impala_mlp_fwd_tcx(const float* x, const float* params, float* out, int M, int O, int H, int N2,
                        cudaStream_t st);
