@@ -199,6 +199,26 @@ int impala_vtrace_loss(const float* cur_logits, const float* beh_logits, const i
                        float policy_loss_c, float entropy_c, float inv_batch, int mode,
                        void* stream);
 
+/* Workspace of impala_vtrace_loss_diag (same zero-once rule; larger than impala_vtrace_loss's). */
+int64_t impala_vtrace_loss_diag_workspace(int T, int B, int A);
+
+/* impala_vtrace_loss (bit-identical vs, pg_adv, dlogits, dv and scalars) plus the off-policy
+ * diagnostics of the batch: diag[0..8) (float64, overwritten) are sums over the valid steps
+ * (t < lens[b]), NOT scaled by inv_batch, so they add across ranks:
+ *   [0] n, the number of valid steps       [1] sum log pi(a_t) - log mu(a_t)  (natural log)
+ *   [2] #{ratio_t > rho_bar}               [3] #{ratio_t > c_bar}
+ *   [4] sum KL(mu_t || pi_t)               [5] sum vs_t
+ *   [6] sum vs_t^2                         [7] sum (vs_t - v_t)
+ * pi = softmax(cur_logits), mu = softmax(beh_logits), ratio_t = pi(a_t) / mu(a_t), vs_t the value
+ * written to vs.  Combined in a fixed order like the scalars (bitwise reproducible). */
+int impala_vtrace_loss_diag(const float* cur_logits, const float* beh_logits, const int32_t* actions,
+                            const float* rewards, const uint8_t* done, const int32_t* lens,
+                            const float* v, float* vs, float* pg_adv, float* dlogits, float* dv,
+                            double* scalars, double* diag, void* workspace, int64_t workspace_bytes,
+                            int T, int B, int A, float gamma, float rho_bar, float c_bar,
+                            float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch,
+                            int mode, void* stream);
+
 /* Per-group gradient clipping + Adam in one launch (learner.py:176-183).
  *   params/m/v: f32 [n_total]; grad: f64 [n_total] (the possibly all-reduced sum);
  *   group 0 = [0, n_policy) (policy net), group 1 = [n_policy, n_total) (value net);

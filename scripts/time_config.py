@@ -7,7 +7,10 @@ slab i+1 runs under step i; a step's window also waits for that DMA), with the G
 maximum SM clock read in the same run.
 --compare-frames alternates the dense engine and a frame engine (--frames k stacked frames stored once per frame,
 --obs-dtype) on the same values the same way, and times the unstacking launch alone (median of 200 launches,
-L2 flushed before each) against its HBM floor (frame bytes read + dense bytes written at 3.35 TB/s)."""
+L2 flushed before each) against its HBM floor (frame bytes read + dense bytes written at 3.35 TB/s).
+--compare-diag alternates a diagnostics=False and a diagnostics=True engine on the same batch the same way, and
+times impala_vtrace_loss against impala_vtrace_loss_diag alone on the engine's buffers (median of 200 launches
+each, alternating, L2 flushed before each)."""
 import argparse
 import os
 import statistics
@@ -49,6 +52,7 @@ ap.add_argument("--compare-obs", action="store_true", help="alternate float32 an
 ap.add_argument("--compare-frames", action="store_true", help="alternate dense and frame-stacked observation slabs")
 ap.add_argument("--frames", type=int, default=4, help="stacked frames of --compare-frames")
 ap.add_argument("--obs-dtype", default="float32", choices=["float32", "uint8"], help="slab obs type of --compare-frames")
+ap.add_argument("--compare-diag", action="store_true", help="alternate engines without / with off-policy diagnostics")
 a = ap.parse_args()
 w = CFG[a.config]
 hp = default_hparams(batch_size=w["B"], max_timesteps=w["T"])
@@ -60,6 +64,12 @@ if a.compare_obs:
     arms = {"obs float32": arms["default"], "obs uint8": arms["default"]}
     obs_dt = {"obs float32": "float32", "obs uint8": "uint8"}
 n_frames = {}
+diag_arm = {}
+if a.compare_diag:
+    arms = {"diagnostics off": arms["default"], "diagnostics on": arms["default"]}
+    diag_arm = {"diagnostics on": True}
+    # byte observations where the flagship users of the shape have them (Atari RAM, MinAtar)
+    obs_dt = {name: "uint8" if a.config in ("ram", "ram4", "ram8", "minatar", "ram_a6") else "float32" for name in arms}
 if a.compare_frames:
     arms = {f"dense {a.obs_dtype}": arms["default"], f"frames={a.frames} {a.obs_dtype}": arms["default"]}
     obs_dt = {name: a.obs_dtype for name in arms}
@@ -69,9 +79,10 @@ for name, tc in arms.items():
     os.environ["IMPALA_MLP_TC"] = tc  # read by the C library at every launch (and at graph capture)
     dt = obs_dt.get(name, "float32")
     k = n_frames.get(name, 1)
-    eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k)
+    eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k,
+                        diagnostics=diag_arm.get(name, False))
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
-    byte_obs = a.compare_obs or (a.compare_frames and dt == "uint8")
+    byte_obs = a.compare_obs or (a.compare_frames and dt == "uint8") or (a.compare_diag and dt == "uint8")
     if a.compare_frames:  # the same observation values in both arms: the dense arm gets the stacked frames
         batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if byte_obs else "normal",
                                  frames=a.frames)
@@ -142,6 +153,41 @@ if a.compare_frames:  # the unstacking launch alone, back to back
     print(f"impala_obs_unstack {a.config} frames={a.frames} {a.obs_dtype} -> {eng.obs_dense.dtype}: {us:.1f} us, "
           f"{nbytes / 1e6:.1f} MB moved, HBM floor {nbytes / 3.35e12 * 1e6:.1f} us at 3.35 TB/s "
           f"({nbytes / 3.35e12 * 1e6 / us:.0%} of it)")
+if a.compare_diag:  # the V-trace + loss kernel alone, plain and diag entry points alternating
+    import ctypes
+
+    eng = engines["diagnostics on"]
+    d = eng.d_views[0]
+    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    ins = (P(eng.logits), P(d["beh_logits"]), P(d["actions"]), P(d["rewards"]), P(d["done"]), P(d["lens"]),
+           P(eng.values), P(eng.vs), P(eng.pg_adv), P(eng.dlogits), P(eng.dv))
+    scal = ctypes.c_void_p(eng.comm.data_ptr() + 8 * eng.n_total)
+    diag = ctypes.c_void_p(eng.comm.data_ptr() + 8 * (eng.n_total + 4))
+    ws_plain = torch.zeros(int(eng.lib.impala_vtrace_loss_workspace(w["T"], w["B"], w["A"])), dtype=torch.uint8,
+                           device="cuda")
+    tail = (w["T"], w["B"], w["A"], hp.gamma, hp.rho_bar, hp.c_bar, hp.v_loss_c, hp.policy_loss_c, hp.entropy_c,
+            1.0 / w["B"], 0)
+    calls = {"impala_vtrace_loss": lambda st: eng.lib.impala_vtrace_loss(*ins, scal, P(ws_plain), ws_plain.numel(),
+                                                                        *tail, st),
+             "impala_vtrace_loss_diag": lambda st: eng.lib.impala_vtrace_loss_diag(*ins, scal, diag, P(eng.ws_vt),
+                                                                                  eng.ws_vt_bytes, *tail, st)}
+    tk = {name: [] for name in calls}
+    with torch.cuda.stream(eng.stream):
+        st = ctypes.c_void_p(eng.stream.cuda_stream)
+        for i in range(220):
+            for name, fn in calls.items():
+                flush.zero_()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(eng.stream)
+                rc = fn(st)
+                e1.record(eng.stream)
+                e1.synchronize()
+                assert rc == 0, (name, rc)
+                if i >= 20:
+                    tk[name].append(e0.elapsed_time(e1) * 1e3)
+    k0, k1 = statistics.median(tk["impala_vtrace_loss"]), statistics.median(tk["impala_vtrace_loss_diag"])
+    print(f"V-trace + loss kernel {a.config}: impala_vtrace_loss {k0:.1f} us, impala_vtrace_loss_diag {k1:.1f} us "
+          f"(+{k1 - k0:.1f} us, {100 * (k1 / k0 - 1):+.1f} %)")
 q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
                     "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 print(f"GPU (nvidia-smi): {q}")
@@ -151,3 +197,9 @@ for name, eng in engines.items():
         if te[name] else ""
     print(f"{a.config} {w} [{name}] on {dev}: median {med:.1f} us/step ({1e6 / med:.0f} steps/s){e2e}, "
           f"loss {eng.read_scalars()['total_loss']:.5f}")
+if a.compare_diag:
+    m0, m1 = statistics.median(ts["diagnostics off"]), statistics.median(ts["diagnostics on"])
+    sc = engines["diagnostics on"].read_scalars()
+    print(f"diagnostics overhead {a.config}: {m1 - m0:+.1f} us/step ({100 * (m1 / m0 - 1):+.1f} %); "
+          f"rho clipped {100 * sc['rho_clip_fraction']:.1f} %, kl {sc['kl_behaviour_current']:.4f}, "
+          f"explained variance {sc['value_explained_variance']:.4f}")

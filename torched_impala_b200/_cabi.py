@@ -67,6 +67,8 @@ SIGNATURES = {
     "impala_vtrace": (_i, [_p] * 9 + [_i, _i, _i, _f, _f, _f, _i, _p]),
     "impala_vtrace_loss_workspace": (_i64, [_i, _i, _i]),
     "impala_vtrace_loss": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p]),
+    "impala_vtrace_loss_diag_workspace": (_i64, [_i, _i, _i]),
+    "impala_vtrace_loss_diag": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p]),
     "impala_clip_adam": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _f, _f, _f, _f, _p, _p]),
     "impala_policy_terms": (_i, [_p, _p, _p, _p, _i, _i, _p]),
     "impala_policy_terms_backward": (_i, [_p, _p, _p, _p, _p, _i, _i, _p]),

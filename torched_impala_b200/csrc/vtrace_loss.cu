@@ -21,6 +21,7 @@
 #include <math.h>
 
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -65,11 +66,18 @@ struct VtArgs {
     float* dlogits;
     float* dv;
     double* scalars;
-    double* partials;        // [gridDim.x][4] per-CTA loss sums (workspace)
+    double* partials;        // [gridDim.x][4] per-CTA loss sums ([12] with the off-policy sums; workspace)
     unsigned int* counter;   // CTA arrival counter (workspace; zero on entry, zero on exit)
     int T, B, A, mode;
     float gamma, rho_bar, c_bar, v_loss_c, policy_loss_c, entropy_c, inv_batch;
 };
+// DIAG instantiations take the off-policy sums' destination as well (the others keep VtArgs, so their
+// parameter block and code are those of the plain loss kernel).
+struct VtDiagArgs : VtArgs {
+    double* diag;  // [8] sums over the valid steps, see impala_vtrace_loss_diag
+};
+template <bool DIAG>
+using VtArgsT = typename std::conditional<DIAG, VtDiagArgs, VtArgs>::type;
 
 // Row loads / stores of the (T, B, A) logits: lane = trajectory, so a warp reads 32 * A consecutive
 // floats of a time step.  VEC (A == AP, 16-byte aligned bases): one 128-bit (A = 4), one 64-bit
@@ -129,6 +137,26 @@ __device__ __forceinline__ void row_lse2(const float* __restrict__ p, unsigned e
     *shift = sh, *lse2 = lg2f(se), *za = z_a;
 }
 
+// KL(mu || pi) / ln 2 of one streaming row pair (VEC rows), from the shifts and log-sum-exps row_lse2 returned:
+// both rows are read again four logits at a time (L1 / L2 hits), so no whole row is held.
+template <int AP>
+__device__ __forceinline__ float row_kl2(const float* __restrict__ pc, const float* __restrict__ pb, unsigned elem,
+                                         float shc, float lsec, float shb, float lseb) {
+    float kl = 0.f;
+#pragma unroll
+    for (int k = 0; k < AP; k += 4) {
+        const float4 qc = __ldg(reinterpret_cast<const float4*>(pc + elem * AP + k));
+        const float4 qb = __ldg(reinterpret_cast<const float4*>(pb + elem * AP + k));
+        const float zc[4] = {qc.x, qc.y, qc.z, qc.w}, zb[4] = {qb.x, qb.y, qb.z, qb.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float lpi = fmaf(zc[j], kLog2e, shc) - lsec, lmu = fmaf(zb[j], kLog2e, shb) - lseb;
+            kl = fmaf(ex2f(lmu), lmu - lpi, kl);
+        }
+    }
+    return kl;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Lane = trajectory, warp = time segment.
 //
@@ -152,15 +180,30 @@ __device__ __forceinline__ void row_lse2(const float* __restrict__ p, unsigned e
 // of both logit vectors would be ~130 registers on their own); step 2 reduces each row as it loads
 // (row_lse2) and keeps the two taken-action logits, and step 4 re-reads the current row (an L1 / L2
 // hit) for the entropy and the logit gradient.
+//
+// DIAG (with WITH_LOSS): also the eight off-policy sums of impala_vtrace_loss_diag.  Each thread keeps
+// them as seven float32 registers for the whole unroll (at most ceil(T / (S nseg)) S steps per thread:
+// 2 at T = 20, 16 at T = 100 for the default shapes) and converts to float64 only in the final
+// reduction, next to the loss sums (the loss scalars keep the plain kernel's combination order, so they
+// are bit-identical to it); the count of valid steps is sum_b lens[b], added by segment 0.
+// Seven floats rather than float64 accumulators (14 registers) or float64 folds per chunk keeps the
+// register budget of the plain kernel.  The log-ratio sum and the clip counts come from step 2, KL
+// from step 2 as well: on the register path from the behaviour row's 2^zb terms already summed for its
+// log-sum-exp (KL / ln 2 = sum_k 2^zb_k (zb_k - zc_k) / sum_k 2^zb_k + lse - lseb, both rows shifted by
+// their maximum); on the streaming path VEC rows re-read both rows four logits at a time right after
+// row_lse2 reduced them (row_kl2), non-VEC rows re-read the behaviour row in step 4 next to the current
+// row's re-read (whichever keeps the twin's zero spills); vs and vs - v come from step 4.
 // ------------------------------------------------------------------------------------------------
-template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool VEC>
-__global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a) {
+template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool VEC, bool DIAG>
+__global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<DIAG> a) {
     constexpr bool STREAM = AP > 16;
     constexpr int SR = STREAM ? 1 : S, AR = STREAM ? 1 : AP;  // extent of the held logit rows
     static_assert(!STREAM || S == 1, "the streaming rows keep one step per thread");
+    static_assert(!DIAG || WITH_LOSS, "the off-policy sums ride the loss reduction");
+    constexpr int NV = DIAG ? 12 : 4;  // per-CTA sums: 4 loss sums (+ 8 off-policy sums)
     __shared__ float2 s_map[2][kMaxSeg][32];
     __shared__ float2 s_cta[2][32];  // this CTA's segments composed into one map (read by the cluster)
-    __shared__ double s_red[kMaxSeg][4];
+    __shared__ double s_red[kMaxSeg][NV];
     pdl_wait();  // logits / values come from the forward kernel
     // Long unrolls: the time segments of a trajectory group are spread over a thread-block CLUSTER
     // (csize CTAs x nw warps x S steps per chunk - T = 100 fits ONE chunk of 8 x 7 x 2 steps), so a
@@ -181,6 +224,8 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
     const bool ref_mode = a.mode == IMPALA_MODE_REFERENCE;
 
     double sum_vl = 0.0, sum_pl = 0.0, sum_ent = 0.0, sum_rw = 0.0;
+    // DIAG: sum of log2 ratio, #ratio > rho_bar, #ratio > c_bar, sum KL / ln 2, sum vs, sum vs^2, sum (vs - v)
+    float d_lr = 0.f, d_nrho = 0.f, d_nc = 0.f, d_kl = 0.f, d_vs = 0.f, d_vs2 = 0.f, d_err = 0.f;
     float chunk_carry = 0.f;  // accumulator at the first step after the current chunk
     // One chunk's raw rows of this thread (registers).  Unpredicated loads: steps past the unroll
     // (last chunk only) re-read step T - 1 and dead lanes read trajectory B - 1; both are masked
@@ -222,20 +267,33 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
                 row_lse2<AP, VEC>(a.cur_logits, e, A, R.act[i], &shc[i], &lsec[i], &z_a);
                 row_lse2<AP, VEC>(a.beh_logits, e, A, R.act[i], &shb, &lseb, &zb_a);
                 lse = lsec[i];
+                if constexpr (DIAG && VEC) {
+                    if (valid) d_kl += row_kl2<AP>(a.cur_logits, a.beh_logits, e, shc[i], lsec[i], shb, lseb);
+                } else if constexpr (DIAG) {
+                    // non-VEC rows: KL in step 4 next to the current row's re-read (row_kl2 here spills); the
+                    // behaviour row's shift and lse2 are parked in the row slots the streaming path leaves unused
+                    R.zb[i][0] = shb, R.zc[i][0] = lseb;
+                }
             } else {
                 float mx = R.zc[i][0], mxb = R.zb[i][0];
 #pragma unroll
                 for (int k = 1; k < AP; ++k)
                     if (k < A) mx = fmaxf(mx, R.zc[i][k]), mxb = fmaxf(mxb, R.zb[i][k]);
-                float se = 0.f, seb = 0.f;
+                float se = 0.f, seb = 0.f, klw = 0.f;  // DIAG: klw = sum_k 2^zb_k (zb_k - zc_k), shifted rows
                 const float mxl = -mx * kLog2e, mxbl = -mxb * kLog2e;
 #pragma unroll
                 for (int k = 0; k < AP; ++k) {
                     R.zc[i][k] = fmaf(R.zc[i][k], kLog2e, mxl);   // (z - max) log2(e), one rounding
                     R.zb[i][k] = fmaf(R.zb[i][k], kLog2e, mxbl);
                     if (k < A) se += ex2f(R.zc[i][k]), seb += ex2f(R.zb[i][k]);
+                    if constexpr (DIAG) {
+                        if (k < A) klw = fmaf(ex2f(R.zb[i][k]), R.zb[i][k] - R.zc[i][k], klw);  // same ex2 as seb's
+                    }
                 }
                 lse = lg2f(se), lseb = lg2f(seb);
+                if constexpr (DIAG) {
+                    if (valid) d_kl += __fdividef(klw, seb) + (lse - lseb);  // KL(mu || pi) / ln 2
+                }
                 z_a = R.zc[i][0], zb_a = R.zb[i][0];
 #pragma unroll
                 for (int k = 1; k < AP; ++k) {
@@ -249,6 +307,13 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
             const float ratio = ex2f(lp2a[i] - (zb_a - lseb));                 // :121-123
             rho[i] = valid ? fminf(ratio, a.rho_bar) : 0.f;                    // :124
             const float cc = valid ? fminf(ratio, a.c_bar) : 0.f;              // :125
+            if constexpr (DIAG) {
+                if (valid) {
+                    d_lr += lp2a[i] - (zb_a - lseb);
+                    d_nrho += ratio > a.rho_bar ? 1.f : 0.f;
+                    d_nc += ratio > a.c_bar ? 1.f : 0.f;
+                }
+            }
             disc[i] = (valid && R.dn[i] == 0) ? a.gamma : 0.f;                       // :109
             g[i] = disc[i] * cc;
             if (ref_mode) {
@@ -324,6 +389,20 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
                         dz[k] = fmaf(dz[k], kLog2e, shc[i]) - lsec[i];
                         if (k < A) ent -= ex2f(dz[k]) * (dz[k] * kLn2);
                     }
+                    if constexpr (DIAG && !VEC) {
+                        // KL(mu || pi) / ln 2 against the log2 pi(k) in dz: the behaviour row again
+                        if (valid) {
+                            const unsigned eb = (unsigned)t * (unsigned)B + (unsigned)bl;
+                            float kl = 0.f;
+#pragma unroll
+                            for (int k = 0; k < AP; ++k) {
+                                const float zb = k < A ? __ldg(a.beh_logits + eb * A + k) : 0.f;
+                                const float lmu = fmaf(zb, kLog2e, R.zb[i][0]) - R.zc[i][0];  // log2 mu(k)
+                                if (k < A) kl = fmaf(ex2f(lmu), lmu - dz[k], kl);
+                            }
+                            d_kl += kl;
+                        }
+                    }
 #pragma unroll
                     for (int k = 0; k < AP; ++k) {
                         const float lz = dz[k] * kLn2, pk = (k < A) ? ex2f(dz[k]) : 0.f;
@@ -358,6 +437,10 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
                     sum_pl += (double)(-(lp2a[i] * kLn2) * pg);                // :317-321
                     sum_ent += (double)ent;
                     sum_rw += (double)R.r[i];                                    // :108
+                    if constexpr (DIAG) {
+                        const float vs_t = acc[i] + R.vv[i];  // the value written to vs
+                        d_vs += vs_t, d_vs2 = fmaf(vs_t, vs_t, d_vs2), d_err += acc[i];
+                    }
                 }
             }
         }
@@ -384,18 +467,28 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
         // per-CTA sums -> workspace; the last CTA to arrive adds them up in a fixed order
         // (bitwise reproducible, no float64 atomics, no memset node) and re-arms the counter.
         __shared__ bool s_last;
-        __shared__ double s_fin[32][4];
+        __shared__ double s_fin[32][NV];
         const int tid = threadIdx.x;
         sum_vl = warp_sum_f64(sum_vl);
         sum_pl = warp_sum_f64(sum_pl);
         sum_ent = warp_sum_f64(sum_ent);
         sum_rw = warp_sum_f64(sum_rw);
         if (lane == 0) s_red[w][0] = sum_vl, s_red[w][1] = sum_pl, s_red[w][2] = sum_ent, s_red[w][3] = sum_rw;
+        if constexpr (DIAG) {
+            constexpr double kLn2d = 0.6931471805599453;
+            double dg[8] = {seg == 0 ? (double)L : 0.0, (double)d_lr * kLn2d, (double)d_nrho, (double)d_nc,
+                            (double)d_kl * kLn2d, (double)d_vs, (double)d_vs2, (double)d_err};
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                dg[j] = warp_sum_f64(dg[j]);
+                if (lane == 0) s_red[w][4 + j] = dg[j];
+            }
+        }
         __syncthreads();
-        if (tid < 4) {
+        if (tid < NV) {
             double s = 0.0;
             for (int i = 0; i < nw; ++i) s += s_red[i][tid];
-            a.partials[(size_t)blockIdx.x * 4 + tid] = s;
+            a.partials[(size_t)blockIdx.x * NV + tid] = s;
             __threadfence();
         }
         __syncthreads();
@@ -406,18 +499,34 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgs a)
             const int nthr = (int)blockDim.x, which = tid & 3, stripe = tid >> 2, nstripes = nthr >> 2;
             double s = 0.0;
             for (unsigned cta = stripe; cta < gridDim.x; cta += nstripes)
-                s += __ldcg(a.partials + (size_t)cta * 4 + which);
+                s += __ldcg(a.partials + (size_t)cta * NV + which);
             // fixed-order tree over the stripes of each scalar: lanes {which, which + 4, ...} of a warp,
             // then the warps through shared memory
             s += __shfl_xor_sync(IMPALA_FULL_MASK, s, 4);
             s += __shfl_xor_sync(IMPALA_FULL_MASK, s, 8);
             s += __shfl_xor_sync(IMPALA_FULL_MASK, s, 16);
             if (lane < 4) s_fin[w][lane] = s;
+            if constexpr (DIAG) {
+                // the eight off-policy sums by the same scheme over stripes of 8 (the loss scalars above keep
+                // exactly the plain kernel's order, so they stay bit-identical to it)
+                const int wd = tid & 7, sd = tid >> 3, nsd = nthr >> 3;
+                double q = 0.0;
+                for (unsigned cta = sd; cta < gridDim.x; cta += nsd)
+                    q += __ldcg(a.partials + (size_t)cta * NV + 4 + wd);
+                q += __shfl_xor_sync(IMPALA_FULL_MASK, q, 8);
+                q += __shfl_xor_sync(IMPALA_FULL_MASK, q, 16);
+                if (lane < 8) s_fin[w][4 + lane] = q;
+            }
             __syncthreads();
-            if (tid < 4) {
+            if (tid < NV) {
                 double tot = 0.0;
                 for (int i = 0; i < nw; ++i) tot += s_fin[i][tid];
-                a.scalars[tid] = tot * (double)a.inv_batch;
+                if constexpr (DIAG) {
+                    if (tid < 4) a.scalars[tid] = tot * (double)a.inv_batch;
+                    else a.diag[tid - 4] = tot;  // not scaled: the off-policy sums add across ranks
+                } else {
+                    a.scalars[tid] = tot * (double)a.inv_batch;
+                }
             }
             if (tid == 0) *a.counter = 0u;
         }
@@ -436,11 +545,11 @@ int pick_ap(int A) {
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS>
-int launch_s(const VtArgs& a, bool vec, unsigned groups, int nw, int cl, cudaStream_t st) {
+template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool DIAG>
+int launch_s(const VtArgsT<DIAG>& a, bool vec, unsigned groups, int nw, int cl, cudaStream_t st) {
     const cudaError_t e =
-        vec ? impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, true>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
-            : impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, false>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
+        vec ? impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, true, DIAG>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
+            : impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, false, DIAG>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
     if (e != cudaSuccess) return (int)e;
     return impala_launch_status();
 }
@@ -453,8 +562,8 @@ constexpr int kMaxCluster = 8;  // portable cluster size
 // over a thread-block cluster (DSMEM carry exchange, cl = 4 / 8) works, but its cluster barriers
 // replace a cheap chunk loop, so cl = 1 unless overridden (scripts/tune_vtrace.py compares them).
 // IMPALA_VTRACE_S / IMPALA_VTRACE_NSEG (warps per CTA) / IMPALA_VTRACE_CLUSTER override the choice.
-template <bool WITH_LOSS>
-int launch(VtArgs& a, cudaStream_t st) {
+template <bool WITH_LOSS, bool DIAG = false>
+int launch(VtArgsT<DIAG>& a, cudaStream_t st) {
     if (a.T < 1 || a.B < 1 || a.A < 1) return IMPALA_ERR_BAD_ARG;
     const int AP = pick_ap(a.A);
     if (!AP) return IMPALA_ERR_UNSUPPORTED_SHAPE;
@@ -477,16 +586,16 @@ int launch(VtArgs& a, cudaStream_t st) {
     if (n_env >= 1 && n_env <= max_w) nw = n_env;
 #define VT_AP(APV)                                                                                      \
     if (AP == APV) {                                                                                    \
-        if (S == 5) return launch_s<APV, 5, 320, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);             \
-        if (S == 1) return launch_s<APV, 1, 1024, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);            \
-        return launch_s<APV, 2, 512, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);                         \
+        if (S == 5) return launch_s<APV, 5, 320, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);       \
+        if (S == 1) return launch_s<APV, 1, 1024, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);      \
+        return launch_s<APV, 2, 512, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);                   \
     }
     VT_AP(2)
     VT_AP(4)
 #undef VT_AP
-    if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);
-    if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);
-    return launch_s<32, 1, 512, 1, WITH_LOSS>(a, vec, groups, nw, cl, st);
+    if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);
+    if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);
+    return launch_s<32, 1, 512, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);
 }
 
 }  // namespace
@@ -507,29 +616,26 @@ extern "C" int impala_vtrace(const float* cur_logits, const float* beh_logits,
     return launch<false>(a, (cudaStream_t)stream);
 }
 
-extern "C" int64_t impala_vtrace_loss_workspace(int T, int B, int A) {
+// Per-CTA partial rows: 4 loss sums (plain) or [4 loss sums | 8 off-policy sums] (diag).
+static int64_t loss_workspace(int T, int B, int A, int row) {
     if (T < 1 || B < 1 || A < 1) return IMPALA_ERR_BAD_ARG;
     const int64_t grid = (((int64_t)B + 31) / 32) * kMaxCluster;  // one row per CTA, clusters of up to 8 per group
-    return grid * 4 * (int64_t)sizeof(double) + 16;  // per-CTA sums + arrival counter
+    return grid * row * (int64_t)sizeof(double) + 16;  // per-CTA sums + arrival counter
 }
 
-extern "C" int impala_vtrace_loss(const float* cur_logits, const float* beh_logits,
-                                  const int32_t* actions, const float* rewards,
-                                  const uint8_t* done, const int32_t* lens, const float* v,
-                                  float* vs, float* pg_adv, float* dlogits, float* dv,
-                                  double* scalars, void* workspace, int64_t workspace_bytes, int T,
-                                  int B, int A, float gamma, float rho_bar, float c_bar,
-                                  float v_loss_c, float policy_loss_c, float entropy_c,
-                                  float inv_batch, int mode, void* stream) {
+// Argument checks and packing shared by impala_vtrace_loss and impala_vtrace_loss_diag.
+static int loss_args(VtArgs& a, const float* cur_logits, const float* beh_logits, const int32_t* actions,
+                     const float* rewards, const uint8_t* done, const int32_t* lens, const float* v, float* vs,
+                     float* pg_adv, float* dlogits, float* dv, double* scalars, void* workspace,
+                     int64_t workspace_bytes, int64_t need, int T, int B, int A, float gamma, float rho_bar,
+                     float c_bar, float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch, int mode) {
     if (!cur_logits || !beh_logits || !actions || !rewards || !done || !lens || !v || !dlogits ||
         !dv || !scalars || !workspace)
         return IMPALA_ERR_BAD_ARG;
     if (mode != IMPALA_MODE_REFERENCE && mode != IMPALA_MODE_PAPER) return IMPALA_ERR_BAD_ARG;
-    const int64_t need = impala_vtrace_loss_workspace(T, B, A);
     if (need < 0) return (int)need;
     if (workspace_bytes < need) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
     if (reinterpret_cast<uintptr_t>(workspace) & 15) return IMPALA_ERR_BAD_ARG;
-    VtArgs a{};
     a.cur_logits = cur_logits, a.beh_logits = beh_logits, a.actions = actions, a.rewards = rewards;
     a.done = done, a.lens = lens, a.v = v, a.vs = vs, a.pg_adv = pg_adv, a.dlogits = dlogits;
     a.dv = dv, a.scalars = scalars;
@@ -540,5 +646,44 @@ extern "C" int impala_vtrace_loss(const float* cur_logits, const float* beh_logi
     a.gamma = gamma, a.rho_bar = rho_bar, a.c_bar = c_bar;
     a.v_loss_c = v_loss_c, a.policy_loss_c = policy_loss_c, a.entropy_c = entropy_c;
     a.inv_batch = inv_batch;
+    return 0;
+}
+
+extern "C" int64_t impala_vtrace_loss_workspace(int T, int B, int A) { return loss_workspace(T, B, A, 4); }
+
+extern "C" int impala_vtrace_loss(const float* cur_logits, const float* beh_logits,
+                                  const int32_t* actions, const float* rewards,
+                                  const uint8_t* done, const int32_t* lens, const float* v,
+                                  float* vs, float* pg_adv, float* dlogits, float* dv,
+                                  double* scalars, void* workspace, int64_t workspace_bytes, int T,
+                                  int B, int A, float gamma, float rho_bar, float c_bar,
+                                  float v_loss_c, float policy_loss_c, float entropy_c,
+                                  float inv_batch, int mode, void* stream) {
+    VtArgs a{};
+    const int rc = loss_args(a, cur_logits, beh_logits, actions, rewards, done, lens, v, vs, pg_adv, dlogits, dv,
+                             scalars, workspace, workspace_bytes, impala_vtrace_loss_workspace(T, B, A), T, B, A,
+                             gamma, rho_bar, c_bar, v_loss_c, policy_loss_c, entropy_c, inv_batch, mode);
+    if (rc) return rc;
     return launch<true>(a, (cudaStream_t)stream);
+}
+
+extern "C" int64_t impala_vtrace_loss_diag_workspace(int T, int B, int A) { return loss_workspace(T, B, A, 12); }
+
+extern "C" int impala_vtrace_loss_diag(const float* cur_logits, const float* beh_logits,
+                                       const int32_t* actions, const float* rewards,
+                                       const uint8_t* done, const int32_t* lens, const float* v,
+                                       float* vs, float* pg_adv, float* dlogits, float* dv,
+                                       double* scalars, double* diag, void* workspace,
+                                       int64_t workspace_bytes, int T, int B, int A, float gamma,
+                                       float rho_bar, float c_bar, float v_loss_c,
+                                       float policy_loss_c, float entropy_c, float inv_batch,
+                                       int mode, void* stream) {
+    if (!diag) return IMPALA_ERR_BAD_ARG;
+    VtDiagArgs a{};
+    const int rc = loss_args(a, cur_logits, beh_logits, actions, rewards, done, lens, v, vs, pg_adv, dlogits, dv,
+                             scalars, workspace, workspace_bytes, impala_vtrace_loss_diag_workspace(T, B, A), T, B,
+                             A, gamma, rho_bar, c_bar, v_loss_c, policy_loss_c, entropy_c, inv_batch, mode);
+    if (rc) return rc;
+    a.diag = diag;
+    return launch<true, true>(a, (cudaStream_t)stream);
 }

@@ -35,7 +35,8 @@ def main():
         hp = Hyperparameters(**c["hp"])
         eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], hp, global_batch=c["B"],
                             device=dev, mode=c["mode"], process_group=dist.group.WORLD,
-                            obs_dtype=c.get("obs_dtype", "float32"), frames=c.get("frames", 1))
+                            obs_dtype=c.get("obs_dtype", "float32"), frames=c.get("frames", 1),
+                            diagnostics=c.get("diagnostics", False))
         z = np.load(spec["state"])
         state = {"policy": {}, "value_fn": {}}
         for key in z.files:

@@ -8,6 +8,8 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
     impala_ingest              pinned host slab -> device slab (one DMA)        learner.py:104-109,117
     impala_mlp_forward_pair    policy logits (T*B rows) + values ((T+1)*B)      learner.py:112-113
     impala_vtrace_loss         V-trace, 3 losses, dL/dlogits, dL/dv, scalars    learner.py:116-162
+      diagnostics=True: impala_vtrace_loss_diag, the same outputs plus eight off-policy sums (ratio
+      clipping, KL(behaviour || current), value explained variance) that ride the all-reduce with the scalars
     impala_mlp_backward_pair   parameter gradients of both nets (float64)       learner.py:175
     impala_clip_adam           per-net clip + Adam + step counter               learner.py:176-183
       N > 1 (new; SURVEY 8e): the all-reduce of [grads | scalars] is a PUSH over NVLink peer memory -
@@ -46,9 +48,31 @@ from . import _cabi
 
 PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
 SCALAR_NAMES = ("value_fn_loss", "policy_loss", "policy_entropy", "batch_mean_reward")
+DIAG_NAMES = ("log_ratio_mean", "rho_clip_fraction", "c_clip_fraction", "kl_behaviour_current",
+              "value_explained_variance", "valid_steps")
 _BATCH_FIELDS = (("obs", np.float32), ("beh_logits", np.float32), ("actions", np.int32),
                  ("rewards", np.float32), ("done", np.uint8), ("lens", np.int32))
 _TORCH_DT = {np.float32: torch.float32, np.int32: torch.int32, np.uint8: torch.uint8}
+
+
+def diagnostic_values(sums, value_fn_loss: float, global_batch: int) -> dict:
+    """The logged off-policy diagnostics from the eight sums of impala_vtrace_loss_diag (all ranks added).
+
+    sum (vs - v)^2 over the valid steps is not summed again: it is 2 B value_fn_loss (the baseline loss
+    is 0.5 sum (v - vs)^2 over t <= lens, and its t = lens term is 0).  value_explained_variance =
+    1 - Var(vs - v) / Var(vs) (population variances over the valid steps), NaN when n < 2 or Var(vs) <= 0."""
+    n, s_lr, n_rho, n_c, s_kl, s_vs, s_vs2, s_err = (float(x) for x in sums)
+    nan = float("nan")
+    out = {"valid_steps": n}
+    if n <= 0:
+        out.update(dict.fromkeys(DIAG_NAMES[:5], nan))
+        return out
+    out.update(log_ratio_mean=s_lr / n, rho_clip_fraction=n_rho / n, c_clip_fraction=n_c / n,
+               kl_behaviour_current=s_kl / n)
+    var_vs = s_vs2 / n - (s_vs / n) ** 2
+    var_err = 2.0 * global_batch * value_fn_loss / n - (s_err / n) ** 2
+    out["value_explained_variance"] = 1.0 - var_err / var_vs if n >= 2 and var_vs > 0.0 else nan
+    return out
 
 
 def _ptr(t: torch.Tensor) -> C.c_void_p:
@@ -70,7 +94,7 @@ class LearnerEngine:
     def __init__(self, T: int, B_local: int, O: int, A: int, H_pi: int, H_v: int, hp,
                  global_batch: int | None = None, device: str | torch.device = "cuda:0",
                  mode: str = "reference", process_group=None, use_graph: bool = True,
-                 slabs: int = 2, obs_dtype: str = "float32", frames: int = 1):
+                 slabs: int = 2, obs_dtype: str = "float32", frames: int = 1, diagnostics: bool = False):
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
@@ -84,6 +108,9 @@ class LearnerEngine:
         torch.cuda.set_device(self.dev)
         self.T, self.B, self.O, self.A, self.H_pi, self.H_v = T, B_local, O, A, H_pi, H_v
         self.hp = hp
+        # off-policy diagnostics of every update (impala_vtrace_loss_diag); every rank must agree on it
+        self.diagnostics = bool(diagnostics)
+        self.n_extra = 12 if self.diagnostics else 4  # logged float64 values after the gradient in `comm`
         self.mode = _cabi.MODES[mode]
         self.pg = process_group
         self.world = 1
@@ -107,8 +134,9 @@ class LearnerEngine:
         self.adam_m = torch.zeros(self.n_total, **f32)
         self.adam_v = torch.zeros(self.n_total, **f32)
         self.adam_step = torch.zeros(3, dtype=torch.int64, device=self.dev)  # step, beta1^t, beta2^t bits
-        # float64 [gradient | 4 loss scalars | pad]: the all-reduce payload
-        self.comm = torch.zeros(self.n_total + 8, dtype=torch.float64, device=self.dev)
+        # float64 [gradient | 4 loss scalars | (diagnostics: 8 off-policy sums |) pad]: the all-reduce payload
+        self.n_comm = self.n_total + self.n_extra + 4
+        self.comm = torch.zeros(self.n_comm, dtype=torch.float64, device=self.dev)
         self.norms = torch.zeros(2, dtype=torch.float64, device=self.dev)
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts
@@ -160,9 +188,11 @@ class LearnerEngine:
         if frames > 1:
             self.obs_dense = self.obs_f32 if self.obs_f32 is not None else torch.zeros(
                 (T + 1) * B_local * O, dtype=torch.uint8 if self.obs_u8_native else torch.float32, device=self.dev)
-        self.ws_vt_bytes = int(self.lib.impala_vtrace_loss_workspace(T, B_local, A))
+        ws_fn = self.lib.impala_vtrace_loss_diag_workspace if self.diagnostics else self.lib.impala_vtrace_loss_workspace
+        self.ws_vt_bytes = int(ws_fn(T, B_local, A))
         self.ws_vt = torch.zeros(self.ws_vt_bytes, dtype=torch.uint8, device=self.dev)  # zeroed once
-        self.h_scalars = torch.zeros(4, 8, dtype=torch.float64).pin_memory()  # ring of 4 tickets
+        # ring of 4 tickets: [4 scalars | 2 norms | peer error | pad (| 8 off-policy sums)]
+        self.h_scalars = torch.zeros(4, 16 if self.diagnostics else 8, dtype=torch.float64).pin_memory()
         self._scalar_events = [torch.cuda.Event() for _ in range(4)]
         self._ticket = 0
 
@@ -189,7 +219,7 @@ class LearnerEngine:
         rank, world = dist.get_rank(self.pg), self.world
         ok, err, mine = os.environ.get("IMPALA_ALLREDUCE", "peer") != "nccl" and world <= 8, "", {}
         lib = self.lib
-        slot = self.n_total + 8                         # LL elements per rank slot: [gradient | scalars | pad]
+        slot = self.n_comm                              # LL elements per rank slot: [gradient | scalars | pad]
         buf = world * slot                              # LL elements per parity buffer
         if ok:
             try:
@@ -373,19 +403,23 @@ class LearnerEngine:
             _cabi.check(lib.impala_mlp_forward_pair(obs, p_pi, p_vf, _ptr(self.logits), _ptr(self.values),
                                                     self.M_pi, self.M_vf, O, self.H_pi, self.H_v, A, st),
                         "impala_mlp_forward_pair")
-        _cabi.check(lib.impala_vtrace_loss(
-            _ptr(self.logits), _ptr(d["beh_logits"]), _ptr(d["actions"]),
-            _ptr(d["rewards"]), _ptr(d["done"]), _ptr(d["lens"]), _ptr(self.values),
-            _ptr(self.vs), _ptr(self.pg_adv), _ptr(self.dlogits), _ptr(self.dv), scal,
-            _ptr(self.ws_vt), self.ws_vt_bytes, T, B, A,
-            float(hp.gamma), float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c),
-            float(hp.policy_loss_c), float(hp.entropy_c), float(self.inv_batch), self.mode, st),
-            "impala_vtrace_loss")
+        vt_in = (_ptr(self.logits), _ptr(d["beh_logits"]), _ptr(d["actions"]),
+                 _ptr(d["rewards"]), _ptr(d["done"]), _ptr(d["lens"]), _ptr(self.values),
+                 _ptr(self.vs), _ptr(self.pg_adv), _ptr(self.dlogits), _ptr(self.dv), scal)
+        vt_hp = (T, B, A, float(hp.gamma), float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c),
+                 float(hp.policy_loss_c), float(hp.entropy_c), float(self.inv_batch), self.mode, st)
+        if self.diagnostics:  # the eight sums land right after the four scalars
+            _cabi.check(lib.impala_vtrace_loss_diag(*vt_in, C.c_void_p(gbase + 8 * (self.n_total + 4)),
+                                                    _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp),
+                        "impala_vtrace_loss_diag")
+        else:
+            _cabi.check(lib.impala_vtrace_loss(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp),
+                        "impala_vtrace_loss")
         pr = self.peer
         if pr and pr["fused"]:
             _cabi.check(lib.impala_mlp_backward_pair_push(
                 obs, p_pi, p_vf, _ptr(self.dlogits), _ptr(self.dv), _ptr(self.ws_pi), self.ws_pi_bytes,
-                _ptr(self.ws_vf), self.ws_vf_bytes, self.M_pi, self.M_vf, O, self.H_pi, self.H_v, A, scal, 4,
+                _ptr(self.ws_vf), self.ws_vf_bytes, self.M_pi, self.M_vf, O, self.H_pi, self.H_v, A, scal, self.n_extra,
                 _ptr(pr["gather_ptrs"]), _ptr(pr["seq"]), pr["slot"], pr["buf"], pr["rank"], self.world, st),
                 "impala_mlp_backward_pair_push")
         else:
@@ -400,8 +434,8 @@ class LearnerEngine:
                     obs, p_pi, p_vf, _ptr(self.dlogits), _ptr(self.dv), g_pi, g_vf, _ptr(self.ws_pi),
                     self.ws_pi_bytes, _ptr(self.ws_vf), self.ws_vf_bytes, self.M_pi, self.M_vf, O, self.H_pi,
                     self.H_v, A, st), "impala_mlp_backward_pair")
-            if pr:  # stand-alone producer: comm[0 : n_total + 8) -> every rank's gather buffer
-                _cabi.check(lib.impala_peer_push(_ptr(self.comm), self.n_total + 8, _ptr(pr["gather_ptrs"]),
+            if pr:  # stand-alone producer: all of comm -> every rank's gather buffer
+                _cabi.check(lib.impala_peer_push(_ptr(self.comm), self.n_comm, _ptr(pr["gather_ptrs"]),
                                                  _ptr(pr["seq"]), pr["slot"], pr["buf"], pr["rank"], self.world, st),
                             "impala_peer_push")
         return int(lib.impala_launch_count() - launched)  # kernels actually launched / captured
@@ -412,7 +446,7 @@ class LearnerEngine:
             pr = self.peer
             _cabi.check(self.lib.impala_gather_clip_adam(
                 _ptr(self.params), _ptr(self.comm), C.c_void_p(pr["gather"]), _ptr(pr["seq"]),
-                pr["slot"], pr["buf"], self.world, 4, _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step),
+                pr["slot"], pr["buf"], self.world, self.n_extra, _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step),
                 self.n_pi, self.n_total, float(hp.max_norm), float(0.95 * hp.lr), 0.9, 0.999, 1e-8,
                 _ptr(self.norms), _ptr(pr["err"]), pr["timeout_s"], st), "impala_gather_clip_adam")
             return 1
@@ -507,6 +541,8 @@ class LearnerEngine:
             self.h_scalars[k, 4:6].copy_(self.norms, non_blocking=True)
             if self.peer:
                 self.h_scalars[k, 6:7].copy_(self.peer["err"].to(torch.float64), non_blocking=True)
+            if self.diagnostics:
+                self.h_scalars[k, 8:16].copy_(self.comm[self.n_total + 4:self.n_total + 12], non_blocking=True)
             self._scalar_events[k].record(self.stream)
         return k
 
@@ -522,6 +558,8 @@ class LearnerEngine:
         out["total_loss"] = (hp.v_loss_c * out["value_fn_loss"] + hp.policy_loss_c * out["policy_loss"]
                              - hp.entropy_c * out["policy_entropy"])  # learner.py:154-159
         out["norm_policy"], out["norm_value"] = s[4], s[5]
+        if self.diagnostics:
+            out.update(diagnostic_values(s[8:16], out["value_fn_loss"], self.global_batch))
         return out
 
     def synchronize(self) -> None:

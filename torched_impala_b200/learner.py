@@ -236,7 +236,7 @@ class _Publisher:
 class Learner:
     def __init__(self, id, hparams, policy, value_fn, q, update_counter, log_path=None,
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
-                 evaluator=None, obs_dtype="float32", frames=1):
+                 evaluator=None, obs_dtype="float32", frames=1, diagnostics=False):
         self.id = id
         if obs_dtype not in ("float32", "uint8"):
             raise ValueError(f"obs_dtype must be 'float32' or 'uint8', got {obs_dtype!r}")
@@ -261,6 +261,8 @@ class Learner:
         self.device = self.devices[0]
         self.mode = mode
         self.publish_every = max(1, int(publish_every))
+        # off-policy diagnostics of every update (ratio clipping, behaviour KL, value explained variance)
+        self.diagnostics = bool(diagnostics)
         for name, mod in (("policy", policy), ("value_fn", value_fn)):
             if any(p.is_cuda for p in mod.parameters()):
                 raise ValueError(
@@ -311,7 +313,7 @@ class Learner:
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
-                    obs_dtype=self.obs_dtype, frames=self.frames)
+                    obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -321,7 +323,7 @@ class Learner:
             raise ValueError(f"batch_size {c['B']} does not divide over {world} devices")
         eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], self.hp,
                             global_batch=c["B"], device=self.device, mode=self.mode, process_group=process_group,
-                            obs_dtype=c["obs_dtype"], frames=c["frames"])
+                            obs_dtype=c["obs_dtype"], frames=c["frames"], diagnostics=c["diagnostics"])
         eng.load_state(self._init_state())
         return eng
 
@@ -414,10 +416,13 @@ class Learner:
         return reward
 
     def _report(self, writer, n, reward, sc):
-        """Console line + the five TensorBoard scalars of learner.py:188-192,217-240."""
+        """Console line + the five TensorBoard scalars of learner.py:188-192,217-240 (+ the off-policy
+        diagnostics when they are on)."""
         if self.hp.verbose >= 1:
+            diag = (f", rho clipped {100.0 * sc['rho_clip_fraction']:.1f} %, kl {sc['kl_behaviour_current']:.4f}"
+                    if self.diagnostics else "")
             print(f"[learner_{self.id}] update {n}: batch mean reward {reward:.2f}, "
-                  f"loss {sc['total_loss']:.2f}")
+                  f"loss {sc['total_loss']:.2f}{diag}")
         if writer is None:
             return
         tag = f"learner_{self.id}"
@@ -426,6 +431,10 @@ class Learner:
                           ("loss/policy_entropy", sc["policy_entropy"]),
                           ("loss/total_loss", sc["total_loss"])):
             writer.add_scalar(f"{tag}/{name}", val, n)
+        if self.diagnostics:
+            for name in ("log_ratio_mean", "rho_clip_fraction", "c_clip_fraction", "kl_behaviour_current"):
+                writer.add_scalar(f"{tag}/offpolicy/{name}", sc[name], n)
+            writer.add_scalar(f"{tag}/value/explained_variance", sc["value_explained_variance"], n)
 
     def _due(self, n) -> bool:
         hp = self.hp

@@ -197,6 +197,30 @@ def vtrace_loss(cur_logits, beh_logits, actions, rewards, done, lens, v, hp, inv
     return dict(vs=vs, pg_adv=pg, dlogits=dlogits, dv=dv, scalars=scalars)
 
 
+def vtrace_loss_diag(cur_logits, beh_logits, actions, rewards, done, lens, v, hp, inv_batch,
+                     mode="reference"):
+    """vtrace_loss plus `diag`: the eight float64 off-policy sums of impala_vtrace_loss_diag (see
+    engine.diagnostic_values for the logged values derived from them)."""
+    _need_cuda(cur_logits, beh_logits, actions, rewards, done, lens, v)
+    T, B, A = cur_logits.shape
+    dev = v.device
+    vs = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    pg = torch.empty(T, B, dtype=torch.float32, device=dev)
+    dlogits = torch.empty(T, B, A, dtype=torch.float32, device=dev)
+    dv = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    scalars = torch.empty(4, dtype=torch.float64, device=dev)
+    diag = torch.empty(8, dtype=torch.float64, device=dev)
+    lib = _cabi.lib()
+    ws_bytes = int(lib.impala_vtrace_loss_diag_workspace(T, B, A))
+    ws = torch.zeros(ws_bytes, dtype=torch.uint8, device=dev)
+    _cabi.check(lib.impala_vtrace_loss_diag(
+        _p(cur_logits), _p(beh_logits), _p(actions), _p(rewards), _p(done), _p(lens), _p(v), _p(vs),
+        _p(pg), _p(dlogits), _p(dv), _p(scalars), _p(diag), _p(ws), ws_bytes, T, B, A, float(hp.gamma),
+        float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c), float(hp.policy_loss_c), float(hp.entropy_c),
+        float(inv_batch), _cabi.MODES[mode], _st()), "impala_vtrace_loss_diag")
+    return dict(vs=vs, pg_adv=pg, dlogits=dlogits, dv=dv, scalars=scalars, diag=diag)
+
+
 def clip_adam(params, grad, m, v, step, n_policy, max_norm, lr, beta1=0.9, beta2=0.999, eps=1e-8):
     _need_cuda(params, grad, m, v, step)
     norms = torch.empty(2, dtype=torch.float64, device=params.device)
