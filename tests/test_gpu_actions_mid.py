@@ -3,14 +3,13 @@ tensor-core MLP kernels.
 
 The forward runs the 16-output epilogue at one, two or four K atoms and the backward the 16-output
 layer-2-through-shared-memory kernel at one or two (at four it keeps the 32-output padded kernel).  Both
-are held to the float64 oracle with every logit written (the output starts as NaN), the launches are
-checked by name in a profiler trace, and the whole learner step - eager engine, byte observations,
-forked Learner behind a RingQueue - is checked at A = 6 and A = 9.
+are held to the float64 oracle with every logit written (the output starts as NaN), and the whole learner
+step - eager engine, byte observations, forked Learner behind a RingQueue - is checked at A = 6 and A = 9.
+Which kernels the launches take is checked in test_gpu_mlp_routes.py.
 """
 import ctypes
 import json
 import os
-import re
 import subprocess
 import sys
 
@@ -105,49 +104,6 @@ def test_backward_matches_oracle(ops, M, O, H, N2):
         assert got[k].shape == w.shape
         tol = 5e-5 * np.abs(w).max() + (3 * one_row if k in PKEYS[:2] else 0.0)
         assert np.abs(got[k] - w).max() < tol, (k, float(np.abs(got[k] - w).max()), float(np.abs(w).max()))
-
-
-def _kernel_names(fn):
-    fn()  # first launches (occupancy queries, shared-memory opt-in) stay out of the trace
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    return {ev.name for ev in prof.events() if ev.device_type == torch.autograd.DeviceType.CUDA}
-
-
-def _has(names, kernel, *targs):
-    """A launch of `kernel<targs>` (demangled or mangled name)."""
-    demangled = re.escape(kernel) + "<" + r",\s*".join(map(str, targs)) + ">"
-    mangled = re.escape(kernel) + "I" + "".join(f"Li{t}E" for t in targs) + "E"
-    return any(re.search(demangled, n) or re.search(mangled, n) for n in names)
-
-
-# O -> (forward, backward) instantiations at A = 6, H = 256
-ROUTES = {24: (("mlp_fwd_tc_kernel", 16, 1), ("mlp_bwd_tcw_kernel", 16, 1)),
-          128: (("mlp_fwd_tc_kernel", 16, 4), ("mlp_bwd_tcw_kernel", 32, 4))}
-
-
-@pytest.mark.parametrize("tensor_cores", ["1", "0"])
-@pytest.mark.parametrize("O", sorted(ROUTES))
-def test_launches_take_the_16_output_kernels(ops, monkeypatch, O, tensor_cores):
-    monkeypatch.setenv("IMPALA_MLP_TC", tensor_cores)
-    M, H, N2 = 4096, 256, 6
-    rng = np.random.default_rng(O)
-    p = ops.pack_params(synth.init_params(1, O, N2, H)["policy"])
-    x = dev(rng.standard_normal((M, O), dtype=np.float32))
-    dout = dev(rng.standard_normal((M, N2), dtype=np.float32))
-    fwd = _kernel_names(lambda: ops.mlp_forward(x, p, O, H, N2))
-    bwd = _kernel_names(lambda: ops.mlp_backward(x, p, dout, O, H, N2))
-    print(O, tensor_cores, sorted(fwd), sorted(bwd))
-    fp32_fwd = any("mlp_fwd_kernel" in n for n in fwd)
-    fp32_bwd = any("mlp_bwd_kernel" in n for n in bwd)
-    if tensor_cores == "1":
-        assert _has(fwd, *ROUTES[O][0]) and not fp32_fwd, fwd
-        assert _has(bwd, *ROUTES[O][1]) and not fp32_bwd, bwd
-    else:
-        assert fp32_fwd and not any("_tc" in n for n in fwd), fwd
-        assert fp32_bwd and not any("_tc" in n for n in bwd), bwd
 
 
 # name: (T, B, O, A, H, ragged)

@@ -53,6 +53,11 @@ static inline cudaError_t impala_sm_count(int* out) {
     return cudaSuccess;
 }
 
+// Resident CTAs per SM of `kernel` launched with `threads` threads and `smem` bytes of dynamic shared
+// memory (defined in mlp.cu).  Opts the kernel in to `smem` first; the opt-in is only ever raised, and
+// the occupancy is cached per (kernel, device, threads, smem).
+cudaError_t impala_resident_ctas(const void* kernel, int threads, size_t smem, int* per_sm);
+
 static inline int impala_env_int(const char* name, int dflt) {
     const char* v = getenv(name);
     return (v && *v) ? atoi(v) : dflt;

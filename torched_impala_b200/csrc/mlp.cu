@@ -13,10 +13,9 @@
 // deterministic; wide hidden layers are split over blockIdx.y.  Per-CTA partials are then
 // summed in float64 by a second small kernel.
 //
-// This file: host-side configuration, occupancy cache, the partial reduction and the
-// C-ABI entry points.  Kernel templates: mlp_kernels.cuh; instantiations: mlp_inst.cu.
+// This file: the route that picks the kernels of every MLP call, the FP32 configuration, the occupancy
+// cache, the partial reduction and the C-ABI entry points.  Kernel templates: mlp_kernels.cuh; instantiations: mlp_inst.cu.
 #include <algorithm>
-#include <cstdlib>
 #include <map>
 #include <mutex>
 #include <tuple>
@@ -24,17 +23,6 @@
 #include "mlp_kernels.cuh"
 
 namespace {
-
-struct GridInfo {
-    int ctas_per_sm, sms;
-};
-std::mutex g_cfg_mutex;
-std::map<std::tuple<const void*, int, int, size_t>, GridInfo> g_cfg_cache;
-// cudaFuncAttributeMaxDynamicSharedMemorySize is a property of the KERNEL (per device), not of one launch
-// configuration: it is only ever raised.  (Setting it per (threads, smem) entry lowered it when the same
-// instantiation was used with a narrower hidden layer, and the next launch of the wider, already
-// cached configuration failed with cudaErrorInvalidValue.)
-std::map<std::pair<const void*, int>, size_t> g_smem_opt_in;
 
 // grad[i] = sum_c ws[c][i] in float64.  A CTA covers 32 consecutive entries (one 128-byte
 // line per partial row); its 8 warps split the partial rows, so every load instruction is
@@ -109,14 +97,13 @@ bool pick_config(int O, int H, int N2, bool bwd, MlpConfig* c) {
     return true;
 }
 
-bool fill_args(MlpArgs* a, MlpConfig* c, size_t* smem, bool bwd, int M, int O, int H, int N2) {
-    if (M < 1 || !pick_config(O, H, N2, bwd, c)) return false;
+// Arguments and dynamic shared memory of the FP32 kernels in configuration c (pick_config).
+size_t fill_args(MlpArgs* a, const MlpConfig& c, bool bwd, int M, int O, int H, int N2) {
     a->M = M, a->O = O, a->H = H, a->N2 = N2;
     a->num_tiles = (M + kRows - 1) / kRows;
     a->lay = impala_make_layout(O, H, N2);
-    const size_t tail = bwd ? (size_t)kRows * c->np : (size_t)(c->threads / 32) * kRows * c->np;
-    *smem = ((size_t)kRows * c->op + tail) * sizeof(float);
-    return true;
+    const size_t tail = bwd ? (size_t)kRows * c.np : (size_t)(c.threads / 32) * kRows * c.np;
+    return ((size_t)kRows * c.op + tail) * sizeof(float);
 }
 
 int dispatch(bool bwd, const MlpArgs& a, const MlpConfig& c, size_t smem, cudaStream_t st,
@@ -130,109 +117,94 @@ int dispatch(bool bwd, const MlpArgs& a, const MlpConfig& c, size_t smem, cudaSt
     }
 }
 
-}  // namespace
+bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
 
-// Persistent grid = resident CTAs per SM x SM count, computed once per
-// (kernel, device, block size, shared memory) and cached.
-int impala_mlp_launch(void (*kernel)(MlpArgs), const MlpArgs& a, const MlpConfig& c, size_t smem,
-                      cudaStream_t st, int* grid_out) {
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return (int)e;
-    GridInfo gi;
-    {
-        std::lock_guard<std::mutex> lock(g_cfg_mutex);
-        const auto key = std::make_tuple((const void*)kernel, dev, c.threads, smem);
-        auto it = g_cfg_cache.find(key);
-        if (it == g_cfg_cache.end()) {
-            size_t& opted = g_smem_opt_in[std::make_pair((const void*)kernel, dev)];
-            if (smem > opted) {
-                e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e != cudaSuccess) return (int)e;
-                opted = smem;
-            }
-            e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&gi.ctas_per_sm, kernel, c.threads, smem);
-            if (e != cudaSuccess) return (int)e;
-            e = cudaDeviceGetAttribute(&gi.sms, cudaDevAttrMultiProcessorCount, dev);
-            if (e != cudaSuccess) return (int)e;
-            if (gi.ctas_per_sm < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-            g_cfg_cache[key] = gi;
-        } else {
-            gi = it->second;
-        }
+// The one place that decides which kernels run an MLP call: the first row below that takes the shape.
+// Returns IMPALA_OK and the plan, or the error of the call: IMPALA_ERR_UNSUPPORTED_SHAPE when no kernel
+// takes the shape, IMPALA_ERR_WORKSPACE_TOO_SMALL when a backward's ws_bytes is below p->ws.
+//
+//   O > 128 or byte rows  Obs: 128 < O <= 1024, O % 4 == 0, H = 128 k <= 1024, N2 <= 32.  There is no FP32
+//                         kernel for these widths, and byte rows of O <= 128 are refused (their callers
+//                         widen them once with impala_obs_u8_to_f32).  Shape, then workspace, then alignment.
+//   backward              the FP32 configuration and the workspace first: the FP32 kernels size it for all
+//   Narrow                O = 4 k <= 28, N2 <= 4; forward H = 32 k <= 256, backward H = 128 or 256 with dout
+//                         and grad 16-byte aligned as well
+//   Wide                  O = 4 k <= 128, H = 128 k <= 4096, N2 <= 32
+//   Fp32                  otherwise (O <= 128, N2 <= 32; the forward holds the hidden layer in one CTA)
+//
+// x_al: x aligned as the tensor-core kernels load it (16 bytes for float rows, 4 for byte rows).  Every
+// tensor-core row needs it; a misaligned float x at O <= 128 goes to the FP32 kernels.  IMPALA_MLP_TC=0
+// turns off every tensor-core row and IMPALA_MLP_TCW=0 all but Narrow.  Both are read on every call, so a
+// process may flip them between steps.
+int route(bool bwd, int M, int O, int H, int N2, bool bytes, bool x_al, bool dout_al, bool grad_al, int64_t ws_bytes,
+          MlpPlan* p) {
+    const bool tc = impala_env_int("IMPALA_MLP_TC", 1) != 0;
+    const bool tcw = tc && impala_env_int("IMPALA_MLP_TCW", 1) != 0;
+    *p = MlpPlan{};
+    if (O > 128 || bytes) {
+        if (O <= 128 || !tcw || M < 1 || O > 1024 || O % 4 || H < 128 || H > 1024 || H % 128 || N2 < 1 || N2 > 32)
+            return IMPALA_ERR_UNSUPPORTED_SHAPE;
+        p->kernel = MlpKernel::Obs, p->np = N2 == 1 ? 1 : N2 <= 4 ? 4 : 32;
+        if (bwd && ws_bytes < (p->ws = kWsHeader + impala_mlp_obs_bwd_layout(M, O, H, N2).bytes))
+            return IMPALA_ERR_WORKSPACE_TOO_SMALL;
+        return x_al ? IMPALA_OK : IMPALA_ERR_UNSUPPORTED_SHAPE;
     }
-    int grid = gi.ctas_per_sm * gi.sms / c.slices;
-    if (grid < 1) grid = 1;
-    if (grid > a.num_tiles) grid = a.num_tiles;
-    if (grid > kMaxParts) grid = kMaxParts;
-    kernel<<<dim3(grid, c.slices), c.threads, smem, st>>>(a);
-    *grid_out = grid;
-    return impala_launch_status();
+    if (bwd) {
+        if (M < 1 || !pick_config(O, H, N2, true, &p->fp32)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+        const int64_t tiles = std::min<int64_t>((M + kRows - 1) / kRows, kMaxParts);
+        p->ws = kWsHeader + tiles * impala_make_layout(O, H, N2).total * (int64_t)sizeof(float);
+        if (ws_bytes < p->ws) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
+    }
+    const bool tc_shape = tc && x_al && M >= 1 && O >= 4 && O % 4 == 0 && N2 >= 1;
+    if (tc_shape && O <= 28 && N2 <= 4 &&
+        (bwd ? (H == 128 || H == 256) && dout_al && grad_al : H >= 32 && H <= 256 && H % 32 == 0)) {
+        // one K atom, the whole hidden layer in one pass (forward) or one 64-unit block per CTA (backward)
+        p->kernel = MlpKernel::Narrow, p->np = N2 == 1 ? 1 : 4, p->ka = 1, p->hb = H, p->rows = 64;
+        p->reduce_in_kernel = bwd;
+        return IMPALA_OK;
+    }
+    if (tcw && tc_shape && H >= 128 && H % 128 == 0 && H <= 4096 && N2 <= 32) {
+        p->kernel = MlpKernel::Wide, p->rows = 64;
+        // 256 hidden units per pass fit at 16 outputs too: 88 064 B at one K atom, 219 136 B at two
+        p->hb = H <= 256 ? H : H % 256 ? 128 : 256;
+        if (O <= 64 && N2 <= 16) {
+            p->np = N2 == 1 ? 1 : N2 <= 4 ? 4 : 16, p->ka = O <= 32 ? 1 : 2;
+        } else if (bwd) {
+            // four K atoms, GEMM2 in 64-feature halves, 32-row tiles; 5..32 outputs padded to 32
+            p->np = N2 == 1 ? 1 : N2 <= 4 ? 4 : 32, p->ka = 4, p->rows = 32;
+        } else if (N2 > 16 && O <= 64) {
+            p->np = 32, p->ka = O <= 32 ? 1 : 2;
+            if (p->ka == 2) p->hb = 128;  // 256 units would need 235 520 B with the padded W2 rows
+        } else {
+            // four K atoms: 64 hidden units per pass keep W1 hi / lo + both warpgroups' x stages in 227 KB
+            p->np = N2 > 16 ? 32 : N2 > 4 ? 16 : N2 == 1 ? 1 : 4, p->ka = 4, p->hb = 64;
+        }
+        return IMPALA_OK;
+    }
+    if (!bwd && (M < 1 || !pick_config(O, H, N2, false, &p->fp32))) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    p->kernel = MlpKernel::Fp32;
+    return IMPALA_OK;
 }
 
-extern "C" int impala_mlp_forward(const float* x, const float* params, float* out, int M, int O,
-                                  int H, int N2, void* stream) {
-    if (!x || !params || !out) return IMPALA_ERR_BAD_ARG;
-    // GEMM-shaped layers go to the tensor cores (IMPALA_MLP_TC=0 forces the FP32 kernels).
-    const char* tc_env = std::getenv("IMPALA_MLP_TC");
-    if (!(tc_env && tc_env[0] == '0') && impala_mlp_fwd_tc_eligible(x, M, O, H, N2))
-        return impala_mlp_fwd_tc(x, params, out, M, O, H, N2, (cudaStream_t)stream);
-    if (!(tc_env && tc_env[0] == '0') && impala_mlp_tcw_eligible(x, M, O, H, N2))
-        return impala_mlp_fwd_tcw(x, params, out, M, O, H, N2, (cudaStream_t)stream);
-    if (!(tc_env && tc_env[0] == '0') && impala_mlp_fwd_tcx_eligible(x, M, O, H, N2))
-        return impala_mlp_fwd_tcx(x, params, out, M, O, H, N2, (cudaStream_t)stream);
-    if (O > 128 && impala_mlp_obs_shape_ok(M, O, H, N2))  // wide observations: K-streamed kernels
-        return impala_mlp_fwd_obs(x, params, out, M, O, H, N2, (cudaStream_t)stream);
+int forward(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
+            cudaStream_t st) {
+    if (p.kernel == MlpKernel::Obs) return impala_mlp_fwd_obs(p, x, params, out, M, O, H, N2, st);
+    if (p.kernel != MlpKernel::Fp32) return impala_mlp_fwd_tc(p, x, params, out, M, O, H, N2, st);
     MlpArgs a{};
-    MlpConfig c{};
-    size_t smem;
-    if (!fill_args(&a, &c, &smem, false, M, O, H, N2)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    const size_t smem = fill_args(&a, p.fp32, false, M, O, H, N2);
     a.x = x, a.params = params, a.out = out;
     int grid = 0;
-    return dispatch(false, a, c, smem, (cudaStream_t)stream, &grid);
-}
-
-static bool pair_enabled() {
-    const char* tc_env = std::getenv("IMPALA_MLP_TC");
-    const char* pr_env = std::getenv("IMPALA_MLP_PAIR");
-    return !(tc_env && tc_env[0] == '0') && !(pr_env && pr_env[0] == '0');
-}
-
-extern "C" int impala_mlp_forward_pair(const float* x, const float* params_pi, const float* params_vf,
-                                       float* logits, float* values, int M_pi, int M_vf, int O,
-                                       int H_pi, int H_vf, int A, void* stream) {
-    if (!x || !params_pi || !params_vf || !logits || !values) return IMPALA_ERR_BAD_ARG;
-    if (pair_enabled() && A >= 2 && A <= 4 && impala_mlp_fwd_tc_eligible(x, M_pi, O, H_pi, A) &&
-        impala_mlp_fwd_tc_eligible(x, M_vf, O, H_vf, 1))
-        return impala_mlp_fwd_tc_pair(x, params_pi, params_vf, logits, values, M_pi, M_vf, O, H_pi, H_vf, A,
-                                      (cudaStream_t)stream);
-    const int rc = impala_mlp_forward(x, params_pi, logits, M_pi, O, H_pi, A, stream);
-    if (rc != IMPALA_OK) return rc;
-    return impala_mlp_forward(x, params_vf, values, M_vf, O, H_vf, 1, stream);
-}
-
-extern "C" int64_t impala_mlp_backward_workspace(int M, int O, int H, int N2) {
-    if (O > 128) {
-        ObsBwdLayout L;
-        return impala_mlp_obs_bwd_layout(M, O, H, N2, &L) ? kWsHeader + L.bytes : IMPALA_ERR_UNSUPPORTED_SHAPE;
-    }
-    MlpConfig c{};
-    if (M < 1 || !pick_config(O, H, N2, true, &c)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    int64_t tiles = (M + kRows - 1) / kRows;
-    if (tiles > kMaxParts) tiles = kMaxParts;
-    return kWsHeader + tiles * impala_make_layout(O, H, N2).total * (int64_t)sizeof(float);
+    return dispatch(false, a, p.fp32, smem, st, &grid);
 }
 
 // Wide observations (O > 128, float or byte rows): DP^T and two sets of partial rows in the workspace,
 // each summed in float64.
 template <typename XT>
-static int backward_obs(const XT* x, const float* params, const float* dout, double* grad, void* workspace,
-                        int64_t workspace_bytes, int M, int O, int H, int N2, cudaStream_t st) {
-    ObsBwdLayout L;
-    if (!impala_mlp_obs_bwd_layout(M, O, H, N2, &L)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    if (workspace_bytes < kWsHeader + L.bytes) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
+int backward_obs(const MlpPlan& p, const XT* x, const float* params, const float* dout, double* grad,
+                 void* workspace, int M, int O, int H, int N2, cudaStream_t st) {
+    const ObsBwdLayout L = impala_mlp_obs_bwd_layout(M, O, H, N2);
     char* ws = static_cast<char*>(workspace) + kWsHeader;
-    const int rc = impala_mlp_bwd_obs(x, params, dout, ws, L, M, O, H, N2, st);
+    const int rc = impala_mlp_bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st);
     if (rc != IMPALA_OK) return rc;
     const MlpLayout lay = impala_make_layout(O, H, N2);
     const int64_t nr = lay.total - lay.ob1;
@@ -244,38 +216,118 @@ static int backward_obs(const XT* x, const float* params, const float* dout, dou
     return impala_launch_status();
 }
 
+int backward(const MlpPlan& p, const float* x, const float* params, const float* dout, double* grad, void* workspace,
+             int M, int O, int H, int N2, cudaStream_t st) {
+    if (p.kernel == MlpKernel::Obs) return backward_obs(p, x, params, dout, grad, workspace, M, O, H, N2, st);
+    // workspace = [control words (kWsHeader bytes, zero-filled once by the caller) | partial rows]
+    float* ws = reinterpret_cast<float*>(static_cast<char*>(workspace) + kWsHeader);
+    if (p.reduce_in_kernel)
+        return impala_mlp_bwd_tc(x, params, dout, ws, grad, static_cast<unsigned int*>(workspace), M, O, H, N2, st);
+    int grid = 0, rc;
+    if (p.kernel == MlpKernel::Wide) {
+        rc = impala_mlp_bwd_tcw(p, x, params, dout, ws, M, O, H, N2, st, &grid);
+    } else {
+        MlpArgs a{};
+        const size_t smem = fill_args(&a, p.fp32, true, M, O, H, N2);
+        a.x = x, a.params = params, a.dout = dout, a.ws = ws;
+        rc = dispatch(true, a, p.fp32, smem, st, &grid);
+    }
+    if (rc != IMPALA_OK) return rc;
+    const int64_t total = impala_make_layout(O, H, N2).total;
+    reduce_partials_kernel<<<(unsigned)((total + 31) / 32), kRedWarps * 32, 0, st>>>(ws, grad, grid, total);
+    return impala_launch_status();
+}
+
+// The paired backward that pushes to the peers: both networks on Narrow plans, >= 2 tiles between them.
+bool push_plans(int M_pi, int M_vf, int O, int H_pi, int H_vf, int A, bool x_al, bool dlogits_al, bool dv_al,
+                MlpPlan* pi, MlpPlan* vf) {
+    return A >= 2 && A <= 4 && route(true, M_pi, O, H_pi, A, false, x_al, dlogits_al, true, INT64_MAX, pi) == IMPALA_OK &&
+           pi->kernel == MlpKernel::Narrow &&
+           route(true, M_vf, O, H_vf, 1, false, x_al, dv_al, true, INT64_MAX, vf) == IMPALA_OK &&
+           vf->kernel == MlpKernel::Narrow && (M_pi + 63) / 64 + (M_vf + 63) / 64 >= 2;
+}
+
+}  // namespace
+
+cudaError_t impala_resident_ctas(const void* kernel, int threads, size_t smem, int* per_sm) {
+    static std::mutex mu;
+    // The dynamic shared-memory limit is a property of the KERNEL (per device), not of one launch
+    // configuration: it is only ever raised.  (Setting it per (threads, smem) entry lowered it when the same
+    // instantiation was used with a narrower hidden layer, and the next launch of the wider, already
+    // cached configuration failed with cudaErrorInvalidValue.)
+    static std::map<std::pair<const void*, int>, size_t> opted;
+    static std::map<std::tuple<const void*, int, int, size_t>, int> cached;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    std::lock_guard<std::mutex> lock(mu);
+    const auto key = std::make_tuple(kernel, dev, threads, smem);
+    if (const auto it = cached.find(key); it != cached.end()) return *per_sm = it->second, cudaSuccess;
+    size_t& o = opted[std::make_pair(kernel, dev)];
+    if (smem > o) {
+        if ((e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
+            return e;
+        o = smem;
+    }
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, kernel, threads, smem)) != cudaSuccess) return e;
+    cached[key] = *per_sm;
+    return cudaSuccess;
+}
+
+// Persistent grid = resident CTAs per SM x SM count / slices.
+int impala_mlp_launch(void (*kernel)(MlpArgs), const MlpArgs& a, const MlpConfig& c, size_t smem,
+                      cudaStream_t st, int* grid_out) {
+    int per_sm = 0, sms = 0;
+    cudaError_t e;
+    if ((e = impala_resident_ctas((const void*)kernel, c.threads, smem, &per_sm)) != cudaSuccess) return (int)e;
+    if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
+    if (per_sm < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    int grid = per_sm * sms / c.slices;
+    if (grid < 1) grid = 1;
+    if (grid > a.num_tiles) grid = a.num_tiles;
+    if (grid > kMaxParts) grid = kMaxParts;
+    kernel<<<dim3(grid, c.slices), c.threads, smem, st>>>(a);
+    *grid_out = grid;
+    return impala_launch_status();
+}
+
+extern "C" int impala_mlp_forward(const float* x, const float* params, float* out, int M, int O,
+                                  int H, int N2, void* stream) {
+    if (!x || !params || !out) return IMPALA_ERR_BAD_ARG;
+    MlpPlan p;
+    const int rc = route(false, M, O, H, N2, false, aligned(x, 16), true, true, 0, &p);
+    return rc != IMPALA_OK ? rc : forward(p, x, params, out, M, O, H, N2, (cudaStream_t)stream);
+}
+
+extern "C" int impala_mlp_forward_pair(const float* x, const float* params_pi, const float* params_vf,
+                                       float* logits, float* values, int M_pi, int M_vf, int O,
+                                       int H_pi, int H_vf, int A, void* stream) {
+    if (!x || !params_pi || !params_vf || !logits || !values) return IMPALA_ERR_BAD_ARG;
+    const cudaStream_t st = (cudaStream_t)stream;
+    MlpPlan pi, vf;
+    int rc = route(false, M_pi, O, H_pi, A, false, aligned(x, 16), true, true, 0, &pi);
+    if (rc == IMPALA_OK) rc = route(false, M_vf, O, H_vf, 1, false, aligned(x, 16), true, true, 0, &vf);
+    if (rc != IMPALA_OK) return rc;
+    if (A >= 2 && A <= 4 && pi.kernel == MlpKernel::Narrow && vf.kernel == MlpKernel::Narrow)
+        return impala_mlp_fwd_tc_pair(x, params_pi, params_vf, logits, values, M_pi, M_vf, O, H_pi, H_vf, A, st);
+    if ((rc = forward(pi, x, params_pi, logits, M_pi, O, H_pi, A, st)) != IMPALA_OK) return rc;
+    return forward(vf, x, params_vf, values, M_vf, O, H_vf, 1, st);
+}
+
+extern "C" int64_t impala_mlp_backward_workspace(int M, int O, int H, int N2) {
+    MlpPlan p;
+    const int rc = route(true, M, O, H, N2, false, true, true, true, INT64_MAX, &p);
+    return rc != IMPALA_OK ? rc : p.ws;
+}
+
 extern "C" int impala_mlp_backward(const float* x, const float* params, const float* dout,
                                    double* grad, void* workspace, int64_t workspace_bytes, int M,
                                    int O, int H, int N2, void* stream) {
     if (!x || !params || !dout || !grad || !workspace) return IMPALA_ERR_BAD_ARG;
-    if (O > 128)
-        return backward_obs(x, params, dout, grad, workspace, workspace_bytes, M, O, H, N2, (cudaStream_t)stream);
-    MlpArgs a{};
-    MlpConfig c{};
-    size_t smem;
-    if (!fill_args(&a, &c, &smem, true, M, O, H, N2)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    if (workspace_bytes < impala_mlp_backward_workspace(M, O, H, N2))
-        return IMPALA_ERR_WORKSPACE_TOO_SMALL;
-    // workspace = [control words (kWsHeader bytes, zero-filled once by the caller) | partial rows]
-    a.x = x, a.params = params, a.dout = dout;
-    a.ws = reinterpret_cast<float*>(static_cast<char*>(workspace) + kWsHeader);
-    int grid = 0;
-    const char* tc_env = std::getenv("IMPALA_MLP_TC");
-    if (!(tc_env && tc_env[0] == '0') && impala_mlp_bwd_tc_eligible(x, dout, M, O, H, N2) &&
-        (reinterpret_cast<uintptr_t>(grad) & 15) == 0)
-        return impala_mlp_bwd_tc(x, params, dout, a.ws, grad, static_cast<unsigned int*>(workspace), M, O, H,
-                                 N2, (cudaStream_t)stream);  // reduces in-kernel
-    const bool tc_on = !(tc_env && tc_env[0] == '0');
-    const bool wide = tc_on && impala_mlp_tcw_eligible(x, M, O, H, N2);
-    const bool widex = tc_on && !wide && impala_mlp_bwd_tcx_eligible(x, M, O, H, N2);
-    const int rc = wide    ? impala_mlp_bwd_tcw(x, params, dout, a.ws, M, O, H, N2, (cudaStream_t)stream, &grid)
-                   : widex ? impala_mlp_bwd_tcx(x, params, dout, a.ws, M, O, H, N2, (cudaStream_t)stream, &grid)
-                           : dispatch(true, a, c, smem, (cudaStream_t)stream, &grid);
-    if (rc != IMPALA_OK) return rc;
-    const int64_t total = a.lay.total;
-    reduce_partials_kernel<<<(unsigned)((total + 31) / 32), kRedWarps * 32, 0,
-                             (cudaStream_t)stream>>>(a.ws, grad, grid, total);
-    return impala_launch_status();
+    MlpPlan p;
+    const int rc = route(true, M, O, H, N2, false, aligned(x, 16), aligned(dout, 16), aligned(grad, 16),
+                         workspace_bytes, &p);
+    return rc != IMPALA_OK ? rc : backward(p, x, params, dout, grad, workspace, M, O, H, N2, (cudaStream_t)stream);
 }
 
 // ---- byte observations: the K-streamed kernels read uint8 rows (O > 128); narrower shapes are refused,
@@ -283,16 +335,78 @@ extern "C" int impala_mlp_backward(const float* x, const float* params, const fl
 extern "C" int impala_mlp_forward_u8(const uint8_t* x, const float* params, float* out, int M, int O, int H, int N2,
                                      void* stream) {
     if (!x || !params || !out) return IMPALA_ERR_BAD_ARG;
-    if (O <= 128 || !impala_mlp_obs_shape_ok(M, O, H, N2)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    return impala_mlp_fwd_obs(x, params, out, M, O, H, N2, (cudaStream_t)stream);
+    MlpPlan p;
+    const int rc = route(false, M, O, H, N2, true, aligned(x, 4), true, true, 0, &p);
+    return rc != IMPALA_OK ? rc : impala_mlp_fwd_obs(p, x, params, out, M, O, H, N2, (cudaStream_t)stream);
 }
 
 extern "C" int impala_mlp_backward_u8(const uint8_t* x, const float* params, const float* dout, double* grad,
                                       void* workspace, int64_t workspace_bytes, int M, int O, int H, int N2,
                                       void* stream) {
     if (!x || !params || !dout || !grad || !workspace) return IMPALA_ERR_BAD_ARG;
-    if (O <= 128) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    return backward_obs(x, params, dout, grad, workspace, workspace_bytes, M, O, H, N2, (cudaStream_t)stream);
+    MlpPlan p;
+    const int rc = route(true, M, O, H, N2, true, aligned(x, 4), true, true, workspace_bytes, &p);
+    return rc != IMPALA_OK ? rc
+                           : backward_obs(p, x, params, dout, grad, workspace, M, O, H, N2, (cudaStream_t)stream);
+}
+
+extern "C" int impala_mlp_backward_pair(const float* x, const float* params_pi, const float* params_vf,
+                                        const float* dlogits, const float* dv, double* grad_pi,
+                                        double* grad_vf, void* workspace_pi, int64_t workspace_pi_bytes,
+                                        void* workspace_vf, int64_t workspace_vf_bytes, int M_pi, int M_vf,
+                                        int O, int H_pi, int H_vf, int A, void* stream) {
+    if (!x || !params_pi || !params_vf || !dlogits || !dv || !grad_pi || !grad_vf || !workspace_pi ||
+        !workspace_vf)
+        return IMPALA_ERR_BAD_ARG;
+    const cudaStream_t st = (cudaStream_t)stream;
+    MlpPlan pi, vf;
+    int rc = route(true, M_pi, O, H_pi, A, false, aligned(x, 16), aligned(dlogits, 16), aligned(grad_pi, 16),
+                   workspace_pi_bytes, &pi);
+    if (rc == IMPALA_OK)
+        rc = route(true, M_vf, O, H_vf, 1, false, aligned(x, 16), aligned(dv, 16), aligned(grad_vf, 16),
+                   workspace_vf_bytes, &vf);
+    if (rc != IMPALA_OK) return rc;
+    if (A >= 2 && A <= 4 && pi.kernel == MlpKernel::Narrow && vf.kernel == MlpKernel::Narrow)
+        return impala_mlp_bwd_tc_pair(
+            x, params_pi, params_vf, dlogits, dv,
+            reinterpret_cast<float*>(static_cast<char*>(workspace_pi) + kWsHeader),
+            reinterpret_cast<float*>(static_cast<char*>(workspace_vf) + kWsHeader), grad_pi, grad_vf,
+            static_cast<unsigned int*>(workspace_pi), M_pi, M_vf, O, H_pi, H_vf, A, st);
+    if ((rc = backward(pi, x, params_pi, dlogits, grad_pi, workspace_pi, M_pi, O, H_pi, A, st)) != IMPALA_OK) return rc;
+    return backward(vf, x, params_vf, dv, grad_vf, workspace_vf, M_vf, O, H_vf, 1, st);
+}
+
+// ---- data-parallel learner: the paired backward that pushes its result to the peers (optim.cu)
+extern "C" int impala_mlp_backward_pair_push_supported(int M_pi, int M_vf, int O, int H_pi, int H_vf, int A) {
+    MlpPlan pi, vf;
+    return push_plans(M_pi, M_vf, O, H_pi, H_vf, A, true, true, true, &pi, &vf);
+}
+
+extern "C" int impala_mlp_backward_pair_push(const float* x, const float* params_pi, const float* params_vf,
+                                             const float* dlogits, const float* dv, void* workspace_pi,
+                                             int64_t workspace_pi_bytes, void* workspace_vf,
+                                             int64_t workspace_vf_bytes, int M_pi, int M_vf, int O, int H_pi,
+                                             int H_vf, int A, const double* extra, int n_extra,
+                                             void* const* peer_gather, const long long* seq,
+                                             int64_t slot_stride, int64_t buf_stride, int rank, int world,
+                                             void* stream) {
+    if (!x || !params_pi || !params_vf || !dlogits || !dv || !workspace_pi || !workspace_vf || !peer_gather ||
+        !seq || (n_extra > 0 && !extra))
+        return IMPALA_ERR_BAD_ARG;
+    if (world < 1 || world > 8 || rank < 0 || rank >= world || n_extra < 0 || n_extra > 32) return IMPALA_ERR_BAD_ARG;
+    MlpPlan pi, vf;
+    if (!push_plans(M_pi, M_vf, O, H_pi, H_vf, A, aligned(x, 16), aligned(dlogits, 16), aligned(dv, 16), &pi, &vf))
+        return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    const int64_t n_pi = impala_make_layout(O, H_pi, A).total, n_vf = impala_make_layout(O, H_vf, 1).total;
+    if (slot_stride < n_pi + n_vf + n_extra || buf_stride < (int64_t)world * slot_stride) return IMPALA_ERR_BAD_ARG;
+    if (workspace_pi_bytes < pi.ws || workspace_vf_bytes < vf.ws) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
+    const PushArgs push{reinterpret_cast<ulonglong2* const*>(peer_gather), seq, slot_stride, buf_stride, rank, world};
+    return impala_mlp_bwd_tc_pair(
+        x, params_pi, params_vf, dlogits, dv,
+        reinterpret_cast<float*>(static_cast<char*>(workspace_pi) + kWsHeader),
+        reinterpret_cast<float*>(static_cast<char*>(workspace_vf) + kWsHeader), nullptr, nullptr,
+        static_cast<unsigned int*>(workspace_pi), M_pi, M_vf, O, H_pi, H_vf, A, (cudaStream_t)stream, &push, extra,
+        n_extra);
 }
 
 // out[i] = x[i] (exact): 4 bytes -> one float4 per thread and iteration when both pointers allow it
@@ -326,70 +440,4 @@ extern "C" int impala_obs_u8_to_f32(const uint8_t* x, float* out, int64_t n, voi
     else
         obs_u8_to_f32_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, out, n);
     return impala_launch_status();
-}
-
-extern "C" int impala_mlp_backward_pair(const float* x, const float* params_pi, const float* params_vf,
-                                        const float* dlogits, const float* dv, double* grad_pi,
-                                        double* grad_vf, void* workspace_pi, int64_t workspace_pi_bytes,
-                                        void* workspace_vf, int64_t workspace_vf_bytes, int M_pi, int M_vf,
-                                        int O, int H_pi, int H_vf, int A, void* stream) {
-    if (!x || !params_pi || !params_vf || !dlogits || !dv || !grad_pi || !grad_vf || !workspace_pi ||
-        !workspace_vf)
-        return IMPALA_ERR_BAD_ARG;
-    if (pair_enabled() && A >= 2 && A <= 4 && impala_mlp_bwd_tc_eligible(x, dlogits, M_pi, O, H_pi, A) &&
-        impala_mlp_bwd_tc_eligible(x, dv, M_vf, O, H_vf, 1) &&
-        ((reinterpret_cast<uintptr_t>(grad_pi) | reinterpret_cast<uintptr_t>(grad_vf)) & 15) == 0) {
-        const int64_t need_pi = impala_mlp_backward_workspace(M_pi, O, H_pi, A);
-        const int64_t need_vf = impala_mlp_backward_workspace(M_vf, O, H_vf, 1);
-        if (need_pi < 0 || need_vf < 0) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-        if (workspace_pi_bytes < need_pi || workspace_vf_bytes < need_vf) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
-        return impala_mlp_bwd_tc_pair(
-            x, params_pi, params_vf, dlogits, dv,
-            reinterpret_cast<float*>(static_cast<char*>(workspace_pi) + kWsHeader),
-            reinterpret_cast<float*>(static_cast<char*>(workspace_vf) + kWsHeader), grad_pi, grad_vf,
-            static_cast<unsigned int*>(workspace_pi), M_pi, M_vf, O, H_pi, H_vf, A, (cudaStream_t)stream);
-    }
-    const int rc = impala_mlp_backward(x, params_pi, dlogits, grad_pi, workspace_pi, workspace_pi_bytes, M_pi,
-                                       O, H_pi, A, stream);
-    if (rc != IMPALA_OK) return rc;
-    return impala_mlp_backward(x, params_vf, dv, grad_vf, workspace_vf, workspace_vf_bytes, M_vf, O, H_vf, 1,
-                               stream);
-}
-
-// ---- data-parallel learner: the paired backward that pushes its result to the peers (optim.cu)
-extern "C" int impala_mlp_backward_pair_push_supported(int M_pi, int M_vf, int O, int H_pi, int H_vf, int A) {
-    alignas(16) static const float probe[4] = {0.f, 0.f, 0.f, 0.f};  // alignment stand-in for the data pointers
-    return pair_enabled() && A >= 2 && A <= 4 && impala_mlp_bwd_tc_eligible(probe, probe, M_pi, O, H_pi, A) &&
-           impala_mlp_bwd_tc_eligible(probe, probe, M_vf, O, H_vf, 1) &&
-           (M_pi + 63) / 64 + (M_vf + 63) / 64 >= 2;
-}
-
-extern "C" int impala_mlp_backward_pair_push(const float* x, const float* params_pi, const float* params_vf,
-                                             const float* dlogits, const float* dv, void* workspace_pi,
-                                             int64_t workspace_pi_bytes, void* workspace_vf,
-                                             int64_t workspace_vf_bytes, int M_pi, int M_vf, int O, int H_pi,
-                                             int H_vf, int A, const double* extra, int n_extra,
-                                             void* const* peer_gather, const long long* seq,
-                                             int64_t slot_stride, int64_t buf_stride, int rank, int world,
-                                             void* stream) {
-    if (!x || !params_pi || !params_vf || !dlogits || !dv || !workspace_pi || !workspace_vf || !peer_gather ||
-        !seq || (n_extra > 0 && !extra))
-        return IMPALA_ERR_BAD_ARG;
-    if (world < 1 || world > 8 || rank < 0 || rank >= world || n_extra < 0 || n_extra > 32) return IMPALA_ERR_BAD_ARG;
-    if (!impala_mlp_backward_pair_push_supported(M_pi, M_vf, O, H_pi, H_vf, A) ||
-        !impala_mlp_bwd_tc_eligible(x, dlogits, M_pi, O, H_pi, A) || !impala_mlp_bwd_tc_eligible(x, dv, M_vf, O, H_vf, 1))
-        return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    const int64_t n_pi = impala_make_layout(O, H_pi, A).total, n_vf = impala_make_layout(O, H_vf, 1).total;
-    if (slot_stride < n_pi + n_vf + n_extra || buf_stride < (int64_t)world * slot_stride) return IMPALA_ERR_BAD_ARG;
-    const int64_t need_pi = impala_mlp_backward_workspace(M_pi, O, H_pi, A);
-    const int64_t need_vf = impala_mlp_backward_workspace(M_vf, O, H_vf, 1);
-    if (need_pi < 0 || need_vf < 0) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    if (workspace_pi_bytes < need_pi || workspace_vf_bytes < need_vf) return IMPALA_ERR_WORKSPACE_TOO_SMALL;
-    const PushArgs push{reinterpret_cast<ulonglong2* const*>(peer_gather), seq, slot_stride, buf_stride, rank, world};
-    return impala_mlp_bwd_tc_pair(
-        x, params_pi, params_vf, dlogits, dv,
-        reinterpret_cast<float*>(static_cast<char*>(workspace_pi) + kWsHeader),
-        reinterpret_cast<float*>(static_cast<char*>(workspace_vf) + kWsHeader), nullptr, nullptr,
-        static_cast<unsigned int*>(workspace_pi), M_pi, M_vf, O, H_pi, H_vf, A, (cudaStream_t)stream, &push, extra,
-        n_extra);
 }

@@ -30,7 +30,7 @@
 // partial gradient row (same layout as the FP32 kernels) and the rows are summed in float64 in a fixed
 // order.
 //
-// Narrow shapes (impala_mlp_bwd_tc_eligible: one K atom, <= 4 outputs; bwd_blk_body): a CTA owns ONE
+// Narrow shapes (Narrow plans: one K atom, <= 4 outputs; bwd_blk_body): a CTA owns ONE
 // 64-unit hidden block of one network for the whole launch, so W1 of the block is loaded once and held
 // in registers as GEMM1's A operand (only the x tile is read from shared memory).  Its two warpgroups
 // are independent - each takes alternate tiles of the CTA's share, with its own x stage and named
@@ -42,10 +42,6 @@
 //
 // Wide shapes (bwd_tc_body): one CTA = 2 warpgroups = 128 hidden units per pass, wider layers walked
 // in passes (x is re-read once per pass); reduce_partials_kernel sums the rows.
-#include <map>
-#include <mutex>
-#include <tuple>
-
 #include "mlp_kernels.cuh"
 #include "tc_common.cuh"
 
@@ -954,24 +950,6 @@ __global__ void __launch_bounds__(kThreads) mlp_bwd_tcw_kernel(const __grid_cons
 
 static_assert(kWarps * 64 * sizeof(double) <= 2 * kXAtomBytes, "reduction scratch fits the x stage");
 
-// Dynamic shared memory opt-in (only ever raised, per kernel and device).
-template <typename K>
-cudaError_t opt_in(K kernel, size_t smem) {
-    static std::mutex mu;
-    static std::map<std::pair<const void*, int>, size_t> opted;
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    std::lock_guard<std::mutex> lock(mu);
-    size_t& o = opted[std::make_pair((const void*)kernel, dev)];
-    if (smem > o) {
-        if ((e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-            return e;
-        o = smem;
-    }
-    return cudaSuccess;
-}
-
 BwdTcArgs make_bwd_args(const float* x, const float* params, const float* dout, float* ws, double* grad,
                         unsigned int* ctl, int M, int O, int H, int N2) {
     BwdTcArgs a{};
@@ -999,12 +977,6 @@ void split_sets(int tiles_a, int tiles_b, int grid, int ga, int gb, int64_t wa, 
 
 }  // namespace
 
-bool impala_mlp_bwd_tc_eligible(const float* x, const float* dout, int M, int O, int H, int N2) {
-    return M >= 1 && O >= 4 && O <= 28 && (O & 3) == 0 && (H == 128 || H == 256) && N2 >= 1 &&
-           N2 <= 4 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
-           (reinterpret_cast<uintptr_t>(dout) & 15) == 0;
-}
-
 // Per-CTA partial gradient rows go to ws (same layout as the FP32 kernel), their float64 sum to
 // grad; ctl = two zeroed control words (see the grid barrier in the kernel).
 int impala_mlp_bwd_tc(const float* x, const float* params, const float* dout, float* ws,
@@ -1015,7 +987,8 @@ int impala_mlp_bwd_tc(const float* x, const float* params, const float* dout, fl
     int sms = 0;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
     auto kernel = N2 == 1 ? mlp_bwd_tc_kernel<1> : mlp_bwd_tc_kernel<4>;
-    if ((e = opt_in(kernel, smem)) != cudaSuccess) return (int)e;
+    int per_sm = 0;  // unused: the cooperative launch fails when the grid cannot be resident
+    if ((e = impala_resident_ctas((const void*)kernel, kThreads, smem, &per_sm)) != cudaSuccess) return (int)e;
     // every hidden block gets the same number of CTAs, no more than there are tiles (= partial rows the
     // workspace holds); grid <= SM count: the grid barrier needs residency
     const int nblk = H / 64;
@@ -1026,7 +999,7 @@ int impala_mlp_bwd_tc(const float* x, const float* params, const float* dout, fl
     return impala_launch_status();
 }
 
-// Both networks in one launch; the caller has checked eligibility of each and 2 <= A <= 4.
+// Both networks in one launch; the caller has routed each to a Narrow plan and checked 2 <= A <= 4.
 // push != nullptr: data-parallel variant (see mlp_bwd_tc_pair_kernel).
 int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* params_vf,
                            const float* dlogits, const float* dv, float* ws_pi, float* ws_vf,
@@ -1039,7 +1012,9 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
     cudaError_t e;
     int sms = 0;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
-    e = push ? opt_in(mlp_bwd_tc_pair_kernel<true>, smem) : opt_in(mlp_bwd_tc_pair_kernel<false>, smem);
+    int per_sm = 0;  // unused: the cooperative launch fails when the grid cannot be resident
+    e = impala_resident_ctas(push ? (const void*)mlp_bwd_tc_pair_kernel<true> : (const void*)mlp_bwd_tc_pair_kernel<false>,
+                             kThreads, smem, &per_sm);
     if (e != cudaSuccess) return (int)e;
     // a CTA does one hidden block of a tile whatever H is: the per-tile weights do not scale with H.  A
     // policy tile (4-output epilogue) costs about 1.25 value-function tiles (scripts/tune_pair_split.py)
@@ -1059,50 +1034,21 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
     return impala_launch_status();
 }
 
-// Wide shapes (impala_mlp_tcw_eligible): per-CTA float32 partial gradient rows into ws (row stride =
-// layout total); *nparts = rows written.
-int impala_mlp_bwd_tcw(const float* x, const float* params, const float* dout, float* ws, int M, int O, int H,
-                       int N2, cudaStream_t st, int* nparts) {
-    const BwdTcArgs a = make_bwd_args(x, params, dout, ws, nullptr, nullptr, M, O, H, N2);
-    const int ka = O <= 32 ? 1 : 2;
-    const int np = N2 == 1 ? 1 : (N2 <= 4 ? 4 : 16);
-    const size_t smem = bwd_smem_bytes(ka, np);
-    auto kernel = ka == 1 ? (np == 1 ? mlp_bwd_tcw_kernel<1, 1> : np == 4 ? mlp_bwd_tcw_kernel<4, 1> : mlp_bwd_tcw_kernel<16, 1>)
-                          : (np == 1 ? mlp_bwd_tcw_kernel<1, 2> : np == 4 ? mlp_bwd_tcw_kernel<4, 2> : mlp_bwd_tcw_kernel<16, 2>);
-    cudaError_t e;
-    int sms = 0, per_sm = 0;
-    if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
-    if ((e = opt_in(kernel, smem)) != cudaSuccess) return (int)e;
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem)) != cudaSuccess) return (int)e;
-    if (per_sm < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    int grid = per_sm * sms;
-    if (grid > a.num_tiles) grid = a.num_tiles;
-    if (grid > kMaxParts) grid = kMaxParts;
-    if ((e = impala_launch(kernel, grid, kThreads, smem, st, true, a)) != cudaSuccess) return (int)e;
-    *nparts = grid;
-    return impala_launch_status();
-}
-
-// Beyond the wide kernels' limits (impala_mlp_bwd_tcx_eligible): four K atoms, GEMM2 in 64-feature halves,
-// 32-row tiles; 5..32 outputs through shared memory, padded to 32.  Partial rows as impala_mlp_bwd_tcw.
-bool impala_mlp_bwd_tcx_eligible(const float* x, int M, int O, int H, int N2) {
-    return M >= 1 && O >= 4 && O <= 128 && (O & 3) == 0 && H >= 128 && H % 128 == 0 && H <= 4096 && N2 >= 1 &&
-           N2 <= 32 && (O > 64 || N2 > 16) && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
-           impala_env_int("IMPALA_MLP_TCW", 1) != 0;
-}
-
-int impala_mlp_bwd_tcx(const float* x, const float* params, const float* dout, float* ws, int M, int O, int H,
-                       int N2, cudaStream_t st, int* nparts) {
+// Wide plans: per-CTA float32 partial gradient rows into ws (row stride = layout total); *nparts = rows
+// written.  At four K atoms (GEMM2 in 64-feature halves) the tiles are 32 rows high.
+int impala_mlp_bwd_tcw(const MlpPlan& p, const float* x, const float* params, const float* dout, float* ws, int M,
+                       int O, int H, int N2, cudaStream_t st, int* nparts) {
     BwdTcArgs a = make_bwd_args(x, params, dout, ws, nullptr, nullptr, M, O, H, N2);
-    a.num_tiles = (M + 31) / 32;  // 32-row tiles at four K atoms
-    const int np = N2 == 1 ? 1 : (N2 <= 4 ? 4 : 32);
-    const size_t smem = bwd_smem_bytes(4, np);
-    auto kernel = np == 1 ? mlp_bwd_tcw_kernel<1, 4> : (np == 4 ? mlp_bwd_tcw_kernel<4, 4> : mlp_bwd_tcw_kernel<32, 4>);
+    a.num_tiles = (M + p.rows - 1) / p.rows;
+    const int np = p.np;
+    auto kernel = p.ka == 1   ? (np == 1 ? mlp_bwd_tcw_kernel<1, 1> : np == 4 ? mlp_bwd_tcw_kernel<4, 1> : mlp_bwd_tcw_kernel<16, 1>)
+                  : p.ka == 2 ? (np == 1 ? mlp_bwd_tcw_kernel<1, 2> : np == 4 ? mlp_bwd_tcw_kernel<4, 2> : mlp_bwd_tcw_kernel<16, 2>)
+                              : (np == 1 ? mlp_bwd_tcw_kernel<1, 4> : np == 4 ? mlp_bwd_tcw_kernel<4, 4> : mlp_bwd_tcw_kernel<32, 4>);
+    const size_t smem = bwd_smem_bytes(p.ka, np);
     cudaError_t e;
     int sms = 0, per_sm = 0;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
-    if ((e = opt_in(kernel, smem)) != cudaSuccess) return (int)e;
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem)) != cudaSuccess) return (int)e;
+    if ((e = impala_resident_ctas((const void*)kernel, kThreads, smem, &per_sm)) != cudaSuccess) return (int)e;
     if (per_sm < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
     int grid = per_sm * sms;
     if (grid > a.num_tiles) grid = a.num_tiles;

@@ -26,10 +26,6 @@
 // layers walk their blocks in passes: out[row] = ((b2 + z_0) + z_1) + ...  where the thread that
 // owns a row adds the block's partial second-layer sum to what the SAME thread wrote in the
 // previous pass (fixed order, bitwise reproducible, no workspace).
-#include <map>
-#include <mutex>
-#include <tuple>
-
 #include "mlp_fwd_tc.cuh"
 #include "tc_common.cuh"
 
@@ -341,41 +337,24 @@ mlp_fwd_tc_pair_kernel(const __grid_constant__ FwdTcArgs a_pi, const __grid_cons
     fwd_rs_body<4, 1>(a, pi ? (int)blockIdx.x : (int)blockIdx.x - n_pi, pi ? n_pi : (int)gridDim.x - n_pi);
 }
 
-FwdTcArgs make_fwd_args(const float* x, const float* params, float* out, int M, int O, int H, int N2) {
+FwdTcArgs make_fwd_args(const float* x, const float* params, float* out, int M, int O, int H, int N2, int hb) {
     FwdTcArgs a{};
     a.x = x, a.params = params, a.out = out;
     a.M = M, a.O = O, a.H = H, a.N2 = N2;
     a.num_tiles = (M + kTileM - 1) / kTileM;
-    a.hb = H <= 256 ? H : (H % 256 == 0 ? 256 : 128);
+    a.hb = hb;
     a.lay = impala_make_layout(O, H, N2);
     return a;
 }
 
-// Resident CTAs per SM of `kernel` at `smem` bytes (dynamic shared memory opted in on first use;
-// the attribute is only ever raised) times the SM count.
-template <typename K>
-int resident_grid(K kernel, size_t smem, int* grid) {
-    static std::mutex mu;
-    static std::map<std::pair<const void*, int>, size_t> opted;          // (kernel, dev) -> smem opted in
-    static std::map<std::tuple<const void*, int, size_t>, int> cached;  // (kernel, dev, smem) -> grid
-    int dev = 0, sms = 0;
+// Resident CTAs of `kernel` on the whole device at `smem` bytes.
+int resident_grid(const void* kernel, size_t smem, int* grid) {
+    int per_sm = 0, sms = 0;
     cudaError_t e;
-    if ((e = cudaGetDevice(&dev)) != cudaSuccess) return (int)e;
-    std::lock_guard<std::mutex> lock(mu);
-    const auto key = std::make_tuple((const void*)kernel, dev, smem);
-    auto it = cached.find(key);
-    if (it != cached.end()) return *grid = it->second, IMPALA_OK;
-    size_t& o = opted[std::make_pair((const void*)kernel, dev)];
-    if (smem > o) {
-        if ((e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-            return (int)e;
-        o = smem;
-    }
-    int per_sm = 0;
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem)) != cudaSuccess) return (int)e;
+    if ((e = impala_resident_ctas(kernel, kThreads, smem, &per_sm)) != cudaSuccess) return (int)e;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
     if (per_sm < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    *grid = cached[key] = per_sm * sms;
+    *grid = per_sm * sms;
     return IMPALA_OK;
 }
 
@@ -383,41 +362,42 @@ template <int NP, int KA>
 int launch_fwd(const FwdTcArgs& a, cudaStream_t st) {
     const size_t smem = fwd_smem_bytes(a.hb, KA, NP);
     int grid = 0;
-    const int rc = resident_grid(mlp_fwd_tc_kernel<NP, KA>, smem, &grid);
+    const int rc = resident_grid((const void*)mlp_fwd_tc_kernel<NP, KA>, smem, &grid);
     if (rc != IMPALA_OK) return rc;
     const int want = (a.num_tiles + kWG - 1) / kWG;
     mlp_fwd_tc_kernel<NP, KA><<<want < grid ? want : grid, kThreads, smem, st>>>(a);
     return impala_launch_status();
 }
 
+template <int KA>
+int launch_fwd_ka(int np, const FwdTcArgs& a, cudaStream_t st) {
+    return np == 1 ? launch_fwd<1, KA>(a, st) : np == 4 ? launch_fwd<4, KA>(a, st)
+                   : np == 16 ? launch_fwd<16, KA>(a, st) : launch_fwd<32, KA>(a, st);
+}
+
 }  // namespace
 
-// Shapes the narrow tensor-core path covers (one K atom, the whole hidden layer in one pass).
-bool impala_mlp_fwd_tc_eligible(const float* x, int M, int O, int H, int N2) {
-    return M >= 1 && O >= 4 && O <= 28 && (O & 3) == 0 && H >= 16 && H <= 256 && (H & 31) == 0 &&
-           N2 >= 1 && N2 <= 4 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
-}
-
-int impala_mlp_fwd_tc(const float* x, const float* params, float* out, int M, int O, int H, int N2,
+int impala_mlp_fwd_tc(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
                       cudaStream_t st) {
-    const FwdTcArgs a = make_fwd_args(x, params, out, M, O, H, N2);
-    return N2 == 1 ? launch_fwd<1, 1>(a, st) : launch_fwd<4, 1>(a, st);
+    const FwdTcArgs a = make_fwd_args(x, params, out, M, O, H, N2, p.hb);
+    return p.ka == 1 ? launch_fwd_ka<1>(p.np, a, st) : p.ka == 2 ? launch_fwd_ka<2>(p.np, a, st)
+                                                     : launch_fwd_ka<4>(p.np, a, st);
 }
 
-// Both networks in one launch (policy: 2..4 outputs, value fn: 1 output); the caller has checked
-// impala_mlp_fwd_tc_eligible for each.  Per-tile cost weights split the CTAs between the two tile
-// lists; both networks run the same MMAs and the same 4-output epilogue per tile, so the default
-// weighs a policy tile as one value-function tile.
+// Both networks in one launch (policy: 2..4 outputs, value fn: 1 output); the caller has routed each
+// to a Narrow plan, which holds the whole hidden layer in one pass.  Per-tile cost weights split the
+// CTAs between the two tile lists; both networks run the same MMAs and the same 4-output epilogue per
+// tile, so the default weighs a policy tile as one value-function tile.
 int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* params_vf, float* logits,
                            float* values, int M_pi, int M_vf, int O, int H_pi, int H_vf, int A,
                            cudaStream_t st) {
-    const FwdTcArgs a_pi = make_fwd_args(x, params_pi, logits, M_pi, O, H_pi, A);
-    const FwdTcArgs a_vf = make_fwd_args(x, params_vf, values, M_vf, O, H_vf, 1);
+    const FwdTcArgs a_pi = make_fwd_args(x, params_pi, logits, M_pi, O, H_pi, A, H_pi);
+    const FwdTcArgs a_vf = make_fwd_args(x, params_vf, values, M_vf, O, H_vf, 1, H_vf);
     // both networks stage W2 in the 4-output layout (one body instantiation, see the kernel)
     const size_t s_pi = fwd_smem_bytes(a_pi.hb, 1, 4), s_vf = fwd_smem_bytes(a_vf.hb, 1, 4);
     const size_t smem = s_pi > s_vf ? s_pi : s_vf;
     int grid = 0;
-    const int rc = resident_grid(mlp_fwd_tc_pair_kernel, smem, &grid);
+    const int rc = resident_grid((const void*)mlp_fwd_tc_pair_kernel, smem, &grid);
     if (rc != IMPALA_OK) return rc;
     const int units_pi = (a_pi.num_tiles + kWG - 1) / kWG, units_vf = (a_vf.num_tiles + kWG - 1) / kWG;
     if (grid > units_pi + units_vf) grid = units_pi + units_vf;
@@ -426,46 +406,4 @@ int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* 
                                        100 * (H_vf / 32));
     mlp_fwd_tc_pair_kernel<<<grid, kThreads, smem, st>>>(a_pi, a_vf, n_pi);
     return impala_launch_status();
-}
-
-// Wide shapes (observation width up to 64 = two K atoms, hidden layers a multiple of 128 of any
-// size, walked in passes, up to 16 outputs): BASELINE config c5 (obs = 64, hidden = 512), and policies
-// with an Atari minimal action set (5..16 actions; epilogue padded to 16 outputs).  IMPALA_MLP_TCW=0
-// disables.
-bool impala_mlp_tcw_eligible(const float* x, int M, int O, int H, int N2) {
-    return M >= 1 && O >= 4 && O <= 64 && (O & 3) == 0 && H >= 128 && H % 128 == 0 && H <= 4096 && N2 >= 1 &&
-           N2 <= 16 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && impala_env_int("IMPALA_MLP_TCW", 1) != 0;
-}
-
-int impala_mlp_fwd_tcw(const float* x, const float* params, float* out, int M, int O, int H, int N2,
-                       cudaStream_t st) {
-    // 256 hidden units per pass fit at 16 outputs too: 88 064 B at one K atom, 219 136 B at two
-    const FwdTcArgs a = make_fwd_args(x, params, out, M, O, H, N2);
-    if (O <= 32) return N2 == 1 ? launch_fwd<1, 1>(a, st) : N2 <= 4 ? launch_fwd<4, 1>(a, st) : launch_fwd<16, 1>(a, st);
-    return N2 == 1 ? launch_fwd<1, 2>(a, st) : N2 <= 4 ? launch_fwd<4, 2>(a, st) : launch_fwd<16, 2>(a, st);
-}
-
-// Beyond the wide kernels' limits: observations up to 128 (four K atoms) or 17..32 outputs (the
-// epilogue keeps 2 x 32 partial sums per thread).  Shapes that the kernels above take never get here.
-bool impala_mlp_fwd_tcx_eligible(const float* x, int M, int O, int H, int N2) {
-    return M >= 1 && O >= 4 && O <= 128 && (O & 3) == 0 && H >= 128 && H % 128 == 0 && H <= 4096 && N2 >= 1 &&
-           N2 <= 32 && (O > 64 || N2 > 16) && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
-           impala_env_int("IMPALA_MLP_TCW", 1) != 0;
-}
-
-int impala_mlp_fwd_tcx(const float* x, const float* params, float* out, int M, int O, int H, int N2,
-                       cudaStream_t st) {
-    FwdTcArgs a = make_fwd_args(x, params, out, M, O, H, N2);
-    if (N2 > 16) {
-        if (O <= 32) return launch_fwd<32, 1>(a, st);
-        if (O <= 64) {
-            a.hb = 128;  // 256 units would need 235 520 B with the padded W2 rows
-            return launch_fwd<32, 2>(a, st);
-        }
-    }
-    // four K atoms: 64 hidden units per pass keep W1 hi / lo + both warpgroups' x stages in 227 KB
-    a.hb = 64;
-    if (N2 > 16) return launch_fwd<32, 4>(a, st);
-    if (N2 > 4) return launch_fwd<16, 4>(a, st);
-    return N2 == 1 ? launch_fwd<1, 4>(a, st) : launch_fwd<4, 4>(a, st);
 }

@@ -30,18 +30,33 @@ constexpr int kMaxParts = 1024;  // upper bound on persistent CTAs (= per-CTA pa
 int impala_mlp_launch(void (*kernel)(MlpArgs), const MlpArgs& a, const MlpConfig& c, size_t smem,
                       cudaStream_t st, int* grid_out);
 
-// Tensor-core (wgmma, 3xTF32) forward for GEMM-shaped layers, defined in mlp_fwd_tc.cu.
-bool impala_mlp_fwd_tc_eligible(const float* x, int M, int O, int H, int N2);
-int impala_mlp_fwd_tc(const float* x, const float* params, float* out, int M, int O, int H, int N2,
+// Which kernels run one MLP call: decided by the route in mlp.cu, carried out by the launchers below.
+enum class MlpKernel {
+    Fp32,    // FP32 CUDA-core kernels (mlp_kernels.cuh / mlp_inst.cu), configuration `fp32`
+    Narrow,  // tensor-core block kernels: forward mlp_fwd_tc_kernel<NP, 1>, backward mlp_bwd_tc_kernel<NP>
+    Wide,    // tensor-core pass kernels: mlp_fwd_tc_kernel<NP, KA>, mlp_bwd_tcw_kernel<NP, KA>
+    Obs,     // K-streamed tensor-core kernels for O > 128 (mlp_obs_tc.cu)
+};
+struct MlpPlan {
+    MlpKernel kernel;
+    int np, ka;             // template parameters <NP, KA> (padded outputs, 32-feature K atoms)
+    int hb;                 // forward: hidden units per pass
+    int rows;               // backward: batch rows per tile
+    bool reduce_in_kernel;  // backward: the kernel sums its partial rows into grad itself
+    int64_t ws;             // backward: workspace bytes the call needs
+    MlpConfig fp32;         // the FP32 kernels' configuration (backward: always, it sizes the workspace)
+};
+
+// Tensor-core (wgmma, 3xTF32) forward of the Narrow and Wide plans, defined in mlp_fwd_tc.cu.
+int impala_mlp_fwd_tc(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
                       cudaStream_t st);
 
-// Policy + value network in one launch (CTA ranges per network); A in 2..4, both nets eligible.
+// Policy + value network in one launch (CTA ranges per network); A in 2..4, both nets on Narrow plans.
 int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* params_vf, float* logits,
                            float* values, int M_pi, int M_vf, int O, int H_pi, int H_vf, int A,
                            cudaStream_t st);
 
-// Tensor-core backward (mlp_bwd_tc.cu): per-CTA partial rows into ws, reduced in-kernel to grad.
-bool impala_mlp_bwd_tc_eligible(const float* x, const float* dout, int M, int O, int H, int N2);
+// Tensor-core backward of a Narrow plan (mlp_bwd_tc.cu): per-CTA partial rows into ws, reduced in-kernel to grad.
 int impala_mlp_bwd_tc(const float* x, const float* params, const float* dout, float* ws,
                       double* grad, unsigned int* ctl, int M, int O, int H, int N2, cudaStream_t st);
 
@@ -51,43 +66,28 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
                            int H_pi, int H_vf, int A, cudaStream_t st, const PushArgs* push = nullptr,
                            const double* extra = nullptr, int n_extra = 0);
 
-// Wide tensor-core kernels (forward in mlp_fwd_tc.cu, backward in mlp_bwd_tc.cu): O <= 64, H a multiple
-// of 128, N2 <= 16 (BASELINE c5: O = 64, H = 512).  The forward needs no workspace; the backward leaves *nparts float32 partial rows in ws for
-// reduce_partials_kernel.  IMPALA_MLP_TCW=0 disables them.
-bool impala_mlp_tcw_eligible(const float* x, int M, int O, int H, int N2);
-int impala_mlp_fwd_tcw(const float* x, const float* params, float* out, int M, int O, int H, int N2,
-                       cudaStream_t st);
-int impala_mlp_bwd_tcw(const float* x, const float* params, const float* dout, float* ws, int M, int O, int H,
-                       int N2, cudaStream_t st, int* nparts);
+// Tensor-core backward of a Wide plan (mlp_bwd_tc.cu): *nparts float32 partial rows in ws for
+// reduce_partials_kernel.
+int impala_mlp_bwd_tcw(const MlpPlan& p, const float* x, const float* params, const float* dout, float* ws, int M,
+                       int O, int H, int N2, cudaStream_t st, int* nparts);
 
-// Wide tensor-core forward of the shapes beyond the limits above (O in 65..128 = four K atoms, or N2 in
-// 17..32; O in 65..128 takes N2 in 5..16 as well): O % 4 == 0, H a multiple of 128 up to 4096.
-// IMPALA_MLP_TCW=0 disables them too.
-bool impala_mlp_fwd_tcx_eligible(const float* x, int M, int O, int H, int N2);
-int impala_mlp_fwd_tcx(const float* x, const float* params, float* out, int M, int O, int H, int N2,
+// Obs plans (mlp_obs_tc.cu): 128 < O <= 1024, K streamed.  Byte observations (values 0..255) enter the
+// network as they are.
+int impala_mlp_fwd_obs(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
                        cudaStream_t st);
-// ... and its backward (mlp_bwd_tc.cu): per-CTA float32 partial rows in ws, *nparts of them.
-bool impala_mlp_bwd_tcx_eligible(const float* x, int M, int O, int H, int N2);
-int impala_mlp_bwd_tcx(const float* x, const float* params, const float* dout, float* ws, int M, int O, int H,
-                       int N2, cudaStream_t st, int* nparts);
-
-// Wide observations (mlp_obs_tc.cu): 128 < O <= 1024, O % 4 == 0, H a multiple of 128 up to 1024, N2 <= 32,
-// K streamed; false under IMPALA_MLP_TC=0 / IMPALA_MLP_TCW=0 (there is no FP32 kernel for these widths).
-bool impala_mlp_obs_shape_ok(int M, int O, int H, int N2);
-int impala_mlp_fwd_obs(const float* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st);
-// The same with byte observations (values 0..255 enter the network as they are); x 4-byte aligned.
-int impala_mlp_fwd_obs(const uint8_t* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st);
+int impala_mlp_fwd_obs(const MlpPlan& p, const uint8_t* x, const float* params, float* out, int M, int O, int H,
+                       int N2, cudaStream_t st);
 // Backward workspace past the control header: byte offsets of DP^T and of the two sets of float32 partial
 // rows (r1 rows of layout entries [ob1, total), p2 rows of [0, ob1)) for reduce_partials_kernel.
 struct ObsBwdLayout {
     int64_t dpt_off, rest_off, w1_off, bytes;
     int mp, r1, p2;
 };
-bool impala_mlp_obs_bwd_layout(int M, int O, int H, int N2, ObsBwdLayout* L);
-int impala_mlp_bwd_obs(const float* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L, int M,
-                       int O, int H, int N2, cudaStream_t st);
-int impala_mlp_bwd_obs(const uint8_t* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L,
-                       int M, int O, int H, int N2, cudaStream_t st);
+ObsBwdLayout impala_mlp_obs_bwd_layout(int M, int O, int H, int N2);
+int impala_mlp_bwd_obs(const MlpPlan& p, const float* x, const float* params, const float* dout, void* ws,
+                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st);
+int impala_mlp_bwd_obs(const MlpPlan& p, const uint8_t* x, const float* params, const float* dout, void* ws,
+                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st);
 
 // One per padded observation width / direction, defined in mlp_inst.cu.
 #define IMPALA_DECL_DISPATCH(OPV)                                                             \

@@ -36,9 +36,6 @@
 // keep their order and the first of a chunk takes over scale-d = 0, so each accumulator sees the same
 // non-zero additions in the same order as the float kernels on the same values converted to float.
 #include <algorithm>
-#include <cstdlib>
-#include <map>
-#include <mutex>
 
 #include "mlp_fwd_tc.cuh"
 #include "tc_common.cuh"
@@ -478,38 +475,18 @@ constexpr size_t kPreSmem(int np) {
 }
 constexpr size_t kDw1Smem = 1024 + kStageBytes;
 
-// Dynamic shared memory opt-in (only ever raised, per kernel and device) and launch.
 template <typename... KArgs, typename... Args>
 int launch(void (*kernel)(KArgs...), dim3 grid, size_t smem, cudaStream_t st, Args&&... args) {
-    static std::mutex mu;
-    static std::map<std::pair<const void*, int>, size_t> opted;
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return (int)e;
-    {
-        std::lock_guard<std::mutex> lock(mu);
-        size_t& o = opted[std::make_pair((const void*)kernel, dev)];
-        if (smem > o) {
-            if ((e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-                return (int)e;
-            o = smem;
-        }
-    }
+    int per_sm = 0;  // unused: the grid is one CTA per tile / block whatever the residency
+    if (const cudaError_t e = impala_resident_ctas((const void*)kernel, kT, smem, &per_sm); e != cudaSuccess)
+        return (int)e;
     kernel<<<grid, kT, smem, st>>>(static_cast<Args&&>(args)...);
     return impala_launch_status();
 }
 
-int np_of(int N2) { return N2 == 1 ? 1 : (N2 <= 4 ? 4 : 32); }
-
-// x alignment the loads need: 16 bytes for float rows, 4 for byte rows (O % 4 == 0 keeps every row aligned)
 template <typename XT>
-bool x_aligned(const XT* x) {
-    return (reinterpret_cast<uintptr_t>(x) & (sizeof(XT) == 4 ? 15 : 3)) == 0;
-}
-
-template <typename XT>
-int fwd_obs(const XT* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st) {
-    if (!impala_mlp_obs_shape_ok(M, O, H, N2) || !x_aligned(x)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+int fwd_obs(const MlpPlan& p, const XT* x, const float* params, float* out, int M, int O, int H, int N2,
+            cudaStream_t st) {
     FwdTcArgs a{};
     a.x = sizeof(XT) == 4 ? reinterpret_cast<const float*>(x) : nullptr, a.params = params, a.out = out;
     a.M = M, a.O = O, a.H = H, a.N2 = N2;
@@ -517,7 +494,7 @@ int fwd_obs(const XT* x, const float* params, float* out, int M, int O, int H, i
     a.hb = kHBlk;
     a.lay = impala_make_layout(O, H, N2);
     const dim3 grid(a.num_tiles);
-    switch (np_of(N2)) {
+    switch (p.np) {
         case 1: return launch(mlp_fwd_obs_kernel<1, XT>, grid, kFwdSmem(1), st, a, x);
         case 4: return launch(mlp_fwd_obs_kernel<4, XT>, grid, kFwdSmem(4), st, a, x);
         default: return launch(mlp_fwd_obs_kernel<32, XT>, grid, kFwdSmem(32), st, a, x);
@@ -525,9 +502,8 @@ int fwd_obs(const XT* x, const float* params, float* out, int M, int O, int H, i
 }
 
 template <typename XT>
-int bwd_obs(const XT* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L, int M, int O,
-            int H, int N2, cudaStream_t st) {
-    if (!x_aligned(x)) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+int bwd_obs(const MlpPlan& p, const XT* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L,
+            int M, int O, int H, int N2, cudaStream_t st) {
     ObsBwdArgs a{};
     a.x = x, a.params = params, a.dout = dout;
     a.dpt = reinterpret_cast<float*>(static_cast<char*>(ws) + L.dpt_off);
@@ -539,7 +515,7 @@ int bwd_obs(const XT* x, const float* params, const float* dout, void* ws, const
     a.lay = impala_make_layout(O, H, N2);
     const dim3 g1(L.r1, H / kHBlk);
     int rc;
-    switch (np_of(N2)) {
+    switch (p.np) {
         case 1: rc = launch(mlp_bwd_obs_pre_kernel<1, XT>, g1, kPreSmem(1), st, a); break;
         case 4: rc = launch(mlp_bwd_obs_pre_kernel<4, XT>, g1, kPreSmem(4), st, a); break;
         default: rc = launch(mlp_bwd_obs_pre_kernel<32, XT>, g1, kPreSmem(32), st, a); break;
@@ -550,43 +526,39 @@ int bwd_obs(const XT* x, const float* params, const float* dout, void* ws, const
 
 }  // namespace
 
-bool impala_mlp_obs_shape_ok(int M, int O, int H, int N2) {
-    const char* tc_env = std::getenv("IMPALA_MLP_TC");
-    return M >= 1 && O > 128 && O <= 1024 && (O & 3) == 0 && H >= 128 && H <= 1024 && H % 128 == 0 && N2 >= 1 &&
-           N2 <= 32 && !(tc_env && tc_env[0] == '0') && impala_env_int("IMPALA_MLP_TCW", 1) != 0;
+int impala_mlp_fwd_obs(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
+                       cudaStream_t st) {
+    return fwd_obs(p, x, params, out, M, O, H, N2, st);
 }
-
-int impala_mlp_fwd_obs(const float* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st) {
-    return fwd_obs(x, params, out, M, O, H, N2, st);
-}
-int impala_mlp_fwd_obs(const uint8_t* x, const float* params, float* out, int M, int O, int H, int N2, cudaStream_t st) {
-    return fwd_obs(x, params, out, M, O, H, N2, st);
+int impala_mlp_fwd_obs(const MlpPlan& p, const uint8_t* x, const float* params, float* out, int M, int O, int H,
+                       int N2, cudaStream_t st) {
+    return fwd_obs(p, x, params, out, M, O, H, N2, st);
 }
 
 // Workspace past the control header: DP^T [H][mp] | r1 partial rows of [ob1, total) | p2 partial rows of
 // [0, ob1), each region 256-byte aligned.  r1 (backward-1 CTAs per hidden block) and p2 (batch-row ranges
 // of backward 2) depend on the shape only: about 512 CTAs per phase, so the partial rows stay small next
 // to DP^T.
-bool impala_mlp_obs_bwd_layout(int M, int O, int H, int N2, ObsBwdLayout* L) {
-    if (!impala_mlp_obs_shape_ok(M, O, H, N2)) return false;
+ObsBwdLayout impala_mlp_obs_bwd_layout(int M, int O, int H, int N2) {
+    ObsBwdLayout L;
     const MlpLayout lay = impala_make_layout(O, H, N2);
     const int tiles = (M + kTileM - 1) / kTileM, nblk = H / kHBlk, nfb = (O + kFBlk - 1) / kFBlk;
     const int nc = tiles * kTileM / 32;
-    L->mp = tiles * kTileM;
-    L->r1 = std::min(tiles, (512 + nblk - 1) / nblk);
-    L->p2 = std::min(nc, std::max(1, 512 / (nblk * nfb)));
-    L->dpt_off = 0;
-    L->rest_off = impala_round_up((int64_t)H * L->mp * (int64_t)sizeof(float), 256);
-    L->w1_off = L->rest_off + impala_round_up((int64_t)L->r1 * (lay.total - lay.ob1) * (int64_t)sizeof(float), 256);
-    L->bytes = L->w1_off + (int64_t)L->p2 * lay.ob1 * (int64_t)sizeof(float);
-    return true;
+    L.mp = tiles * kTileM;
+    L.r1 = std::min(tiles, (512 + nblk - 1) / nblk);
+    L.p2 = std::min(nc, std::max(1, 512 / (nblk * nfb)));
+    L.dpt_off = 0;
+    L.rest_off = impala_round_up((int64_t)H * L.mp * (int64_t)sizeof(float), 256);
+    L.w1_off = L.rest_off + impala_round_up((int64_t)L.r1 * (lay.total - lay.ob1) * (int64_t)sizeof(float), 256);
+    L.bytes = L.w1_off + (int64_t)L.p2 * lay.ob1 * (int64_t)sizeof(float);
+    return L;
 }
 
-int impala_mlp_bwd_obs(const float* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L, int M,
-                       int O, int H, int N2, cudaStream_t st) {
-    return bwd_obs(x, params, dout, ws, L, M, O, H, N2, st);
+int impala_mlp_bwd_obs(const MlpPlan& p, const float* x, const float* params, const float* dout, void* ws,
+                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st) {
+    return bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st);
 }
-int impala_mlp_bwd_obs(const uint8_t* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L,
-                       int M, int O, int H, int N2, cudaStream_t st) {
-    return bwd_obs(x, params, dout, ws, L, M, O, H, N2, st);
+int impala_mlp_bwd_obs(const MlpPlan& p, const uint8_t* x, const float* params, const float* dout, void* ws,
+                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st) {
+    return bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st);
 }
