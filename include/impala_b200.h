@@ -109,6 +109,19 @@ int impala_ingest_shard_frames(void* dev_slab, const void* host_slab, int T, int
 int impala_obs_unstack(const void* frames, int in_dtype, void* out, int out_dtype, int R, int B, int F, int k,
                        void* stream);
 
+/* Experience replay: build the dense B-column training slab (impala_batch_layout_frames(T, B, ...)) out of a
+ * store of Bf-column slabs (impala_batch_layout_frames(T, Bf, ...) each, store_slab_bytes apart, the fresh
+ * batches of past updates).  For every one of the six tensors, column j of the training slab is column
+ * plan[2j+1] of store slab plan[2j]; a negative slab index gives the empty trajectory (every byte zero,
+ * lens = 0).  Pure data movement on bytes, one launch: any obs_dtype, dense and frame slabs.  plan is a device
+ * array of B int32 pairs, 8-byte aligned.  16-byte loads and stores for the tensors whose bytes per (row,
+ * column) are a multiple of 16 when both slabs and store_slab_bytes are 16-byte aligned, 4-byte words or single
+ * bytes otherwise.  Bf <= 0, Bf >= B, store_slab_bytes smaller than the Bf-column slab, a NULL pointer or
+ * arguments impala_batch_layout_frames refuses return IMPALA_ERR_BAD_ARG.  The plan's entries are not
+ * checked: slab indices and columns < Bf are the caller's to keep in range. */
+int impala_batch_compose(void* dst_slab, const void* store, int64_t store_slab_bytes, const int32_t* plan, int T,
+                         int B, int Bf, int F, int frames, int A, int obs_dtype, void* stream);
+
 /* out[i] = (float)x[i] for i < n: exact widening of byte observations, for the MLP shapes that read
  * float32 rows only (O <= 128). */
 int impala_obs_u8_to_f32(const uint8_t* x, float* out, int64_t n, void* stream);

@@ -3,6 +3,7 @@
 
     python scripts/learner_e2e.py [--config c3|c4] [--actors 32] [--updates 300] [--devices 1]
                                   [--payload block|trajectory] [--block 128] [--obs-dtype float32|uint8]
+                                  [--replay-slabs R --replay-columns Br]
 
 Prints ONE JSON line: learner steps/s and trajectories/s measured on the shared update counter
 between update `warmup` and the last one (wall clock of the launcher, which never touches CUDA -
@@ -12,6 +13,8 @@ format, one `utils.Trajectory` of ~5T tiny tensors per put (what an unmodified a
 --obs-dtype uint8: byte observations (0..255, as Atari RAM) in the ring, the slabs and the MLP kernels.
 --frames k: the observations are k stacked frames, stored once per frame in the ring and the slabs (block
 actors push (T+k, n, O/k) frame blocks, trajectory actors the stacked observations).
+--replay-slabs R --replay-columns Br: experience replay; the ring gets B - Br columns, every update takes that
+many fresh trajectories and Br out of HBM, and the line also reports fresh_trajectories_per_s.
 Run in a fresh interpreter (bench.py spawns it as a subprocess)."""
 import argparse
 import json
@@ -72,6 +75,8 @@ def main():
     ap.add_argument("--deadline", type=float, default=120.0)
     ap.add_argument("--obs-dtype", default="float32", choices=["float32", "uint8"])
     ap.add_argument("--frames", type=int, default=1)
+    ap.add_argument("--replay-slabs", type=int, default=0)
+    ap.add_argument("--replay-columns", type=int, default=0)
     a = ap.parse_args()
     w = CFG[a.config]
     mp.set_start_method("fork", force=True)
@@ -80,14 +85,16 @@ def main():
                          max_updates=a.updates, verbose=0, eval_every=None, save_every=10 ** 9, n_actors=a.actors)
     policy, value_fn = MlpPolicy(w["O"], w["A"], w["H"]), MlpValueFn(w["O"], w["H"])
     policy.share_memory()
-    block = min(a.block, w["B"])
-    while w["B"] % block:
+    B_fresh = w["B"] - a.replay_columns  # trajectories an update takes from the actors
+    block = min(a.block, B_fresh)
+    while B_fresh % block:
         block //= 2
-    ring = RingQueue(w["T"], w["B"], w["O"], w["A"], slabs=3, obs_dtype=a.obs_dtype, frames=a.frames)
+    ring = RingQueue(w["T"], B_fresh, w["O"], w["A"], slabs=3, obs_dtype=a.obs_dtype, frames=a.frames)
     counter = Counter(0)
     devices = [f"cuda:{i}" for i in range(a.devices)]
     lrn = Learner(1, hp, policy, value_fn, ring, counter, log_path=None, timeout=120, devices=devices,
-                  publish_every=a.publish_every, obs_dtype=a.obs_dtype, frames=a.frames)
+                  publish_every=a.publish_every, obs_dtype=a.obs_dtype, frames=a.frames,
+                  replay_slabs=a.replay_slabs, replay_columns=a.replay_columns)
     obs_kind = "bytes" if a.obs_dtype == "uint8" else "normal"
     actors = [mp.Process(target=actor_main, args=(i, ring, lrn.completion, w, a.payload, block, 100 + i, obs_kind, a.frames),
                          daemon=True) for i in range(a.actors)]
@@ -128,7 +135,9 @@ def main():
         what="steps/s through Learner + RingQueue + synthetic actor processes (wall clock on the shared update counter)",
         config=a.config, **w, actors=a.actors, payload=a.payload, block=block if a.payload == "block" else 1,
         devices=a.devices, **({"obs_dtype": a.obs_dtype} if a.obs_dtype != "float32" else {}),
-        **({"frames": a.frames} if a.frames != 1 else {}), updates_timed=c_end - c_w, steps_per_s=sps, trajectories_per_s=sps * w["B"],
+        **({"frames": a.frames} if a.frames != 1 else {}),
+        **(dict(replay_slabs=a.replay_slabs, replay_columns=a.replay_columns, fresh_trajectories_per_s=sps * B_fresh)
+           if a.replay_slabs else {}), updates_timed=c_end - c_w, steps_per_s=sps, trajectories_per_s=sps * w["B"],
         h2d_bytes_per_step=int(ring.slab_bytes), weight_publications=(lrn.policy_version - (v0 or 0)) // 2,
         publish_every=a.publish_every, host_cores=os.cpu_count())))
 

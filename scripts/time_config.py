@@ -10,7 +10,12 @@ maximum SM clock read in the same run.
 L2 flushed before each) against its HBM floor (frame bytes read + dense bytes written at 3.35 TB/s).
 --compare-diag alternates a diagnostics=False and a diagnostics=True engine on the same batch the same way, and
 times impala_vtrace_loss against impala_vtrace_loss_diag alone on the engine's buffers (median of 200 launches
-each, alternating, L2 flushed before each)."""
+each, alternating, L2 flushed before each).
+--compare-replay alternates a plain engine and a replay engine (--replay-slabs R, --replay-columns Br, default
+B/2; --obs-dtype, --frames k if given) the same way: the replay engine's pool is filled first, and the plain
+engine trains on the very slab the replay engine composed, so both steps see the same values.  It also times
+impala_batch_compose alone (median of 200 launches, L2 flushed before each) against its HBM floor (one training
+slab read and written at 3.35 TB/s)."""
 import argparse
 import os
 import statistics
@@ -50,11 +55,16 @@ ap.add_argument("--steps", type=int, default=30)
 ap.add_argument("--compare-tc", action="store_true", help="alternate with IMPALA_MLP_TC=0 and report both")
 ap.add_argument("--compare-obs", action="store_true", help="alternate float32 and uint8 observation slabs")
 ap.add_argument("--compare-frames", action="store_true", help="alternate dense and frame-stacked observation slabs")
-ap.add_argument("--frames", type=int, default=4, help="stacked frames of --compare-frames")
+ap.add_argument("--frames", type=int, default=None, help="stacked frames of --compare-frames (default 4) / --compare-replay (default 1)")
 ap.add_argument("--obs-dtype", default="float32", choices=["float32", "uint8"], help="slab obs type of --compare-frames")
 ap.add_argument("--compare-diag", action="store_true", help="alternate engines without / with off-policy diagnostics")
+ap.add_argument("--compare-replay", action="store_true", help="alternate engines without / with experience replay")
+ap.add_argument("--replay-slabs", type=int, default=2, help="past fresh batches in the pool of --compare-replay")
+ap.add_argument("--replay-columns", type=int, default=None, help="replayed columns of --compare-replay (default B/2)")
 a = ap.parse_args()
 w = CFG[a.config]
+if a.frames is None:
+    a.frames = 1 if a.compare_replay else 4
 hp = default_hparams(batch_size=w["B"], max_timesteps=w["T"])
 arms = {"default": os.environ.get("IMPALA_MLP_TC", "1")}
 obs_dt = {"default": "float32"}
@@ -74,15 +84,26 @@ if a.compare_frames:
     arms = {f"dense {a.obs_dtype}": arms["default"], f"frames={a.frames} {a.obs_dtype}": arms["default"]}
     obs_dt = {name: a.obs_dtype for name in arms}
     n_frames = {f"frames={a.frames} {a.obs_dtype}": a.frames}
+replay_arm = {}
+if a.compare_replay:
+    Br = w["B"] // 2 if a.replay_columns is None else a.replay_columns
+    on = f"replay R={a.replay_slabs} Br={Br}"
+    arms = {"replay off": arms["default"], on: arms["default"]}
+    obs_dt = {name: a.obs_dtype for name in arms}
+    n_frames = {name: a.frames for name in arms}
+    replay_arm = {on: dict(replay_slabs=a.replay_slabs, replay_columns=Br)}
 engines = {}
 for name, tc in arms.items():
     os.environ["IMPALA_MLP_TC"] = tc  # read by the C library at every launch (and at graph capture)
     dt = obs_dt.get(name, "float32")
     k = n_frames.get(name, 1)
     eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k,
-                        diagnostics=diag_arm.get(name, False))
+                        diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}))
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
-    byte_obs = a.compare_obs or (a.compare_frames and dt == "uint8") or (a.compare_diag and dt == "uint8")
+    byte_obs = a.compare_obs or ((a.compare_frames or a.compare_replay) and dt == "uint8") or (a.compare_diag and dt == "uint8")
+    if a.compare_replay:
+        engines[name] = eng
+        continue
     if a.compare_frames:  # the same observation values in both arms: the dense arm gets the stacked frames
         batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if byte_obs else "normal",
                                  frames=a.frames)
@@ -96,6 +117,18 @@ for name, tc in arms.items():
     if a.compare_obs or a.compare_frames:
         eng.load_device_batch(batch, 1)
     engines[name] = eng
+if a.compare_replay:  # fill the pool (R fresh batches, then the one trained on), then hand the composed slab over
+    eng = engines[on]
+    for n in range(a.replay_slabs + 1):
+        eng.load_device_batch(synth.make_batch(1 + n, w["T"], eng.B_fresh, w["O"], w["A"], frames=a.frames,
+                                               obs_kind="bytes" if a.obs_dtype == "uint8" else "normal"))
+        eng.step(0)
+        eng.synchronize()
+    assert (eng.replay_plan[:, 0] >= 0).all()
+    engines["replay off"].d_slabs[0].copy_(eng.d_slabs[0])
+    torch.cuda.synchronize()
+    engines["replay off"].slab_ready[0].record(engines["replay off"].copy_stream)
+    eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))  # both arms start the timed steps from the same weights
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 ts = {name: [] for name in arms}
 for i in range(a.steps + 5):
@@ -153,6 +186,31 @@ if a.compare_frames:  # the unstacking launch alone, back to back
     print(f"impala_obs_unstack {a.config} frames={a.frames} {a.obs_dtype} -> {eng.obs_dense.dtype}: {us:.1f} us, "
           f"{nbytes / 1e6:.1f} MB moved, HBM floor {nbytes / 3.35e12 * 1e6:.1f} us at 3.35 TB/s "
           f"({nbytes / 3.35e12 * 1e6 / us:.0%} of it)")
+if a.compare_replay:  # the compose launch alone
+    import ctypes
+
+    from torched_impala_b200 import _cabi
+
+    eng = engines[on]
+    args = (ctypes.c_void_p(eng.d_slabs[0].data_ptr()), ctypes.c_void_p(eng.store.data_ptr()), eng.slab_bytes,
+            ctypes.c_void_p(eng.d_plans[0].data_ptr()), w["T"], w["B"], eng.B_fresh, eng.F, a.frames, w["A"], eng.obs_code)
+    with torch.cuda.stream(eng.stream):
+        st = ctypes.c_void_p(eng.stream.cuda_stream)
+        tu = []
+        for i in range(220):
+            flush.zero_()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(eng.stream)
+            _cabi.check(eng.lib.impala_batch_compose(*args, st), "impala_batch_compose")
+            e1.record(eng.stream)
+            e1.synchronize()
+            if i >= 20:
+                tu.append(e0.elapsed_time(e1) * 1e3)
+    us, nbytes = statistics.median(tu), 2 * eng.d_slabs[0].numel()
+    print(f"impala_batch_compose {a.config} frames={a.frames} {a.obs_dtype} {on}: {us:.1f} us, {nbytes / 1e6:.1f} MB moved "
+          f"(training slab {nbytes / 2e6:.1f} MB read and written, fresh slab {eng.slab_bytes / 1e6:.1f} MB, store "
+          f"{eng.store.numel() / 1e6:.1f} MB), HBM floor {nbytes / 3.35e12 * 1e6:.1f} us at 3.35 TB/s "
+          f"({nbytes / 3.35e12 * 1e6 / us:.0%} of it)")
 if a.compare_diag:  # the V-trace + loss kernel alone, plain and diag entry points alternating
     import ctypes
 
@@ -197,6 +255,10 @@ for name, eng in engines.items():
         if te[name] else ""
     print(f"{a.config} {w} [{name}] on {dev}: median {med:.1f} us/step ({1e6 / med:.0f} steps/s){e2e}, "
           f"loss {eng.read_scalars()['total_loss']:.5f}")
+if a.compare_replay:
+    m0, m1 = statistics.median(ts["replay off"]), statistics.median(ts[on])
+    print(f"replay overhead {a.config}: {m1 - m0:+.1f} us/step ({100 * (m1 / m0 - 1):+.1f} %), one launch more "
+          f"({engines[on].launches_per_step} against {engines['replay off'].launches_per_step})")
 if a.compare_diag:
     m0, m1 = statistics.median(ts["diagnostics off"]), statistics.median(ts["diagnostics on"])
     sc = engines["diagnostics on"].read_scalars()

@@ -46,6 +46,7 @@ SIGNATURES = {
     "impala_batch_layout_frames": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_i64), C.POINTER(_i64)]),
     "impala_ingest_shard_frames": (_i, [_p, _p] + [_i] * 8 + [_p]),
     "impala_obs_unstack": (_i, [_p, _i, _p, _i, _i, _i, _i, _i, _p]),
+    "impala_batch_compose": (_i, [_p, _p, _i64, _p] + [_i] * 7 + [_p]),
     "impala_obs_u8_to_f32": (_i, [_p, _p, _i64, _p]),
     "impala_mlp_forward": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
     "impala_mlp_forward_u8": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),

@@ -36,6 +36,17 @@ a dedicated copy stream, so the DMA of batch i+1 runs under the kernels of batch
 (`ingest(slot)` / `step(slot)` order themselves with events); the loss scalars come back
 through a small ring of pinned buffers (`post_scalars` / `fetch_scalars`) so the host only
 ever waits for the previous step.
+
+replay_slabs=R, replay_columns=Br (experience replay, both 0 = off): the host slabs, `fill_host` and the
+ingest calls speak the FRESH layout of Bf = B - Br columns, and the DMA of update n lands in slot n mod (R + 2)
+of a store of fresh slabs in HBM that keeps the last R fresh batches.  The step's first launch,
+impala_batch_compose, gathers the B-column training slab out of the store by the update's plan (replay.py):
+its own Bf columns, then Br columns drawn uniformly from the fresh batches of the R updates before it (empty
+columns at update 1).  The plan reaches a small device buffer per training slab on the copy stream, ahead of
+the event the step waits on, so the captured graphs keep fixed pointers.  R + 2 slots: while update n trains,
+the slot that receives update n + 1 is in nobody's pool, so the DMA still runs under the kernels.  The kernels
+after the compose launch are unchanged; the logged `batch_mean_reward` scalar is the composed batch's (sum of
+all B columns' rewards / B), the mean over the fresh trajectories is the caller's (Learner logs that one).
 """
 from __future__ import annotations
 
@@ -45,6 +56,7 @@ import numpy as np
 import torch
 
 from . import _cabi
+from .replay import ReplaySampler, check_replay_args
 
 PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
 SCALAR_NAMES = ("value_fn_loss", "policy_loss", "policy_entropy", "batch_mean_reward")
@@ -94,7 +106,8 @@ class LearnerEngine:
     def __init__(self, T: int, B_local: int, O: int, A: int, H_pi: int, H_v: int, hp,
                  global_batch: int | None = None, device: str | torch.device = "cuda:0",
                  mode: str = "reference", process_group=None, use_graph: bool = True,
-                 slabs: int = 2, obs_dtype: str = "float32", frames: int = 1, diagnostics: bool = False):
+                 slabs: int = 2, obs_dtype: str = "float32", frames: int = 1, diagnostics: bool = False,
+                 replay_slabs: int = 0, replay_columns: int = 0, replay_seed: int = 0):
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
@@ -108,6 +121,11 @@ class LearnerEngine:
         torch.cuda.set_device(self.dev)
         self.T, self.B, self.O, self.A, self.H_pi, self.H_v = T, B_local, O, A, H_pi, H_v
         self.hp = hp
+        # experience replay: B_fresh of the B columns of an update arrive from the host, the rest from the store
+        self.B_fresh = check_replay_args(B_local, replay_slabs, replay_columns)
+        self.replay_slabs, self.replay_columns = int(replay_slabs), int(replay_columns)
+        if self.replay_slabs and process_group is not None:
+            raise ValueError("experience replay runs on one device: the store is not sharded over a process group")
         # off-policy diagnostics of every update (impala_vtrace_loss_diag); every rank must agree on it
         self.diagnostics = bool(diagnostics)
         self.n_extra = 12 if self.diagnostics else 4  # logged float64 values after the gradient in `comm`
@@ -139,32 +157,44 @@ class LearnerEngine:
         self.comm = torch.zeros(self.n_comm, dtype=torch.float64, device=self.dev)
         self.norms = torch.zeros(2, dtype=torch.float64, device=self.dev)
 
-        # ---- batch slab (device) and pinned staging slabs (host), identical layouts
-        self.slab_off, self.slab_bytes = _cabi.batch_layout(T, B_local, O, A, obs_dtype, frames)
+        # ---- batch slab (device) and pinned staging slabs (host), identical layouts (replay: the host slabs
+        # hold the B_fresh columns that cross the host link, the device slabs the B columns trained on)
+        train_off, train_bytes = _cabi.batch_layout(T, B_local, O, A, obs_dtype, frames)
+        self.slab_off, self.slab_bytes = train_off, train_bytes
+        if self.replay_slabs:
+            self.slab_off, self.slab_bytes = _cabi.batch_layout(T, self.B_fresh, O, A, obs_dtype, frames)
         self.fields = ((("obs", np.uint8 if obs_dtype == "uint8" else np.float32),) + _BATCH_FIELDS[1:])
         self.n_slabs = slabs
-        self.d_slabs = [torch.zeros(self.slab_bytes, dtype=torch.uint8, device=self.dev)
+        self.d_slabs = [torch.zeros(train_bytes, dtype=torch.uint8, device=self.dev)
                         for _ in range(slabs)]
         self.h_slabs = [torch.zeros(self.slab_bytes, dtype=torch.uint8).pin_memory()
                         for _ in range(slabs)]
-        shapes = {"obs": (T + frames, B_local, self.F), "beh_logits": (T, B_local, A),
-                  "actions": (T, B_local), "rewards": (T, B_local), "done": (T, B_local),
-                  "lens": (B_local,)}
-        self.shapes = shapes
+        self.shapes = self._shapes(B_local)
+        h_shapes = self._shapes(self.B_fresh)
         self.d_views, self.h_views = [], []
         for dslab, hslab in zip(self.d_slabs, self.h_slabs):
             arr = hslab.numpy()
             dv, hv = {}, {}
-            for (name, dt), off in zip(self.fields, self.slab_off):
-                n = int(np.prod(shapes[name])) * np.dtype(dt).itemsize
-                dv[name] = dslab[off:off + n].view(_TORCH_DT[dt]).view(shapes[name])
-                hv[name] = arr[off:off + n].view(dt).reshape(shapes[name])
+            for (name, dt), d_off, h_off in zip(self.fields, train_off, self.slab_off):
+                item = np.dtype(dt).itemsize
+                nd, nh = int(np.prod(self.shapes[name])) * item, int(np.prod(h_shapes[name])) * item
+                dv[name] = dslab[d_off:d_off + nd].view(_TORCH_DT[dt]).view(self.shapes[name])
+                hv[name] = arr[h_off:h_off + nh].view(dt).reshape(h_shapes[name])
             self.d_views.append(dv)
             self.h_views.append(hv)
         self.d = self.d_views[0]
         self.slab_ready = [torch.cuda.Event() for _ in range(slabs)]  # H2D into slab done
         self.slab_free = [torch.cuda.Event() for _ in range(slabs)]   # last consumer of slab done
         self._slab_used = [False] * slabs
+        if self.replay_slabs:
+            self.sampler = ReplaySampler(replay_seed, self.replay_slabs, self.B_fresh, self.replay_columns)
+            self.store = torch.zeros(self.replay_slabs + 2, self.slab_bytes, dtype=torch.uint8, device=self.dev)
+            self.d_plans = [torch.zeros(B_local, 2, dtype=torch.int32, device=self.dev) for _ in range(slabs)]
+            self.h_plans = [torch.zeros(B_local, 2, dtype=torch.int32).pin_memory() for _ in range(slabs)]
+            self.replay_plan = None  # plan of the last ingested update: (B, 2) int32 (store slot, column)
+            self._slab_update = [0] * slabs  # update number held by each training slab
+            self._ingested = self._stepped = 0  # updates whose DMA / whose step has been enqueued
+            self._update_done = [torch.cuda.Event() for _ in range(3)]  # store reads of update u: index u % 3
 
         # ---- activations / gradients of the non-MLP part
         self.logits = torch.zeros(T, B_local, A, **f32)
@@ -265,6 +295,12 @@ class LearnerEngine:
         torch.cuda.synchronize(self.dev)
         dist.barrier(group=self.pg)
 
+    def _shapes(self, B: int) -> dict:
+        """Shapes of the six batch tensors in a slab of B columns."""
+        T, A = self.T, self.A
+        return {"obs": (T + self.frames, B, self.F), "beh_logits": (T, B, A), "actions": (T, B), "rewards": (T, B),
+                "done": (T, B), "lens": (B,)}
+
     def _ws_bytes(self, M, O, H, N2):
         n = self.lib.impala_mlp_backward_workspace(M, O, H, N2)
         if n < 0:
@@ -329,11 +365,30 @@ class LearnerEngine:
         cs = self.copy_stream
         if self._slab_used[slot]:
             cs.wait_event(self.slab_free[slot])  # the step that last read this slab is done
-        _cabi.check(self.lib.impala_ingest(_ptr(self.d_slabs[slot]),
+        _cabi.check(self.lib.impala_ingest(self._ingest_target(slot),
                                            C.c_void_p(self.h_slabs[slot].data_ptr()),
                                            self.slab_bytes, C.c_void_p(cs.cuda_stream)),
                     "impala_ingest")
         self.slab_ready[slot].record(cs)
+
+    def _ingest_target(self, slot: int) -> C.c_void_p:
+        """Device address the DMA for training slab `slot` writes: the slab itself, or with replay the store
+        slot of the update being ingested, after the update's plan has been queued on the copy stream."""
+        if not self.replay_slabs:
+            return _ptr(self.d_slabs[slot])
+        n, cs = self._ingested + 1, self.copy_stream
+        if self._stepped < n - 2:
+            raise RuntimeError(f"replay: update {n} ingested before the step of update {n - 2} was enqueued; its "
+                               "store slot may still be read (at most two updates in flight)")
+        if n > 2:  # the store slot last held update n - R - 2, which update n - 2 may have sampled
+            cs.wait_event(self._update_done[(n - 2) % 3])
+        self.slab_ready[slot].synchronize()  # the pinned plan buffer's previous copy has left the host
+        plan = self.sampler.plan(n)
+        self.h_plans[slot].numpy()[...] = plan
+        _cabi.check(self.lib.impala_ingest(_ptr(self.d_plans[slot]), C.c_void_p(self.h_plans[slot].data_ptr()),
+                                           plan.nbytes, C.c_void_p(cs.cuda_stream)), "impala_ingest(plan)")
+        self.replay_plan, self._ingested, self._slab_update[slot] = plan, n, n
+        return C.c_void_p(self.store.data_ptr() + (n % self.sampler.slots) * self.slab_bytes)
 
     def register_host(self, address: int, nbytes: int) -> None:
         """Page-lock caller-owned host memory (e.g. a shared-memory trajectory ring) for DMA."""
@@ -347,13 +402,15 @@ class LearnerEngine:
         cs = self.copy_stream
         if self._slab_used[slot]:
             cs.wait_event(self.slab_free[slot])
-        _cabi.check(self.lib.impala_ingest(_ptr(self.d_slabs[slot]), C.c_void_p(host_address),
+        _cabi.check(self.lib.impala_ingest(self._ingest_target(slot), C.c_void_p(host_address),
                                            self.slab_bytes, C.c_void_p(cs.cuda_stream)), "impala_ingest")
         self.slab_ready[slot].record(cs)
 
     def ingest_shard_from(self, host_address: int, b0: int, B_total: int, slot: int = 0) -> None:
         """Data-parallel ingest: columns [b0, b0 + B_local) of a caller-owned (registered) host slab
         laid out for B_total columns -> device slab `slot` (impala_ingest_shard)."""
+        if self.replay_slabs:
+            raise ValueError("experience replay runs on one device: there is no sharded ingest into the store")
         cs = self.copy_stream
         if self._slab_used[slot]:
             cs.wait_event(self.slab_free[slot])
@@ -375,6 +432,10 @@ class LearnerEngine:
         launched = lib.impala_launch_count()
         d = self.d_views[slot]
         T, B, O, A = self.T, self.B, self.O, self.A
+        if self.replay_slabs:  # the training slab out of the store, by the plan ingest left in d_plans[slot]
+            _cabi.check(lib.impala_batch_compose(_ptr(self.d_slabs[slot]), _ptr(self.store), self.slab_bytes,
+                                                 _ptr(self.d_plans[slot]), T, B, self.B_fresh, self.F, self.frames, A,
+                                                 self.obs_code, st), "impala_batch_compose")
         p_pi = C.c_void_p(self.params.data_ptr())
         p_vf = C.c_void_p(self.params.data_ptr() + 4 * self.n_pi)
         # this rank's [gradient | scalars] goes to `comm` (final at N = 1, reduced in place by NCCL,
@@ -508,6 +569,10 @@ class LearnerEngine:
                 fused_opt = False
             self.slab_free[slot].record(self.stream)
             self._slab_used[slot] = True
+            if self.replay_slabs:  # the store reads of this update are enqueued: ingest of update u + 2 waits here
+                u = self._slab_update[slot]
+                self._update_done[u % 3].record(self.stream)
+                self._stepped = max(self._stepped, u)
             if self.world > 1 and not self.peer:
                 import torch.distributed as dist
 

@@ -30,7 +30,10 @@ path of the device (SURVEY 8f-2, 8f-4):
   * evaluation (`learner.py:195-214`) runs on a frozen copy of the policy in a background thread,
     it no longer blocks updates and no longer flips the training module's mode;
   * `devices=[...]`: data-parallel over the GPUs of one node, still ONE learner object/process
-    for the launcher (dp.py): rank 0 lives here, publishes weights and logs.
+    for the launcher (dp.py): rank 0 lives here, publishes weights and logs;
+  * `replay_slabs=R, replay_columns=Br` (experience replay, off by default): every update consumes
+    `batch_size - Br` trajectories from the queue and fills its other Br columns from the fresh batches of
+    the last R updates, kept in HBM (engine.py, replay.py); one device only.
 
 CUDA is initialised inside the learner process only (`train.py:42` forces the fork start method,
 so the parent must never touch the device); a policy / value_fn that already lives on a CUDA
@@ -53,6 +56,8 @@ from pathlib import Path
 import numpy as np
 import torch
 import torch.multiprocessing as mp
+
+from .replay import check_replay_args
 
 PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
 
@@ -236,7 +241,8 @@ class _Publisher:
 class Learner:
     def __init__(self, id, hparams, policy, value_fn, q, update_counter, log_path=None,
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
-                 evaluator=None, obs_dtype="float32", frames=1, diagnostics=False):
+                 evaluator=None, obs_dtype="float32", frames=1, diagnostics=False,
+                 replay_slabs=0, replay_columns=0):
         self.id = id
         if obs_dtype not in ("float32", "uint8"):
             raise ValueError(f"obs_dtype must be 'float32' or 'uint8', got {obs_dtype!r}")
@@ -249,6 +255,14 @@ class Learner:
         if hasattr(q, "collect_batch") and getattr(q, "frames", 1) != frames:
             raise ValueError(f"the RingQueue stores observations as {getattr(q, 'frames', 1)} frames, "
                              f"the learner was built for frames={frames}")
+        # experience replay: B_fresh trajectories per update come off the queue, replay_columns out of HBM
+        self.B_fresh = check_replay_args(hparams.batch_size, replay_slabs, replay_columns)
+        self.replay_slabs, self.replay_columns = int(replay_slabs), int(replay_columns)
+        if self.replay_slabs and devices and len(devices) > 1:
+            raise ValueError(f"experience replay runs on one device, got devices={list(devices)}")
+        if hasattr(q, "collect_batch") and self.replay_slabs and q.B != self.B_fresh:
+            raise ValueError(f"with replay_columns={replay_columns} an update takes batch_size - replay_columns = "
+                             f"{self.B_fresh} trajectories from the queue; the RingQueue was built for {q.B}")
         self.obs_dtype = obs_dtype  # "uint8": byte observations end to end (ring / slabs / MLP kernels)
         self.frames = frames  # > 1: each of the stacked frames stored once (ring / slabs), unstacked on the device
         self.hp = hparams
@@ -313,7 +327,8 @@ class Learner:
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
-                    obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics)
+                    obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics,
+                    replay_slabs=self.replay_slabs, replay_columns=self.replay_columns)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -323,7 +338,8 @@ class Learner:
             raise ValueError(f"batch_size {c['B']} does not divide over {world} devices")
         eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], self.hp,
                             global_batch=c["B"], device=self.device, mode=self.mode, process_group=process_group,
-                            obs_dtype=c["obs_dtype"], frames=c["frames"], diagnostics=c["diagnostics"])
+                            obs_dtype=c["obs_dtype"], frames=c["frames"], diagnostics=c["diagnostics"],
+                            replay_slabs=c["replay_slabs"], replay_columns=c["replay_columns"])
         eng.load_state(self._init_state())
         return eng
 
@@ -397,10 +413,11 @@ class Learner:
 
     # ---------------------------------------------------------------- the update loop
     def _collect(self, views, writer):
-        """Pull hp.batch_size trajectories off the queue into one host slab (learner.py:89-109)."""
+        """Pull hp.batch_size trajectories (B_fresh of them with replay) off the queue into one host slab
+        (learner.py:89-109)."""
         hp = self.hp
         reward = 0.0
-        for b in range(hp.batch_size):
+        for b in range(self.B_fresh):
             try:
                 traj = self.q.get(timeout=self.timeout)
             except queue.Empty:
@@ -411,7 +428,7 @@ class Learner:
                 raise
             if hp.verbose >= 2:
                 print(f"[learner_{self.id}] packing traj_{traj.id} into column {b}")
-            reward += pack_trajectory(views, b, traj, hp.max_timesteps) / hp.batch_size
+            reward += pack_trajectory(views, b, traj, hp.max_timesteps) / self.B_fresh
             del traj  # drop the shared-memory handles of its ~5T tensors right away
         return reward
 

@@ -133,6 +133,26 @@ def obs_unstack(frames, k: int, out_dtype=None):
     return out
 
 
+def batch_compose(store, plan, T: int, B: int, Bf: int, F: int, frames: int, A: int, obs_dtype: str = "float32",
+                  out=None):
+    """The B-column training slab (uint8 bytes, _cabi.batch_layout(T, B, ...)) gathered from `store`, a
+    (slabs, slab_bytes) uint8 tensor of Bf-column slabs, by `plan` (B, 2) int32 (slab, column), slab < 0 = an
+    empty column (impala_batch_compose).  `out`: a uint8 tensor of the slab's size to write into."""
+    _need_cuda(store, plan)
+    if store.dtype != torch.uint8 or store.dim() != 2 or plan.dtype != torch.int32 or tuple(plan.shape) != (B, 2):
+        raise _cabi.ImpalaCudaError(f"batch_compose takes a (slabs, bytes) uint8 store and a ({B}, 2) int32 plan, got "
+                                    f"{tuple(store.shape)} {store.dtype}, {tuple(plan.shape)} {plan.dtype}")
+    _, total = _cabi.batch_layout(T, B, F * frames, A, obs_dtype, frames)
+    if out is None:
+        out = torch.empty(total, dtype=torch.uint8, device=store.device)
+    _need_cuda(out)
+    if out.dtype != torch.uint8 or out.numel() != total:
+        raise _cabi.ImpalaCudaError(f"batch_compose writes a slab of {total} bytes, got {out.numel()} {out.dtype}")
+    _cabi.check(_cabi.lib().impala_batch_compose(_p(out), _p(store), store.shape[1], _p(plan), T, B, Bf, F, frames, A,
+                                                 _cabi.obs_dtype_code(obs_dtype), _st()), "impala_batch_compose")
+    return out
+
+
 def mlp_forward_pair(x, params_pi, params_vf, M_pi: int, M_vf: int, O: int, H_pi: int, H_vf: int, A: int):
     """Policy logits on the first M_pi rows of x and values on the first M_vf rows, one call."""
     _need_cuda(x, params_pi, params_vf)
