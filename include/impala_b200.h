@@ -236,7 +236,9 @@ int impala_vtrace_loss_diag(const float* cur_logits, const float* beh_logits, co
  *   params/m/v: f32 [n_total]; grad: f64 [n_total] (the possibly all-reduced sum);
  *   group 0 = [0, n_policy) (policy net), group 1 = [n_policy, n_total) (value net);
  *   each group is scaled by min(1, max_norm / (||g||_2 + 1e-6)) as
- *   torch.nn.utils.clip_grad_norm_ does, then one Adam step (no weight decay) with
+ *   torch.nn.utils.clip_grad_norm_ does - a NaN norm (a NaN entry in the group) scales by NaN,
+ *   so every parameter, m and v of that group becomes NaN, as in torch; an infinite entry gives
+ *   coefficient 0 - then one Adam step (no weight decay) with
  *   bias correction from the device-side optimizer state (updated by the kernel):
  *   state = int64[3] {step count, beta1^step, beta2^step as float64 bits}; all zero = fresh.
  *   norms_out (f64[2], may be NULL) receives the two pre-clip norms. */

@@ -134,9 +134,11 @@ def losses(v, vs, cur_logits, actions, pg_adv, lens, hp_v_loss_c, hp_policy_loss
 
 # --------------------------------------------------------------------- clip + Adam
 def clip_coef(grads, max_norm):
-    """torch.nn.utils.clip_grad_norm_ as called at learner.py:176-181 (L2, eps 1e-6, clamp 1)."""
+    """torch.nn.utils.clip_grad_norm_ as called at learner.py:176-181 (L2, eps 1e-6, clamp 1).
+
+    A NaN norm gives a NaN coefficient, as torch.clamp propagates it (Python's min(1.0, nan) is 1.0)."""
     total = np.sqrt(sum(float((g.astype(F64) ** 2).sum()) for g in grads))
-    return min(1.0, max_norm / (total + 1e-6)), total
+    return (total if np.isnan(total) else min(1.0, max_norm / (total + 1e-6))), total
 
 
 class Adam:

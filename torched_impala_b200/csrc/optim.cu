@@ -89,8 +89,9 @@ clip_adam_kernel(float* __restrict__ params, const double* __restrict__ grad, fl
         double s = 0.0;
         for (int r = 0; r < kAdamCluster; ++r) s += *cluster.map_shared_rank(&s_cta[tid], r);
         const double norm = sqrt(s);
-        // torch.nn.utils.clip_grad_norm_: coef = max_norm / (norm + 1e-6), clamped to 1
-        s_coef[tid] = (float)fmin(1.0, (double)max_norm / (norm + 1e-6));
+        // torch.nn.utils.clip_grad_norm_: coef = max_norm / (norm + 1e-6), clamped to 1; a NaN norm
+        // gives a NaN coefficient (torch.clamp propagates NaN, fmin would return the 1)
+        s_coef[tid] = isnan(norm) ? (float)norm : (float)fmin(1.0, (double)max_norm / (norm + 1e-6));
         if (norms_out && cluster.block_rank() == 0) norms_out[tid] = norm;
     }
     __syncthreads();
@@ -191,7 +192,7 @@ gather_clip_adam_kernel(float* __restrict__ params, double* __restrict__ reduced
     const int64_t stride = (int64_t)kAdamCluster * kAdamThreads;
 
     // optimizer state that does not depend on the peers: issued before anything else
-    constexpr int kKeep = 2, kMaxWorld = 8;  // one NVLink node
+    constexpr int kKeep = 2, kMaxWorld = 8, kPoll = 2;  // one NVLink node
     float pk[kKeep], mk[kKeep], vk[kKeep];
 #pragma unroll
     for (int k = 0; k < kKeep; ++k) {
@@ -213,30 +214,35 @@ gather_clip_adam_kernel(float* __restrict__ params, double* __restrict__ reduced
     const unsigned step = (unsigned)step64;
     __syncthreads();
 
-    // rank-ordered sum of entry i: all `world` loads are issued together, then each is re-polled
-    // until it carries this step's tag (local memory: the peers' values arrive by themselves)
+    // rank-ordered sum of entry i: the loads of kPoll ranks are issued together, then each is re-polled
+    // until it carries this step's tag (local memory: the peers' values arrive by themselves).  kPoll = 2:
+    // more 16-byte words in flight at the three inlined call sites exceed the 64 registers a 1024-thread
+    // CTA allows (all eight spilled 232 bytes to local memory, four still 12).
     const ulonglong2* gb = gather + (step64 & 1) * buf_stride;
     const unsigned long long t_start = global_ns();
     bool ok = true;
     auto gsum = [&](int64_t i) {
-        ulonglong2 w[kMaxWorld];
-#pragma unroll
-        for (int r = 0; r < kMaxWorld; ++r)
-            if (r < world) w[r] = ll_load(gb + r * slot_stride + i);
         double s = 0.0;
 #pragma unroll
-        for (int r = 0; r < kMaxWorld; ++r) {
-            if (r < world) {
-                unsigned spins = 0;
-                while (!ll_ready(w[r], step)) {
-                    if ((++spins & 255u) == 0 && global_ns() - t_start > timeout_ns) {
-                        ok = false;
-                        break;
+        for (int r0 = 0; r0 < kMaxWorld; r0 += kPoll) {
+            ulonglong2 w[kPoll];
+#pragma unroll
+            for (int r = 0; r < kPoll; ++r)
+                if (r0 + r < world) w[r] = ll_load(gb + (r0 + r) * slot_stride + i);
+#pragma unroll
+            for (int r = 0; r < kPoll; ++r) {
+                if (r0 + r < world) {
+                    unsigned spins = 0;
+                    while (!ll_ready(w[r], step)) {
+                        if ((++spins & 255u) == 0 && global_ns() - t_start > timeout_ns) {
+                            ok = false;
+                            break;
+                        }
+                        if (spins > 16) __nanosleep(20);
+                        w[r] = ll_load(gb + (r0 + r) * slot_stride + i);
                     }
-                    if (spins > 16) __nanosleep(20);
-                    w[r] = ll_load(gb + r * slot_stride + i);
+                    s += ll_value(w[r]);
                 }
-                s += ll_value(w[r]);
             }
         }
         return s;
@@ -278,7 +284,7 @@ gather_clip_adam_kernel(float* __restrict__ params, double* __restrict__ reduced
         double s = 0.0;
         for (int r = 0; r < kAdamCluster; ++r) s += *cluster.map_shared_rank(&s_cta[tid], r);
         const double norm = sqrt(s);
-        s_coef[tid] = (float)fmin(1.0, (double)max_norm / (norm + 1e-6));
+        s_coef[tid] = isnan(norm) ? (float)norm : (float)fmin(1.0, (double)max_norm / (norm + 1e-6));  // as above
         if (norms_out && crank == 0) norms_out[tid] = norm;
     }
     __syncthreads();
