@@ -3,7 +3,7 @@ tensor-core MLP kernels.
 
 The forward runs the 16-output epilogue at one, two or four K atoms and the backward the 16-output
 layer-2-through-shared-memory kernel at one or two (at four it keeps the 32-output padded kernel).  Both
-are held to the float64 oracle with every logit written (the output starts as NaN), and the whole learner
+are held to the float64 error bound of tests/mlp_bounds.py with every logit written (the output starts as NaN), and the whole learner
 step - eager engine, byte observations, forked Learner behind a RingQueue - is checked at A = 6 and A = 9.
 Which kernels the launches take is checked in test_gpu_mlp_routes.py.
 """
@@ -17,15 +17,16 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import PKEYS
-from oracle import impala_oracle as orc
+from mlp_bounds import check_backward, check_forward
 from oracle.check import first_step_parity
+from test_gpu_parity import backward_case, forward_case
 from torched_impala_b200 import _cabi, synth
 from torched_impala_b200.utils import default_hparams
 
 pytestmark = pytest.mark.gpu
 
-ATOL = 1e-5
+REL = 5e-5  # the backward's precision floor here (mlp_bounds.GRAD_REL elsewhere)
+
 SHAPES = [
     # (M, O, H, N2): four K atoms (the 16-output forward replaces one that wrote 4 logits) ...
     (20 * 1024, 128, 256, 6), (5000, 100, 512, 9), (5, 128, 128, 16),
@@ -76,34 +77,18 @@ def backward_into_nan(x, params, dout, M, O, H, N2):
 
 @pytest.mark.parametrize("M,O,H,N2", SHAPES)
 def test_forward_matches_oracle(ops, M, O, H, N2):
-    rng = np.random.default_rng(M + O + H + N2)
-    p = synth.init_params(M, O, N2, H)["policy"]
-    x = rng.standard_normal((M, O), dtype=np.float32)
-    want, _ = orc.mlp_forward(x.astype(np.float64), *[p[k].astype(np.float64) for k in PKEYS])
-    got = forward_into_nan(dev(x), ops.pack_params(p), M, O, H, N2).cpu().numpy()
-    assert np.isfinite(got).all(), np.argwhere(~np.isfinite(got))[:4]
-    assert np.abs(got - want).max() < ATOL
+    x, p = forward_case(M, O, H, N2)
+    got = forward_into_nan(dev(x), ops.pack_params(p), M, O, H, N2)
+    check_forward(got, x, p, f"fwd {M},{O},{H},{N2}")  # a NaN left in the output fails it
 
 
 @pytest.mark.parametrize("M,O,H,N2", SHAPES)
 def test_backward_matches_oracle(ops, M, O, H, N2):
-    """5e-5 of the largest entry; W1 / b1 also get the ReLU-tie allowance of test_gpu_wide_shapes.py (one
-    batch row's contribution, three times)."""
-    rng = np.random.default_rng(7 * M + O + H + N2)
-    p = synth.init_params(M + 1, O, N2, H)["policy"]
-    x = rng.standard_normal((M, O), dtype=np.float32)
-    dout = (rng.standard_normal((M, N2), dtype=np.float32) / M).astype(np.float32)
-    p64 = [p[k].astype(np.float64) for k in PKEYS]
-    _, pre = orc.mlp_forward(x.astype(np.float64), *p64)
-    want = orc.mlp_backward(x.astype(np.float64), pre, p64[2], dout.astype(np.float64))
+    """Every entry within its float64 error bound (ReLU ties allowed only in the entries they move); W2, b2 and the
+    W1 / b1 rows without a tie within REL of their tensor's largest entry."""
+    x, p, dout = backward_case(M, O, H, N2)
     flat = backward_into_nan(dev(x), ops.pack_params(p), dev(dout), M, O, H, N2)
-    assert bool(torch.isfinite(flat).all())
-    got = ops.unpack_grad(flat, O, H, N2)
-    one_row = float(np.abs(dout).max() * np.abs(p[PKEYS[2]]).max() * max(1.0, np.abs(x).max()))
-    for k, w in zip(PKEYS, want):
-        assert got[k].shape == w.shape
-        tol = 5e-5 * np.abs(w).max() + (3 * one_row if k in PKEYS[:2] else 0.0)
-        assert np.abs(got[k] - w).max() < tol, (k, float(np.abs(got[k] - w).max()), float(np.abs(w).max()))
+    check_backward(flat, x, p, dout, f"bwd {M},{O},{H},{N2}", rel=REL)
 
 
 # name: (T, B, O, A, H, ragged)
@@ -116,7 +101,7 @@ CASES = {
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_first_step_matches_oracle(ops, name):
-    from test_gpu_wide_shapes import _check_grad_with_relu_ties
+    from test_gpu_wide_shapes import check_engine_mlp, check_grad_end_to_end
     from torched_impala_b200.engine import LearnerEngine
 
     T, B, O, A, H, ragged = CASES[name]
@@ -130,8 +115,9 @@ def test_first_step_matches_oracle(ops, name):
     assert par["max_abs_pg"] < 1e-5, par
     for k, v in par["scalars"].items():
         assert v["abs_err"] < 1e-5, (k, v)
+    check_engine_mlp(eng, params)
     if par["max_rel_grad"] >= 5e-5:
-        _check_grad_with_relu_ties(eng, params, batch, hp)
+        check_grad_end_to_end(eng, params, batch, hp)
     assert par["max_abs_param_after_1_update"] < 5e-5, par
     assert par["frac_params_off"] < 1e-3, par
     for k in ("norm_policy", "norm_value"):

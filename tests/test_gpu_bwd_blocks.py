@@ -5,15 +5,14 @@ writes only that block's entries of its partial row.  These cases pin what that 
 right: every entry of the summed rows written exactly once (the workspace is filled with NaN before
 the launch, so an entry no CTA writes shows), CTAs and warpgroups that get no tile, hidden widths
 that differ between the two networks (different numbers of CTA groups per network), a ragged last
-tile, and a reduction that is bitwise reproducible from launch to launch.  Everything is held
-against the float64 oracle.
+tile, and a reduction that is bitwise reproducible from launch to launch.  Every gradient entry is held to
+its float64 error bound (tests/mlp_bounds.py).
 """
 import numpy as np
 import pytest
 import torch
 
-from conftest import PKEYS
-from oracle import impala_oracle as orc
+from mlp_bounds import check_backward
 from torched_impala_b200 import _cabi, ops, synth
 
 pytestmark = pytest.mark.gpu
@@ -54,24 +53,6 @@ def _single(x, params, dout, M, O, H, N2, ws):
     return grad
 
 
-def _check_oracle(flat, x, p, dout, O, H, N2):
-    """As test_gpu_parity.test_mlp_backward: relative to the largest entry, one ReLU tie allowed in
-    W1 / b1; pad entries exactly zero."""
-    p64 = [p[k].astype(np.float64) for k in PKEYS]
-    _, pre = orc.mlp_forward(x.astype(np.float64), *p64)
-    want = orc.mlp_backward(x.astype(np.float64), pre, p64[2], dout.astype(np.float64))
-    got = ops.unpack_grad(flat, O, H, N2)
-    one_row = float(np.abs(dout).max() * np.abs(p[PKEYS[2]]).max() * max(1.0, np.abs(x).max()))
-    for k, w in zip(PKEYS, want):
-        tol = 2e-5 * np.abs(w).max() + (3 * one_row if k in PKEYS[:2] else 0.0)
-        assert np.isfinite(got[k]).all(), k
-        assert np.abs(got[k] - w).max() < tol, (k, float(np.abs(got[k] - w).max()), tol)
-    assert torch.isfinite(flat).all()
-    total = float(flat.abs().sum().cpu())
-    real = sum(np.abs(g).sum() for g in got.values())
-    assert abs(total - real) <= 1e-12 * max(1.0, real)
-
-
 PAIR_SHAPES = [
     # (T, B, O, H_pi, H_vf, A): M_pi = T*B, M_vf = (T+1)*B
     (5, 7, 8, 128, 256, 2),      # one tile per network: most warpgroups idle; 2 + 4 hidden blocks
@@ -82,8 +63,8 @@ PAIR_SHAPES = [
 ]
 
 
-@pytest.mark.parametrize("T,B,O,H_pi,H_vf,A", PAIR_SHAPES)
-def test_pair_against_oracle(T, B, O, H_pi, H_vf, A):
+def pair_cases(T, B, O, H_pi, H_vf, A):
+    """(x, params, dout) of the policy and of the value network, seeded as test_pair_against_oracle."""
     rng = np.random.default_rng(11 * T + B + O + H_pi)
     M_pi, M_vf = T * B, (T + 1) * B
     p_pi = synth.init_params(3, O, A, H_pi)["policy"]
@@ -91,11 +72,20 @@ def test_pair_against_oracle(T, B, O, H_pi, H_vf, A):
     x = rng.standard_normal((M_vf, O), dtype=np.float32)
     dlog = (rng.standard_normal((M_pi, A), dtype=np.float32) / M_pi).astype(np.float32)
     dv = (rng.standard_normal((M_vf,), dtype=np.float32) / M_vf).astype(np.float32)
-    xd, dlogd, dvd = (torch.from_numpy(a).cuda() for a in (x, dlog, dv))
+    return (x[:M_pi], p_pi, dlog), (x, p_vf, dv.reshape(-1, 1))
+
+
+@pytest.mark.parametrize("T,B,O,H_pi,H_vf,A", PAIR_SHAPES)
+def test_pair_against_oracle(T, B, O, H_pi, H_vf, A):
+    """Both networks' gradients, every entry within its float64 error bound (tests/mlp_bounds.py) and pad
+    entries exactly zero."""
+    (_, p_pi, dlog), (x, p_vf, dv) = pair_cases(T, B, O, H_pi, H_vf, A)
+    M_pi, M_vf = T * B, (T + 1) * B
+    xd, dlogd, dvd = (torch.from_numpy(a).cuda() for a in (x, dlog, dv.reshape(-1)))
     g_pi, g_vf = _pair(xd, ops.pack_params(p_pi), ops.pack_params(p_vf), dlogd, dvd, M_pi, M_vf, O, H_pi, H_vf, A,
                        _workspace(M_pi, O, H_pi, A), _workspace(M_vf, O, H_vf, 1))
-    _check_oracle(g_pi, x[:M_pi], p_pi, dlog, O, H_pi, A)
-    _check_oracle(g_vf, x, p_vf, dv.reshape(-1, 1), O, H_vf, 1)
+    check_backward(g_pi, x[:M_pi], p_pi, dlog, f"pair policy {T},{B},{O},{H_pi},{A}")
+    check_backward(g_vf, x, p_vf, dv, f"pair value {T},{B},{O},{H_vf}")
 
 
 SINGLE_SHAPES = [
@@ -104,15 +94,19 @@ SINGLE_SHAPES = [
 ]
 
 
-@pytest.mark.parametrize("M,O,H,N2", SINGLE_SHAPES)
-def test_single_against_oracle(M, O, H, N2):
+def single_case(M, O, H, N2):
     rng = np.random.default_rng(5 * M + O + H + N2)
     p = synth.init_params(M + 2, O, N2, H)["policy"]
     x = rng.standard_normal((M, O), dtype=np.float32)
-    dout = (rng.standard_normal((M, N2), dtype=np.float32) / M).astype(np.float32)
+    return x, p, (rng.standard_normal((M, N2), dtype=np.float32) / M).astype(np.float32)
+
+
+@pytest.mark.parametrize("M,O,H,N2", SINGLE_SHAPES)
+def test_single_against_oracle(M, O, H, N2):
+    x, p, dout = single_case(M, O, H, N2)
     grad = _single(torch.from_numpy(x).cuda(), ops.pack_params(p), torch.from_numpy(dout).cuda(), M, O, H, N2,
                    _workspace(M, O, H, N2))
-    _check_oracle(grad, x, p, dout, O, H, N2)
+    check_backward(grad, x, p, dout, f"single {M},{O},{H},{N2}")
 
 
 def test_pair_is_bitwise_reproducible_at_c4():

@@ -14,7 +14,7 @@ import pytest
 import torch
 
 from oracle.check import first_step_parity
-from test_gpu_wide_shapes import _check_grad_with_relu_ties
+from test_gpu_wide_shapes import check_engine_mlp, check_grad_end_to_end
 from torched_impala_b200 import _cabi, synth
 from torched_impala_b200.utils import default_hparams
 
@@ -135,8 +135,9 @@ def test_ram4_u8_frames_first_step_matches_oracle():
     assert par["max_abs_pg"] < 1e-5, par
     for key, v in par["scalars"].items():
         assert v["abs_err"] < 1e-5 * max(1.0, abs(v["ref"])), (key, v)
+    check_engine_mlp(eng, params)
     if par["max_rel_grad"] >= 5e-5:
-        _check_grad_with_relu_ties(eng, params, dense, hp)
+        check_grad_end_to_end(eng, params, dense, hp)
     assert par["max_abs_param_after_1_update"] < 5e-5, par
     assert par["frac_params_off"] < 1e-3, par
 

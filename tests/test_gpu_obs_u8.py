@@ -16,7 +16,7 @@ import pytest
 import torch
 
 from oracle.check import first_step_parity
-from test_gpu_wide_shapes import _check_grad_with_relu_ties
+from test_gpu_wide_shapes import check_engine_mlp, check_grad_end_to_end
 from torched_impala_b200 import _cabi, synth
 from torched_impala_b200.utils import default_hparams
 
@@ -126,8 +126,9 @@ def test_u8_first_step_matches_oracle_minatar_planes():
     assert par["max_abs_pg"] < 1e-5, par
     for k, v in par["scalars"].items():
         assert v["abs_err"] < 1e-5, (k, v)
+    check_engine_mlp(eng, params)
     if par["max_rel_grad"] >= 5e-5:
-        _check_grad_with_relu_ties(eng, params, batch, hp)
+        check_grad_end_to_end(eng, params, batch, hp)
     assert par["max_abs_param_after_1_update"] < 5e-5, par
     assert par["frac_params_off"] < 1e-3, par
     for k in ("norm_policy", "norm_value"):

@@ -4,7 +4,8 @@ The forward and the two-phase backward (recompute + DP^T, then dW1 = DP^T X) aga
 with N(0, 1), binary {0, 1} (MinAtar) and uniform [0, 1] (Atari RAM / 255) observations; output and
 workspace buffers NaN-filled so that an entry no CTA writes shows up; bitwise determinism; the refused
 shapes; first-step parity of the whole learner step; graph replay; the forked Learner behind a RingQueue.
-Tolerances are those of test_gpu_wide_shapes.py.
+Every output and gradient entry is held to its float64 error bound (tests/mlp_bounds.py); the engine checks
+are those of test_gpu_wide_shapes.py.
 """
 import json
 import os
@@ -15,16 +16,13 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import PKEYS
-from oracle import impala_oracle as orc
+from mlp_bounds import check_backward, check_forward
 from oracle.check import first_step_parity
-from test_gpu_wide_shapes import _check_grad_with_relu_ties
+from test_gpu_wide_shapes import check_engine_mlp, check_grad_end_to_end
 from torched_impala_b200 import _cabi, synth
 from torched_impala_b200.utils import default_hparams
 
 pytestmark = pytest.mark.gpu
-
-ATOL = 1e-5
 
 OBS_SHAPES = [
     # (M, O, H, N2)
@@ -55,6 +53,19 @@ def make_x(rng, M, O, kind):
     return rng.standard_normal((M, O), dtype=np.float32)
 
 
+def forward_case(M, O, H, N2, kind):
+    rng = np.random.default_rng(M + O + H + N2)
+    p = synth.init_params(M, O, N2, H)["policy"]
+    return make_x(rng, M, O, kind), p
+
+
+def backward_case(M, O, H, N2, kind):
+    rng = np.random.default_rng(7 * M + O + H + N2)
+    p = synth.init_params(M + 1, O, N2, H)["policy"]
+    x = make_x(rng, M, O, kind)
+    return x, p, (rng.standard_normal((M, N2), dtype=np.float32) / M).astype(np.float32)
+
+
 def forward(ops, x, params, M, O, H, N2):
     """impala_mlp_forward into an output buffer NaN-filled past M rows."""
     out = torch.full(((M + 64) * N2,), float("nan"), dtype=torch.float32, device="cuda")
@@ -82,42 +93,20 @@ def backward(ops, x, params, dout, M, O, H, N2):
 @pytest.mark.parametrize("kind", INPUTS)
 @pytest.mark.parametrize("M,O,H,N2", OBS_SHAPES)
 def test_obs_mlp_forward(ops, M, O, H, N2, kind):
-    rng = np.random.default_rng(M + O + H + N2)
-    p = synth.init_params(M, O, N2, H)["policy"]
-    x = make_x(rng, M, O, kind)
-    want, _ = orc.mlp_forward(x.astype(np.float64), *[p[k].astype(np.float64) for k in PKEYS])
+    x, p = forward_case(M, O, H, N2, kind)
     params, xd = ops.pack_params(p), dev(x)
     got = forward(ops, xd, params, M, O, H, N2)
-    err = float(np.abs(got.cpu().numpy() - want).max())
-    print(f"fwd M={M} O={O} H={H} N2={N2} {kind}: max abs err {err:.2e}")
-    assert err < ATOL
+    check_forward(got, x, p, f"fwd {M},{O},{H},{N2} {kind}")
     assert torch.equal(got, forward(ops, xd, params, M, O, H, N2))  # bitwise reproducible
 
 
 @pytest.mark.parametrize("kind", INPUTS)
 @pytest.mark.parametrize("M,O,H,N2", OBS_SHAPES)
 def test_obs_mlp_backward(ops, M, O, H, N2, kind):
-    rng = np.random.default_rng(7 * M + O + H + N2)
-    p = synth.init_params(M + 1, O, N2, H)["policy"]
-    x = make_x(rng, M, O, kind)
-    dout = (rng.standard_normal((M, N2), dtype=np.float32) / M).astype(np.float32)
-    p64 = [p[k].astype(np.float64) for k in PKEYS]
-    _, pre = orc.mlp_forward(x.astype(np.float64), *p64)
-    want = orc.mlp_backward(x.astype(np.float64), pre, p64[2], dout.astype(np.float64))
+    x, p, dout = backward_case(M, O, H, N2, kind)
     params, xd, dd = ops.pack_params(p), dev(x), dev(dout)
     flat = backward(ops, xd, params, dd, M, O, H, N2)
-    assert not torch.isnan(flat).any()
-    got = ops.unpack_grad(flat, O, H, N2)
-    one_row = float(np.abs(dout).max() * np.abs(p[PKEYS[2]]).max() * max(1.0, np.abs(x).max()))
-    for k, w in zip(PKEYS, want):
-        assert got[k].shape == w.shape
-        tol = 2e-5 * np.abs(w).max() + (3 * one_row if k in PKEYS[:2] else 0.0)
-        err = float(np.abs(got[k] - w).max())
-        print(f"bwd M={M} O={O} H={H} N2={N2} {kind} {k}: max abs err {err:.2e} (max |g| {np.abs(w).max():.2e})")
-        assert err < tol, (k, err, tol)
-    total = float(flat.abs().sum().cpu())
-    real = sum(np.abs(g).sum() for g in got.values())
-    assert abs(total - real) <= 1e-12 * max(1.0, real)  # pad entries are exactly zero
+    check_backward(flat, x, p, dout, f"bwd {M},{O},{H},{N2} {kind}")  # also: pad entries exactly zero
     assert torch.equal(flat, backward(ops, xd, params, dd, M, O, H, N2))  # bitwise reproducible
 
 
@@ -166,8 +155,9 @@ def test_obs_first_step_matches_oracle(name):
     assert par["max_abs_pg"] < 1e-5, par
     for k, v in par["scalars"].items():
         assert v["abs_err"] < 1e-5, (k, v)
+    check_engine_mlp(eng, params)
     if par["max_rel_grad"] >= 5e-5:
-        _check_grad_with_relu_ties(eng, params, batch, hp)
+        check_grad_end_to_end(eng, params, batch, hp)
     assert par["max_abs_param_after_1_update"] < 5e-5, par
     assert par["frac_params_off"] < 1e-3, par
     for k in ("norm_policy", "norm_value"):

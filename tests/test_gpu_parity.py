@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from conftest import PKEYS
+from mlp_bounds import check_backward, check_forward
 from oracle import impala_oracle as orc
 from torched_impala_b200 import synth
 from torched_impala_b200.utils import default_hparams
@@ -58,46 +59,46 @@ MLP_SHAPES = [
 ]
 
 
-@pytest.mark.parametrize("tensor_cores", ["1", "0"])
-@pytest.mark.parametrize("M,O,H,N2", MLP_SHAPES)
-def test_mlp_forward(ops, monkeypatch, M, O, H, N2, tensor_cores):
-    """Both forward paths: wgmma 3xTF32 (default where the layer is GEMM-shaped) and FP32 FFMA."""
-    monkeypatch.setenv("IMPALA_MLP_TC", tensor_cores)
+BWD_SHAPES = MLP_SHAPES + [(96, 4, 128, 1), (4100, 8, 256, 3), (2500, 28, 128, 4)]
+
+
+def forward_case(M, O, H, N2):
+    """Seeded rows and parameters of the forward tests here, in test_gpu_wide_shapes.py and test_gpu_actions_mid.py."""
     rng = np.random.default_rng(M + O + H + N2)
-    p = synth.init_params(M, O, N2, H)["policy"]
-    x = rng.standard_normal((M, O), dtype=np.float32)
-    want, _ = orc.mlp_forward(x.astype(np.float64), *[p[k].astype(np.float64) for k in PKEYS])
-    got = ops.mlp_forward(dev(x), ops.pack_params(p), O, H, N2).cpu().numpy()
-    assert got.shape == (M, N2)
-    assert np.abs(got - want).max() < ATOL
+    return rng.standard_normal((M, O), dtype=np.float32), synth.init_params(M, O, N2, H)["policy"]
 
 
-@pytest.mark.parametrize("tensor_cores", ["1", "0"])
-@pytest.mark.parametrize("M,O,H,N2", MLP_SHAPES + [(96, 4, 128, 1), (4100, 8, 256, 3), (2500, 28, 128, 4)])
-def test_mlp_backward(ops, monkeypatch, M, O, H, N2, tensor_cores):
-    """Both backward paths (wgmma 3xTF32 for H in {128,256}, O%4==0, O<=28; FP32 FFMA otherwise).
-
-    A ReLU unit whose pre-activation is within rounding of 0 may be switched differently than in
-    float64; that moves one entry by one row's contribution, hence the tolerance term below."""
-    monkeypatch.setenv("IMPALA_MLP_TC", tensor_cores)
+def backward_case(M, O, H, N2):
+    """Seeded rows, parameters and output gradient of the backward tests of the same three files."""
     rng = np.random.default_rng(7 * M + O + H + N2)
     p = synth.init_params(M + 1, O, N2, H)["policy"]
     x = rng.standard_normal((M, O), dtype=np.float32)
     dout = (rng.standard_normal((M, N2), dtype=np.float32) / M).astype(np.float32)
-    p64 = [p[k].astype(np.float64) for k in PKEYS]
-    _, pre = orc.mlp_forward(x.astype(np.float64), *p64)
-    want = orc.mlp_backward(x.astype(np.float64), pre, p64[2], dout.astype(np.float64))
+    return x, p, dout
+
+
+@pytest.mark.parametrize("tensor_cores", ["1", "0"])
+@pytest.mark.parametrize("M,O,H,N2", MLP_SHAPES)
+def test_mlp_forward(ops, monkeypatch, M, O, H, N2, tensor_cores):
+    """Both forward paths: wgmma 3xTF32 (default where the layer is GEMM-shaped) and FP32 FFMA, every output
+    within its float64 error bound (tests/mlp_bounds.py)."""
+    monkeypatch.setenv("IMPALA_MLP_TC", tensor_cores)
+    x, p = forward_case(M, O, H, N2)
+    got = ops.mlp_forward(dev(x), ops.pack_params(p), O, H, N2)
+    assert got.shape == (M, N2)
+    check_forward(got, x, p, f"fwd {M},{O},{H},{N2} tc={tensor_cores}")
+
+
+@pytest.mark.parametrize("tensor_cores", ["1", "0"])
+@pytest.mark.parametrize("M,O,H,N2", BWD_SHAPES)
+def test_mlp_backward(ops, monkeypatch, M, O, H, N2, tensor_cores):
+    """Both backward paths (wgmma 3xTF32 for H in {128,256}, O%4==0, O<=28; FP32 FFMA otherwise): every
+    gradient entry within its float64 error bound, which allows a ReLU tie only in the entries it moves; pad
+    entries of the parameter block exactly zero (they enter the clip norm)."""
+    monkeypatch.setenv("IMPALA_MLP_TC", tensor_cores)
+    x, p, dout = backward_case(M, O, H, N2)
     flat = ops.mlp_backward(dev(x), ops.pack_params(p), dev(dout), O, H, N2)
-    got = ops.unpack_grad(flat, O, H, N2)
-    one_row = float(np.abs(dout).max() * np.abs(p[PKEYS[2]]).max() * max(1.0, np.abs(x).max()))
-    for k, w in zip(PKEYS, want):
-        assert got[k].shape == w.shape
-        tol = 2e-5 * np.abs(w).max() + (3 * one_row if k in PKEYS[:2] else 0.0)
-        assert np.abs(got[k] - w).max() < tol, (k, rel_err(got[k], w))
-    # pad entries of the parameter block must be exactly zero (they enter the clip norm)
-    total = float(flat.abs().sum().cpu())
-    real = sum(np.abs(g).sum() for g in got.values())
-    assert abs(total - real) <= 1e-12 * max(1.0, real)
+    check_backward(flat, x, p, dout, f"bwd {M},{O},{H},{N2} tc={tensor_cores}")
 
 
 PAIR_SHAPES = [
