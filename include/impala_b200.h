@@ -246,6 +246,27 @@ int impala_clip_adam(float* params, const double* grad, float* m, float* v, int6
                      int64_t n_policy, int64_t n_total, float max_norm, float lr, float beta1,
                      float beta2, float eps, double* norms_out, void* stream);
 
+/* Update rules of impala_clip_optim / impala_gather_clip_optim. */
+#define IMPALA_OPT_ADAM 0    /* torch.optim.Adam, no weight decay:  h0 = beta1, h1 = beta2 */
+#define IMPALA_OPT_RMSPROP 1 /* torch.optim.RMSprop, not centered, no weight decay:  h0 = alpha, h1 = momentum */
+
+/* impala_clip_adam with a choice of update rule and a learning-rate SCHEDULE read from device memory:
+ * the update after n completed ones (n = state[0]) uses lr_table[min(n, n_lr - 1)] - torch's
+ * LambdaLR(lambda) with lr_table[e] = lr * lambda(e).  The table is only read, so one captured CUDA graph
+ * serves every update of a schedule.  Clipping, norms_out and the float32 state are as in impala_clip_adam.
+ *   IMPALA_OPT_ADAM     m = exp_avg, v = exp_avg_sq, state = {step, beta1^step, beta2^step bits}: a table of
+ *                       one constant lr gives the bits of impala_clip_adam with that lr.
+ *   IMPALA_OPT_RMSPROP  per entry, on the clipped gradient g:  v = alpha v + (1 - alpha) g^2,
+ *                       avg = sqrt(v) + eps (eps OUTSIDE the root, as torch);  momentum > 0:  m = momentum m +
+ *                       g / avg, param -= lr m;  momentum = 0:  param -= lr g / avg and m is neither read nor
+ *                       written.  v = square_avg, m = momentum_buffer (both start at 0); state[0] counts the
+ *                       steps, state[1] and state[2] are left as they are.
+ * Returns IMPALA_ERR_BAD_ARG before any launch for the arguments impala_clip_adam refuses, a NULL lr_table,
+ * n_lr < 1, an unknown rule, eps < 0, and for RMSprop alpha outside [0, 1) or momentum < 0 (NaN included). */
+int impala_clip_optim(float* params, const double* grad, float* m, float* v, int64_t* state,
+                      int64_t n_policy, int64_t n_total, float max_norm, const float* lr_table, int64_t n_lr,
+                      int rule, float h0, float h1, float eps, double* norms_out, void* stream);
+
 /* Node-local buffers that the other ranks (one process per GPU) map into their address space
  * for the push-model all-reduce below: impala_peer_alloc = cudaMalloc + zero-fill on the current
  * device and its 64-byte CUDA IPC handle (to be sent to the peers, e.g. through
@@ -300,6 +321,13 @@ int impala_gather_clip_adam(float* params, double* reduced, const void* gather, 
                             float* v, int64_t* state, int64_t n_policy, int64_t n_total,
                             float max_norm, float lr, float beta1, float beta2, float eps,
                             double* norms_out, int* err, double timeout_s, void* stream);
+/* impala_gather_clip_adam whose update is impala_clip_optim's (rule, h0, h1, eps, learning-rate table);
+ * refuses what either of the two refuses.  The table entry is read before the wait on the backward. */
+int impala_gather_clip_optim(float* params, double* reduced, const void* gather, long long* seq,
+                             int64_t slot_stride, int64_t buf_stride, int world, int n_extra, float* m,
+                             float* v, int64_t* state, int64_t n_policy, int64_t n_total, float max_norm,
+                             const float* lr_table, int64_t n_lr, int rule, float h0, float h1, float eps,
+                             double* norms_out, int* err, double timeout_s, void* stream);
 
 /* Pieces of the reference's module-level loss helpers (learner.py:298-321) for callers that use
  * them individually instead of impala_vtrace_loss.  logits (M,A) f32 row-major, actions (M) i32.

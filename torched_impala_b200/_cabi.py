@@ -19,6 +19,10 @@ OBS_F32 = 0
 OBS_U8 = 1
 OBS_DTYPES = {"float32": OBS_F32, "uint8": OBS_U8}  # batch-slab observation types (impala_batch_layout_obs)
 
+OPT_ADAM = 0
+OPT_RMSPROP = 1
+OPT_RULES = {"adam": OPT_ADAM, "rmsprop": OPT_RMSPROP}  # update rules of impala_clip_optim
+
 
 def obs_dtype_code(obs_dtype: str) -> int:
     if obs_dtype not in OBS_DTYPES:
@@ -71,6 +75,9 @@ SIGNATURES = {
     "impala_vtrace_loss_diag_workspace": (_i64, [_i, _i, _i]),
     "impala_vtrace_loss_diag": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p]),
     "impala_clip_adam": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _f, _f, _f, _f, _p, _p]),
+    "impala_clip_optim": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i, _f, _f, _f, _p, _p]),
+    "impala_gather_clip_optim": (_i, [_p] * 4 + [_i64, _i64, _i, _i, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i]
+                                 + [_f] * 3 + [_p, _p, C.c_double, _p]),
     "impala_policy_terms": (_i, [_p, _p, _p, _p, _i, _i, _p]),
     "impala_policy_terms_backward": (_i, [_p, _p, _p, _p, _p, _i, _i, _p]),
     "impala_reduce": (_i, [_p, _p, _i64, _i, _p, _p]),

@@ -1,4 +1,4 @@
-// Per-group gradient clipping + Adam + step counter in ONE launch
+// Per-group gradient clipping + Adam (or RMSprop) + step counter in ONE launch
 // (reference learner.py:176-183: two clip_grad_norm_ calls, Adam.step, LambdaLR.step).
 //
 // The parameter vector is tiny (14 144 floats at H=256, 69 312 at H=512) but the two clip
@@ -6,9 +6,14 @@
 // cluster of 8 CTAs (8 x 1024 threads, co-scheduled by hardware) does both phases in a
 // single launch: each CTA reduces the squares of its slice in float64, the 8 partial pairs
 // are exchanged through distributed shared memory, one cluster barrier later every CTA
-// holds the same two norms and applies Adam to its slice.  The gradient arrives as float64
+// holds the same two norms and applies the update to its slice.  The gradient arrives as float64
 // (sum of per-CTA float32 partials, possibly all-reduced over ranks) and the norms are reduced
 // in float64; optimizer state stays float32 in HBM and the per-element update runs in float32.
+//
+// Both kernels are written once, as a body templated on the update rule (AdamRule, RmspropRule)
+// and on where the learning rate comes from (LrScalar: a launch argument; LrTable: a device table
+// indexed by the step counter, so one captured CUDA graph serves a whole learning-rate schedule).
+// impala_clip_adam / impala_gather_clip_adam are the <AdamRule, LrScalar> instantiations.
 #include <cooperative_groups.h>
 #include <math.h>
 
@@ -21,18 +26,96 @@ namespace {
 constexpr int kAdamThreads = 1024;
 constexpr int kAdamCluster = 8;
 
-// state[0] = step count (int64), state[1] / state[2] = beta1^t / beta2^t as float64 bit patterns
+// ---- learning-rate sources: the rate of the update after `t` completed ones (t = state[0])
+struct LrScalar {
+    float lr;
+    __device__ __forceinline__ float at(int64_t) const { return lr; }
+};
+
+// LambdaLR as a table: update n (1-based) uses table[n - 1]; steps past the end keep the last entry.
+// The table is only read, so the rate changes from one replay of a captured graph to the next.
+struct LrTable {
+    const float* __restrict__ table;
+    int64_t n;
+    __device__ __forceinline__ float at(int64_t t) const { return table[t <= 0 ? 0 : (t < n ? t : n - 1)]; }
+};
+
+// ---- update rules.  Each rule sees the clipped float32 gradient g of one entry with its float32 state
+// (p, m, v) and writes what it changes; k0 / k1 are the two per-step constants `prepare` left for every
+// thread (thread 64 runs `prepare` once, before the update; `finish` advances the state at the very end).
+
+// torch.optim.Adam (no weight decay).  state = int64[3] {step count, beta1^t, beta2^t as float64 bits}
 // (all-zero state = fresh optimizer): running powers replace two float64 pow() calls per step.
-__global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
-clip_adam_kernel(float* __restrict__ params, const double* __restrict__ grad, float* __restrict__ m,
-                 float* __restrict__ v, int64_t* __restrict__ state, int64_t n_policy,
-                 int64_t n_total, float max_norm, float lr, float beta1, float beta2, float eps,
-                 double* __restrict__ norms_out) {
+struct AdamRule {
+    float b1, b2, eps;
+    __device__ __forceinline__ bool reads_m() const { return true; }
+    __device__ __forceinline__ void prepare(const int64_t* __restrict__ state, float lr, float* s_k,
+                                            double* s_pow) const {
+        const double p1 = state[0] == 0 ? 1.0 : __longlong_as_double(state[1]);
+        const double p2 = state[0] == 0 ? 1.0 : __longlong_as_double(state[2]);
+        s_pow[0] = p1 * (double)b1, s_pow[1] = p2 * (double)b2;
+        s_k[0] = (float)((double)lr / (1.0 - s_pow[0]));  // step_size = lr / (1 - beta1^t)
+        s_k[1] = (float)(1.0 / sqrt(1.0 - s_pow[1]));     // 1 / sqrt(1 - beta2^t)
+    }
+    __device__ __forceinline__ void apply(int64_t i, float g, float p, float mi, float vi, float step_size,
+                                          float inv_bc2_sqrt, float* __restrict__ params, float* __restrict__ m,
+                                          float* __restrict__ v) const {
+        mi = fmaf(b1, mi, (1.f - b1) * g);
+        vi = fmaf(b2, vi, (1.f - b2) * g * g);
+        const float denom = fmaf(sqrtf(vi), inv_bc2_sqrt, eps);
+        params[i] = p - step_size * mi / denom;
+        m[i] = mi;
+        v[i] = vi;
+    }
+    __device__ __forceinline__ void finish(int64_t* __restrict__ state, const double* s_pow) const {
+        state[0] += 1;
+        state[1] = __double_as_longlong(s_pow[0]);
+        state[2] = __double_as_longlong(s_pow[1]);
+    }
+};
+
+// torch.optim.RMSprop (not centered, no weight decay): square_avg in v, the momentum buffer in m (neither read
+// nor written when momentum = 0), eps added outside the square root as torch does.  Only state[0] is used.
+struct RmspropRule {
+    float alpha, momentum, eps;
+    __device__ __forceinline__ bool reads_m() const { return momentum > 0.f; }
+    __device__ __forceinline__ void prepare(const int64_t* __restrict__, float lr, float* s_k, double*) const {
+        s_k[0] = lr;
+        s_k[1] = 0.f;
+    }
+    __device__ __forceinline__ void apply(int64_t i, float g, float p, float mi, float vi, float lr, float,
+                                          float* __restrict__ params, float* __restrict__ m,
+                                          float* __restrict__ v) const {
+        vi = fmaf(alpha, vi, (1.f - alpha) * g * g);
+        const float avg = sqrtf(vi) + eps;
+        if (momentum > 0.f) {
+            mi = fmaf(momentum, mi, g / avg);
+            params[i] = p - lr * mi;
+            m[i] = mi;
+        } else {
+            params[i] = p - lr * (g / avg);
+        }
+        v[i] = vi;
+    }
+    __device__ __forceinline__ void finish(int64_t* __restrict__ state, const double*) const { state[0] += 1; }
+};
+
+// torch.nn.utils.clip_grad_norm_: coef = max_norm / (norm + 1e-6), clamped to 1; a NaN norm gives a NaN
+// coefficient (torch.clamp propagates NaN, fmin would return the 1)
+__device__ __forceinline__ float clip_coef(double norm, float max_norm) {
+    return isnan(norm) ? (float)norm : (float)fmin(1.0, (double)max_norm / (norm + 1e-6));
+}
+
+template <class Rule, class Lr>
+__device__ __forceinline__ void clip_update(float* __restrict__ params, const double* __restrict__ grad,
+                                            float* __restrict__ m, float* __restrict__ v,
+                                            int64_t* __restrict__ state, int64_t n_policy, int64_t n_total,
+                                            float max_norm, Lr lr, Rule rule, double* __restrict__ norms_out) {
     cg::cluster_group cluster = cg::this_cluster();
     __shared__ double s_warp[2][kAdamThreads / 32];
     __shared__ double s_cta[2];   // this CTA's partial sums of squares (read by the peers)
     __shared__ float s_coef[2];
-    __shared__ float s_bias[2];   // step_size = lr / (1 - beta1^t), 1 / sqrt(1 - beta2^t)
+    __shared__ float s_bias[2];   // the rule's two per-step constants
     __shared__ double s_pow[2];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int64_t first = (int64_t)cluster.block_rank() * kAdamThreads + tid;
@@ -48,7 +131,7 @@ clip_adam_kernel(float* __restrict__ params, const double* __restrict__ grad, fl
     for (int k = 0; k < kKeep; ++k) {  // optimizer state: not touched by the backward, loaded before the wait
         const int64_t i = first + k * stride;
         pk[k] = i < n_total ? params[i] : 0.f;
-        mk[k] = i < n_total ? m[i] : 0.f;
+        mk[k] = i < n_total && rule.reads_m() ? m[i] : 0.f;
         vk[k] = i < n_total ? v[i] : 0.f;
     }
     pdl_wait();  // the gradient comes from the backward kernel
@@ -71,13 +154,8 @@ clip_adam_kernel(float* __restrict__ params, const double* __restrict__ grad, fl
     ss0 = warp_sum_f64(ss0);
     ss1 = warp_sum_f64(ss1);
     if (lane == 0) s_warp[0][warp] = ss0, s_warp[1][warp] = ss1;
-    if (tid == 64) {  // bias corrections from the running powers (nobody writes state before the end)
-        const double p1 = state[0] == 0 ? 1.0 : __longlong_as_double(state[1]);
-        const double p2 = state[0] == 0 ? 1.0 : __longlong_as_double(state[2]);
-        s_pow[0] = p1 * (double)beta1, s_pow[1] = p2 * (double)beta2;
-        s_bias[0] = (float)((double)lr / (1.0 - s_pow[0]));
-        s_bias[1] = (float)(1.0 / sqrt(1.0 - s_pow[1]));
-    }
+    if (tid == 64)  // learning rate and bias corrections (nobody writes state before the end)
+        rule.prepare(state, lr.at(state[0]), s_bias, s_pow);
     __syncthreads();
     if (tid < 2) {
         double s = 0.0;
@@ -89,23 +167,15 @@ clip_adam_kernel(float* __restrict__ params, const double* __restrict__ grad, fl
         double s = 0.0;
         for (int r = 0; r < kAdamCluster; ++r) s += *cluster.map_shared_rank(&s_cta[tid], r);
         const double norm = sqrt(s);
-        // torch.nn.utils.clip_grad_norm_: coef = max_norm / (norm + 1e-6), clamped to 1; a NaN norm
-        // gives a NaN coefficient (torch.clamp propagates NaN, fmin would return the 1)
-        s_coef[tid] = isnan(norm) ? (float)norm : (float)fmin(1.0, (double)max_norm / (norm + 1e-6));
+        s_coef[tid] = clip_coef(norm, max_norm);
         if (norms_out && cluster.block_rank() == 0) norms_out[tid] = norm;
     }
     __syncthreads();
-    // phase 2: Adam in float32 arithmetic (the state is float32; one step's rounding is ~1e-7)
-    const float b1 = beta1, b2 = beta2, step_size = s_bias[0], inv_bc2_sqrt = s_bias[1];
+    // phase 2: the update in float32 arithmetic (the state is float32; one step's rounding is ~1e-7)
+    const float k0 = s_bias[0], k1 = s_bias[1];
     const float c0 = s_coef[0], c1 = s_coef[1];
     auto update = [&](int64_t i, float g, float p, float mi, float vi) {
-        g *= (i < n_policy ? c0 : c1);
-        mi = fmaf(b1, mi, (1.f - b1) * g);
-        vi = fmaf(b2, vi, (1.f - b2) * g * g);
-        const float denom = fmaf(sqrtf(vi), inv_bc2_sqrt, eps);
-        params[i] = p - step_size * mi / denom;
-        m[i] = mi;
-        v[i] = vi;
+        rule.apply(i, g * (i < n_policy ? c0 : c1), p, mi, vi, k0, k1, params, m, v);
     };
 #pragma unroll
     for (int k = 0; k < kKeep; ++k) {
@@ -113,13 +183,29 @@ clip_adam_kernel(float* __restrict__ params, const double* __restrict__ grad, fl
         if (i < n_total) update(i, (float)gk[k], pk[k], mk[k], vk[k]);
     }
     for (int64_t i = first + kKeep * stride; i < n_total; i += stride)
-        update(i, (float)grad[i], params[i], m[i], v[i]);
+        update(i, (float)grad[i], params[i], rule.reads_m() ? m[i] : 0.f, v[i]);
     cluster.sync();  // peers finished reading this CTA's shared memory; every CTA has read state
-    if (cluster.block_rank() == 0 && tid == 64) {
-        state[0] += 1;
-        state[1] = __double_as_longlong(s_pow[0]);
-        state[2] = __double_as_longlong(s_pow[1]);
-    }
+    if (cluster.block_rank() == 0 && tid == 64) rule.finish(state, s_pow);
+}
+
+__global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
+clip_adam_kernel(float* __restrict__ params, const double* __restrict__ grad, float* __restrict__ m,
+                 float* __restrict__ v, int64_t* __restrict__ state, int64_t n_policy,
+                 int64_t n_total, float max_norm, float lr, float beta1, float beta2, float eps,
+                 double* __restrict__ norms_out) {
+    clip_update(params, grad, m, v, state, n_policy, n_total, max_norm, LrScalar{lr}, AdamRule{beta1, beta2, eps},
+                norms_out);
+}
+
+// Rule = AdamRule: h0, h1 = beta1, beta2.  Rule = RmspropRule: h0, h1 = alpha, momentum.
+template <class Rule>
+__global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
+clip_optim_kernel(float* __restrict__ params, const double* __restrict__ grad, float* __restrict__ m,
+                  float* __restrict__ v, int64_t* __restrict__ state, int64_t n_policy, int64_t n_total,
+                  float max_norm, const float* __restrict__ lr_table, int64_t n_lr, float h0, float h1, float eps,
+                  double* __restrict__ norms_out) {
+    clip_update(params, grad, m, v, state, n_policy, n_total, max_norm, LrTable{lr_table, n_lr}, Rule{h0, h1, eps},
+                norms_out);
 }
 
 
@@ -134,7 +220,7 @@ clip_adam_kernel(float* __restrict__ params, const double* __restrict__ grad, fl
 // posted NVLink writes, nobody waits for a round trip, no fence, no flag.  The optimizer kernel of
 // each rank polls the `world` slots of its OWN buffer (local memory) until each element carries
 // the current step, adds them in rank order - every rank forms bit-identical sums, so the
-// replicas cannot drift - and runs the clip norms and Adam on the sum.  The data path costs one
+// replicas cannot drift - and runs the clip norms and the update on the sum.  The data path costs one
 // NVLink one-way latency.
 //
 // The buffers are double-buffered by step parity, which makes an "I have read your slot" message
@@ -169,15 +255,15 @@ peer_push_kernel(const double* __restrict__ local, int64_t n, PushArgs p) {
     }
 }
 
-// Consumer: poll the local slots, add them in rank order, clip + Adam.
-__global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
-gather_clip_adam_kernel(float* __restrict__ params, double* __restrict__ reduced,
-                        const ulonglong2* __restrict__ gather, long long* __restrict__ seq,
-                        int64_t slot_stride, int64_t buf_stride, int world, int n_extra,
-                        float* __restrict__ m, float* __restrict__ v, int64_t* __restrict__ state,
-                        int64_t n_policy, int64_t n_total, float max_norm, float lr, float beta1,
-                        float beta2, float eps, double* __restrict__ norms_out, int* __restrict__ err,
-                        unsigned long long timeout_ns) {
+// Consumer: poll the local slots, add them in rank order, clip + update.
+template <class Rule, class Lr>
+__device__ __forceinline__ void gather_clip_update(float* __restrict__ params, double* __restrict__ reduced,
+                                                   const ulonglong2* __restrict__ gather, long long* __restrict__ seq,
+                                                   int64_t slot_stride, int64_t buf_stride, int world, int n_extra,
+                                                   float* __restrict__ m, float* __restrict__ v,
+                                                   int64_t* __restrict__ state, int64_t n_policy, int64_t n_total,
+                                                   float max_norm, Lr lr, Rule rule, double* __restrict__ norms_out,
+                                                   int* __restrict__ err, unsigned long long timeout_ns) {
     cg::cluster_group cluster = cg::this_cluster();
     __shared__ double s_warp[2][kAdamThreads / 32];
     __shared__ double s_cta[2];
@@ -198,17 +284,12 @@ gather_clip_adam_kernel(float* __restrict__ params, double* __restrict__ reduced
     for (int k = 0; k < kKeep; ++k) {
         const int64_t i = first + k * stride;
         pk[k] = i < n_total ? params[i] : 0.f;
-        mk[k] = i < n_total ? m[i] : 0.f;
+        mk[k] = i < n_total && rule.reads_m() ? m[i] : 0.f;
         vk[k] = i < n_total ? v[i] : 0.f;
     }
     if (tid == 0) s_abort = 0;
-    if (tid == 64) {  // bias corrections from the running powers (nobody writes state before the end)
-        const double p1 = state[0] == 0 ? 1.0 : __longlong_as_double(state[1]);
-        const double p2 = state[0] == 0 ? 1.0 : __longlong_as_double(state[2]);
-        s_pow[0] = p1 * (double)beta1, s_pow[1] = p2 * (double)beta2;
-        s_bias[0] = (float)((double)lr / (1.0 - s_pow[0]));
-        s_bias[1] = (float)(1.0 / sqrt(1.0 - s_pow[1]));
-    }
+    if (tid == 64)  // learning rate and bias corrections (nobody writes state before the end)
+        rule.prepare(state, lr.at(state[0]), s_bias, s_pow);
     pdl_wait();  // orders this kernel behind the local backward (its successors rely on that)
     const long long step64 = *seq + 1;
     const unsigned step = (unsigned)step64;
@@ -284,21 +365,15 @@ gather_clip_adam_kernel(float* __restrict__ params, double* __restrict__ reduced
         double s = 0.0;
         for (int r = 0; r < kAdamCluster; ++r) s += *cluster.map_shared_rank(&s_cta[tid], r);
         const double norm = sqrt(s);
-        s_coef[tid] = isnan(norm) ? (float)norm : (float)fmin(1.0, (double)max_norm / (norm + 1e-6));  // as above
+        s_coef[tid] = clip_coef(norm, max_norm);
         if (norms_out && crank == 0) norms_out[tid] = norm;
     }
     __syncthreads();
     if (!s_any_abort) {
-        const float b1 = beta1, b2 = beta2, step_size = s_bias[0], inv_bc2_sqrt = s_bias[1];
+        const float k0 = s_bias[0], k1 = s_bias[1];
         const float c0 = s_coef[0], c1 = s_coef[1];
         auto update = [&](int64_t i, float g, float p, float mi, float vi) {
-            g *= (i < n_policy ? c0 : c1);
-            mi = fmaf(b1, mi, (1.f - b1) * g);
-            vi = fmaf(b2, vi, (1.f - b2) * g * g);
-            const float denom = fmaf(sqrtf(vi), inv_bc2_sqrt, eps);
-            params[i] = p - step_size * mi / denom;
-            m[i] = mi;
-            v[i] = vi;
+            rule.apply(i, g * (i < n_policy ? c0 : c1), p, mi, vi, k0, k1, params, m, v);
         };
 #pragma unroll
         for (int k = 0; k < kKeep; ++k) {
@@ -306,19 +381,54 @@ gather_clip_adam_kernel(float* __restrict__ params, double* __restrict__ reduced
             if (i < n_total) update(i, (float)gk[k], pk[k], mk[k], vk[k]);
         }
         for (int64_t i = first + kKeep * stride; i < n_total; i += stride)
-            update(i, (float)reduced[i], params[i], m[i], v[i]);
+            update(i, (float)reduced[i], params[i], rule.reads_m() ? m[i] : 0.f, v[i]);
     }
     cluster.sync();  // peers finished reading this CTA's shared memory; every CTA has read state
     if (crank == 0 && tid == 64) {
         if (s_any_abort) {
             if (err) *err = 1;  // the host raises; state and seq stay as they were
         } else {
-            state[0] += 1;
-            state[1] = __double_as_longlong(s_pow[0]);
-            state[2] = __double_as_longlong(s_pow[1]);
+            rule.finish(state, s_pow);
             *seq = step64;
         }
     }
+}
+
+__global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
+gather_clip_adam_kernel(float* __restrict__ params, double* __restrict__ reduced,
+                        const ulonglong2* __restrict__ gather, long long* __restrict__ seq,
+                        int64_t slot_stride, int64_t buf_stride, int world, int n_extra,
+                        float* __restrict__ m, float* __restrict__ v, int64_t* __restrict__ state,
+                        int64_t n_policy, int64_t n_total, float max_norm, float lr, float beta1,
+                        float beta2, float eps, double* __restrict__ norms_out, int* __restrict__ err,
+                        unsigned long long timeout_ns) {
+    gather_clip_update(params, reduced, gather, seq, slot_stride, buf_stride, world, n_extra, m, v, state, n_policy,
+                       n_total, max_norm, LrScalar{lr}, AdamRule{beta1, beta2, eps}, norms_out, err, timeout_ns);
+}
+
+template <class Rule>
+__global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
+gather_clip_optim_kernel(float* __restrict__ params, double* __restrict__ reduced,
+                         const ulonglong2* __restrict__ gather, long long* __restrict__ seq,
+                         int64_t slot_stride, int64_t buf_stride, int world, int n_extra,
+                         float* __restrict__ m, float* __restrict__ v, int64_t* __restrict__ state,
+                         int64_t n_policy, int64_t n_total, float max_norm, const float* __restrict__ lr_table,
+                         int64_t n_lr, float h0, float h1, float eps, double* __restrict__ norms_out,
+                         int* __restrict__ err, unsigned long long timeout_ns) {
+    gather_clip_update(params, reduced, gather, seq, slot_stride, buf_stride, world, n_extra, m, v, state, n_policy,
+                       n_total, max_norm, LrTable{lr_table, n_lr}, Rule{h0, h1, eps}, norms_out, err, timeout_ns);
+}
+
+// The checks of impala_clip_optim / impala_gather_clip_optim beyond those of the Adam entry points.
+bool bad_optim_args(const float* lr_table, int64_t n_lr, int rule, float h0, float h1, float eps) {
+    if (!lr_table || n_lr < 1 || !(eps >= 0.f)) return true;
+    if (rule == IMPALA_OPT_ADAM) return false;
+    if (rule == IMPALA_OPT_RMSPROP) return !(h0 >= 0.f && h0 < 1.f) || !(h1 >= 0.f);
+    return true;
+}
+
+unsigned long long timeout_ns_of(double timeout_s) {
+    return timeout_s > 0 ? (unsigned long long)(timeout_s * 1e9) : 600ull * 1000000000ull;
 }
 
 }  // namespace
@@ -331,6 +441,20 @@ extern "C" int impala_clip_adam(float* params, const double* grad, float* m, flo
     if (n_total < 1 || n_policy < 0 || n_policy > n_total) return IMPALA_ERR_BAD_ARG;
     const cudaError_t e = impala_launch(clip_adam_kernel, kAdamCluster, kAdamThreads, 0, (cudaStream_t)stream, true, params,
                                         grad, m, v, state, n_policy, n_total, max_norm, lr, beta1, beta2, eps, norms_out);
+    if (e != cudaSuccess) return (int)e;
+    return impala_launch_status();
+}
+
+extern "C" int impala_clip_optim(float* params, const double* grad, float* m, float* v, int64_t* state,
+                                 int64_t n_policy, int64_t n_total, float max_norm, const float* lr_table,
+                                 int64_t n_lr, int rule, float h0, float h1, float eps, double* norms_out,
+                                 void* stream) {
+    if (!params || !grad || !m || !v || !state) return IMPALA_ERR_BAD_ARG;
+    if (n_total < 1 || n_policy < 0 || n_policy > n_total) return IMPALA_ERR_BAD_ARG;
+    if (bad_optim_args(lr_table, n_lr, rule, h0, h1, eps)) return IMPALA_ERR_BAD_ARG;
+    const auto kernel = rule == IMPALA_OPT_ADAM ? clip_optim_kernel<AdamRule> : clip_optim_kernel<RmspropRule>;
+    const cudaError_t e = impala_launch(kernel, kAdamCluster, kAdamThreads, 0, (cudaStream_t)stream, true, params, grad,
+                                        m, v, state, n_policy, n_total, max_norm, lr_table, n_lr, h0, h1, eps, norms_out);
     if (e != cudaSuccess) return (int)e;
     return impala_launch_status();
 }
@@ -351,22 +475,47 @@ extern "C" int impala_peer_push(const double* local, int64_t n, void* const* pee
     return impala_launch_status();
 }
 
+// The checks both gather entry points make.
+static bool bad_gather_args(float* params, double* reduced, const void* gather, long long* seq, int64_t slot_stride,
+                            int64_t buf_stride, int world, int n_extra, float* m, float* v, int64_t* state,
+                            int64_t n_policy, int64_t n_total) {
+    if (!params || !reduced || !gather || !seq || !m || !v || !state) return true;
+    if (n_total < 1 || n_policy < 0 || n_policy > n_total) return true;
+    if (world < 1 || world > 8 || n_extra < 0 || n_extra > kAdamThreads) return true;
+    if (slot_stride < n_total + n_extra || buf_stride < (int64_t)world * slot_stride) return true;
+    return (reinterpret_cast<uintptr_t>(gather) & 15) != 0;
+}
+
 extern "C" int impala_gather_clip_adam(float* params, double* reduced, const void* gather, long long* seq,
                                        int64_t slot_stride, int64_t buf_stride, int world, int n_extra, float* m,
                                        float* v, int64_t* state, int64_t n_policy, int64_t n_total, float max_norm,
                                        float lr, float beta1, float beta2, float eps, double* norms_out, int* err,
                                        double timeout_s, void* stream) {
-    if (!params || !reduced || !gather || !seq || !m || !v || !state) return IMPALA_ERR_BAD_ARG;
-    if (n_total < 1 || n_policy < 0 || n_policy > n_total) return IMPALA_ERR_BAD_ARG;
-    if (world < 1 || world > 8 || n_extra < 0 || n_extra > kAdamThreads) return IMPALA_ERR_BAD_ARG;
-    if (slot_stride < n_total + n_extra || buf_stride < (int64_t)world * slot_stride) return IMPALA_ERR_BAD_ARG;
-    if (reinterpret_cast<uintptr_t>(gather) & 15) return IMPALA_ERR_BAD_ARG;
-    const unsigned long long timeout_ns =
-        timeout_s > 0 ? (unsigned long long)(timeout_s * 1e9) : 600ull * 1000000000ull;
+    if (bad_gather_args(params, reduced, gather, seq, slot_stride, buf_stride, world, n_extra, m, v, state, n_policy,
+                        n_total))
+        return IMPALA_ERR_BAD_ARG;
     const cudaError_t e = impala_launch(gather_clip_adam_kernel, kAdamCluster, kAdamThreads, 0, (cudaStream_t)stream, true,
                                         params, reduced, static_cast<const ulonglong2*>(gather), seq, slot_stride, buf_stride,
                                         world, n_extra, m, v, state, n_policy, n_total, max_norm, lr, beta1, beta2, eps,
-                                        norms_out, err, timeout_ns);
+                                        norms_out, err, timeout_ns_of(timeout_s));
+    if (e != cudaSuccess) return (int)e;
+    return impala_launch_status();
+}
+
+extern "C" int impala_gather_clip_optim(float* params, double* reduced, const void* gather, long long* seq,
+                                        int64_t slot_stride, int64_t buf_stride, int world, int n_extra, float* m,
+                                        float* v, int64_t* state, int64_t n_policy, int64_t n_total, float max_norm,
+                                        const float* lr_table, int64_t n_lr, int rule, float h0, float h1, float eps,
+                                        double* norms_out, int* err, double timeout_s, void* stream) {
+    if (bad_gather_args(params, reduced, gather, seq, slot_stride, buf_stride, world, n_extra, m, v, state, n_policy,
+                        n_total))
+        return IMPALA_ERR_BAD_ARG;
+    if (bad_optim_args(lr_table, n_lr, rule, h0, h1, eps)) return IMPALA_ERR_BAD_ARG;
+    const auto kernel = rule == IMPALA_OPT_ADAM ? gather_clip_optim_kernel<AdamRule> : gather_clip_optim_kernel<RmspropRule>;
+    const cudaError_t e = impala_launch(kernel, kAdamCluster, kAdamThreads, 0, (cudaStream_t)stream, true, params, reduced,
+                                        static_cast<const ulonglong2*>(gather), seq, slot_stride, buf_stride, world,
+                                        n_extra, m, v, state, n_policy, n_total, max_norm, lr_table, n_lr, h0, h1, eps,
+                                        norms_out, err, timeout_ns_of(timeout_s));
     if (e != cudaSuccess) return (int)e;
     return impala_launch_status();
 }

@@ -103,11 +103,36 @@ def _wait(pred, timeout: float, what: str, ctl: ShardControl | None = None):
         time.sleep(_POLL_S)
 
 
+LR_TABLE_KEY = "optim/lr_table"  # init_state.npz entry of the learning-rate table (absent: the default)
+
+
+def write_init_state(path: str, init_state: dict, lr_table=None) -> None:
+    """The worker ranks' start: both networks' parameters and the learning-rate table (tabulated on rank 0: a
+    lambda need not pickle, and a command-line argument is capped at 128 KiB on Linux)."""
+    arrays = {f"{g}/{k}": np.asarray(v) for g, d in init_state.items() for k, v in d.items()}
+    if lr_table is not None:
+        arrays[LR_TABLE_KEY] = np.asarray(lr_table, np.float32)
+    np.savez(path, **arrays)
+
+
+def read_init_state(path: str):
+    """(state, lr_table or None) from the init_state.npz DpLeader writes."""
+    z = np.load(path)
+    state, table = {"policy": {}, "value_fn": {}}, None
+    for key in z.files:
+        if key == LR_TABLE_KEY:
+            table = z[key]
+            continue
+        g, k = key.split("/", 1)
+        state[g][k] = z[key]
+    return state, table
+
+
 class DpLeader:
     """Rank 0's handle on the worker ranks (lives inside the learner process, post-fork)."""
 
     def __init__(self, devices, cfg: dict, init_state: dict, slab_shm_name: str, slab_bytes: int,
-                 n_slabs: int, timeout: float = 200.0):
+                 n_slabs: int, timeout: float = 200.0, lr_table=None):
         self.world = len(devices)
         self.devices = list(devices)
         self.timeout = timeout
@@ -116,7 +141,7 @@ class DpLeader:
         self.step_no = 0
         self._tmp = tempfile.mkdtemp(prefix="impala_dp_")
         state_path = os.path.join(self._tmp, "init_state.npz")
-        np.savez(state_path, **{f"{g}/{k}": np.asarray(v) for g, d in init_state.items() for k, v in d.items()})
+        write_init_state(state_path, init_state, lr_table)
         self.procs = []
         root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
         for r in range(1, self.world):

@@ -33,15 +33,12 @@ def main():
                                 device_id=torch.device(dev))
         c = spec["cfg"]
         hp = Hyperparameters(**c["hp"])
+        state, lr_table = dp.read_init_state(spec["state"])
         eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], hp, global_batch=c["B"],
                             device=dev, mode=c["mode"], process_group=dist.group.WORLD,
                             obs_dtype=c.get("obs_dtype", "float32"), frames=c.get("frames", 1),
-                            diagnostics=c.get("diagnostics", False))
-        z = np.load(spec["state"])
-        state = {"policy": {}, "value_fn": {}}
-        for key in z.files:
-            g, k = key.split("/", 1)
-            state[g][k] = z[key]
+                            diagnostics=c.get("diagnostics", False), optimizer=c.get("optimizer", "adam"),
+                            optimizer_kwargs=c.get("optimizer_kwargs"), lr_table=lr_table)
         eng.load_state(state)
         shm = dp.attach_untracked(spec["slab_shm"])
         base = np.ndarray((1,), dtype=np.uint8, buffer=shm.buf).ctypes.data

@@ -18,6 +18,9 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       every rank's gather buffer; impala_gather_clip_adam polls its local slots, adds them in rank
       order and applies the update.  IMPALA_ALLREDUCE=nccl: torch.distributed all-reduce between the
       backward and impala_clip_adam instead.
+      optimizer="rmsprop" or an lr_lambda (learning-rate schedule): impala_clip_optim /
+      impala_gather_clip_optim in place of the two Adam entry points, with the rate of every update read
+      from a float32 table in device memory (optim.py) - the captured graphs stay valid for every update.
 
 obs_dtype="uint8" (byte observations): the slabs hold obs as uint8 (impala_batch_layout_obs).  For
 O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one after the other as the
@@ -56,6 +59,7 @@ import numpy as np
 import torch
 
 from . import _cabi
+from .optim import optim_config
 from .replay import ReplaySampler, check_replay_args
 
 PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
@@ -107,7 +111,11 @@ class LearnerEngine:
                  global_batch: int | None = None, device: str | torch.device = "cuda:0",
                  mode: str = "reference", process_group=None, use_graph: bool = True,
                  slabs: int = 2, obs_dtype: str = "float32", frames: int = 1, diagnostics: bool = False,
-                 replay_slabs: int = 0, replay_columns: int = 0, replay_seed: int = 0):
+                 replay_slabs: int = 0, replay_columns: int = 0, replay_seed: int = 0,
+                 optimizer: str = "adam", optimizer_kwargs: dict | None = None, lr_lambda=None, lr_table=None):
+        # update rule and learning-rate schedule, checked before any device work (optim.optim_config); the
+        # default - Adam at 0.95 * hp.lr - keeps impala_clip_adam with the rate as a launch argument
+        self.optim = optim_config(hp, optimizer, optimizer_kwargs, lr_lambda, lr_table)
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
@@ -156,6 +164,10 @@ class LearnerEngine:
         self.n_comm = self.n_total + self.n_extra + 4
         self.comm = torch.zeros(self.n_comm, dtype=torch.float64, device=self.dev)
         self.norms = torch.zeros(2, dtype=torch.float64, device=self.dev)
+        # the schedule (rmsprop or an lr_lambda): update n reads entry min(n - 1, len - 1); the state buffers
+        # keep their Adam names, RMSprop's square_avg lives in adam_v and its momentum buffer in adam_m
+        self.lr_table = (None if self.optim.lr_table is None
+                         else torch.from_numpy(self.optim.lr_table.copy()).to(self.dev))
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts (replay: the host slabs
         # hold the B_fresh columns that cross the host link, the device slabs the B columns trained on)
@@ -501,8 +513,14 @@ class LearnerEngine:
                             "impala_peer_push")
         return int(lib.impala_launch_count() - launched)  # kernels actually launched / captured
 
+    def lr_of(self, n: int) -> float:
+        """The learning rate update n (1-based) uses (host-side, no device read)."""
+        return self.optim.lr_of(n)
+
     def _enqueue_opt(self) -> int:
         hp, st = self.hp, C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        if self.lr_table is not None:
+            return self._enqueue_optim(st)
         if self.peer:
             pr = self.peer
             _cabi.check(self.lib.impala_gather_clip_adam(
@@ -516,6 +534,23 @@ class LearnerEngine:
             _ptr(self.adam_step), self.n_pi, self.n_total, float(hp.max_norm),
             float(0.95 * hp.lr),  # LambdaLR(lambda e: 0.95): constant factor, learner.py:42
             0.9, 0.999, 1e-8, _ptr(self.norms), st), "impala_clip_adam")
+        return 1
+
+    def _enqueue_optim(self, st) -> int:
+        """The chosen rule with the scheduled rate, on the same buffers and paths as _enqueue_opt."""
+        o, hp = self.optim, self.hp
+        rule = (_ptr(self.lr_table), self.lr_table.numel(), o.rule_code, o.h0, o.h1, o.eps)
+        if self.peer:
+            pr = self.peer
+            _cabi.check(self.lib.impala_gather_clip_optim(
+                _ptr(self.params), _ptr(self.comm), C.c_void_p(pr["gather"]), _ptr(pr["seq"]),
+                pr["slot"], pr["buf"], self.world, self.n_extra, _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step),
+                self.n_pi, self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), _ptr(pr["err"]), pr["timeout_s"],
+                st), "impala_gather_clip_optim")
+            return 1
+        _cabi.check(self.lib.impala_clip_optim(
+            _ptr(self.params), _ptr(self.comm), _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step), self.n_pi,
+            self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), st), "impala_clip_optim")
         return 1
 
     def _capture(self, slot: int):

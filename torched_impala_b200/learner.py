@@ -33,7 +33,10 @@ path of the device (SURVEY 8f-2, 8f-4):
     for the launcher (dp.py): rank 0 lives here, publishes weights and logs;
   * `replay_slabs=R, replay_columns=Br` (experience replay, off by default): every update consumes
     `batch_size - Br` trajectories from the queue and fills its other Br columns from the fresh batches of
-    the last R updates, kept in HBM (engine.py, replay.py); one device only.
+    the last R updates, kept in HBM (engine.py, replay.py); one device only;
+  * `optimizer="rmsprop"`, `optimizer_kwargs` (torch's RMSprop keywords) and `lr_lambda` (a LambdaLR
+    lambda, tabulated over hp.max_updates updates): the IMPALA paper's recipe (optim.py); the default is
+    the reference's Adam at 0.95 * hp.lr.  With a log_path and either one set, `optim/lr` is logged.
 
 CUDA is initialised inside the learner process only (`train.py:42` forces the fork start method,
 so the parent must never touch the device); a policy / value_fn that already lives on a CUDA
@@ -57,6 +60,7 @@ import numpy as np
 import torch
 import torch.multiprocessing as mp
 
+from .optim import optim_config
 from .replay import check_replay_args
 
 PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
@@ -242,8 +246,12 @@ class Learner:
     def __init__(self, id, hparams, policy, value_fn, q, update_counter, log_path=None,
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
                  evaluator=None, obs_dtype="float32", frames=1, diagnostics=False,
-                 replay_slabs=0, replay_columns=0):
+                 replay_slabs=0, replay_columns=0, optimizer="adam", optimizer_kwargs=None, lr_lambda=None):
         self.id = id
+        # update rule and learning-rate schedule: checked and tabulated here, in the launching process (a lambda
+        # need not pickle; data-parallel worker ranks receive the table)
+        self.optimizer, self.optimizer_kwargs = optimizer, dict(optimizer_kwargs or {})
+        self.optim = optim_config(hparams, optimizer, optimizer_kwargs, lr_lambda)
         if obs_dtype not in ("float32", "uint8"):
             raise ValueError(f"obs_dtype must be 'float32' or 'uint8', got {obs_dtype!r}")
         if hasattr(q, "collect_batch") and getattr(q, "obs_dtype", "float32") != obs_dtype:
@@ -328,7 +336,8 @@ class Learner:
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
                     obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics,
-                    replay_slabs=self.replay_slabs, replay_columns=self.replay_columns)
+                    replay_slabs=self.replay_slabs, replay_columns=self.replay_columns, optimizer=self.optimizer,
+                    optimizer_kwargs=self.optimizer_kwargs)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -339,7 +348,9 @@ class Learner:
         eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], self.hp,
                             global_batch=c["B"], device=self.device, mode=self.mode, process_group=process_group,
                             obs_dtype=c["obs_dtype"], frames=c["frames"], diagnostics=c["diagnostics"],
-                            replay_slabs=c["replay_slabs"], replay_columns=c["replay_columns"])
+                            replay_slabs=c["replay_slabs"], replay_columns=c["replay_columns"],
+                            optimizer=c["optimizer"], optimizer_kwargs=c["optimizer_kwargs"],
+                            lr_table=self.optim.lr_table)
         eng.load_state(self._init_state())
         return eng
 
@@ -502,7 +513,8 @@ class Learner:
 
                 slabs = ring if ring is not None else stage
                 leader = dp.DpLeader(self.devices, self._cfg(), self._init_state(), slabs.shm.name,
-                                     slabs.slab_bytes, slabs.K, timeout=max(60.0, float(self.timeout)))
+                                     slabs.slab_bytes, slabs.K, timeout=max(60.0, float(self.timeout)),
+                                     lr_table=self.optim.lr_table)
                 torch.cuda.set_device(torch.device(self.device))
                 pg = leader.init_process_group(self.device)
             eng = self._make_engine(pg, world)  # first CUDA call of this process (post-fork)
@@ -632,6 +644,8 @@ class Learner:
         if ticket is not None:
             sc = eng.fetch_scalars(ticket)
             self._report(writer, n, reward, sc)
+        if writer is not None and not self.optim.is_default:  # the rate update n used
+            writer.add_scalar(f"learner_{self.id}/optim/lr", eng.lr_of(n), n)
         self._periodic(writer, n, eng, pub)
 
     # ------------------------------------------------------ checkpoints (learner.py:277-295)

@@ -249,3 +249,17 @@ def clip_adam(params, grad, m, v, step, n_policy, max_norm, lr, beta1=0.9, beta2
                                              float(lr), float(beta1), float(beta2), float(eps),
                                              _p(norms), _st()), "impala_clip_adam")
     return norms
+
+
+def clip_optim(params, grad, m, v, step, n_policy, max_norm, lr_table, rule="adam", h0=0.9, h1=0.999, eps=1e-8):
+    """impala_clip_optim: clip + one Adam ("adam": h0, h1 = beta1, beta2) or RMSprop ("rmsprop": h0, h1 = alpha,
+    momentum) step with the learning rate lr_table[min(step[0], len - 1)] (float32 CUDA tensor)."""
+    _need_cuda(params, grad, m, v, step, lr_table)
+    if lr_table.dtype != torch.float32:
+        raise _cabi.ImpalaCudaError(f"lr_table must be float32, got {lr_table.dtype}")
+    norms = torch.empty(2, dtype=torch.float64, device=params.device)
+    _cabi.check(_cabi.lib().impala_clip_optim(_p(params), _p(grad), _p(m), _p(v), _p(step), int(n_policy),
+                                              params.numel(), float(max_norm), _p(lr_table), lr_table.numel(),
+                                              _cabi.OPT_RULES[rule], float(h0), float(h1), float(eps), _p(norms),
+                                              _st()), "impala_clip_optim")
+    return norms
