@@ -232,6 +232,24 @@ int impala_vtrace_loss_diag(const float* cur_logits, const float* beh_logits, co
                             float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch,
                             int mode, void* stream);
 
+/* impala_vtrace_loss_diag with PopArt value normalization (van Hasselt et al. 2016, single task).
+ * popart: float64 device statistics {mu, nu, sigma, ...} (the layout impala_clip_optim_popart keeps),
+ * read once; v holds the NORMALIZED value output n, the value in reward units is sigma n + mu.
+ *   V-trace runs on sigma n + mu for every value read (v[:1] of IMPALA_MODE_REFERENCE included), so vs is
+ *   in reward units; pg_adv = rho (r + gamma vs' - v) / sigma, the normalized advantage the policy gradient
+ *   and policy loss use; the value loss is 0.5 sum ((v - vs) / sigma)^2, so dv = v_loss_c (v - vs) / (sigma B)
+ *   (B = 1 / inv_batch); entropy and reward are unchanged; scalars[0..1] are the normalized losses.
+ *   diag[0..8) are impala_vtrace_loss_diag's sums, in reward units.
+ * Workspace: impala_vtrace_loss_diag_workspace.  At mu = 0, sigma = 1 every output is bit-identical to
+ * impala_vtrace_loss_diag.  Returns IMPALA_ERR_BAD_ARG for a NULL popart and whatever that entry refuses. */
+int impala_vtrace_loss_popart(const float* cur_logits, const float* beh_logits, const int32_t* actions,
+                              const float* rewards, const uint8_t* done, const int32_t* lens,
+                              const float* v, float* vs, float* pg_adv, float* dlogits, float* dv,
+                              double* scalars, double* diag, void* workspace, int64_t workspace_bytes,
+                              int T, int B, int A, float gamma, float rho_bar, float c_bar,
+                              float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch,
+                              int mode, const double* popart, void* stream);
+
 /* Per-group gradient clipping + Adam in one launch (learner.py:176-183).
  *   params/m/v: f32 [n_total]; grad: f64 [n_total] (the possibly all-reduced sum);
  *   group 0 = [0, n_policy) (policy net), group 1 = [n_policy, n_total) (value net);
@@ -328,6 +346,36 @@ int impala_gather_clip_optim(float* params, double* reduced, const void* gather,
                              float* v, int64_t* state, int64_t n_policy, int64_t n_total, float max_norm,
                              const float* lr_table, int64_t n_lr, int rule, float h0, float h1, float eps,
                              double* norms_out, int* err, double timeout_s, void* stream);
+
+/* Size of the PopArt statistics, float64 {mu, nu, sigma, mu_loss, sigma_loss}: the running mean and second
+ * moment of the value targets and sigma = clamp(sqrt(max(nu - mu^2, 0)), 1e-4, 1e6), then the (mu, sigma)
+ * the loss of the last update used.  A fresh run starts at {0, 1, 1, 0, 1}. */
+#define IMPALA_POPART_STATS 5
+
+/* impala_clip_optim (resp. impala_gather_clip_optim) followed, in the same launch, by the PopArt step:
+ *   n = grad[sums_at], S1 = grad[sums_at + 5], S2 = grad[sums_at + 6] (impala_vtrace_loss_popart's diag
+ *   sums; the gather variant reads them from `reduced`, added in rank order, so sums_at + 8 <= n_total +
+ *   n_extra), then with b = beta:
+ *     mu' = (1 - b) mu + b S1 / n,  nu' = (1 - b) nu + b S2 / n,  sigma' = clamp(sqrt(max(nu' - mu'^2, 0)), 1e-4, 1e6)
+ *   (n = 0 leaves mu, nu, sigma as they are), and, after the optimizer step, the value head is rescaled so that
+ *   sigma' n + mu' is the output sigma n + mu of the updated head:
+ *     params[w2_off, w2_off + w2_len) *= sigma / sigma',  params[b2_off] = (sigma b2 + mu - mu') / sigma'.
+ *   The optimizer state (m, v) is not touched.  popart[3], popart[4] receive the (mu, sigma) the update's
+ *   loss used.  A timed-out gather leaves the statistics untouched, like the parameters.
+ * Returns IMPALA_ERR_BAD_ARG before any launch for what impala_clip_optim / impala_gather_clip_optim refuse,
+ * a NULL popart, beta outside (0, 1] (NaN included), sums_at < n_total, w2_len < 1, a W2 block or b2 outside
+ * [n_policy, n_total), or b2 inside the W2 block. */
+int impala_clip_optim_popart(float* params, const double* grad, float* m, float* v, int64_t* state,
+                             int64_t n_policy, int64_t n_total, float max_norm, const float* lr_table, int64_t n_lr,
+                             int rule, float h0, float h1, float eps, double* norms_out, double* popart,
+                             int64_t sums_at, int64_t w2_off, int64_t w2_len, int64_t b2_off, float beta,
+                             void* stream);
+int impala_gather_clip_optim_popart(float* params, double* reduced, const void* gather, long long* seq,
+                                    int64_t slot_stride, int64_t buf_stride, int world, int n_extra, float* m,
+                                    float* v, int64_t* state, int64_t n_policy, int64_t n_total, float max_norm,
+                                    const float* lr_table, int64_t n_lr, int rule, float h0, float h1, float eps,
+                                    double* norms_out, int* err, double timeout_s, double* popart, int64_t sums_at,
+                                    int64_t w2_off, int64_t w2_len, int64_t b2_off, float beta, void* stream);
 
 /* Pieces of the reference's module-level loss helpers (learner.py:298-321) for callers that use
  * them individually instead of impala_vtrace_loss.  logits (M,A) f32 row-major, actions (M) i32.

@@ -15,7 +15,12 @@ each, alternating, L2 flushed before each).
 B/2; --obs-dtype, --frames k if given) the same way: the replay engine's pool is filled first, and the plain
 engine trains on the very slab the replay engine composed, so both steps see the same values.  It also times
 impala_batch_compose alone (median of 200 launches, L2 flushed before each) against its HBM floor (one training
-slab read and written at 3.35 TB/s)."""
+slab read and written at 3.35 TB/s).
+--compare-popart alternates a popart=False and a popart=True engine on the same batch the same way (the same
+launch count; the PopArt arm adds one FMA per value load, the 1 / sigma scaling and the optimizer's head
+epilogue), and times impala_vtrace_loss_diag against impala_vtrace_loss_popart and impala_clip_optim against
+impala_clip_optim_popart alone on the engine's buffers (median of 200 launches each, alternating, L2 flushed
+before each)."""
 import argparse
 import os
 import statistics
@@ -58,6 +63,7 @@ ap.add_argument("--compare-frames", action="store_true", help="alternate dense a
 ap.add_argument("--frames", type=int, default=None, help="stacked frames of --compare-frames (default 4) / --compare-replay (default 1)")
 ap.add_argument("--obs-dtype", default="float32", choices=["float32", "uint8"], help="slab obs type of --compare-frames")
 ap.add_argument("--compare-diag", action="store_true", help="alternate engines without / with off-policy diagnostics")
+ap.add_argument("--compare-popart", action="store_true", help="alternate engines without / with PopArt")
 ap.add_argument("--compare-replay", action="store_true", help="alternate engines without / with experience replay")
 ap.add_argument("--replay-slabs", type=int, default=2, help="past fresh batches in the pool of --compare-replay")
 ap.add_argument("--replay-columns", type=int, default=None, help="replayed columns of --compare-replay (default B/2)")
@@ -84,6 +90,11 @@ if a.compare_frames:
     arms = {f"dense {a.obs_dtype}": arms["default"], f"frames={a.frames} {a.obs_dtype}": arms["default"]}
     obs_dt = {name: a.obs_dtype for name in arms}
     n_frames = {f"frames={a.frames} {a.obs_dtype}": a.frames}
+popart_arm = {}
+if a.compare_popart:
+    arms = {"popart off": arms["default"], "popart on": arms["default"]}
+    popart_arm = {"popart on": dict(popart=True)}
+    obs_dt = {name: "uint8" if a.config in ("ram", "ram4", "ram8", "minatar", "ram_a6") else "float32" for name in arms}
 replay_arm = {}
 if a.compare_replay:
     Br = w["B"] // 2 if a.replay_columns is None else a.replay_columns
@@ -98,9 +109,10 @@ for name, tc in arms.items():
     dt = obs_dt.get(name, "float32")
     k = n_frames.get(name, 1)
     eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k,
-                        diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}))
+                        diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}), **popart_arm.get(name, {}))
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
-    byte_obs = a.compare_obs or ((a.compare_frames or a.compare_replay) and dt == "uint8") or (a.compare_diag and dt == "uint8")
+    byte_obs = (a.compare_obs or ((a.compare_frames or a.compare_replay) and dt == "uint8")
+                or ((a.compare_diag or a.compare_popart) and dt == "uint8"))
     if a.compare_replay:
         engines[name] = eng
         continue
@@ -246,6 +258,52 @@ if a.compare_diag:  # the V-trace + loss kernel alone, plain and diag entry poin
     k0, k1 = statistics.median(tk["impala_vtrace_loss"]), statistics.median(tk["impala_vtrace_loss_diag"])
     print(f"V-trace + loss kernel {a.config}: impala_vtrace_loss {k0:.1f} us, impala_vtrace_loss_diag {k1:.1f} us "
           f"(+{k1 - k0:.1f} us, {100 * (k1 / k0 - 1):+.1f} %)")
+if a.compare_popart:  # the two launches PopArt changes, alone, plain and PopArt entry points alternating
+    import ctypes
+
+    from torched_impala_b200 import _cabi
+
+    eng = engines["popart on"]
+    d = eng.d_views[0]
+    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    ins = (P(eng.logits), P(d["beh_logits"]), P(d["actions"]), P(d["rewards"]), P(d["done"]), P(d["lens"]),
+           P(eng.values), P(eng.vs), P(eng.pg_adv), P(eng.dlogits), P(eng.dv))
+    scal = ctypes.c_void_p(eng.comm.data_ptr() + 8 * eng.n_total)
+    diag = ctypes.c_void_p(eng.comm.data_ptr() + 8 * (eng.n_total + 4))
+    tail = (w["T"], w["B"], w["A"], hp.gamma, hp.rho_bar, hp.c_bar, hp.v_loss_c, hp.policy_loss_c, hp.entropy_c,
+            1.0 / w["B"], 0)
+    # the optimizer on copies of the engine's state, so the timed launches do not move the engine
+    cp = {k: getattr(eng, k).clone() for k in ("params", "adam_m", "adam_v", "adam_step", "popart_buf")}
+    o = eng.optim
+    rule = (P(eng.lr_table), eng.lr_table.numel(), o.rule_code, o.h0, o.h1, o.eps)
+    opt_head = (P(cp["params"]), P(eng.comm), P(cp["adam_m"]), P(cp["adam_v"]), P(cp["adam_step"]), eng.n_pi,
+                eng.n_total, float(hp.max_norm))
+    calls = {"impala_vtrace_loss_diag": lambda st: eng.lib.impala_vtrace_loss_diag(*ins, scal, diag, P(eng.ws_vt),
+                                                                                  eng.ws_vt_bytes, *tail, st),
+             "impala_vtrace_loss_popart": lambda st: eng.lib.impala_vtrace_loss_popart(
+                 *ins, scal, diag, P(eng.ws_vt), eng.ws_vt_bytes, *tail, P(eng.popart_buf), st),
+             "impala_clip_optim": lambda st: eng.lib.impala_clip_optim(*opt_head, *rule, P(eng.norms), st),
+             "impala_clip_optim_popart": lambda st: eng.lib.impala_clip_optim_popart(
+                 *opt_head, *rule, P(eng.norms), P(cp["popart_buf"]), eng.n_total + 4, eng.w2_at, w["H"], eng.b2_at,
+                 float(eng.popart_beta), st)}
+    tk = {name: [] for name in calls}
+    with torch.cuda.stream(eng.stream):
+        st = ctypes.c_void_p(eng.stream.cuda_stream)
+        for i in range(220):
+            for name, fn in calls.items():
+                flush.zero_()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(eng.stream)
+                rc = fn(st)
+                e1.record(eng.stream)
+                e1.synchronize()
+                assert rc == 0, (name, rc)
+                if i >= 20:
+                    tk[name].append(e0.elapsed_time(e1) * 1e3)
+    for plain, pop in (("impala_vtrace_loss_diag", "impala_vtrace_loss_popart"),
+                       ("impala_clip_optim", "impala_clip_optim_popart")):
+        k0, k1 = statistics.median(tk[plain]), statistics.median(tk[pop])
+        print(f"{a.config}: {plain} {k0:.1f} us, {pop} {k1:.1f} us (+{k1 - k0:.1f} us, {100 * (k1 / k0 - 1):+.1f} %)")
 q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
                     "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 print(f"GPU (nvidia-smi): {q}")
@@ -265,3 +323,9 @@ if a.compare_diag:
     print(f"diagnostics overhead {a.config}: {m1 - m0:+.1f} us/step ({100 * (m1 / m0 - 1):+.1f} %); "
           f"rho clipped {100 * sc['rho_clip_fraction']:.1f} %, kl {sc['kl_behaviour_current']:.4f}, "
           f"explained variance {sc['value_explained_variance']:.4f}")
+if a.compare_popart:
+    m0, m1 = statistics.median(ts["popart off"]), statistics.median(ts["popart on"])
+    st = engines["popart on"].popart_stats()
+    print(f"popart overhead {a.config}: {m1 - m0:+.1f} us/step ({100 * (m1 / m0 - 1):+.1f} %), launches "
+          f"{engines['popart on'].launches_per_step} against {engines['popart off'].launches_per_step}; "
+          f"mu {st['mu']:.4f}, sigma {st['sigma']:.4f}")

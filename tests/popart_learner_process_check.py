@@ -1,0 +1,106 @@
+"""Run the drop-in Learner with PopArt as a forked process behind a RingQueue, then resume from its checkpoint.
+
+    python tests/popart_learner_process_check.py <log dir> <out.npz>
+
+Executed by test_gpu_popart.py in a fresh interpreter (the parent of a forked CUDA process must not have
+initialised CUDA).  Feeds the golden c1 batches with popart=True and a large step size, checks that the
+checkpoint holds the folded value function (the value_fn module's weights) and the "popart" key, and that the
+event file holds popart/mu and popart/sigma at every update.  Then load()s the checkpoint into a new Learner and
+builds its engine in this process (no fork follows): its normalized weights and statistics are saved to
+<out.npz> next to the forked run's folded weights, for the test to compare.
+"""
+import glob
+import os
+import sys
+import threading
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+import torch.multiprocessing as mp  # noqa: E402
+
+from conftest import PKEYS, Golden  # noqa: E402
+from torched_impala_b200 import synth  # noqa: E402
+from torched_impala_b200.learner import Learner  # noqa: E402
+from torched_impala_b200.models import MlpPolicy, MlpValueFn  # noqa: E402
+from torched_impala_b200.ring import RingQueue  # noqa: E402
+from torched_impala_b200.utils import Counter  # noqa: E402
+
+BETA = 0.2
+
+
+def modules(c, init):
+    policy, value_fn = MlpPolicy(c["O"], c["A"], c["H_pi"]), MlpValueFn(c["O"], c["H_v"])
+    policy.load_state_dict({k: torch.as_tensor(np.asarray(init["policy"][k])).double() for k in PKEYS})
+    value_fn.load_state_dict({k: torch.as_tensor(np.asarray(init["value_fn"][k])).double() for k in PKEYS})
+    return policy, value_fn
+
+
+def main():
+    mp.set_start_method("fork", force=True)
+    log_dir, out = sys.argv[1], sys.argv[2]
+    g = Golden("c1_cartpole_ragged")
+    c = g.case
+    hp = g.hp._replace(max_updates=g.updates, verbose=0, eval_every=None, save_every=g.updates)
+    policy, value_fn = modules(c, g.init_params())
+    policy.share_memory()
+    value_fn.share_memory()  # the learner process writes both modules back at the end
+    q = RingQueue(c["T"], c["B"], c["O"], c["A"], slabs=2)
+    counter = Counter(0)
+    lrn = Learner(1, hp, policy, value_fn, q, counter, log_path=log_dir, timeout=60, popart=True, popart_beta=BETA)
+
+    def feed():
+        for u in range(g.updates):
+            for tr in synth.to_trajectories(g.batch(u)):
+                q.put(tr, timeout=60)
+
+    lrn.start()
+    t = threading.Thread(target=feed, daemon=True)
+    t.start()
+    ok = lrn.completion.wait(timeout=180)
+    lrn.join()
+    t.join(timeout=5)
+    q.close()
+    assert ok and lrn.p.exitcode == 0, f"learner failed (exit code {lrn.p.exitcode})"
+    assert counter.value == g.updates, counter.value
+
+    ckpts = glob.glob(os.path.join(log_dir, "l1", "*.pt"))
+    assert len(ckpts) == 1, ckpts
+    ck = torch.load(ckpts[0])
+    assert set(ck) == {"policy_state_dict", "value_fn_state_dict", "popart"}, set(ck)
+    mu, nu = float(ck["popart"]["mu"]), float(ck["popart"]["nu"])
+    assert mu != 0.0 and nu != 1.0, (mu, nu)
+    for k in PKEYS:  # the checkpoint's value function is the module's: folded, in reward units
+        assert torch.equal(ck["value_fn_state_dict"][k], value_fn.state_dict()[k]), k
+        assert torch.equal(ck["policy_state_dict"][k], policy.state_dict()[k]), k
+
+    from tensorboard.backend.event_processing.event_accumulator import EventAccumulator
+
+    acc = EventAccumulator(os.path.join(log_dir, "l1"))
+    acc.Reload()
+    for tag in ("popart/mu", "popart/sigma"):
+        ev = acc.Scalars(f"learner_1/{tag}")
+        assert [e.step for e in ev] == list(range(1, g.updates + 1)), (tag, [e.step for e in ev])
+    last_mu = acc.Scalars("learner_1/popart/mu")[-1].value
+    assert abs(last_mu - mu) <= 1e-6 * max(1.0, abs(mu)), (last_mu, mu)
+
+    # resume: a new Learner load()s the checkpoint and builds its engine here
+    p2, v2 = modules(c, g.init_params())
+    lrn2 = Learner(2, hp, p2, v2, RingQueue(c["T"], c["B"], c["O"], c["A"], slabs=2), Counter(0), popart=True,
+                   popart_beta=BETA)
+    lrn2.load(ckpts[0])
+    eng = lrn2._make_engine()
+    st, norm = eng.popart_stats(), eng.normalized_state()
+    assert st["mu"] == mu and st["nu"] == nu, (st, mu, nu)
+    np.savez(out, **{f"policy/{k}": v.numpy() for k, v in policy.state_dict().items()},
+             **{f"value_fn/{k}": v.numpy() for k, v in value_fn.state_dict().items()},
+             **{f"resumed/{g_}/{k}": norm[g_][k].numpy() for g_ in norm for k in PKEYS},
+             mu=mu, nu=nu)
+    print(f"POPART_LEARNER_OK updates={counter.value} mu={mu:.6f} nu={nu:.6f}")
+
+
+if __name__ == "__main__":
+    main()

@@ -22,6 +22,7 @@ OBS_DTYPES = {"float32": OBS_F32, "uint8": OBS_U8}  # batch-slab observation typ
 OPT_ADAM = 0
 OPT_RMSPROP = 1
 OPT_RULES = {"adam": OPT_ADAM, "rmsprop": OPT_RMSPROP}  # update rules of impala_clip_optim
+POPART_STATS = 5  # float64 {mu, nu, sigma, mu_loss, sigma_loss} (IMPALA_POPART_STATS)
 
 
 def obs_dtype_code(obs_dtype: str) -> int:
@@ -74,10 +75,15 @@ SIGNATURES = {
     "impala_vtrace_loss": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p]),
     "impala_vtrace_loss_diag_workspace": (_i64, [_i, _i, _i]),
     "impala_vtrace_loss_diag": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p]),
+    "impala_vtrace_loss_popart": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p]),
     "impala_clip_adam": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _f, _f, _f, _f, _p, _p]),
     "impala_clip_optim": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i, _f, _f, _f, _p, _p]),
     "impala_gather_clip_optim": (_i, [_p] * 4 + [_i64, _i64, _i, _i, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i]
                                  + [_f] * 3 + [_p, _p, C.c_double, _p]),
+    "impala_clip_optim_popart": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i, _f, _f, _f, _p, _p]
+                                 + [_i64] * 4 + [_f, _p]),
+    "impala_gather_clip_optim_popart": (_i, [_p] * 4 + [_i64, _i64, _i, _i, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i]
+                                        + [_f] * 3 + [_p, _p, C.c_double, _p] + [_i64] * 4 + [_f, _p]),
     "impala_policy_terms": (_i, [_p, _p, _p, _p, _i, _i, _p]),
     "impala_policy_terms_backward": (_i, [_p, _p, _p, _p, _p, _i, _i, _p]),
     "impala_reduce": (_i, [_p, _p, _i64, _i, _p, _p]),

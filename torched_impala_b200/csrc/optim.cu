@@ -14,6 +14,11 @@
 // and on where the learning rate comes from (LrScalar: a launch argument; LrTable: a device table
 // indexed by the step counter, so one captured CUDA graph serves a whole learning-rate schedule).
 // impala_clip_adam / impala_gather_clip_adam are the <AdamRule, LrScalar> instantiations.
+//
+// The body's third parameter is the value normalization (NoPopart, Popart): with Popart one thread of CTA 0
+// forms the new value statistics from the eight V-trace sums before the norm exchange's cluster barrier, the
+// other CTAs read them through distributed shared memory, and phase 2 rescales the value head's entries right
+// after their update, so the PopArt step needs no launch of its own.
 #include <cooperative_groups.h>
 #include <math.h>
 
@@ -100,18 +105,62 @@ struct RmspropRule {
     __device__ __forceinline__ void finish(int64_t* __restrict__ state, const double*) const { state[0] += 1; }
 };
 
+// ---- value normalization.  NoPopart: the plain kernels (every member compiles to nothing).
+struct NoPopart {
+    static constexpr bool kOn = false;
+    static constexpr int kShared = 1;
+    __device__ __forceinline__ void form(const double*, double*) const {}
+    __device__ __forceinline__ void rescale(int64_t, float*, const double*) const {}
+    __device__ __forceinline__ void finish(const double*) const {}
+};
+
+// PopArt (van Hasselt et al. 2016), single task: stats = float64 {mu, nu, sigma, mu_loss, sigma_loss} in device
+// memory, the first three the running statistics, the last two those the update's loss used (written with the
+// new ones, so a logged copy of the five is self-consistent).  `form` (one thread) turns the sums of the batch
+// (sums[0] = n, [5] = sum vs, [6] = sum vs^2, impala_vtrace_loss_diag's layout) into
+//   s = {mu', nu', sigma', sigma / sigma', (mu - mu') / sigma', mu, sigma}
+// and `rescale` keeps the unnormalized value output sigma n + mu of the updated head: W2 <- W2 sigma / sigma',
+// b2 <- (sigma b2 + mu - mu') / sigma'.  n = 0 keeps the statistics (and the rescale is the identity).
+struct Popart {
+    static constexpr bool kOn = true;
+    static constexpr int kShared = 7;
+    double* __restrict__ stats;
+    int64_t sums_at, w2_off, w2_len, b2_off;
+    float beta;
+    __device__ __forceinline__ void form(const double* sums, double* s) const {
+        const double mu = stats[0], nu = stats[1], sg = stats[2], n = sums[0];
+        double mu1 = mu, nu1 = nu, sg1 = sg;
+        if (n > 0.0) {
+            const double b = (double)beta;
+            mu1 = (1.0 - b) * mu + b * (sums[5] / n);
+            nu1 = (1.0 - b) * nu + b * (sums[6] / n);
+            sg1 = fmin(fmax(sqrt(fmax(nu1 - mu1 * mu1, 0.0)), 1e-4), 1e6);
+        }
+        s[0] = mu1, s[1] = nu1, s[2] = sg1, s[3] = sg / sg1, s[4] = (mu - mu1) / sg1, s[5] = mu, s[6] = sg;
+    }
+    __device__ __forceinline__ void rescale(int64_t i, float* __restrict__ params, const double* s) const {
+        if (i >= w2_off && i < w2_off + w2_len) params[i] = (float)((double)params[i] * s[3]);
+        else if (i == b2_off) params[i] = (float)fma((double)params[i], s[3], s[4]);
+    }
+    __device__ __forceinline__ void finish(const double* s) const {
+        stats[0] = s[0], stats[1] = s[1], stats[2] = s[2], stats[3] = s[5], stats[4] = s[6];
+    }
+};
+
 // torch.nn.utils.clip_grad_norm_: coef = max_norm / (norm + 1e-6), clamped to 1; a NaN norm gives a NaN
 // coefficient (torch.clamp propagates NaN, fmin would return the 1)
 __device__ __forceinline__ float clip_coef(double norm, float max_norm) {
     return isnan(norm) ? (float)norm : (float)fmin(1.0, (double)max_norm / (norm + 1e-6));
 }
 
-template <class Rule, class Lr>
+template <class Rule, class Lr, class Pop = NoPopart>
 __device__ __forceinline__ void clip_update(float* __restrict__ params, const double* __restrict__ grad,
                                             float* __restrict__ m, float* __restrict__ v,
                                             int64_t* __restrict__ state, int64_t n_policy, int64_t n_total,
-                                            float max_norm, Lr lr, Rule rule, double* __restrict__ norms_out) {
+                                            float max_norm, Lr lr, Rule rule, double* __restrict__ norms_out,
+                                            Pop pop = Pop{}) {
     cg::cluster_group cluster = cg::this_cluster();
+    __shared__ double s_pop[Pop::kShared];  // Popart: the statistics CTA 0 forms (read by the peers)
     __shared__ double s_warp[2][kAdamThreads / 32];
     __shared__ double s_cta[2];   // this CTA's partial sums of squares (read by the peers)
     __shared__ float s_coef[2];
@@ -156,13 +205,16 @@ __device__ __forceinline__ void clip_update(float* __restrict__ params, const do
     if (lane == 0) s_warp[0][warp] = ss0, s_warp[1][warp] = ss1;
     if (tid == 64)  // learning rate and bias corrections (nobody writes state before the end)
         rule.prepare(state, lr.at(state[0]), s_bias, s_pow);
+    if constexpr (Pop::kOn) {
+        if (cluster.block_rank() == 0 && tid == 96) pop.form(grad + pop.sums_at, s_pop);
+    }
     __syncthreads();
     if (tid < 2) {
         double s = 0.0;
         for (int i = 0; i < kAdamThreads / 32; ++i) s += s_warp[tid][i];
         s_cta[tid] = s;
     }
-    cluster.sync();  // all 8 partial pairs are in place
+    cluster.sync();  // all 8 partial pairs (and CTA 0's statistics) are in place
     if (tid < 2) {
         double s = 0.0;
         for (int r = 0; r < kAdamCluster; ++r) s += *cluster.map_shared_rank(&s_cta[tid], r);
@@ -174,8 +226,10 @@ __device__ __forceinline__ void clip_update(float* __restrict__ params, const do
     // phase 2: the update in float32 arithmetic (the state is float32; one step's rounding is ~1e-7)
     const float k0 = s_bias[0], k1 = s_bias[1];
     const float c0 = s_coef[0], c1 = s_coef[1];
+    const double* pop_s = Pop::kOn ? cluster.map_shared_rank(s_pop, 0) : s_pop;
     auto update = [&](int64_t i, float g, float p, float mi, float vi) {
         rule.apply(i, g * (i < n_policy ? c0 : c1), p, mi, vi, k0, k1, params, m, v);
+        pop.rescale(i, params, pop_s);  // the value head, right after its update
     };
 #pragma unroll
     for (int k = 0; k < kKeep; ++k) {
@@ -185,7 +239,10 @@ __device__ __forceinline__ void clip_update(float* __restrict__ params, const do
     for (int64_t i = first + kKeep * stride; i < n_total; i += stride)
         update(i, (float)grad[i], params[i], rule.reads_m() ? m[i] : 0.f, v[i]);
     cluster.sync();  // peers finished reading this CTA's shared memory; every CTA has read state
-    if (cluster.block_rank() == 0 && tid == 64) rule.finish(state, s_pow);
+    if (cluster.block_rank() == 0 && tid == 64) {
+        rule.finish(state, s_pow);
+        pop.finish(s_pop);
+    }
 }
 
 __global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
@@ -206,6 +263,16 @@ clip_optim_kernel(float* __restrict__ params, const double* __restrict__ grad, f
                   double* __restrict__ norms_out) {
     clip_update(params, grad, m, v, state, n_policy, n_total, max_norm, LrTable{lr_table, n_lr}, Rule{h0, h1, eps},
                 norms_out);
+}
+
+template <class Rule>
+__global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
+clip_optim_popart_kernel(float* __restrict__ params, const double* __restrict__ grad, float* __restrict__ m,
+                         float* __restrict__ v, int64_t* __restrict__ state, int64_t n_policy, int64_t n_total,
+                         float max_norm, const float* __restrict__ lr_table, int64_t n_lr, float h0, float h1,
+                         float eps, double* __restrict__ norms_out, Popart pop) {
+    clip_update(params, grad, m, v, state, n_policy, n_total, max_norm, LrTable{lr_table, n_lr}, Rule{h0, h1, eps},
+                norms_out, pop);
 }
 
 
@@ -256,15 +323,17 @@ peer_push_kernel(const double* __restrict__ local, int64_t n, PushArgs p) {
 }
 
 // Consumer: poll the local slots, add them in rank order, clip + update.
-template <class Rule, class Lr>
+template <class Rule, class Lr, class Pop = NoPopart>
 __device__ __forceinline__ void gather_clip_update(float* __restrict__ params, double* __restrict__ reduced,
                                                    const ulonglong2* __restrict__ gather, long long* __restrict__ seq,
                                                    int64_t slot_stride, int64_t buf_stride, int world, int n_extra,
                                                    float* __restrict__ m, float* __restrict__ v,
                                                    int64_t* __restrict__ state, int64_t n_policy, int64_t n_total,
                                                    float max_norm, Lr lr, Rule rule, double* __restrict__ norms_out,
-                                                   int* __restrict__ err, unsigned long long timeout_ns) {
+                                                   int* __restrict__ err, unsigned long long timeout_ns,
+                                                   Pop pop = Pop{}) {
     cg::cluster_group cluster = cg::this_cluster();
+    __shared__ double s_pop[Pop::kShared];  // Popart: the statistics CTA 0 forms from the summed extras
     __shared__ double s_warp[2][kAdamThreads / 32];
     __shared__ double s_cta[2];
     __shared__ int s_abort;     // a thread of this CTA gave up waiting (read by the peers of the cluster)
@@ -350,12 +419,15 @@ __device__ __forceinline__ void gather_clip_update(float* __restrict__ params, d
     ss1 = warp_sum_f64(ss1);
     if (lane == 0) s_warp[0][warp] = ss0, s_warp[1][warp] = ss1;
     __syncthreads();
+    if constexpr (Pop::kOn) {  // the rank-ordered sums of all ranks' V-trace sums are in `reduced` now
+        if (crank == 0 && tid == 96) pop.form(reduced + pop.sums_at, s_pop);
+    }
     if (tid < 2) {
         double s = 0.0;
         for (int i = 0; i < kAdamThreads / 32; ++i) s += s_warp[tid][i];
         s_cta[tid] = s;
     }
-    cluster.sync();  // all 8 partial pairs (and abort flags) are in place
+    cluster.sync();  // all 8 partial pairs (and abort flags, CTA 0's statistics) are in place
     if (tid == 0) {
         int ab = 0;
         for (int r = 0; r < kAdamCluster; ++r) ab |= *cluster.map_shared_rank(&s_abort, r);
@@ -372,8 +444,10 @@ __device__ __forceinline__ void gather_clip_update(float* __restrict__ params, d
     if (!s_any_abort) {
         const float k0 = s_bias[0], k1 = s_bias[1];
         const float c0 = s_coef[0], c1 = s_coef[1];
+        const double* pop_s = Pop::kOn ? cluster.map_shared_rank(s_pop, 0) : s_pop;
         auto update = [&](int64_t i, float g, float p, float mi, float vi) {
             rule.apply(i, g * (i < n_policy ? c0 : c1), p, mi, vi, k0, k1, params, m, v);
+            pop.rescale(i, params, pop_s);
         };
 #pragma unroll
         for (int k = 0; k < kKeep; ++k) {
@@ -386,9 +460,10 @@ __device__ __forceinline__ void gather_clip_update(float* __restrict__ params, d
     cluster.sync();  // peers finished reading this CTA's shared memory; every CTA has read state
     if (crank == 0 && tid == 64) {
         if (s_any_abort) {
-            if (err) *err = 1;  // the host raises; state and seq stay as they were
+            if (err) *err = 1;  // the host raises; state, statistics and seq stay as they were
         } else {
             rule.finish(state, s_pow);
+            pop.finish(s_pop);
             *seq = step64;
         }
     }
@@ -419,12 +494,35 @@ gather_clip_optim_kernel(float* __restrict__ params, double* __restrict__ reduce
                        n_total, max_norm, LrTable{lr_table, n_lr}, Rule{h0, h1, eps}, norms_out, err, timeout_ns);
 }
 
+template <class Rule>
+__global__ void __cluster_dims__(kAdamCluster, 1, 1) __launch_bounds__(kAdamThreads)
+gather_clip_optim_popart_kernel(float* __restrict__ params, double* __restrict__ reduced,
+                                const ulonglong2* __restrict__ gather, long long* __restrict__ seq,
+                                int64_t slot_stride, int64_t buf_stride, int world, int n_extra,
+                                float* __restrict__ m, float* __restrict__ v, int64_t* __restrict__ state,
+                                int64_t n_policy, int64_t n_total, float max_norm, const float* __restrict__ lr_table,
+                                int64_t n_lr, float h0, float h1, float eps, double* __restrict__ norms_out,
+                                int* __restrict__ err, unsigned long long timeout_ns, Popart pop) {
+    gather_clip_update(params, reduced, gather, seq, slot_stride, buf_stride, world, n_extra, m, v, state, n_policy,
+                       n_total, max_norm, LrTable{lr_table, n_lr}, Rule{h0, h1, eps}, norms_out, err, timeout_ns, pop);
+}
+
 // The checks of impala_clip_optim / impala_gather_clip_optim beyond those of the Adam entry points.
 bool bad_optim_args(const float* lr_table, int64_t n_lr, int rule, float h0, float h1, float eps) {
     if (!lr_table || n_lr < 1 || !(eps >= 0.f)) return true;
     if (rule == IMPALA_OPT_ADAM) return false;
     if (rule == IMPALA_OPT_RMSPROP) return !(h0 >= 0.f && h0 < 1.f) || !(h1 >= 0.f);
     return true;
+}
+
+// The checks of the PopArt entry points beyond those of impala_clip_optim: the statistics, beta in (0, 1] and a
+// value head (W2 block and b2, disjoint) inside the value net's entries [n_policy, n_total).
+bool bad_popart_args(const double* popart, int64_t n_policy, int64_t n_total, int64_t w2_off, int64_t w2_len,
+                     int64_t b2_off, float beta) {
+    if (!popart || !(beta > 0.f && beta <= 1.f)) return true;
+    if (w2_len < 1 || w2_off < n_policy || w2_off > n_total - w2_len) return true;
+    if (b2_off < n_policy || b2_off >= n_total) return true;
+    return b2_off >= w2_off && b2_off < w2_off + w2_len;
 }
 
 unsigned long long timeout_ns_of(double timeout_s) {
@@ -516,6 +614,52 @@ extern "C" int impala_gather_clip_optim(float* params, double* reduced, const vo
                                         static_cast<const ulonglong2*>(gather), seq, slot_stride, buf_stride, world,
                                         n_extra, m, v, state, n_policy, n_total, max_norm, lr_table, n_lr, h0, h1, eps,
                                         norms_out, err, timeout_ns_of(timeout_s));
+    if (e != cudaSuccess) return (int)e;
+    return impala_launch_status();
+}
+
+extern "C" int impala_clip_optim_popart(float* params, const double* grad, float* m, float* v, int64_t* state,
+                                        int64_t n_policy, int64_t n_total, float max_norm, const float* lr_table,
+                                        int64_t n_lr, int rule, float h0, float h1, float eps, double* norms_out,
+                                        double* popart, int64_t sums_at, int64_t w2_off, int64_t w2_len,
+                                        int64_t b2_off, float beta, void* stream) {
+    if (!params || !grad || !m || !v || !state) return IMPALA_ERR_BAD_ARG;
+    if (n_total < 1 || n_policy < 0 || n_policy > n_total) return IMPALA_ERR_BAD_ARG;
+    if (bad_optim_args(lr_table, n_lr, rule, h0, h1, eps)) return IMPALA_ERR_BAD_ARG;
+    if (bad_popart_args(popart, n_policy, n_total, w2_off, w2_len, b2_off, beta) || sums_at < n_total)
+        return IMPALA_ERR_BAD_ARG;
+    const Popart pop{popart, sums_at, w2_off, w2_len, b2_off, beta};
+    const auto kernel =
+        rule == IMPALA_OPT_ADAM ? clip_optim_popart_kernel<AdamRule> : clip_optim_popart_kernel<RmspropRule>;
+    const cudaError_t e = impala_launch(kernel, kAdamCluster, kAdamThreads, 0, (cudaStream_t)stream, true, params, grad,
+                                        m, v, state, n_policy, n_total, max_norm, lr_table, n_lr, h0, h1, eps, norms_out,
+                                        pop);
+    if (e != cudaSuccess) return (int)e;
+    return impala_launch_status();
+}
+
+extern "C" int impala_gather_clip_optim_popart(float* params, double* reduced, const void* gather, long long* seq,
+                                               int64_t slot_stride, int64_t buf_stride, int world, int n_extra,
+                                               float* m, float* v, int64_t* state, int64_t n_policy, int64_t n_total,
+                                               float max_norm, const float* lr_table, int64_t n_lr, int rule, float h0,
+                                               float h1, float eps, double* norms_out, int* err, double timeout_s,
+                                               double* popart, int64_t sums_at, int64_t w2_off, int64_t w2_len,
+                                               int64_t b2_off, float beta, void* stream) {
+    if (bad_gather_args(params, reduced, gather, seq, slot_stride, buf_stride, world, n_extra, m, v, state, n_policy,
+                        n_total))
+        return IMPALA_ERR_BAD_ARG;
+    if (bad_optim_args(lr_table, n_lr, rule, h0, h1, eps)) return IMPALA_ERR_BAD_ARG;
+    // the eight sums must be among the gathered extras
+    if (bad_popart_args(popart, n_policy, n_total, w2_off, w2_len, b2_off, beta) || sums_at < n_total ||
+        sums_at + 8 > n_total + n_extra)
+        return IMPALA_ERR_BAD_ARG;
+    const Popart pop{popart, sums_at, w2_off, w2_len, b2_off, beta};
+    const auto kernel = rule == IMPALA_OPT_ADAM ? gather_clip_optim_popart_kernel<AdamRule>
+                                                : gather_clip_optim_popart_kernel<RmspropRule>;
+    const cudaError_t e = impala_launch(kernel, kAdamCluster, kAdamThreads, 0, (cudaStream_t)stream, true, params, reduced,
+                                        static_cast<const ulonglong2*>(gather), seq, slot_stride, buf_stride, world,
+                                        n_extra, m, v, state, n_policy, n_total, max_norm, lr_table, n_lr, h0, h1, eps,
+                                        norms_out, err, timeout_ns_of(timeout_s), pop);
     if (e != cudaSuccess) return (int)e;
     return impala_launch_status();
 }

@@ -76,8 +76,13 @@ struct VtArgs {
 struct VtDiagArgs : VtArgs {
     double* diag;  // [8] sums over the valid steps, see impala_vtrace_loss_diag
 };
-template <bool DIAG>
-using VtArgsT = typename std::conditional<DIAG, VtDiagArgs, VtArgs>::type;
+// POPART instantiations (on top of DIAG) read the value statistics as well: v is the normalized output.
+struct VtPopArgs : VtDiagArgs {
+    const double* popart;  // {mu, nu, sigma, ...}, see impala_vtrace_loss_popart
+};
+template <bool DIAG, bool POPART = false>
+using VtArgsT = typename std::conditional<POPART, VtPopArgs,
+                                          typename std::conditional<DIAG, VtDiagArgs, VtArgs>::type>::type;
 
 // Row loads / stores of the (T, B, A) logits: lane = trajectory, so a warp reads 32 * A consecutive
 // floats of a time step.  VEC (A == AP, 16-byte aligned bases): one 128-bit (A = 4), one 64-bit
@@ -157,6 +162,15 @@ __device__ __forceinline__ float row_kl2(const float* __restrict__ pc, const flo
     return kl;
 }
 
+// POPART: {mu, sigma, 1 / sigma} as float32 in shared memory, read through a volatile pointer at every use so
+// that the three values take no register across the unroll (the DIAG twins are at their register limit).
+struct PopVals {
+    const volatile float* s;
+    __device__ __forceinline__ float mu() const { return s[0]; }
+    __device__ __forceinline__ float sigma() const { return s[1]; }
+    __device__ __forceinline__ float inv() const { return s[2]; }
+};
+
 // ------------------------------------------------------------------------------------------------
 // Lane = trajectory, warp = time segment.
 //
@@ -193,18 +207,32 @@ __device__ __forceinline__ float row_kl2(const float* __restrict__ pc, const flo
 // their maximum); on the streaming path VEC rows re-read both rows four logits at a time right after
 // row_lse2 reduced them (row_kl2), non-VEC rows re-read the behaviour row in step 4 next to the current
 // row's re-read (whichever keeps the twin's zero spills); vs and vs - v come from step 4.
+//
+// POPART (with DIAG): v holds the normalized values n; every value row is turned into reward units
+// v = sigma n + mu by one FMA as it is loaded (v[:1] included), so the recurrence, vs and the eight sums are
+// those of the value function sigma n + mu.  The accumulator acc = vs - v enters dv, pg and the two loss
+// sums scaled by 1 / sigma: the loss is that of the normalized targets, 0.5 sum ((v - vs) / sigma)^2, and
+// the advantage pg / sigma.  mu = 0, sigma = 1 leaves every value as it is (FMA with 1 and 0, products by 1).
 // ------------------------------------------------------------------------------------------------
-template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool VEC, bool DIAG>
-__global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<DIAG> a) {
+template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool VEC, bool DIAG, bool POPART = false>
+__global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<DIAG, POPART> a) {
     constexpr bool STREAM = AP > 16;
     constexpr int SR = STREAM ? 1 : S, AR = STREAM ? 1 : AP;  // extent of the held logit rows
     static_assert(!STREAM || S == 1, "the streaming rows keep one step per thread");
     static_assert(!DIAG || WITH_LOSS, "the off-policy sums ride the loss reduction");
+    static_assert(!POPART || DIAG, "the value statistics are formed from the DIAG sums");
     constexpr int NV = DIAG ? 12 : 4;  // per-CTA sums: 4 loss sums (+ 8 off-policy sums)
     __shared__ float2 s_map[2][kMaxSeg][32];
     __shared__ float2 s_cta[2][32];  // this CTA's segments composed into one map (read by the cluster)
     __shared__ double s_red[kMaxSeg][NV];
     pdl_wait();  // logits / values come from the forward kernel
+    // POPART: v = sigma n + mu (reward units); acc / sigma = acc * (1 / sigma) (normalized)
+    __shared__ float s_pop[POPART ? 3 : 1];
+    const PopVals pop{s_pop};
+    if constexpr (POPART) {
+        if (threadIdx.x == 0) s_pop[0] = (float)a.popart[0], s_pop[1] = (float)a.popart[2], s_pop[2] = (float)(1.0 / a.popart[2]);
+        __syncthreads();
+    }
     // Long unrolls: the time segments of a trajectory group are spread over a thread-block CLUSTER
     // (csize CTAs x nw warps x S steps per chunk - T = 100 fits ONE chunk of 8 x 7 x 2 steps), so a
     // thread's critical path is one load -> math -> exchange -> fix-up -> store sequence instead of
@@ -218,7 +246,7 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
     const bool live = b < B;
     const int bl = live ? b : B - 1;  // column this lane loads
     const int L = live ? min(max(__ldg(a.lens + bl), 0), T) : 0;
-    const float v0 = __ldg(a.v + bl);  // V(x_0): the reference's v[:1]
+    const float v0 = POPART ? fmaf(pop.sigma(), __ldg(a.v + bl), pop.mu()) : __ldg(a.v + bl);  // V(x_0): the reference's v[:1]
     const int rows = S * nseg;
     const int nch = (T + rows - 1) / rows;
     const bool ref_mode = a.mode == IMPALA_MODE_REFERENCE;
@@ -249,7 +277,10 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
             R.dn[i] = __ldg(a.done + e);
         }
 #pragma unroll
-        for (int i = 0; i <= S; ++i) R.vv[i] = __ldg(a.v + (unsigned)min(tb + i, T) * (unsigned)B + (unsigned)bl);
+        for (int i = 0; i <= S; ++i) {
+            const float n = __ldg(a.v + (unsigned)min(tb + i, T) * (unsigned)B + (unsigned)bl);
+            R.vv[i] = POPART ? fmaf(pop.sigma(), n, pop.mu()) : n;  // reward units
+        }
     };
     auto process = [&](Rows& R, const int c) {
         const int tb = c * rows + seg * S;  // first step of this thread's segment
@@ -371,7 +402,8 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
             const bool valid = t < L;
             acc[i] = fmaf(P[i], mine, acc[i]);
             const float vs_n = acc[i + 1] + R.vv[i + 1];                         // :131
-            const float pg = rho[i] * (R.r[i] + disc[i] * vs_n - R.vv[i]);         // :135
+            const float pg_r = rho[i] * (R.r[i] + disc[i] * vs_n - R.vv[i]);        // :135
+            const float pg = POPART ? pg_r * pop.inv() : pg_r;  // the normalized advantage: pg_adv, dlogits, the loss
             const unsigned e = (unsigned)t * (unsigned)B + (unsigned)b;
             if (live && t < T) {
                 if (a.vs) a.vs[e] = (t <= L) ? acc[i] + R.vv[i] : 0.f;
@@ -428,12 +460,14 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
                     }
                 }
                 if (live && t < T) {
-                    a.dv[e] = valid ? -a.v_loss_c * a.inv_batch * acc[i] : 0.f;
+                    // POPART: the normalized error (v - vs) / sigma in dv and the value loss
+                    a.dv[e] = valid ? -a.v_loss_c * a.inv_batch * (POPART ? acc[i] * pop.inv() : acc[i]) : 0.f;
                     if (t == T - 1) a.dv[e + B] = 0.f;
                     store_logits<AP, VEC>(a.dlogits, e, A, dz);
                 }
                 if (valid) {
-                    sum_vl += 0.5 * (double)acc[i] * (double)acc[i];
+                    const float err_n = POPART ? acc[i] * pop.inv() : acc[i];
+                    sum_vl += 0.5 * (double)err_n * (double)err_n;
                     sum_pl += (double)(-(lp2a[i] * kLn2) * pg);                // :317-321
                     sum_ent += (double)ent;
                     sum_rw += (double)R.r[i];                                    // :108
@@ -545,11 +579,11 @@ int pick_ap(int A) {
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool DIAG>
-int launch_s(const VtArgsT<DIAG>& a, bool vec, unsigned groups, int nw, int cl, cudaStream_t st) {
+template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool DIAG, bool POPART>
+int launch_s(const VtArgsT<DIAG, POPART>& a, bool vec, unsigned groups, int nw, int cl, cudaStream_t st) {
     const cudaError_t e =
-        vec ? impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, true, DIAG>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
-            : impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, false, DIAG>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
+        vec ? impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, true, DIAG, POPART>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
+            : impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, false, DIAG, POPART>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
     if (e != cudaSuccess) return (int)e;
     return impala_launch_status();
 }
@@ -562,8 +596,8 @@ constexpr int kMaxCluster = 8;  // portable cluster size
 // over a thread-block cluster (DSMEM carry exchange, cl = 4 / 8) works, but its cluster barriers
 // replace a cheap chunk loop, so cl = 1 unless overridden (scripts/tune_vtrace.py compares them).
 // IMPALA_VTRACE_S / IMPALA_VTRACE_NSEG (warps per CTA) / IMPALA_VTRACE_CLUSTER override the choice.
-template <bool WITH_LOSS, bool DIAG = false>
-int launch(VtArgsT<DIAG>& a, cudaStream_t st) {
+template <bool WITH_LOSS, bool DIAG = false, bool POPART = false>
+int launch(VtArgsT<DIAG, POPART>& a, cudaStream_t st) {
     if (a.T < 1 || a.B < 1 || a.A < 1) return IMPALA_ERR_BAD_ARG;
     const int AP = pick_ap(a.A);
     if (!AP) return IMPALA_ERR_UNSUPPORTED_SHAPE;
@@ -586,16 +620,16 @@ int launch(VtArgsT<DIAG>& a, cudaStream_t st) {
     if (n_env >= 1 && n_env <= max_w) nw = n_env;
 #define VT_AP(APV)                                                                                      \
     if (AP == APV) {                                                                                    \
-        if (S == 5) return launch_s<APV, 5, 320, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);       \
-        if (S == 1) return launch_s<APV, 1, 1024, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);      \
-        return launch_s<APV, 2, 512, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);                   \
+        if (S == 5) return launch_s<APV, 5, 320, 1, WITH_LOSS, DIAG, POPART>(a, vec, groups, nw, cl, st); \
+        if (S == 1) return launch_s<APV, 1, 1024, 1, WITH_LOSS, DIAG, POPART>(a, vec, groups, nw, cl, st);\
+        return launch_s<APV, 2, 512, 1, WITH_LOSS, DIAG, POPART>(a, vec, groups, nw, cl, st);             \
     }
     VT_AP(2)
     VT_AP(4)
 #undef VT_AP
-    if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);
-    if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);
-    return launch_s<32, 1, 512, 1, WITH_LOSS, DIAG>(a, vec, groups, nw, cl, st);
+    if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG, POPART>(a, vec, groups, nw, cl, st);
+    if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART>(a, vec, groups, nw, cl, st);
+    return launch_s<32, 1, 512, 1, WITH_LOSS, DIAG, POPART>(a, vec, groups, nw, cl, st);
 }
 
 }  // namespace
@@ -686,4 +720,23 @@ extern "C" int impala_vtrace_loss_diag(const float* cur_logits, const float* beh
     if (rc) return rc;
     a.diag = diag;
     return launch<true, true>(a, (cudaStream_t)stream);
+}
+
+extern "C" int impala_vtrace_loss_popart(const float* cur_logits, const float* beh_logits,
+                                         const int32_t* actions, const float* rewards,
+                                         const uint8_t* done, const int32_t* lens, const float* v,
+                                         float* vs, float* pg_adv, float* dlogits, float* dv,
+                                         double* scalars, double* diag, void* workspace,
+                                         int64_t workspace_bytes, int T, int B, int A, float gamma,
+                                         float rho_bar, float c_bar, float v_loss_c,
+                                         float policy_loss_c, float entropy_c, float inv_batch,
+                                         int mode, const double* popart, void* stream) {
+    if (!diag || !popart) return IMPALA_ERR_BAD_ARG;
+    VtPopArgs a{};
+    const int rc = loss_args(a, cur_logits, beh_logits, actions, rewards, done, lens, v, vs, pg_adv, dlogits, dv,
+                             scalars, workspace, workspace_bytes, impala_vtrace_loss_diag_workspace(T, B, A), T, B,
+                             A, gamma, rho_bar, c_bar, v_loss_c, policy_loss_c, entropy_c, inv_batch, mode);
+    if (rc) return rc;
+    a.diag = diag, a.popart = popart;
+    return launch<true, true, true>(a, (cudaStream_t)stream);
 }

@@ -21,6 +21,11 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       optimizer="rmsprop" or an lr_lambda (learning-rate schedule): impala_clip_optim /
       impala_gather_clip_optim in place of the two Adam entry points, with the rate of every update read
       from a float32 table in device memory (optim.py) - the captured graphs stay valid for every update.
+    popart=True (PopArt value normalization): impala_vtrace_loss_popart in place of the V-trace launch and
+      impala_clip_optim_popart / impala_gather_clip_optim_popart in place of the optimizer launch (the default
+      Adam as a one-entry table).  The value net outputs normalized values; the statistics (float64 in device
+      memory, `popart`) are read by the V-trace kernel and updated, with the value head's output-preserving
+      rescale, inside the optimizer launch from the eight V-trace sums that ride `comm`.  No launch is added.
 
 obs_dtype="uint8" (byte observations): the slabs hold obs as uint8 (impala_batch_layout_obs).  For
 O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one after the other as the
@@ -59,7 +64,7 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .optim import optim_config
+from .optim import POPART_BETA, check_popart_args, optim_config
 from .replay import ReplaySampler, check_replay_args
 
 PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
@@ -91,6 +96,11 @@ def diagnostic_values(sums, value_fn_loss: float, global_batch: int) -> dict:
     return out
 
 
+def popart_sigma(mu: float, nu: float) -> float:
+    """sigma of the PopArt statistics (mu, nu), as the optimizer kernel forms it."""
+    return min(max(max(nu - mu * mu, 0.0) ** 0.5, 1e-4), 1e6)
+
+
 def _ptr(t: torch.Tensor) -> C.c_void_p:
     return C.c_void_p(t.data_ptr())
 
@@ -112,10 +122,13 @@ class LearnerEngine:
                  mode: str = "reference", process_group=None, use_graph: bool = True,
                  slabs: int = 2, obs_dtype: str = "float32", frames: int = 1, diagnostics: bool = False,
                  replay_slabs: int = 0, replay_columns: int = 0, replay_seed: int = 0,
-                 optimizer: str = "adam", optimizer_kwargs: dict | None = None, lr_lambda=None, lr_table=None):
+                 optimizer: str = "adam", optimizer_kwargs: dict | None = None, lr_lambda=None, lr_table=None,
+                 popart: bool = False, popart_beta: float = POPART_BETA):
         # update rule and learning-rate schedule, checked before any device work (optim.optim_config); the
         # default - Adam at 0.95 * hp.lr - keeps impala_clip_adam with the rate as a launch argument
         self.optim = optim_config(hp, optimizer, optimizer_kwargs, lr_lambda, lr_table)
+        self.popart_beta = check_popart_args(popart, popart_beta)
+        self.popart = bool(popart)
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
@@ -136,7 +149,8 @@ class LearnerEngine:
             raise ValueError("experience replay runs on one device: the store is not sharded over a process group")
         # off-policy diagnostics of every update (impala_vtrace_loss_diag); every rank must agree on it
         self.diagnostics = bool(diagnostics)
-        self.n_extra = 12 if self.diagnostics else 4  # logged float64 values after the gradient in `comm`
+        # logged float64 values after the gradient in `comm`; PopArt forms its statistics from the eight sums
+        self.n_extra = 12 if self.diagnostics or self.popart else 4
         self.mode = _cabi.MODES[mode]
         self.pg = process_group
         self.world = 1
@@ -168,6 +182,12 @@ class LearnerEngine:
         # keep their Adam names, RMSprop's square_avg lives in adam_v and its momentum buffer in adam_m
         self.lr_table = (None if self.optim.lr_table is None
                          else torch.from_numpy(self.optim.lr_table.copy()).to(self.dev))
+        if self.popart and self.lr_table is None:  # the default Adam through the table entry point: same bits
+            self.lr_table = torch.tensor([self.optim.lr_scalar], dtype=torch.float32, device=self.dev)
+        # PopArt statistics {mu, nu, sigma, mu_loss, sigma_loss} (IMPALA_POPART_STATS), a fresh run at mu 0, nu 1
+        self.popart_buf = torch.tensor([0.0, 1.0, 1.0, 0.0, 1.0], dtype=torch.float64, device=self.dev)
+        # the value head inside `params`: W2 (1 x H_v) and b2
+        self.w2_at, self.b2_at = self.n_pi + self.vf_off[2], self.n_pi + self.vf_off[3]
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts (replay: the host slabs
         # hold the B_fresh columns that cross the host link, the device slabs the B columns trained on)
@@ -230,11 +250,14 @@ class LearnerEngine:
         if frames > 1:
             self.obs_dense = self.obs_f32 if self.obs_f32 is not None else torch.zeros(
                 (T + 1) * B_local * O, dtype=torch.uint8 if self.obs_u8_native else torch.float32, device=self.dev)
-        ws_fn = self.lib.impala_vtrace_loss_diag_workspace if self.diagnostics else self.lib.impala_vtrace_loss_workspace
+        ws_fn = (self.lib.impala_vtrace_loss_diag_workspace if self.n_extra == 12
+                 else self.lib.impala_vtrace_loss_workspace)
         self.ws_vt_bytes = int(ws_fn(T, B_local, A))
         self.ws_vt = torch.zeros(self.ws_vt_bytes, dtype=torch.uint8, device=self.dev)  # zeroed once
-        # ring of 4 tickets: [4 scalars | 2 norms | peer error | pad (| 8 off-policy sums)]
-        self.h_scalars = torch.zeros(4, 16 if self.diagnostics else 8, dtype=torch.float64).pin_memory()
+        # ring of 4 tickets: [4 scalars | 2 norms | peer error | pad (| 8 off-policy sums) (| 5 PopArt statistics |
+        # pad)]
+        self.h_scalars = torch.zeros(4, 24 if self.popart else 16 if self.diagnostics else 8,
+                                     dtype=torch.float64).pin_memory()
         self._scalar_events = [torch.cuda.Event() for _ in range(4)]
         self._ticket = 0
 
@@ -329,20 +352,53 @@ class LearnerEngine:
         for key, off, shp in zip(PKEYS, self.vf_off, shp_vf):
             yield "value_fn", key, self.n_pi + off, shp
 
-    def load_state(self, state: dict) -> None:
-        """state = {"policy": state_dict, "value_fn": state_dict} (any float dtype, CPU)."""
+    def load_state(self, state: dict, popart: dict | None = None) -> None:
+        """state = {"policy": state_dict, "value_fn": state_dict} (any float dtype, CPU).
+
+        With PopArt the value function is taken FOLDED, in reward units (what `state()` returns): popart =
+        {"mu": mu, "nu": nu} sets the statistics and unfolds W2 / sigma, (b2 - mu) / sigma (in float64) into the
+        normalized head; popart=None starts from mu = 0, nu = 1, where the folded head is the normalized one."""
+        if popart is not None and not self.popart:
+            raise ValueError("PopArt statistics given to an engine built with popart=False")
+        mu, nu = (0.0, 1.0) if popart is None else (float(popart["mu"]), float(popart["nu"]))
+        sigma = popart_sigma(mu, nu)
         flat = torch.zeros(self.n_total, dtype=torch.float32)
         for grp, key, off, shp in self._segments():
             t = torch.as_tensor(np.asarray(state[grp][key]) if not torch.is_tensor(state[grp][key])
                                 else state[grp][key].detach().cpu())
             if tuple(t.shape) != tuple(shp):
                 raise ValueError(f"{grp}.{key}: expected {shp}, got {tuple(t.shape)}")
+            if self.popart and grp == "value_fn" and key in PKEYS[2:]:
+                t = t.to(torch.float64)
+                t = t / sigma if key == PKEYS[2] else (t - mu) / sigma
             flat[off:off + t.numel()] = t.reshape(-1).to(torch.float32)
         self.params.copy_(flat)
+        if self.popart:
+            self.popart_buf.copy_(torch.tensor([mu, nu, sigma, mu, sigma], dtype=torch.float64))
         torch.cuda.synchronize(self.dev)
+
+    def popart_stats(self) -> dict:
+        """The current PopArt statistics {"mu", "nu", "sigma"} (float; waits for the stream)."""
+        self.stream.synchronize()
+        mu, nu, sigma = self.popart_buf[:3].tolist()
+        return {"mu": mu, "nu": nu, "sigma": sigma}
 
     def state(self, dtype=torch.float64) -> dict:
         """Reference-format state_dicts (CPU, float64 like reference models.py:6)."""
+        self.stream.synchronize()
+        flat = self.params.detach().cpu()
+        out = {"policy": {}, "value_fn": {}}
+        mu, _, sigma = self.popart_buf[:3].tolist() if self.popart else (0.0, 1.0, 1.0)
+        for grp, key, off, shp in self._segments():
+            n = int(np.prod(shp))
+            t = flat[off:off + n].reshape(shp)
+            if self.popart and grp == "value_fn" and key in PKEYS[2:]:  # folded: the value in reward units
+                t = t.to(torch.float64) * sigma + (mu if key == PKEYS[3] else 0.0)
+            out[grp][key] = t.to(dtype).clone()
+        return out
+
+    def normalized_state(self, dtype=torch.float64) -> dict:
+        """Like `state()`, but the value function as the engine holds it (normalized under PopArt)."""
         self.stream.synchronize()
         flat = self.params.detach().cpu()
         out = {"policy": {}, "value_fn": {}}
@@ -481,7 +537,11 @@ class LearnerEngine:
                  _ptr(self.vs), _ptr(self.pg_adv), _ptr(self.dlogits), _ptr(self.dv), scal)
         vt_hp = (T, B, A, float(hp.gamma), float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c),
                  float(hp.policy_loss_c), float(hp.entropy_c), float(self.inv_batch), self.mode, st)
-        if self.diagnostics:  # the eight sums land right after the four scalars
+        if self.popart:  # normalized values under the device statistics; the eight sums after the four scalars
+            _cabi.check(lib.impala_vtrace_loss_popart(*vt_in, C.c_void_p(gbase + 8 * (self.n_total + 4)),
+                                                      _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp[:-1],
+                                                      _ptr(self.popart_buf), st), "impala_vtrace_loss_popart")
+        elif self.diagnostics:  # the eight sums land right after the four scalars
             _cabi.check(lib.impala_vtrace_loss_diag(*vt_in, C.c_void_p(gbase + 8 * (self.n_total + 4)),
                                                     _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp),
                         "impala_vtrace_loss_diag")
@@ -540,6 +600,8 @@ class LearnerEngine:
         """The chosen rule with the scheduled rate, on the same buffers and paths as _enqueue_opt."""
         o, hp = self.optim, self.hp
         rule = (_ptr(self.lr_table), self.lr_table.numel(), o.rule_code, o.h0, o.h1, o.eps)
+        if self.popart:
+            return self._enqueue_popart(st, rule)
         if self.peer:
             pr = self.peer
             _cabi.check(self.lib.impala_gather_clip_optim(
@@ -551,6 +613,23 @@ class LearnerEngine:
         _cabi.check(self.lib.impala_clip_optim(
             _ptr(self.params), _ptr(self.comm), _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step), self.n_pi,
             self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), st), "impala_clip_optim")
+        return 1
+
+    def _enqueue_popart(self, st, rule) -> int:
+        """_enqueue_optim with the PopArt statistics update and value-head rescale in the same launch."""
+        hp = self.hp
+        pop = (_ptr(self.popart_buf), self.n_total + 4, self.w2_at, self.H_v, self.b2_at, float(self.popart_beta))
+        if self.peer:
+            pr = self.peer
+            _cabi.check(self.lib.impala_gather_clip_optim_popart(
+                _ptr(self.params), _ptr(self.comm), C.c_void_p(pr["gather"]), _ptr(pr["seq"]),
+                pr["slot"], pr["buf"], self.world, self.n_extra, _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step),
+                self.n_pi, self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), _ptr(pr["err"]), pr["timeout_s"],
+                *pop, st), "impala_gather_clip_optim_popart")
+            return 1
+        _cabi.check(self.lib.impala_clip_optim_popart(
+            _ptr(self.params), _ptr(self.comm), _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step), self.n_pi,
+            self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), *pop, st), "impala_clip_optim_popart")
         return 1
 
     def _capture(self, slot: int):
@@ -641,8 +720,10 @@ class LearnerEngine:
             self.h_scalars[k, 4:6].copy_(self.norms, non_blocking=True)
             if self.peer:
                 self.h_scalars[k, 6:7].copy_(self.peer["err"].to(torch.float64), non_blocking=True)
-            if self.diagnostics:
+            if self.n_extra == 12:
                 self.h_scalars[k, 8:16].copy_(self.comm[self.n_total + 4:self.n_total + 12], non_blocking=True)
+            if self.popart:  # the statistics after the update and the (mu, sigma) its loss used
+                self.h_scalars[k, 16:21].copy_(self.popart_buf, non_blocking=True)
             self._scalar_events[k].record(self.stream)
         return k
 
@@ -658,8 +739,12 @@ class LearnerEngine:
         out["total_loss"] = (hp.v_loss_c * out["value_fn_loss"] + hp.policy_loss_c * out["policy_loss"]
                              - hp.entropy_c * out["policy_entropy"])  # learner.py:154-159
         out["norm_policy"], out["norm_value"] = s[4], s[5]
+        if self.popart:
+            out["popart_mu"], out["popart_sigma"] = s[16], s[18]
         if self.diagnostics:
-            out.update(diagnostic_values(s[8:16], out["value_fn_loss"], self.global_batch))
+            # explained variance in reward units: the logged value loss is the normalized one of sigma_loss
+            vl = out["value_fn_loss"] * (s[20] ** 2 if self.popart else 1.0)
+            out.update(diagnostic_values(s[8:16], vl, self.global_batch))
         return out
 
     def synchronize(self) -> None:

@@ -36,7 +36,11 @@ path of the device (SURVEY 8f-2, 8f-4):
     the last R updates, kept in HBM (engine.py, replay.py); one device only;
   * `optimizer="rmsprop"`, `optimizer_kwargs` (torch's RMSprop keywords) and `lr_lambda` (a LambdaLR
     lambda, tabulated over hp.max_updates updates): the IMPALA paper's recipe (optim.py); the default is
-    the reference's Adam at 0.95 * hp.lr.  With a log_path and either one set, `optim/lr` is logged.
+    the reference's Adam at 0.95 * hp.lr.  With a log_path and either one set, `optim/lr` is logged;
+  * `popart=True`, `popart_beta` (PopArt value normalization, off by default): the value net trains on targets
+    normalized by running statistics of vs, kept and updated on the device (engine.py).  Checkpoints and
+    `value_fn` hold the FOLDED value function (reward units), plus the statistics under the key "popart";
+    `popart/mu` and `popart/sigma` are logged.
 
 CUDA is initialised inside the learner process only (`train.py:42` forces the fork start method,
 so the parent must never touch the device); a policy / value_fn that already lives on a CUDA
@@ -60,7 +64,7 @@ import numpy as np
 import torch
 import torch.multiprocessing as mp
 
-from .optim import optim_config
+from .optim import POPART_BETA, check_popart_args, optim_config
 from .replay import check_replay_args
 
 PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
@@ -246,8 +250,13 @@ class Learner:
     def __init__(self, id, hparams, policy, value_fn, q, update_counter, log_path=None,
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
                  evaluator=None, obs_dtype="float32", frames=1, diagnostics=False,
-                 replay_slabs=0, replay_columns=0, optimizer="adam", optimizer_kwargs=None, lr_lambda=None):
+                 replay_slabs=0, replay_columns=0, optimizer="adam", optimizer_kwargs=None, lr_lambda=None,
+                 popart=False, popart_beta=POPART_BETA):
         self.id = id
+        # PopArt value normalization: checked here, in the launching process
+        self.popart_beta = check_popart_args(popart, popart_beta)
+        self.popart = bool(popart)
+        self.popart_init = None  # {"mu", "nu"} of the folded value_fn (load() of a PopArt checkpoint sets it)
         # update rule and learning-rate schedule: checked and tabulated here, in the launching process (a lambda
         # need not pickle; data-parallel worker ranks receive the table)
         self.optimizer, self.optimizer_kwargs = optimizer, dict(optimizer_kwargs or {})
@@ -337,7 +346,7 @@ class Learner:
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
                     obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics,
                     replay_slabs=self.replay_slabs, replay_columns=self.replay_columns, optimizer=self.optimizer,
-                    optimizer_kwargs=self.optimizer_kwargs)
+                    optimizer_kwargs=self.optimizer_kwargs, popart=self.popart, popart_beta=self.popart_beta)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -350,9 +359,13 @@ class Learner:
                             obs_dtype=c["obs_dtype"], frames=c["frames"], diagnostics=c["diagnostics"],
                             replay_slabs=c["replay_slabs"], replay_columns=c["replay_columns"],
                             optimizer=c["optimizer"], optimizer_kwargs=c["optimizer_kwargs"],
-                            lr_table=self.optim.lr_table)
-        eng.load_state(self._init_state())
+                            lr_table=self.optim.lr_table, popart=c["popart"], popart_beta=c["popart_beta"])
+        eng.load_state(self._init_state(), self._popart_init())
         return eng
+
+    def _popart_init(self):
+        """The statistics the folded value_fn goes with: those of a loaded checkpoint, else None (mu 0, nu 1)."""
+        return dict(self.popart_init) if self.popart and self.popart_init is not None else None
 
     def _init_state(self):
         return {"policy": {k: v.detach().cpu() for k, v in self.policy.state_dict().items()},
@@ -362,7 +375,10 @@ class Learner:
         """Blocking: everything published so far is visible AND both float64 modules hold the current
         weights (checkpoints, end of run).  The per-update path is `_Publisher.post`."""
         pub.drain()
-        st = eng.state()
+        st = eng.state()  # the value function folded into reward units under PopArt
+        if self.popart:
+            s = eng.popart_stats()
+            self.popart_init = {"mu": s["mu"], "nu": s["nu"]}  # what save() writes next to the folded value_fn
         with torch.no_grad():
             self._version.value += 1
             for mod, grp in ((self.policy, "policy"), (self.value_fn, "value_fn")):
@@ -463,6 +479,9 @@ class Learner:
             for name in ("log_ratio_mean", "rho_clip_fraction", "c_clip_fraction", "kl_behaviour_current"):
                 writer.add_scalar(f"{tag}/offpolicy/{name}", sc[name], n)
             writer.add_scalar(f"{tag}/value/explained_variance", sc["value_explained_variance"], n)
+        if self.popart:
+            writer.add_scalar(f"{tag}/popart/mu", sc["popart_mu"], n)
+            writer.add_scalar(f"{tag}/popart/sigma", sc["popart_sigma"], n)
 
     def _due(self, n) -> bool:
         hp = self.hp
@@ -514,7 +533,7 @@ class Learner:
                 slabs = ring if ring is not None else stage
                 leader = dp.DpLeader(self.devices, self._cfg(), self._init_state(), slabs.shm.name,
                                      slabs.slab_bytes, slabs.K, timeout=max(60.0, float(self.timeout)),
-                                     lr_table=self.optim.lr_table)
+                                     lr_table=self.optim.lr_table, popart=self._popart_init())
                 torch.cuda.set_device(torch.device(self.device))
                 pg = leader.init_process_group(self.device)
             eng = self._make_engine(pg, world)  # first CUDA call of this process (post-fork)
@@ -650,13 +669,17 @@ class Learner:
 
     # ------------------------------------------------------ checkpoints (learner.py:277-295)
     def save(self, path):
-        torch.save({"policy_state_dict": self.policy.state_dict(),
-                    "value_fn_state_dict": self.value_fn.state_dict()}, path)
+        ckpt = {"policy_state_dict": self.policy.state_dict(), "value_fn_state_dict": self.value_fn.state_dict()}
+        if self.popart:  # value_fn is folded (reward units); the statistics that unfold it
+            ckpt["popart"] = dict(self.popart_init or {"mu": 0.0, "nu": 1.0})
+        torch.save(ckpt, path)
 
     def load(self, path):
         checkpoint = torch.load(path)
         self.policy.load_state_dict(checkpoint["policy_state_dict"])
         self.value_fn.load_state_dict(checkpoint["value_fn_state_dict"])
+        if "popart" in checkpoint:
+            self.popart_init = {k: float(checkpoint["popart"][k]) for k in ("mu", "nu")}
 
     @property
     def policy_weights(self):

@@ -263,3 +263,57 @@ def clip_optim(params, grad, m, v, step, n_policy, max_norm, lr_table, rule="ada
                                               _cabi.OPT_RULES[rule], float(h0), float(h1), float(eps), _p(norms),
                                               _st()), "impala_clip_optim")
     return norms
+
+
+def popart_stats(mu=0.0, nu=1.0, device="cuda"):
+    """A float64 PopArt statistics buffer {mu, nu, sigma, mu_loss, sigma_loss} (IMPALA_POPART_STATS) for the
+    value statistics (mu, nu); sigma = clamp(sqrt(max(nu - mu^2, 0)), 1e-4, 1e6)."""
+    sigma = min(max(max(nu - mu * mu, 0.0) ** 0.5, 1e-4), 1e6)
+    return torch.tensor([mu, nu, sigma, mu, sigma], dtype=torch.float64, device=device)
+
+
+def vtrace_loss_popart(cur_logits, beh_logits, actions, rewards, done, lens, v, hp, inv_batch, popart,
+                       mode="reference"):
+    """vtrace_loss_diag on the NORMALIZED values v under the PopArt statistics `popart` (float64 CUDA tensor,
+    popart_stats' layout): vs and `diag` in reward units, pg_adv, dv, dlogits and the two losses normalized
+    (impala_vtrace_loss_popart)."""
+    _need_cuda(cur_logits, beh_logits, actions, rewards, done, lens, v, popart)
+    if popart.dtype != torch.float64 or popart.numel() < 3:
+        raise _cabi.ImpalaCudaError("popart must be a float64 tensor of the statistics (popart_stats)")
+    T, B, A = cur_logits.shape
+    dev = v.device
+    vs = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    pg = torch.empty(T, B, dtype=torch.float32, device=dev)
+    dlogits = torch.empty(T, B, A, dtype=torch.float32, device=dev)
+    dv = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    scalars = torch.empty(4, dtype=torch.float64, device=dev)
+    diag = torch.empty(8, dtype=torch.float64, device=dev)
+    lib = _cabi.lib()
+    ws_bytes = int(lib.impala_vtrace_loss_diag_workspace(T, B, A))
+    ws = torch.zeros(ws_bytes, dtype=torch.uint8, device=dev)
+    _cabi.check(lib.impala_vtrace_loss_popart(
+        _p(cur_logits), _p(beh_logits), _p(actions), _p(rewards), _p(done), _p(lens), _p(v), _p(vs),
+        _p(pg), _p(dlogits), _p(dv), _p(scalars), _p(diag), _p(ws), ws_bytes, T, B, A, float(hp.gamma),
+        float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c), float(hp.policy_loss_c), float(hp.entropy_c),
+        float(inv_batch), _cabi.MODES[mode], _p(popart), _st()), "impala_vtrace_loss_popart")
+    return dict(vs=vs, pg_adv=pg, dlogits=dlogits, dv=dv, scalars=scalars, diag=diag)
+
+
+def clip_optim_popart(params, grad, m, v, step, n_policy, max_norm, lr_table, popart, sums_at, w2_off, w2_len,
+                      b2_off, beta=3e-4, rule="adam", h0=0.9, h1=0.999, eps=1e-8):
+    """impala_clip_optim_popart: clip_optim, then the PopArt statistics update from the eight sums at
+    grad[sums_at:sums_at + 8] and the output-preserving rescale of the value head params[w2_off:w2_off + w2_len]
+    (W2) and params[b2_off] (b2).  `popart` (float64 CUDA tensor, popart_stats' layout) is updated in place."""
+    _need_cuda(params, grad, m, v, step, lr_table, popart)
+    if lr_table.dtype != torch.float32:
+        raise _cabi.ImpalaCudaError(f"lr_table must be float32, got {lr_table.dtype}")
+    if popart.dtype != torch.float64 or popart.numel() < _cabi.POPART_STATS:
+        raise _cabi.ImpalaCudaError("popart must be a float64 tensor of the statistics (popart_stats)")
+    if grad.numel() < sums_at + 8:
+        raise _cabi.ImpalaCudaError(f"grad holds {grad.numel()} entries, the sums end at {sums_at + 8}")
+    norms = torch.empty(2, dtype=torch.float64, device=params.device)
+    _cabi.check(_cabi.lib().impala_clip_optim_popart(
+        _p(params), _p(grad), _p(m), _p(v), _p(step), int(n_policy), params.numel(), float(max_norm), _p(lr_table),
+        lr_table.numel(), _cabi.OPT_RULES[rule], float(h0), float(h1), float(eps), _p(norms), _p(popart),
+        int(sums_at), int(w2_off), int(w2_len), int(b2_off), float(beta), _st()), "impala_clip_optim_popart")
+    return norms

@@ -143,3 +143,17 @@ def optim_config(hp, optimizer: str = "adam", optimizer_kwargs: dict | None = No
     else:
         table = None
     return OptimConfig(optimizer, float(h0), float(h1), float(eps), table, scalar)
+
+
+POPART_BETA = 3e-4  # step size of the PopArt statistics (van Hasselt et al. 2016)
+
+
+def check_popart_args(popart, popart_beta) -> float:
+    """Check LearnerEngine / Learner's PopArt switch and step size; returns beta.  The kernel takes beta as a
+    float32 in (0, 1]; a value that rounds outside raises ValueError."""
+    if not isinstance(popart, (bool, np.bool_)):
+        raise ValueError(f"popart must be True or False, got {popart!r}")
+    beta = _finite_number("popart_beta", popart_beta)
+    if not (0.0 < np.float32(beta) <= 1.0):
+        raise ValueError(f"popart_beta must be in (0, 1], got {popart_beta!r}")
+    return beta
