@@ -250,6 +250,26 @@ int impala_vtrace_loss_popart(const float* cur_logits, const float* beh_logits, 
                               float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch,
                               int mode, const double* popart, void* stream);
 
+#define IMPALA_REWARD_CLIP_ABS_ONE 1         /* r -> clip(r, -1, 1) (Atari) */
+#define IMPALA_REWARD_CLIP_SOFT_ASYMMETRIC 2 /* r -> 5 tanh(r / 5) for r >= 0, 1.5 tanh(r / 5) for r < 0 (DMLab) */
+
+/* impala_vtrace_loss (diag == NULL), impala_vtrace_loss_diag (diag, popart == NULL) or
+ * impala_vtrace_loss_popart (diag and popart) with the reward transform `reward_clip` (IMPALA_REWARD_CLIP_*)
+ * applied to every reward where it enters the recurrence (delta of either mode) and pg_adv.
+ *   scalars[3] (batch_mean_reward) stays the mean of the RAW rewards; everything formed from vs - the losses,
+ *   diag[0..8) and so the PopArt statistics the optimizer forms from them - is in clipped-reward units.
+ *   NaN rewards stay NaN (compare-and-select, as torch.clamp); +-inf saturates.  With rewards already clipped
+ *   on the host (abs_one) the outputs other than scalars[3] are bit-identical to the selected entry point's.
+ * Workspace: that of the selected entry point.  Returns IMPALA_ERR_BAD_ARG for a popart without diag, a
+ * reward_clip outside IMPALA_REWARD_CLIP_* and whatever the selected entry point refuses. */
+int impala_vtrace_loss_rclip(const float* cur_logits, const float* beh_logits, const int32_t* actions,
+                             const float* rewards, const uint8_t* done, const int32_t* lens,
+                             const float* v, float* vs, float* pg_adv, float* dlogits, float* dv,
+                             double* scalars, void* workspace, int64_t workspace_bytes, int T, int B,
+                             int A, float gamma, float rho_bar, float c_bar, float v_loss_c,
+                             float policy_loss_c, float entropy_c, float inv_batch, int mode,
+                             double* diag, const double* popart, int reward_clip, void* stream);
+
 /* Per-group gradient clipping + Adam in one launch (learner.py:176-183).
  *   params/m/v: f32 [n_total]; grad: f64 [n_total] (the possibly all-reduced sum);
  *   group 0 = [0, n_policy) (policy net), group 1 = [n_policy, n_total) (value net);

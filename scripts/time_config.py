@@ -20,7 +20,11 @@ slab read and written at 3.35 TB/s).
 launch count; the PopArt arm adds one FMA per value load, the 1 / sigma scaling and the optimizer's head
 epilogue), and times impala_vtrace_loss_diag against impala_vtrace_loss_popart and impala_clip_optim against
 impala_clip_optim_popart alone on the engine's buffers (median of 200 launches each, alternating, L2 flushed
-before each)."""
+before each).
+--compare-reward-clip alternates engines with reward_clip None, "abs_one" and "soft_asymmetric" on the same batch
+(rewards N(0, 5^2), so both transforms act) the same way, and times impala_vtrace_loss against
+impala_vtrace_loss_rclip in both modes alone on the engine's buffers (median of 200 launches each, alternating,
+L2 flushed before each)."""
 import argparse
 import os
 import statistics
@@ -65,6 +69,7 @@ ap.add_argument("--obs-dtype", default="float32", choices=["float32", "uint8"], 
 ap.add_argument("--compare-diag", action="store_true", help="alternate engines without / with off-policy diagnostics")
 ap.add_argument("--compare-popart", action="store_true", help="alternate engines without / with PopArt")
 ap.add_argument("--compare-replay", action="store_true", help="alternate engines without / with experience replay")
+ap.add_argument("--compare-reward-clip", action="store_true", help="alternate engines without / with reward clipping")
 ap.add_argument("--replay-slabs", type=int, default=2, help="past fresh batches in the pool of --compare-replay")
 ap.add_argument("--replay-columns", type=int, default=None, help="replayed columns of --compare-replay (default B/2)")
 a = ap.parse_args()
@@ -95,6 +100,12 @@ if a.compare_popart:
     arms = {"popart off": arms["default"], "popart on": arms["default"]}
     popart_arm = {"popart on": dict(popart=True)}
     obs_dt = {name: "uint8" if a.config in ("ram", "ram4", "ram8", "minatar", "ram_a6") else "float32" for name in arms}
+rclip_arm = {}
+if a.compare_reward_clip:
+    arms = {"reward_clip None": arms["default"], "reward_clip abs_one": arms["default"],
+            "reward_clip soft_asymmetric": arms["default"]}
+    rclip_arm = {name: dict(reward_clip=name.split()[1]) for name in list(arms)[1:]}
+    obs_dt = {name: "uint8" if a.config in ("ram", "ram4", "ram8", "minatar", "ram_a6") else "float32" for name in arms}
 replay_arm = {}
 if a.compare_replay:
     Br = w["B"] // 2 if a.replay_columns is None else a.replay_columns
@@ -109,10 +120,11 @@ for name, tc in arms.items():
     dt = obs_dt.get(name, "float32")
     k = n_frames.get(name, 1)
     eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k,
-                        diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}), **popart_arm.get(name, {}))
+                        diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}), **popart_arm.get(name, {}),
+                        **rclip_arm.get(name, {}))
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
     byte_obs = (a.compare_obs or ((a.compare_frames or a.compare_replay) and dt == "uint8")
-                or ((a.compare_diag or a.compare_popart) and dt == "uint8"))
+                or ((a.compare_diag or a.compare_popart or a.compare_reward_clip) and dt == "uint8"))
     if a.compare_replay:
         engines[name] = eng
         continue
@@ -125,6 +137,8 @@ for name, tc in arms.items():
         batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if byte_obs else "normal")
     if dt == "float32":
         batch["obs"] = batch["obs"].astype("float32")
+    if a.compare_reward_clip:
+        batch["rewards"] = batch["rewards"] * 5.0
     eng.load_device_batch(batch)
     if a.compare_obs or a.compare_frames:
         eng.load_device_batch(batch, 1)
@@ -304,6 +318,43 @@ if a.compare_popart:  # the two launches PopArt changes, alone, plain and PopArt
                        ("impala_clip_optim", "impala_clip_optim_popart")):
         k0, k1 = statistics.median(tk[plain]), statistics.median(tk[pop])
         print(f"{a.config}: {plain} {k0:.1f} us, {pop} {k1:.1f} us (+{k1 - k0:.1f} us, {100 * (k1 / k0 - 1):+.1f} %)")
+if a.compare_reward_clip:  # the V-trace + loss kernel alone, without and with either transform, alternating
+    import ctypes
+
+    from torched_impala_b200 import _cabi
+
+    eng = engines["reward_clip abs_one"]
+    d = eng.d_views[0]
+    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    ins = (P(eng.logits), P(d["beh_logits"]), P(d["actions"]), P(d["rewards"]), P(d["done"]), P(d["lens"]),
+           P(eng.values), P(eng.vs), P(eng.pg_adv), P(eng.dlogits), P(eng.dv),
+           ctypes.c_void_p(eng.comm.data_ptr() + 8 * eng.n_total), P(eng.ws_vt), eng.ws_vt_bytes)
+    tail = (w["T"], w["B"], w["A"], hp.gamma, hp.rho_bar, hp.c_bar, hp.v_loss_c, hp.policy_loss_c, hp.entropy_c,
+            1.0 / w["B"], 0)
+    calls = {"impala_vtrace_loss": lambda st: eng.lib.impala_vtrace_loss(*ins, *tail, st)}
+    for rc_name, code in _cabi.REWARD_CLIPS.items():
+        calls[f"impala_vtrace_loss_rclip {rc_name}"] = (
+            lambda st, code=code: eng.lib.impala_vtrace_loss_rclip(*ins, *tail, None, None, code, st))
+    tk = {name: [] for name in calls}
+    with torch.cuda.stream(eng.stream):
+        st = ctypes.c_void_p(eng.stream.cuda_stream)
+        for i in range(220):
+            for name, fn in calls.items():
+                flush.zero_()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(eng.stream)
+                rc = fn(st)
+                e1.record(eng.stream)
+                e1.synchronize()
+                assert rc == 0, (name, rc)
+                if i >= 20:
+                    tk[name].append(e0.elapsed_time(e1) * 1e3)
+    k0 = statistics.median(tk["impala_vtrace_loss"])
+    print(f"V-trace + loss kernel {a.config}: impala_vtrace_loss {k0:.1f} us", end="")
+    for name in list(calls)[1:]:
+        k1 = statistics.median(tk[name])
+        print(f", {name} {k1:.1f} us ({k1 - k0:+.1f} us, {100 * (k1 / k0 - 1):+.1f} %)", end="")
+    print()
 q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
                     "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 print(f"GPU (nvidia-smi): {q}")
@@ -329,3 +380,9 @@ if a.compare_popart:
     print(f"popart overhead {a.config}: {m1 - m0:+.1f} us/step ({100 * (m1 / m0 - 1):+.1f} %), launches "
           f"{engines['popart on'].launches_per_step} against {engines['popart off'].launches_per_step}; "
           f"mu {st['mu']:.4f}, sigma {st['sigma']:.4f}")
+if a.compare_reward_clip:
+    m0 = statistics.median(ts["reward_clip None"])
+    for name in list(arms)[1:]:
+        m1 = statistics.median(ts[name])
+        print(f"{name} overhead {a.config}: {m1 - m0:+.1f} us/step ({100 * (m1 / m0 - 1):+.1f} %), launches "
+              f"{engines[name].launches_per_step} against {engines['reward_clip None'].launches_per_step}")

@@ -23,12 +23,26 @@ OPT_ADAM = 0
 OPT_RMSPROP = 1
 OPT_RULES = {"adam": OPT_ADAM, "rmsprop": OPT_RMSPROP}  # update rules of impala_clip_optim
 POPART_STATS = 5  # float64 {mu, nu, sigma, mu_loss, sigma_loss} (IMPALA_POPART_STATS)
+REWARD_CLIP_ABS_ONE = 1
+REWARD_CLIP_SOFT_ASYMMETRIC = 2
+# reward transforms of impala_vtrace_loss_rclip (IMPALA_REWARD_CLIP_*)
+REWARD_CLIPS = {"abs_one": REWARD_CLIP_ABS_ONE, "soft_asymmetric": REWARD_CLIP_SOFT_ASYMMETRIC}
 
 
 def obs_dtype_code(obs_dtype: str) -> int:
     if obs_dtype not in OBS_DTYPES:
         raise ValueError(f"obs_dtype must be one of {sorted(OBS_DTYPES)}, got {obs_dtype!r}")
     return OBS_DTYPES[obs_dtype]
+
+
+def reward_clip_code(reward_clip) -> int:
+    """The IMPALA_REWARD_CLIP_* code of `reward_clip` ("abs_one" | "soft_asymmetric"), 0 for None (no transform);
+    anything else raises ValueError naming the accepted values."""
+    if reward_clip is None:
+        return 0
+    if not isinstance(reward_clip, str) or reward_clip not in REWARD_CLIPS:
+        raise ValueError(f"reward_clip must be None or one of {sorted(REWARD_CLIPS)}, got {reward_clip!r}")
+    return REWARD_CLIPS[reward_clip]
 
 _ERRORS = {-1: "IMPALA_ERR_BAD_ARG", -2: "IMPALA_ERR_UNSUPPORTED_SHAPE",
            -3: "IMPALA_ERR_WORKSPACE_TOO_SMALL"}
@@ -76,6 +90,7 @@ SIGNATURES = {
     "impala_vtrace_loss_diag_workspace": (_i64, [_i, _i, _i]),
     "impala_vtrace_loss_diag": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p]),
     "impala_vtrace_loss_popart": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p]),
+    "impala_vtrace_loss_rclip": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p]),
     "impala_clip_adam": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _f, _f, _f, _f, _p, _p]),
     "impala_clip_optim": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i, _f, _f, _f, _p, _p]),
     "impala_gather_clip_optim": (_i, [_p] * 4 + [_i64, _i64, _i, _i, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i]

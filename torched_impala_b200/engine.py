@@ -26,6 +26,11 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       Adam as a one-entry table).  The value net outputs normalized values; the statistics (float64 in device
       memory, `popart`) are read by the V-trace kernel and updated, with the value head's output-preserving
       rescale, inside the optimizer launch from the eight V-trace sums that ride `comm`.  No launch is added.
+    reward_clip="abs_one" | "soft_asymmetric" (reward clipping): impala_vtrace_loss_rclip in place of whichever
+      of the three V-trace launches above the step makes, with the same workspace and outputs.  The kernel
+      transforms every reward where it enters V-trace, so the slabs, the replay store and the transport keep raw
+      rewards; the logged batch_mean_reward stays raw, the losses, diagnostics and PopArt statistics are in
+      clipped-reward units.  No launch is added.
 
 obs_dtype="uint8" (byte observations): the slabs hold obs as uint8 (impala_batch_layout_obs).  For
 O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one after the other as the
@@ -123,12 +128,14 @@ class LearnerEngine:
                  slabs: int = 2, obs_dtype: str = "float32", frames: int = 1, diagnostics: bool = False,
                  replay_slabs: int = 0, replay_columns: int = 0, replay_seed: int = 0,
                  optimizer: str = "adam", optimizer_kwargs: dict | None = None, lr_lambda=None, lr_table=None,
-                 popart: bool = False, popart_beta: float = POPART_BETA):
+                 popart: bool = False, popart_beta: float = POPART_BETA, reward_clip: str | None = None):
         # update rule and learning-rate schedule, checked before any device work (optim.optim_config); the
         # default - Adam at 0.95 * hp.lr - keeps impala_clip_adam with the rate as a launch argument
         self.optim = optim_config(hp, optimizer, optimizer_kwargs, lr_lambda, lr_table)
         self.popart_beta = check_popart_args(popart, popart_beta)
         self.popart = bool(popart)
+        # reward transform inside the V-trace kernel (IMPALA_REWARD_CLIP_*; 0 = none), checked before device work
+        self.reward_clip_code = _cabi.reward_clip_code(reward_clip)
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
@@ -537,7 +544,12 @@ class LearnerEngine:
                  _ptr(self.vs), _ptr(self.pg_adv), _ptr(self.dlogits), _ptr(self.dv), scal)
         vt_hp = (T, B, A, float(hp.gamma), float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c),
                  float(hp.policy_loss_c), float(hp.entropy_c), float(self.inv_batch), self.mode, st)
-        if self.popart:  # normalized values under the device statistics; the eight sums after the four scalars
+        if self.reward_clip_code:  # the same kernel as below with the reward transform
+            sums = C.c_void_p(gbase + 8 * (self.n_total + 4)) if self.n_extra == 12 else None
+            _cabi.check(lib.impala_vtrace_loss_rclip(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp[:-1], sums,
+                                                     _ptr(self.popart_buf) if self.popart else None,
+                                                     self.reward_clip_code, st), "impala_vtrace_loss_rclip")
+        elif self.popart:  # normalized values under the device statistics; the eight sums after the four scalars
             _cabi.check(lib.impala_vtrace_loss_popart(*vt_in, C.c_void_p(gbase + 8 * (self.n_total + 4)),
                                                       _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp[:-1],
                                                       _ptr(self.popart_buf), st), "impala_vtrace_loss_popart")

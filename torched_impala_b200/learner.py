@@ -40,7 +40,11 @@ path of the device (SURVEY 8f-2, 8f-4):
   * `popart=True`, `popart_beta` (PopArt value normalization, off by default): the value net trains on targets
     normalized by running statistics of vs, kept and updated on the device (engine.py).  Checkpoints and
     `value_fn` hold the FOLDED value function (reward units), plus the statistics under the key "popart";
-    `popart/mu` and `popart/sigma` are logged.
+    `popart/mu` and `popart/sigma` are logged;
+  * `reward_clip="abs_one"` (clip(r, -1, 1), the paper's Atari setting) or `"soft_asymmetric"` (DMLab's
+    5 tanh(r / 5), 1.5 tanh(r / 5) below 0): the V-trace kernel transforms the rewards it reads, so actors, the
+    transport and replay keep raw rewards and `rewards/batch_mean_reward` stays the raw game score.  A
+    hyperparameter, not state: checkpoints are unchanged.
 
 CUDA is initialised inside the learner process only (`train.py:42` forces the fork start method,
 so the parent must never touch the device); a policy / value_fn that already lives on a CUDA
@@ -64,6 +68,7 @@ import numpy as np
 import torch
 import torch.multiprocessing as mp
 
+from . import _cabi
 from .optim import POPART_BETA, check_popart_args, optim_config
 from .replay import check_replay_args
 
@@ -251,8 +256,11 @@ class Learner:
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
                  evaluator=None, obs_dtype="float32", frames=1, diagnostics=False,
                  replay_slabs=0, replay_columns=0, optimizer="adam", optimizer_kwargs=None, lr_lambda=None,
-                 popart=False, popart_beta=POPART_BETA):
+                 popart=False, popart_beta=POPART_BETA, reward_clip=None):
         self.id = id
+        # reward clipping inside the V-trace kernel: checked here, in the launching process
+        _cabi.reward_clip_code(reward_clip)
+        self.reward_clip = reward_clip
         # PopArt value normalization: checked here, in the launching process
         self.popart_beta = check_popart_args(popart, popart_beta)
         self.popart = bool(popart)
@@ -346,7 +354,8 @@ class Learner:
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
                     obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics,
                     replay_slabs=self.replay_slabs, replay_columns=self.replay_columns, optimizer=self.optimizer,
-                    optimizer_kwargs=self.optimizer_kwargs, popart=self.popart, popart_beta=self.popart_beta)
+                    optimizer_kwargs=self.optimizer_kwargs, popart=self.popart, popart_beta=self.popart_beta,
+                    reward_clip=self.reward_clip)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -359,7 +368,8 @@ class Learner:
                             obs_dtype=c["obs_dtype"], frames=c["frames"], diagnostics=c["diagnostics"],
                             replay_slabs=c["replay_slabs"], replay_columns=c["replay_columns"],
                             optimizer=c["optimizer"], optimizer_kwargs=c["optimizer_kwargs"],
-                            lr_table=self.optim.lr_table, popart=c["popart"], popart_beta=c["popart_beta"])
+                            lr_table=self.optim.lr_table, popart=c["popart"], popart_beta=c["popart_beta"],
+                            reward_clip=c["reward_clip"])
         eng.load_state(self._init_state(), self._popart_init())
         return eng
 

@@ -317,3 +317,41 @@ def clip_optim_popart(params, grad, m, v, step, n_policy, max_norm, lr_table, po
         lr_table.numel(), _cabi.OPT_RULES[rule], float(h0), float(h1), float(eps), _p(norms), _p(popart),
         int(sums_at), int(w2_off), int(w2_len), int(b2_off), float(beta), _st()), "impala_clip_optim_popart")
     return norms
+
+
+def vtrace_loss_rclip(cur_logits, beh_logits, actions, rewards, done, lens, v, hp, inv_batch, reward_clip,
+                      mode="reference", diagnostics=False, popart=None):
+    """vtrace_loss (diagnostics=False, popart=None), vtrace_loss_diag (diagnostics=True) or vtrace_loss_popart
+    (popart: the statistics tensor) with the reward transform `reward_clip` ("abs_one" | "soft_asymmetric")
+    applied to the rewards inside the kernel (impala_vtrace_loss_rclip); scalars[3] stays the raw rewards' mean."""
+    code = _cabi.reward_clip_code(reward_clip)
+    if not code:
+        raise ValueError("vtrace_loss_rclip needs a reward_clip; vtrace_loss is the untransformed kernel")
+    _need_cuda(cur_logits, beh_logits, actions, rewards, done, lens, v)
+    if popart is not None:
+        _need_cuda(popart)
+        if popart.dtype != torch.float64 or popart.numel() < 3:
+            raise _cabi.ImpalaCudaError("popart must be a float64 tensor of the statistics (popart_stats)")
+    with_diag = bool(diagnostics) or popart is not None
+    T, B, A = cur_logits.shape
+    dev = v.device
+    vs = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    pg = torch.empty(T, B, dtype=torch.float32, device=dev)
+    dlogits = torch.empty(T, B, A, dtype=torch.float32, device=dev)
+    dv = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    scalars = torch.empty(4, dtype=torch.float64, device=dev)
+    diag = torch.empty(8, dtype=torch.float64, device=dev) if with_diag else None
+    lib = _cabi.lib()
+    ws_fn = lib.impala_vtrace_loss_diag_workspace if with_diag else lib.impala_vtrace_loss_workspace
+    ws_bytes = int(ws_fn(T, B, A))
+    ws = torch.zeros(ws_bytes, dtype=torch.uint8, device=dev)
+    _cabi.check(lib.impala_vtrace_loss_rclip(
+        _p(cur_logits), _p(beh_logits), _p(actions), _p(rewards), _p(done), _p(lens), _p(v), _p(vs),
+        _p(pg), _p(dlogits), _p(dv), _p(scalars), _p(ws), ws_bytes, T, B, A, float(hp.gamma),
+        float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c), float(hp.policy_loss_c), float(hp.entropy_c),
+        float(inv_batch), _cabi.MODES[mode], None if diag is None else _p(diag),
+        None if popart is None else _p(popart), code, _st()), "impala_vtrace_loss_rclip")
+    out = dict(vs=vs, pg_adv=pg, dlogits=dlogits, dv=dv, scalars=scalars)
+    if with_diag:
+        out["diag"] = diag
+    return out
