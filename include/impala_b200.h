@@ -82,6 +82,20 @@ int impala_batch_layout_obs(int T, int B, int O, int A, int obs_dtype, int64_t o
 int impala_batch_layout_frames(int T, int B, int F, int frames, int A, int obs_dtype, int64_t offsets[6],
                                int64_t* total_bytes);
 
+/* Action distributions of a batch slab and of the V-trace loss kernels.
+ *   IMPALA_ACT_CATEGORICAL: A actions; beh_logits (T,B,A) f32, actions (T,B) i32 (indices).
+ *   IMPALA_ACT_GAUSSIAN: diagonal Gaussian over A action dimensions; the behaviour record is the actor's
+ *     policy output [m | s] (means, then log standard deviations), beh_logits (T,B,2A) f32, and the action the
+ *     unsquashed sample m + e^s eps, actions (T,B,A) f32. */
+#define IMPALA_ACT_CATEGORICAL 0
+#define IMPALA_ACT_GAUSSIAN 1
+
+/* impala_batch_layout_frames for the action distribution act_kind: IMPALA_ACT_CATEGORICAL is exactly
+ * impala_batch_layout_frames, IMPALA_ACT_GAUSSIAN widens beh_logits to (T,B,2A) f32 and actions to (T,B,A) f32.
+ * An unknown act_kind returns IMPALA_ERR_BAD_ARG. */
+int impala_batch_layout_act(int T, int B, int F, int frames, int A, int obs_dtype, int act_kind, int64_t offsets[6],
+                            int64_t* total_bytes);
+
 /* Host slab -> device slab, async on `stream` (host memory should be pinned). */
 int impala_ingest(void* dev_slab, const void* host_slab, int64_t bytes, void* stream);
 
@@ -99,6 +113,10 @@ int impala_ingest_shard_obs(void* dev_slab, const void* host_slab, int T, int B,
  * impala_ingest_shard_obs is its frames = 1 case. */
 int impala_ingest_shard_frames(void* dev_slab, const void* host_slab, int T, int B, int F, int frames, int A,
                                int obs_dtype, int b0, int B_local, void* stream);
+/* The same for slabs laid out by impala_batch_layout_act; impala_ingest_shard_frames is its
+ * IMPALA_ACT_CATEGORICAL case. */
+int impala_ingest_shard_act(void* dev_slab, const void* host_slab, int T, int B, int F, int frames, int A,
+                            int obs_dtype, int act_kind, int b0, int B_local, void* stream);
 
 /* Dense observation rows from frames (pure data movement, one launch):
  *   out[(t B + b) k F + j F + f] = frames[((t + j) B + b) F + f]   for t < R, b < B, j < k, f < F.
@@ -121,6 +139,10 @@ int impala_obs_unstack(const void* frames, int in_dtype, void* out, int out_dtyp
  * checked: slab indices and columns < Bf are the caller's to keep in range. */
 int impala_batch_compose(void* dst_slab, const void* store, int64_t store_slab_bytes, const int32_t* plan, int T,
                          int B, int Bf, int F, int frames, int A, int obs_dtype, void* stream);
+/* The same for slabs laid out by impala_batch_layout_act; impala_batch_compose is its IMPALA_ACT_CATEGORICAL
+ * case.  An unknown act_kind returns IMPALA_ERR_BAD_ARG. */
+int impala_batch_compose_act(void* dst_slab, const void* store, int64_t store_slab_bytes, const int32_t* plan, int T,
+                             int B, int Bf, int F, int frames, int A, int obs_dtype, int act_kind, void* stream);
 
 /* out[i] = (float)x[i] for i < n: exact widening of byte observations, for the MLP shapes that read
  * float32 rows only (O <= 128). */
@@ -268,6 +290,27 @@ int impala_vtrace_loss_rclip(const float* cur_logits, const float* beh_logits, c
                              double* scalars, void* workspace, int64_t workspace_bytes, int T, int B,
                              int A, float gamma, float rho_bar, float c_bar, float v_loss_c,
                              float policy_loss_c, float entropy_c, float inv_batch, int mode,
+                             double* diag, const double* popart, int reward_clip, void* stream);
+
+/* The V-trace loss kernel of impala_vtrace_loss_rclip for diagonal Gaussian policies (IMPALA_ACT_GAUSSIAN) over
+ * A <= 16 action dimensions.  cur_params / beh_params (T,B,2A): the current and the behaviour policy outputs
+ * [m | s], sigma = e^s; actions (T,B,A) f32: the unsquashed samples; dparams (T,B,2A): d total_loss / d params.
+ *   log pi(a) = sum_k [-((a_k - m_k) / sigma_k)^2 / 2 - s_k - log(2 pi) / 2]  (torch Normal.log_prob summed), the
+ *   same for mu with the behaviour outputs; ratio, clipping, V-trace, vs and pg_adv as for categorical policies.
+ *   policy_loss = sum -log pi(a) pg_adv, policy_entropy = sum_k (s_k + (1 + log(2 pi)) / 2), each sum_b .. inv_batch.
+ *   d/dm_k = -policy_loss_c pg_adv (a_k - m_k) / sigma_k^2 inv_batch,
+ *   d/ds_k = (policy_loss_c pg_adv (1 - ((a_k - m_k) / sigma_k)^2) - entropy_c) inv_batch; zero at padded steps.
+ *   diag[4] = sum KL(mu || pi) = sum_k [s_k - sb_k + (sigma_b,k^2 + (mb_k - m_k)^2) / (2 sigma_k^2) - 1/2].
+ * diag == NULL: the loss sums only (workspace impala_vtrace_loss_workspace); diag: the eight off-policy sums as
+ * impala_vtrace_loss_diag (workspace impala_vtrace_loss_diag_workspace); popart (needs diag): PopArt as
+ * impala_vtrace_loss_popart; reward_clip: 0 (none) or IMPALA_REWARD_CLIP_*.  A > 16 returns
+ * IMPALA_ERR_UNSUPPORTED_SHAPE; a popart without diag, an unknown reward_clip and what impala_vtrace_loss refuses
+ * return IMPALA_ERR_BAD_ARG. */
+int impala_vtrace_loss_gauss(const float* cur_params, const float* beh_params, const float* actions,
+                             const float* rewards, const uint8_t* done, const int32_t* lens, const float* v,
+                             float* vs, float* pg_adv, float* dparams, float* dv, double* scalars, void* workspace,
+                             int64_t workspace_bytes, int T, int B, int A, float gamma, float rho_bar, float c_bar,
+                             float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch, int mode,
                              double* diag, const double* popart, int reward_clip, void* stream);
 
 /* Per-group gradient clipping + Adam in one launch (learner.py:176-183).

@@ -44,6 +44,18 @@ def reward_clip_code(reward_clip) -> int:
         raise ValueError(f"reward_clip must be None or one of {sorted(REWARD_CLIPS)}, got {reward_clip!r}")
     return REWARD_CLIPS[reward_clip]
 
+ACT_CATEGORICAL = 0
+ACT_GAUSSIAN = 1
+ACT_DISTS = {"categorical": ACT_CATEGORICAL, "gaussian": ACT_GAUSSIAN}  # action distributions (IMPALA_ACT_*)
+MAX_GAUSSIAN_DIMS = 16  # action dimensions of impala_vtrace_loss_gauss (2A <= 32 policy outputs)
+
+
+def act_kind_code(action_dist: str) -> int:
+    if not isinstance(action_dist, str) or action_dist not in ACT_DISTS:
+        raise ValueError(f"action_dist must be one of {sorted(ACT_DISTS)}, got {action_dist!r}")
+    return ACT_DISTS[action_dist]
+
+
 _ERRORS = {-1: "IMPALA_ERR_BAD_ARG", -2: "IMPALA_ERR_UNSUPPORTED_SHAPE",
            -3: "IMPALA_ERR_WORKSPACE_TOO_SMALL"}
 
@@ -91,6 +103,10 @@ SIGNATURES = {
     "impala_vtrace_loss_diag": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p]),
     "impala_vtrace_loss_popart": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p]),
     "impala_vtrace_loss_rclip": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p]),
+    "impala_vtrace_loss_gauss": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p]),
+    "impala_batch_layout_act": (_i, [_i] * 7 + [C.POINTER(_i64), C.POINTER(_i64)]),
+    "impala_ingest_shard_act": (_i, [_p, _p] + [_i] * 9 + [_p]),
+    "impala_batch_compose_act": (_i, [_p, _p, _i64, _p] + [_i] * 8 + [_p]),
     "impala_clip_adam": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _f, _f, _f, _f, _p, _p]),
     "impala_clip_optim": (_i, [_p, _p, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i, _f, _f, _f, _p, _p]),
     "impala_gather_clip_optim": (_i, [_p] * 4 + [_i64, _i64, _i, _i, _p, _p, _p, _i64, _i64, _f, _p, _i64, _i]
@@ -143,12 +159,20 @@ def param_layout(O: int, H: int, N2: int):
     return list(offs), total.value
 
 
-def batch_layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1):
+def batch_layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1,
+                 action_dist: str = "categorical"):
     """Slab layout for networks of O observation features; frames > 1 stores the O / frames features of
-    each stacked frame once (impala_batch_layout_frames)."""
+    each stacked frame once (impala_batch_layout_frames); action_dist="gaussian" holds (T, B, 2A) behaviour
+    outputs and (T, B, A) float32 actions (impala_batch_layout_act)."""
     offs = (_i64 * 6)()
     total = _i64()
-    if frames == 1:
+    if action_dist != "categorical":
+        if frames < 1 or O % frames:
+            raise ValueError(f"{O} observation features do not split into {frames} frames")
+        check(lib().impala_batch_layout_act(T, B, O // frames, frames, A, obs_dtype_code(obs_dtype),
+                                            act_kind_code(action_dist), offs, C.byref(total)),
+              "impala_batch_layout_act")
+    elif frames == 1:
         check(lib().impala_batch_layout_obs(T, B, O, A, obs_dtype_code(obs_dtype), offs, C.byref(total)),
               "impala_batch_layout_obs")
     else:

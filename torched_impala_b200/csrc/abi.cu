@@ -24,18 +24,21 @@ static int64_t obs_bytes(int obs_dtype) {
     return obs_dtype == IMPALA_OBS_F32 ? 4 : obs_dtype == IMPALA_OBS_U8 ? 1 : 0;
 }
 
-extern "C" int impala_batch_layout_frames(int T, int B, int F, int frames, int A, int obs_dtype, int64_t offsets[6],
-                                          int64_t* total_bytes) {
+static bool act_kind_ok(int act_kind) { return act_kind == IMPALA_ACT_CATEGORICAL || act_kind == IMPALA_ACT_GAUSSIAN; }
+
+extern "C" int impala_batch_layout_act(int T, int B, int F, int frames, int A, int obs_dtype, int act_kind,
+                                       int64_t offsets[6], int64_t* total_bytes) {
     const int64_t ob = obs_bytes(obs_dtype);
-    if (T < 1 || B < 1 || F < 1 || frames < 1 || A < 1 || ob == 0 || !offsets || !total_bytes)
+    if (T < 1 || B < 1 || F < 1 || frames < 1 || A < 1 || ob == 0 || !act_kind_ok(act_kind) || !offsets ||
+        !total_bytes)
         return IMPALA_ERR_BAD_ARG;
     const int64_t al = 256;
     int64_t off = 0;
     const int64_t sizes[6] = {
-        (int64_t)(T + frames) * B * F * ob, // obs frames f32 | u8
-        (int64_t)T * B * A * 4,             // beh_logits f32
-        (int64_t)T * B * 4,                 // actions    i32
-        (int64_t)T * B * 4,                 // rewards    f32
+        (int64_t)(T + frames) * B * F * ob,              // obs frames f32 | u8
+        (int64_t)T * B * impala_beh_width(A, act_kind),  // beh_logits f32 (A | 2A per step)
+        (int64_t)T * B * impala_act_width(A, act_kind),  // actions    i32 | f32 (A per step)
+        (int64_t)T * B * 4,                              // rewards    f32
         (int64_t)T * B,                     // done       u8
         (int64_t)B * 4,                     // lens       i32
     };
@@ -45,6 +48,11 @@ extern "C" int impala_batch_layout_frames(int T, int B, int F, int frames, int A
     }
     *total_bytes = off;
     return IMPALA_OK;
+}
+
+extern "C" int impala_batch_layout_frames(int T, int B, int F, int frames, int A, int obs_dtype, int64_t offsets[6],
+                                          int64_t* total_bytes) {
+    return impala_batch_layout_act(T, B, F, frames, A, obs_dtype, IMPALA_ACT_CATEGORICAL, offsets, total_bytes);
 }
 
 extern "C" int impala_batch_layout_obs(int T, int B, int O, int A, int obs_dtype, int64_t offsets[6],
@@ -66,14 +74,15 @@ extern "C" int impala_ingest(void* dev_slab, const void* host_slab, int64_t byte
 
 // Columns [b0, b0 + B_local) of a host batch slab laid out for B columns -> a device slab laid out
 // for B_local columns: one strided 2-D copy per tensor (rows = time steps or frames), the lens vector 1-D.
-extern "C" int impala_ingest_shard_frames(void* dev_slab, const void* host_slab, int T, int B, int F, int frames, int A,
-                                          int obs_dtype, int b0, int B_local, void* stream) {
+extern "C" int impala_ingest_shard_act(void* dev_slab, const void* host_slab, int T, int B, int F, int frames, int A,
+                                       int obs_dtype, int act_kind, int b0, int B_local, void* stream) {
     if (!dev_slab || !host_slab || b0 < 0 || B_local < 1 || b0 + B_local > B) return IMPALA_ERR_BAD_ARG;
     int64_t ho[6], doff[6], ht, dt;
-    int rc = impala_batch_layout_frames(T, B, F, frames, A, obs_dtype, ho, &ht);
+    int rc = impala_batch_layout_act(T, B, F, frames, A, obs_dtype, act_kind, ho, &ht);
     if (rc != IMPALA_OK) return rc;
-    if ((rc = impala_batch_layout_frames(T, B_local, F, frames, A, obs_dtype, doff, &dt)) != IMPALA_OK) return rc;
-    const int64_t width[5] = {(int64_t)F * obs_bytes(obs_dtype), (int64_t)A * 4, 4, 4, 1};  // bytes per (row, column)
+    if ((rc = impala_batch_layout_act(T, B_local, F, frames, A, obs_dtype, act_kind, doff, &dt)) != IMPALA_OK) return rc;
+    const int64_t width[5] = {(int64_t)F * obs_bytes(obs_dtype), impala_beh_width(A, act_kind),
+                              impala_act_width(A, act_kind), 4, 1};  // bytes per (row, column)
     const int rows[5] = {T + frames, T, T, T, T};
     const char* h = static_cast<const char*>(host_slab);
     char* d = static_cast<char*>(dev_slab);
@@ -86,6 +95,12 @@ extern "C" int impala_ingest_shard_frames(void* dev_slab, const void* host_slab,
     }
     cudaError_t e = cudaMemcpyAsync(d + doff[5], h + ho[5] + (int64_t)b0 * 4, (size_t)B_local * 4, cudaMemcpyHostToDevice, st);
     return e == cudaSuccess ? IMPALA_OK : (int)e;
+}
+
+extern "C" int impala_ingest_shard_frames(void* dev_slab, const void* host_slab, int T, int B, int F, int frames, int A,
+                                          int obs_dtype, int b0, int B_local, void* stream) {
+    return impala_ingest_shard_act(dev_slab, host_slab, T, B, F, frames, A, obs_dtype, IMPALA_ACT_CATEGORICAL, b0,
+                                   B_local, stream);
 }
 
 extern "C" int impala_ingest_shard_obs(void* dev_slab, const void* host_slab, int T, int B, int O, int A,

@@ -64,18 +64,20 @@ __global__ void __launch_bounds__(256) batch_compose_kernel(char* __restrict__ d
 
 }  // namespace
 
-extern "C" int impala_batch_compose(void* dst_slab, const void* store, int64_t store_slab_bytes, const int32_t* plan,
-                                    int T, int B, int Bf, int F, int frames, int A, int obs_dtype, void* stream) {
+extern "C" int impala_batch_compose_act(void* dst_slab, const void* store, int64_t store_slab_bytes,
+                                        const int32_t* plan, int T, int B, int Bf, int F, int frames, int A,
+                                        int obs_dtype, int act_kind, void* stream) {
     if (!dst_slab || !store || !plan || Bf <= 0 || Bf >= B) return IMPALA_ERR_BAD_ARG;
     int64_t so[6], dof[6], st_total, dt_total;
-    int rc = impala_batch_layout_frames(T, Bf, F, frames, A, obs_dtype, so, &st_total);
+    int rc = impala_batch_layout_act(T, Bf, F, frames, A, obs_dtype, act_kind, so, &st_total);
     if (rc != IMPALA_OK) return rc;
-    if ((rc = impala_batch_layout_frames(T, B, F, frames, A, obs_dtype, dof, &dt_total)) != IMPALA_OK) return rc;
+    if ((rc = impala_batch_layout_act(T, B, F, frames, A, obs_dtype, act_kind, dof, &dt_total)) != IMPALA_OK) return rc;
     if (store_slab_bytes < st_total) return IMPALA_ERR_BAD_ARG;
     int sms = 0;
     if (const cudaError_t e = impala_sm_count(&sms); e != cudaSuccess) return (int)e;
 
-    const int64_t width[6] = {(int64_t)F * (obs_dtype == IMPALA_OBS_U8 ? 1 : 4), (int64_t)A * 4, 4, 4, 1, 4};
+    const int64_t width[6] = {(int64_t)F * (obs_dtype == IMPALA_OBS_U8 ? 1 : 4), impala_beh_width(A, act_kind),
+                              impala_act_width(A, act_kind), 4, 1, 4};
     const int64_t rows[6] = {T + frames, T, T, T, T, 1};
     const uintptr_t ptrs = reinterpret_cast<uintptr_t>(dst_slab) | reinterpret_cast<uintptr_t>(store) |
                            (uintptr_t)store_slab_bytes;
@@ -97,4 +99,10 @@ extern "C" int impala_batch_compose(void* dst_slab, const void* store, int64_t s
                                                                  static_cast<const char*>(store), store_slab_bytes,
                                                                  reinterpret_cast<const int2*>(plan), B, Bf, a);
     return impala_launch_status();
+}
+
+extern "C" int impala_batch_compose(void* dst_slab, const void* store, int64_t store_slab_bytes, const int32_t* plan,
+                                    int T, int B, int Bf, int F, int frames, int A, int obs_dtype, void* stream) {
+    return impala_batch_compose_act(dst_slab, store, store_slab_bytes, plan, T, B, Bf, F, frames, A, obs_dtype,
+                                    IMPALA_ACT_CATEGORICAL, stream);
 }

@@ -11,6 +11,14 @@
 
 static inline int64_t impala_round_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 
+// Bytes per (time step, column) of the behaviour record and of the action in a batch slab (IMPALA_ACT_*).
+static inline int64_t impala_beh_width(int A, int act_kind) {
+    return (int64_t)(act_kind == IMPALA_ACT_GAUSSIAN ? 2 * A : A) * 4;
+}
+static inline int64_t impala_act_width(int A, int act_kind) {
+    return act_kind == IMPALA_ACT_GAUSSIAN ? (int64_t)A * 4 : 4;
+}
+
 struct MlpLayout {
     int64_t oW1, ob1, oW2, ob2, total;
 };

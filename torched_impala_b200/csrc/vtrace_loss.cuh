@@ -2,8 +2,9 @@
 // (reference learner.py:116-162 + helpers :298-321 + the non-MLP part of :175).
 //
 // The kernel body and its launcher; vtrace_loss.cu holds the entry points of the plain, diag and PopArt
-// kernels, vtrace_loss_rclip.cu those of the reward-clipping ones (two translation units, so the parallel
-// build compiles the two sets of instantiations side by side).
+// kernels, vtrace_loss_rclip.cu those of the reward-clipping ones and vtrace_loss_gauss.cu those of the
+// diagonal-Gaussian policies (three translation units, so the parallel build compiles the sets of
+// instantiations side by side).
 //
 // Lane = trajectory, warp = time segment (vtrace_lane_kernel below): every tensor of the
 // time-major (T, B[, A]) batch is read and written as fully coalesced row segments straight from /
@@ -187,6 +188,67 @@ __device__ __forceinline__ float row_kl2(const float* __restrict__ pc, const flo
     return kl;
 }
 
+// ---- GAUSS: diagonal Gaussian policies.  A step's policy outputs are [m | s], 2A floats (means, then log
+// standard deviations, sigma = e^s), its action the unsquashed sample, A floats.  VEC (A == AP, 16-byte aligned
+// bases): 128-bit loads and stores (64-bit for the AP = 2 action row); otherwise element accesses, and the
+// entries k >= A are zero, which adds exactly zero to every term below (u = 0, s = 0, sigma ratio 1).
+constexpr float kHalfLog2Pi = 0.9189385332046727f;    // 1/2 log(2 pi)
+constexpr float kHalfLog2PiE = 1.4189385332046727f;   // 1/2 (1 + log(2 pi)): entropy per dimension minus s_k
+template <int AP, bool VEC>
+__device__ __forceinline__ void load_gauss(const float* __restrict__ p, unsigned elem, int A, float (&m)[AP],
+                                           float (&s)[AP]) {
+    if constexpr (VEC) {
+        float z[2 * AP];
+        load_logits<2 * AP, true>(p, elem, 2 * AP, z);
+#pragma unroll
+        for (int k = 0; k < AP; ++k) m[k] = z[k], s[k] = z[AP + k];
+    } else {
+#pragma unroll
+        for (int k = 0; k < AP; ++k) {
+            m[k] = k < A ? __ldg(p + elem * 2 * A + k) : 0.f;
+            s[k] = k < A ? __ldg(p + elem * 2 * A + A + k) : 0.f;
+        }
+    }
+}
+template <int AP, bool VEC>
+__device__ __forceinline__ void store_gauss(float* __restrict__ p, unsigned elem, int A, const float (&dz)[2 * AP]) {
+    if constexpr (VEC) {
+        store_logits<2 * AP, true>(p, elem, 2 * AP, dz);
+    } else {
+#pragma unroll
+        for (int k = 0; k < AP; ++k)
+            if (k < A) p[elem * 2 * A + k] = dz[k], p[elem * 2 * A + A + k] = dz[AP + k];
+    }
+}
+// Step 2 of one Gaussian step, reduced as the three rows load (base 2, like the categorical terms):
+//   *lp2 = log2 pi(a) = log2(e) sum_k [-u_k^2 / 2 - s_k - log(2 pi) / 2],  u_k = (a_k - m_k) / sigma_k
+//   *lr2 = log2 pi(a) - log2 mu(a), summed from the per-dimension differences (the constants cancel)
+//   *kl2 (DIAG) = KL(mu || pi) / ln 2 = log2(e) sum_k [s_k - sb_k + (sigma_b,k^2 + (mb_k - m_k)^2) / (2 sigma_k^2) - 1/2]
+template <int AP, bool VEC, bool DIAG>
+__device__ __forceinline__ void gauss_terms(const float* __restrict__ pc, const float* __restrict__ pb,
+                                            const float* __restrict__ pa, unsigned elem, int A, float* lp2, float* lr2,
+                                            float* kl2) {
+    float m[AP], s[AP], mb[AP], sb[AP], x[AP];
+    load_gauss<AP, VEC>(pc, elem, A, m, s);
+    load_gauss<AP, VEC>(pb, elem, A, mb, sb);
+    load_logits<AP, VEC>(pa, elem, A, x);
+    float q = 0.f, dq = 0.f, ss = 0.f, ds = 0.f, kl = 0.f;
+#pragma unroll
+    for (int k = 0; k < AP; ++k) {
+        const float ic = expf(-s[k]), ib = expf(-sb[k]);  // 1 / sigma, full precision: u^2 reaches ~10
+        const float u = (x[k] - m[k]) * ic, ub = (x[k] - mb[k]) * ib;
+        q = fmaf(u, u, q), dq = fmaf(u - ub, u + ub, dq);  // u^2 - ub^2 per term: no cancellation of the sums
+        ss += s[k], ds += sb[k] - s[k];
+        if constexpr (DIAG) {
+            const float r = ex2f((sb[k] - s[k]) * kLog2e), d = (mb[k] - m[k]) * ic;  // sigma_b / sigma, offset / sigma
+            kl += (s[k] - sb[k]) + 0.5f * (fmaf(r, r, d * d) - 1.f);
+        }
+    }
+    *lp2 = (fmaf(-0.5f, q, -ss) - (float)A * kHalfLog2Pi) * kLog2e;
+    *lr2 = fmaf(-0.5f, dq, ds) * kLog2e;
+    *kl2 = kl * kLog2e;
+}
+
 // POPART: {mu, sigma, 1 / sigma} as float32 in shared memory, read through a volatile pointer at every use so
 // that the three values take no register across the unroll (the DIAG twins are at their register limit).
 struct PopVals {
@@ -233,18 +295,30 @@ struct PopVals {
 // row_lse2 reduced them (row_kl2), non-VEC rows re-read the behaviour row in step 4 next to the current
 // row's re-read (whichever keeps the twin's zero spills); vs and vs - v come from step 4.
 //
+// GAUSS (with WITH_LOSS): the diagonal-Gaussian policy terms in place of the softmax ones; everything else
+// (the recurrence, the segment composition, the reward transform, PopArt and the reductions) is this same code.
+// Like the streaming path no row is held across the chunk: step 2 reduces the current, behaviour and action
+// rows of a step as they load into log2 pi(a), the log2 ratio and (DIAG) KL (gauss_terms); step 4 re-reads the
+// current and action rows (L1 / L2 hits) for the entropy sum_k (s_k + (1 + log 2 pi) / 2) and the 2A gradients
+//   d/dm_k = -policy_loss_c pg (a_k - m_k) / sigma_k^2 / B,   d/ds_k = (policy_loss_c pg (1 - u_k^2) - entropy_c) / B.
+//
 // POPART (with DIAG): v holds the normalized values n; every value row is turned into reward units
 // v = sigma n + mu by one FMA as it is loaded (v[:1] included), so the recurrence, vs and the eight sums are
 // those of the value function sigma n + mu.  The accumulator acc = vs - v enters dv, pg and the two loss
 // sums scaled by 1 / sigma: the loss is that of the normalized targets, 0.5 sum ((v - vs) / sigma)^2, and
 // the advantage pg / sigma.  mu = 0, sigma = 1 leaves every value as it is (FMA with 1 and 0, products by 1).
 // ------------------------------------------------------------------------------------------------
-template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool VEC, bool DIAG, bool POPART = false,
-          bool RCLIP = false>
-__global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<DIAG, POPART, RCLIP> a) {
-    constexpr bool STREAM = AP > 16;
-    constexpr int SR = STREAM ? 1 : S, AR = STREAM ? 1 : AP;  // extent of the held logit rows
+// The body is one device function; vtrace_lane_kernel (softmax policies) and vtrace_gauss_kernel (GAUSS) are its
+// two thin __global__ entries, so the categorical instantiations keep their names and their code.
+template <int AP, int S, bool WITH_LOSS, bool VEC, bool DIAG, bool POPART, bool RCLIP, bool GAUSS>
+__device__ __forceinline__ void vtrace_lane_body(const VtArgsT<DIAG, POPART, RCLIP>& a) {
+    constexpr bool STREAM = !GAUSS && AP > 16;
+    constexpr bool HELD = !STREAM && !GAUSS;  // the logit rows of a chunk are held in registers
+    constexpr int SR = HELD ? S : 1, AR = HELD ? AP : 1;  // extent of the held logit rows
     static_assert(!STREAM || S == 1, "the streaming rows keep one step per thread");
+    static_assert(!GAUSS || (WITH_LOSS && AP <= 16), "Gaussian policies: the loss kernel, up to 16 action dimensions");
+    // GAUSS: the (T, B, A) float32 action samples (the categorical kernels read int32 indices there)
+    const float* const gact = reinterpret_cast<const float*>(a.actions);
     static_assert(!DIAG || WITH_LOSS, "the off-policy sums ride the loss reduction");
     static_assert(!POPART || DIAG, "the value statistics are formed from the DIAG sums");
     static_assert(!RCLIP || WITH_LOSS, "impala_vtrace has no reward transform");
@@ -295,12 +369,12 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
 #pragma unroll
         for (int i = 0; i < S; ++i) {
             const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
-            if constexpr (!STREAM) {
+            if constexpr (HELD) {
                 load_logits<AP, VEC>(a.cur_logits, e, A, R.zc[i]);
                 load_logits<AP, VEC>(a.beh_logits, e, A, R.zb[i]);
             }
             R.r[i] = __ldg(a.rewards + e);
-            R.act[i] = __ldg(a.actions + e);
+            if constexpr (!GAUSS) R.act[i] = __ldg(a.actions + e);
             R.dn[i] = __ldg(a.done + e);
         }
 #pragma unroll
@@ -317,57 +391,68 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
 #pragma unroll
         for (int i = 0; i < S; ++i) {
             const bool valid = tb + i < L;
-            // log-softmax of both logit vectors in the base-2 domain (learner.py:298-303)
-            float z_a, zb_a, lse, lseb;
-            if constexpr (STREAM) {
+            float lr2;  // log2 pi(a) - log2 mu(a)
+            if constexpr (GAUSS) {
                 const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
-                float shb;
-                row_lse2<AP, VEC>(a.cur_logits, e, A, R.act[i], &shc[i], &lsec[i], &z_a);
-                row_lse2<AP, VEC>(a.beh_logits, e, A, R.act[i], &shb, &lseb, &zb_a);
-                lse = lsec[i];
-                if constexpr (DIAG && VEC) {
-                    if (valid) d_kl += row_kl2<AP>(a.cur_logits, a.beh_logits, e, shc[i], lsec[i], shb, lseb);
-                } else if constexpr (DIAG) {
-                    // non-VEC rows: KL in step 4 next to the current row's re-read (row_kl2 here spills); the
-                    // behaviour row's shift and lse2 are parked in the row slots the streaming path leaves unused
-                    R.zb[i][0] = shb, R.zc[i][0] = lseb;
+                float kl2;
+                gauss_terms<AP, VEC, DIAG>(a.cur_logits, a.beh_logits, gact, e, A, &lp2a[i], &lr2, &kl2);
+                if constexpr (DIAG) {
+                    if (valid) d_kl += kl2;
                 }
             } else {
-                float mx = R.zc[i][0], mxb = R.zb[i][0];
-#pragma unroll
-                for (int k = 1; k < AP; ++k)
-                    if (k < A) mx = fmaxf(mx, R.zc[i][k]), mxb = fmaxf(mxb, R.zb[i][k]);
-                float se = 0.f, seb = 0.f, klw = 0.f;  // DIAG: klw = sum_k 2^zb_k (zb_k - zc_k), shifted rows
-                const float mxl = -mx * kLog2e, mxbl = -mxb * kLog2e;
-#pragma unroll
-                for (int k = 0; k < AP; ++k) {
-                    R.zc[i][k] = fmaf(R.zc[i][k], kLog2e, mxl);   // (z - max) log2(e), one rounding
-                    R.zb[i][k] = fmaf(R.zb[i][k], kLog2e, mxbl);
-                    if (k < A) se += ex2f(R.zc[i][k]), seb += ex2f(R.zb[i][k]);
-                    if constexpr (DIAG) {
-                        if (k < A) klw = fmaf(ex2f(R.zb[i][k]), R.zb[i][k] - R.zc[i][k], klw);  // same ex2 as seb's
+                // log-softmax of both logit vectors in the base-2 domain (learner.py:298-303)
+                float z_a, zb_a, lse, lseb;
+                if constexpr (STREAM) {
+                    const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
+                    float shb;
+                    row_lse2<AP, VEC>(a.cur_logits, e, A, R.act[i], &shc[i], &lsec[i], &z_a);
+                    row_lse2<AP, VEC>(a.beh_logits, e, A, R.act[i], &shb, &lseb, &zb_a);
+                    lse = lsec[i];
+                    if constexpr (DIAG && VEC) {
+                        if (valid) d_kl += row_kl2<AP>(a.cur_logits, a.beh_logits, e, shc[i], lsec[i], shb, lseb);
+                    } else if constexpr (DIAG) {
+                        // non-VEC rows: KL in step 4 next to the current row's re-read (row_kl2 here spills); the
+                        // behaviour row's shift and lse2 are parked in the row slots the streaming path leaves unused
+                        R.zb[i][0] = shb, R.zc[i][0] = lseb;
                     }
-                }
-                lse = lg2f(se), lseb = lg2f(seb);
-                if constexpr (DIAG) {
-                    if (valid) d_kl += __fdividef(klw, seb) + (lse - lseb);  // KL(mu || pi) / ln 2
-                }
-                z_a = R.zc[i][0], zb_a = R.zb[i][0];
+                } else {
+                    float mx = R.zc[i][0], mxb = R.zb[i][0];
 #pragma unroll
-                for (int k = 1; k < AP; ++k) {
-                    const bool hit = k == R.act[i];
-                    z_a = selp_f32(hit, R.zc[i][k], z_a), zb_a = selp_f32(hit, R.zb[i][k], zb_a);
-                }
+                    for (int k = 1; k < AP; ++k)
+                        if (k < A) mx = fmaxf(mx, R.zc[i][k]), mxb = fmaxf(mxb, R.zb[i][k]);
+                    float se = 0.f, seb = 0.f, klw = 0.f;  // DIAG: klw = sum_k 2^zb_k (zb_k - zc_k), shifted rows
+                    const float mxl = -mx * kLog2e, mxbl = -mxb * kLog2e;
 #pragma unroll
-                for (int k = 0; k < AP; ++k) R.zc[i][k] -= lse;  // log2 pi(k)
+                    for (int k = 0; k < AP; ++k) {
+                        R.zc[i][k] = fmaf(R.zc[i][k], kLog2e, mxl);   // (z - max) log2(e), one rounding
+                        R.zb[i][k] = fmaf(R.zb[i][k], kLog2e, mxbl);
+                        if (k < A) se += ex2f(R.zc[i][k]), seb += ex2f(R.zb[i][k]);
+                        if constexpr (DIAG) {
+                            if (k < A) klw = fmaf(ex2f(R.zb[i][k]), R.zb[i][k] - R.zc[i][k], klw);  // same ex2 as seb's
+                        }
+                    }
+                    lse = lg2f(se), lseb = lg2f(seb);
+                    if constexpr (DIAG) {
+                        if (valid) d_kl += __fdividef(klw, seb) + (lse - lseb);  // KL(mu || pi) / ln 2
+                    }
+                    z_a = R.zc[i][0], zb_a = R.zb[i][0];
+#pragma unroll
+                    for (int k = 1; k < AP; ++k) {
+                        const bool hit = k == R.act[i];
+                        z_a = selp_f32(hit, R.zc[i][k], z_a), zb_a = selp_f32(hit, R.zb[i][k], zb_a);
+                    }
+#pragma unroll
+                    for (int k = 0; k < AP; ++k) R.zc[i][k] -= lse;  // log2 pi(k)
+                }
+                lp2a[i] = z_a - lse;                                               // log2 pi(a)
+                lr2 = lp2a[i] - (zb_a - lseb);
             }
-            lp2a[i] = z_a - lse;                                               // log2 pi(a)
-            const float ratio = ex2f(lp2a[i] - (zb_a - lseb));                 // :121-123
+            const float ratio = ex2f(lr2);                                     // :121-123
             rho[i] = valid ? fminf(ratio, a.rho_bar) : 0.f;                    // :124
             const float cc = valid ? fminf(ratio, a.c_bar) : 0.f;              // :125
             if constexpr (DIAG) {
                 if (valid) {
-                    d_lr += lp2a[i] - (zb_a - lseb);
+                    d_lr += lr2;
                     d_nrho += ratio > a.rho_bar ? 1.f : 0.f;
                     d_nc += ratio > a.c_bar ? 1.f : 0.f;
                 }
@@ -444,8 +529,24 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
             }
             if constexpr (WITH_LOSS) {
                 // d total / d v = v_loss_c (v - vs) / B = -v_loss_c acc / B  (:149, :306-307)
-                float ent = 0.f, dz[AP];
-                if constexpr (STREAM) {
+                float ent = 0.f, dz[GAUSS ? 2 * AP : AP];
+                if constexpr (GAUSS) {
+                    // re-read the current and action rows: the entropy and the 2A output gradients
+                    float m[AP], s[AP], x[AP];
+                    const unsigned er = (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl;
+                    load_gauss<AP, VEC>(a.cur_logits, er, A, m, s);
+                    load_logits<AP, VEC>(gact, er, A, x);
+                    const float cp = a.policy_loss_c * pg;
+#pragma unroll
+                    for (int k = 0; k < AP; ++k) {
+                        const float iv = ex2f(-2.f * s[k] * kLog2e);  // 1 / sigma^2
+                        const float d = x[k] - m[k], du = d * iv;   // (a - m) / sigma^2
+                        ent += s[k];
+                        dz[k] = valid ? a.inv_batch * (-cp * du) : 0.f;
+                        dz[AP + k] = valid ? a.inv_batch * (cp * fmaf(-d, du, 1.f) - a.entropy_c) : 0.f;
+                    }
+                    ent = fmaf((float)A, kHalfLog2PiE, ent);
+                } else if constexpr (STREAM) {
                     // re-read the row; dz holds log2 pi(k), then the gradient (one row of registers)
                     load_logits<AP, VEC>(a.cur_logits, (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl, A, dz);
 #pragma unroll
@@ -495,7 +596,8 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
                     // POPART: the normalized error (v - vs) / sigma in dv and the value loss
                     a.dv[e] = valid ? -a.v_loss_c * a.inv_batch * (POPART ? acc[i] * pop.inv() : acc[i]) : 0.f;
                     if (t == T - 1) a.dv[e + B] = 0.f;
-                    store_logits<AP, VEC>(a.dlogits, e, A, dz);
+                    if constexpr (GAUSS) store_gauss<AP, VEC>(a.dlogits, e, A, dz);
+                    else store_logits<AP, VEC>(a.dlogits, e, A, dz);
                 }
                 if (valid) {
                     const float err_n = POPART ? acc[i] * pop.inv() : acc[i];
@@ -600,6 +702,16 @@ __global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<D
     if (csize > 1) cluster.sync();  // no CTA leaves while a peer may still read its shared memory
 }
 
+template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool VEC, bool DIAG, bool POPART = false,
+          bool RCLIP = false>
+__global__ void __launch_bounds__(MAXT, MINB) vtrace_lane_kernel(const VtArgsT<DIAG, POPART, RCLIP> a) {
+    vtrace_lane_body<AP, S, WITH_LOSS, VEC, DIAG, POPART, RCLIP, false>(a);
+}
+template <int AP, int S, int MAXT, int MINB, bool VEC, bool DIAG, bool POPART, bool RCLIP>
+__global__ void __launch_bounds__(MAXT, MINB) vtrace_gauss_kernel(const VtArgsT<DIAG, POPART, RCLIP> a) {
+    vtrace_lane_body<AP, S, true, VEC, DIAG, POPART, RCLIP, true>(a);
+}
+
 int pick_ap(int A) {
     if (A <= 2) return 2;
     if (A <= 4) return 4;
@@ -611,11 +723,15 @@ int pick_ap(int A) {
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool DIAG, bool POPART, bool RCLIP>
+template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool DIAG, bool POPART, bool RCLIP, bool GAUSS = false>
 int launch_s(const VtArgsT<DIAG, POPART, RCLIP>& a, bool vec, unsigned groups, int nw, int cl, cudaStream_t st) {
-    const cudaError_t e =
-        vec ? impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, true, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
-            : impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, false, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
+    cudaError_t e;
+    if constexpr (GAUSS)
+        e = vec ? impala_launch_cl(vtrace_gauss_kernel<AP, S, MAXT, MINB, true, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
+                : impala_launch_cl(vtrace_gauss_kernel<AP, S, MAXT, MINB, false, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
+    else
+        e = vec ? impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, true, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
+                : impala_launch_cl(vtrace_lane_kernel<AP, S, MAXT, MINB, WITH_LOSS, false, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
     if (e != cudaSuccess) return (int)e;
     return impala_launch_status();
 }
@@ -628,18 +744,22 @@ constexpr int kMaxCluster = 8;  // portable cluster size
 // over a thread-block cluster (DSMEM carry exchange, cl = 4 / 8) works, but its cluster barriers
 // replace a cheap chunk loop, so cl = 1 unless overridden (scripts/tune_vtrace.py compares them).
 // IMPALA_VTRACE_S / IMPALA_VTRACE_NSEG (warps per CTA) / IMPALA_VTRACE_CLUSTER override the choice.
-template <bool WITH_LOSS, bool DIAG = false, bool POPART = false, bool RCLIP = false>
+// GAUSS: a.A action dimensions (rows of 2A policy outputs), AP = the padded dimension count, at most 16; S = 2 up
+// to AP = 4 and S = 1 from AP = 8 on, where the five rows of two steps in flight would spill (IMPALA_VTRACE_S
+// does not apply).
+constexpr int kMaxGaussA = 16;
+template <bool WITH_LOSS, bool DIAG = false, bool POPART = false, bool RCLIP = false, bool GAUSS = false>
 int launch(VtArgsT<DIAG, POPART, RCLIP>& a, cudaStream_t st) {
     if (a.T < 1 || a.B < 1 || a.A < 1) return IMPALA_ERR_BAD_ARG;
-    const int AP = pick_ap(a.A);
+    const int AP = (GAUSS && a.A > kMaxGaussA) ? 0 : pick_ap(a.A);
     if (!AP) return IMPALA_ERR_UNSUPPORTED_SHAPE;
     // 32-bit element offsets inside the kernel
-    if ((int64_t)(a.T + 1) * a.B * AP >= (int64_t)1 << 31) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    if ((int64_t)(a.T + 1) * a.B * AP * (GAUSS ? 2 : 1) >= (int64_t)1 << 31) return IMPALA_ERR_UNSUPPORTED_SHAPE;
     const unsigned groups = (unsigned)((a.B + 31) / 32);
     const bool vec = a.A == AP && aligned16(a.cur_logits) && aligned16(a.beh_logits) &&
-                     (!WITH_LOSS || aligned16(a.dlogits));
-    int S = AP >= 16 ? 1 : 2;
-    const int s_env = impala_env_int("IMPALA_VTRACE_S", 0);
+                     (!WITH_LOSS || aligned16(a.dlogits)) && (!GAUSS || aligned16(a.actions));
+    int S = AP >= (GAUSS ? 8 : 16) ? 1 : 2;
+    const int s_env = GAUSS ? 0 : impala_env_int("IMPALA_VTRACE_S", 0);
     if (AP <= 4 && (s_env == 1 || s_env == 2 || s_env == 5)) S = s_env;
     const int max_w = S == 5 ? 10 : (AP <= 4 && S == 1 ? kMaxSeg : 16);
     const int nseg = (a.T + S - 1) / S;
@@ -650,6 +770,12 @@ int launch(VtArgsT<DIAG, POPART, RCLIP>& a, cudaStream_t st) {
     if (nw > max_w) nw = max_w;
     const int n_env = impala_env_int("IMPALA_VTRACE_NSEG", 0);
     if (n_env >= 1 && n_env <= max_w) nw = n_env;
+    if constexpr (GAUSS) {
+        if (AP == 2) return launch_s<2, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
+        if (AP == 4) return launch_s<4, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
+        if (AP == 8) return launch_s<8, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
+        return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
+    } else {
 #define VT_AP(APV)                                                                                      \
     if (AP == APV) {                                                                                    \
         if (S == 5) return launch_s<APV, 5, 320, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st); \
@@ -662,6 +788,7 @@ int launch(VtArgsT<DIAG, POPART, RCLIP>& a, cudaStream_t st) {
     if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);
     if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);
     return launch_s<32, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);
+    }
 }
 
 // Per-CTA partial rows: 4 loss sums (plain) or [4 loss sums | 8 off-policy sums] (diag).

@@ -31,6 +31,10 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       transforms every reward where it enters V-trace, so the slabs, the replay store and the transport keep raw
       rewards; the logged batch_mean_reward stays raw, the losses, diagnostics and PopArt statistics are in
       clipped-reward units.  No launch is added.
+    action_dist="gaussian" (continuous actions): A counts action dimensions (at most 16) and the policy has 2A
+      outputs [mean | log std] of a diagonal Gaussian.  The slabs hold the behaviour outputs (T, B, 2A) and the
+      float32 samples (T, B, A) (impala_batch_layout_act); impala_vtrace_loss_gauss takes the V-trace slot of the
+      step with the same flags (diagnostics, PopArt, reward clip) and the same workspace.  No launch is added.
 
 obs_dtype="uint8" (byte observations): the slabs hold obs as uint8 (impala_batch_layout_obs).  For
 O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one after the other as the
@@ -128,7 +132,8 @@ class LearnerEngine:
                  slabs: int = 2, obs_dtype: str = "float32", frames: int = 1, diagnostics: bool = False,
                  replay_slabs: int = 0, replay_columns: int = 0, replay_seed: int = 0,
                  optimizer: str = "adam", optimizer_kwargs: dict | None = None, lr_lambda=None, lr_table=None,
-                 popart: bool = False, popart_beta: float = POPART_BETA, reward_clip: str | None = None):
+                 popart: bool = False, popart_beta: float = POPART_BETA, reward_clip: str | None = None,
+                 action_dist: str = "categorical"):
         # update rule and learning-rate schedule, checked before any device work (optim.optim_config); the
         # default - Adam at 0.95 * hp.lr - keeps impala_clip_adam with the rate as a launch argument
         self.optim = optim_config(hp, optimizer, optimizer_kwargs, lr_lambda, lr_table)
@@ -136,6 +141,13 @@ class LearnerEngine:
         self.popart = bool(popart)
         # reward transform inside the V-trace kernel (IMPALA_REWARD_CLIP_*; 0 = none), checked before device work
         self.reward_clip_code = _cabi.reward_clip_code(reward_clip)
+        # action distribution (IMPALA_ACT_*): the policy has A outputs (categorical) or 2A (Gaussian over A dimensions)
+        self.act_kind = _cabi.act_kind_code(action_dist)
+        self.action_dist = action_dist
+        self.gaussian = self.act_kind == _cabi.ACT_GAUSSIAN
+        if self.gaussian and not 1 <= A <= _cabi.MAX_GAUSSIAN_DIMS:
+            raise ValueError(f"a Gaussian policy takes 1 to {_cabi.MAX_GAUSSIAN_DIMS} action dimensions, got {A}")
+        self.N_pi = 2 * A if self.gaussian else A  # policy outputs
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
@@ -173,7 +185,7 @@ class LearnerEngine:
         self.launches_per_step = 0
 
         # ---- parameter blocks: [policy | value_fn], float32, 128-byte aligned tensors
-        self.pi_off, self.n_pi = _cabi.param_layout(O, H_pi, A)
+        self.pi_off, self.n_pi = _cabi.param_layout(O, H_pi, self.N_pi)
         self.vf_off, self.n_vf = _cabi.param_layout(O, H_v, 1)
         self.n_total = self.n_pi + self.n_vf
         f32 = dict(dtype=torch.float32, device=self.dev)
@@ -198,11 +210,13 @@ class LearnerEngine:
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts (replay: the host slabs
         # hold the B_fresh columns that cross the host link, the device slabs the B columns trained on)
-        train_off, train_bytes = _cabi.batch_layout(T, B_local, O, A, obs_dtype, frames)
+        train_off, train_bytes = _cabi.batch_layout(T, B_local, O, A, obs_dtype, frames, action_dist)
         self.slab_off, self.slab_bytes = train_off, train_bytes
         if self.replay_slabs:
-            self.slab_off, self.slab_bytes = _cabi.batch_layout(T, self.B_fresh, O, A, obs_dtype, frames)
+            self.slab_off, self.slab_bytes = _cabi.batch_layout(T, self.B_fresh, O, A, obs_dtype, frames, action_dist)
         self.fields = ((("obs", np.uint8 if obs_dtype == "uint8" else np.float32),) + _BATCH_FIELDS[1:])
+        if self.gaussian:  # float32 action samples
+            self.fields = self.fields[:2] + (("actions", np.float32),) + self.fields[3:]
         self.n_slabs = slabs
         self.d_slabs = [torch.zeros(train_bytes, dtype=torch.uint8, device=self.dev)
                         for _ in range(slabs)]
@@ -236,14 +250,14 @@ class LearnerEngine:
             self._update_done = [torch.cuda.Event() for _ in range(3)]  # store reads of update u: index u % 3
 
         # ---- activations / gradients of the non-MLP part
-        self.logits = torch.zeros(T, B_local, A, **f32)
+        self.logits = torch.zeros(T, B_local, self.N_pi, **f32)
         self.values = torch.zeros(T + 1, B_local, **f32)
         self.vs = torch.zeros(T + 1, B_local, **f32)
         self.pg_adv = torch.zeros(T, B_local, **f32)
-        self.dlogits = torch.zeros(T, B_local, A, **f32)
+        self.dlogits = torch.zeros(T, B_local, self.N_pi, **f32)
         self.dv = torch.zeros(T + 1, B_local, **f32)
         self.M_pi, self.M_vf = T * B_local, (T + 1) * B_local
-        self.ws_pi_bytes = self._ws_bytes(self.M_pi, O, H_pi, A)
+        self.ws_pi_bytes = self._ws_bytes(self.M_pi, O, H_pi, self.N_pi)
         self.ws_vf_bytes = self._ws_bytes(self.M_vf, O, H_v, 1)
         self.ws_pi = torch.zeros(self.ws_pi_bytes, dtype=torch.uint8, device=self.dev)
         self.ws_vf = torch.zeros(self.ws_vf_bytes, dtype=torch.uint8, device=self.dev)
@@ -327,7 +341,8 @@ class LearnerEngine:
                               "using the NCCL all-reduce between backward and optimizer")
             return
         i64 = dict(dtype=torch.int64, device=self.dev)
-        fused = bool(lib.impala_mlp_backward_pair_push_supported(self.M_pi, self.M_vf, self.O, self.H_pi, self.H_v, self.A))
+        fused = bool(lib.impala_mlp_backward_pair_push_supported(self.M_pi, self.M_vf, self.O, self.H_pi, self.H_v,
+                                                                  self.N_pi))
         if os.environ.get("IMPALA_PUSH_FUSED", "1") == "0":
             fused = False
         self.peer = dict(gather=mine["gather"][0], opened=opened, gather_ptrs=torch.tensor(ptrs["gather"], **i64),
@@ -340,8 +355,8 @@ class LearnerEngine:
     def _shapes(self, B: int) -> dict:
         """Shapes of the six batch tensors in a slab of B columns."""
         T, A = self.T, self.A
-        return {"obs": (T + self.frames, B, self.F), "beh_logits": (T, B, A), "actions": (T, B), "rewards": (T, B),
-                "done": (T, B), "lens": (B,)}
+        return {"obs": (T + self.frames, B, self.F), "beh_logits": (T, B, self.N_pi),
+                "actions": (T, B, A) if self.gaussian else (T, B), "rewards": (T, B), "done": (T, B), "lens": (B,)}
 
     def _ws_bytes(self, M, O, H, N2):
         n = self.lib.impala_mlp_backward_workspace(M, O, H, N2)
@@ -351,8 +366,8 @@ class LearnerEngine:
 
     def _segments(self):
         """(group, key, flat offset, shape) of every parameter tensor in `self.params`."""
-        O, A = self.O, self.A
-        shp_pi = ((self.H_pi, O), (self.H_pi,), (A, self.H_pi), (A,))
+        O, N = self.O, self.N_pi
+        shp_pi = ((self.H_pi, O), (self.H_pi,), (N, self.H_pi), (N,))
         shp_vf = ((self.H_v, O), (self.H_v,), (1, self.H_v), (1,))
         for key, off, shp in zip(PKEYS, self.pi_off, shp_pi):
             yield "policy", key, off, shp
@@ -489,10 +504,16 @@ class LearnerEngine:
         cs = self.copy_stream
         if self._slab_used[slot]:
             cs.wait_event(self.slab_free[slot])
-        _cabi.check(self.lib.impala_ingest_shard_frames(_ptr(self.d_slabs[slot]), C.c_void_p(host_address), self.T,
-                                                        B_total, self.F, self.frames, self.A, self.obs_code, b0,
-                                                        self.B, C.c_void_p(cs.cuda_stream)),
-                    "impala_ingest_shard_frames")
+        if self.gaussian:
+            _cabi.check(self.lib.impala_ingest_shard_act(_ptr(self.d_slabs[slot]), C.c_void_p(host_address), self.T,
+                                                         B_total, self.F, self.frames, self.A, self.obs_code,
+                                                         self.act_kind, b0, self.B, C.c_void_p(cs.cuda_stream)),
+                        "impala_ingest_shard_act")
+        else:
+            _cabi.check(self.lib.impala_ingest_shard_frames(_ptr(self.d_slabs[slot]), C.c_void_p(host_address),
+                                                            self.T, B_total, self.F, self.frames, self.A,
+                                                            self.obs_code, b0, self.B, C.c_void_p(cs.cuda_stream)),
+                        "impala_ingest_shard_frames")
         self.slab_ready[slot].record(cs)
 
     def load_device_batch(self, batch: dict, slot: int = 0) -> None:
@@ -506,8 +527,13 @@ class LearnerEngine:
         lib, hp, st = self.lib, self.hp, C.c_void_p(torch.cuda.current_stream().cuda_stream)
         launched = lib.impala_launch_count()
         d = self.d_views[slot]
-        T, B, O, A = self.T, self.B, self.O, self.A
-        if self.replay_slabs:  # the training slab out of the store, by the plan ingest left in d_plans[slot]
+        T, B, O, A = self.T, self.B, self.O, self.N_pi  # A: the policy's outputs from here on
+        if self.replay_slabs and self.gaussian:
+            _cabi.check(lib.impala_batch_compose_act(_ptr(self.d_slabs[slot]), _ptr(self.store), self.slab_bytes,
+                                                     _ptr(self.d_plans[slot]), T, B, self.B_fresh, self.F, self.frames,
+                                                     self.A, self.obs_code, self.act_kind, st),
+                        "impala_batch_compose_act")
+        elif self.replay_slabs:  # the training slab out of the store, by the plan ingest left in d_plans[slot]
             _cabi.check(lib.impala_batch_compose(_ptr(self.d_slabs[slot]), _ptr(self.store), self.slab_bytes,
                                                  _ptr(self.d_plans[slot]), T, B, self.B_fresh, self.F, self.frames, A,
                                                  self.obs_code, st), "impala_batch_compose")
@@ -544,7 +570,12 @@ class LearnerEngine:
                  _ptr(self.vs), _ptr(self.pg_adv), _ptr(self.dlogits), _ptr(self.dv), scal)
         vt_hp = (T, B, A, float(hp.gamma), float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c),
                  float(hp.policy_loss_c), float(hp.entropy_c), float(self.inv_batch), self.mode, st)
-        if self.reward_clip_code:  # the same kernel as below with the reward transform
+        if self.gaussian:  # the same flags through the Gaussian policy terms; A = action dimensions
+            sums = C.c_void_p(gbase + 8 * (self.n_total + 4)) if self.n_extra == 12 else None
+            _cabi.check(lib.impala_vtrace_loss_gauss(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, T, B, self.A,
+                                                     *vt_hp[3:-1], sums, _ptr(self.popart_buf) if self.popart else None,
+                                                     self.reward_clip_code, st), "impala_vtrace_loss_gauss")
+        elif self.reward_clip_code:  # the same kernel as below with the reward transform
             sums = C.c_void_p(gbase + 8 * (self.n_total + 4)) if self.n_extra == 12 else None
             _cabi.check(lib.impala_vtrace_loss_rclip(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp[:-1], sums,
                                                      _ptr(self.popart_buf) if self.popart else None,

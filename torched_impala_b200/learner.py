@@ -121,24 +121,57 @@ def obs_frames(obs: np.ndarray, k: int, traj=None) -> np.ndarray:
     return np.concatenate([obs[0].reshape(k, F), obs[1:, (k - 1) * F:]], axis=0)
 
 
+def gaussian_steps(traj, L: int, A: int):
+    """A Gaussian trajectory's actions (L, A) and behaviour outputs (L, 2A) as float32.  Raises ValueError, naming
+    the trajectory, for a step of another shape or a non-finite entry: one NaN sample or log std would turn the
+    whole update's gradient into NaN (a categorical index cannot)."""
+    tid = getattr(traj, "id", "?")
+    out = []
+    for name, seq, w in (("action", traj.a, A), ("behaviour [mean | log std]", traj.logits, 2 * A)):
+        rows = [torch.as_tensor(x) for x in seq]
+        bad = next((t for t, x in enumerate(rows) if tuple(x.shape) != (w,)), None)
+        if bad is not None:
+            raise ValueError(f"trajectory {tid}: step {bad} {name} has shape {tuple(rows[bad].shape)}, "
+                             f"a Gaussian policy over {A} dimensions takes ({w},)")
+        v = _np(torch.stack(rows), torch.float32) if rows else np.zeros((0, w), np.float32)
+        if not np.isfinite(v).all():
+            raise ValueError(f"trajectory {tid}: non-finite {name} at step {int(np.argwhere(~np.isfinite(v))[0, 0])}")
+        out.append(v)
+    return out
+
+
+def check_gaussian_block(block: dict, T: int, n: int, A: int) -> None:
+    """put_block's checks of a Gaussian block: (T, n, A) actions and (T, n, 2A) behaviour outputs, all finite."""
+    for name, w in (("actions", A), ("beh_logits", 2 * A)):
+        v = np.asarray(block[name])
+        if v.shape != (T, n, w):
+            raise ValueError(f"Gaussian block {name} of shape {v.shape}; this ring takes {(T, n, w)}")
+        if not np.isfinite(v).all():
+            raise ValueError(f"Gaussian block: non-finite {name} (column {int(np.argwhere(~np.isfinite(v))[0, 1])})")
+
+
 def pack_trajectory(views: dict, b: int, traj, T: int, obs=None) -> float:
     """Write one reference-format trajectory into column `b` of a host batch slab.
 
     Replaces learner.py:104-109,117 (five torch.stack calls + `disc`): float64 -> float32 (or the
     checked uint8 of obs_array for a byte-observation slab), int64 -> int32, bool -> u8, zero padding
     past the trajectory's length.  `obs`: obs_array's result if the caller already has it.  A frame slab
-    (obs (T+k, B, F), k > 1) receives obs_frames' L+k frames.  Returns the trajectory's reward sum
+    (obs (T+k, B, F), k > 1) receives obs_frames' L+k frames.  A Gaussian slab (actions (T, B, A)) takes
+    (A,) actions and (2A,) behaviour outputs per step (gaussian_steps).  Returns the trajectory's reward sum
     (learner.py:108)."""
     L = check_trajectory(traj, T)
+    gauss = views["actions"].ndim == 3
+    if gauss:
+        act, beh = gaussian_steps(traj, L, views["actions"].shape[2])
     obs = obs_array(traj, views["obs"].dtype) if obs is None else obs
     k = views["obs"].shape[0] - T
     if k > 1:
         obs = obs_frames(obs, k, traj)
     views["obs"][:L + k, b] = obs
     views["obs"][L + k:, b] = 0
-    views["beh_logits"][:L, b] = _np(torch.stack(traj.logits), torch.float32)
+    views["beh_logits"][:L, b] = beh if gauss else _np(torch.stack(traj.logits), torch.float32)
     views["beh_logits"][L:, b] = 0
-    views["actions"][:L, b] = _np(torch.stack(traj.a).reshape(L), torch.int32)
+    views["actions"][:L, b] = act if gauss else _np(torch.stack(traj.a).reshape(L), torch.int32)
     views["actions"][L:, b] = 0
     r = torch.stack(traj.r)
     views["rewards"][:L, b] = _np(r, torch.float32)
@@ -150,6 +183,7 @@ def pack_trajectory(views: dict, b: int, traj, T: int, obs=None) -> float:
 
 
 def _dims(policy, value_fn):
+    """(O, policy outputs, H_pi, H_v) of the two modules."""
     sd_p, sd_v = policy.state_dict(), value_fn.state_dict()
     H_pi, O = sd_p[PKEYS[0]].shape
     A = sd_p[PKEYS[2]].shape[0]
@@ -256,8 +290,19 @@ class Learner:
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
                  evaluator=None, obs_dtype="float32", frames=1, diagnostics=False,
                  replay_slabs=0, replay_columns=0, optimizer="adam", optimizer_kwargs=None, lr_lambda=None,
-                 popart=False, popart_beta=POPART_BETA, reward_clip=None):
+                 popart=False, popart_beta=POPART_BETA, reward_clip=None, action_dist="categorical"):
         self.id = id
+        # action distribution: "gaussian" = a diagonal Gaussian policy with 2A outputs [mean | log std]
+        _cabi.act_kind_code(action_dist)
+        self.action_dist = action_dist
+        if action_dist == "gaussian":
+            n_out = _dims(policy, value_fn)[1]
+            if n_out % 2 or not 2 <= n_out <= 2 * _cabi.MAX_GAUSSIAN_DIMS:
+                raise ValueError(f"a Gaussian policy has 2A outputs [mean | log std] for 1 <= A <= "
+                                 f"{_cabi.MAX_GAUSSIAN_DIMS}; this policy has {n_out}")
+        if hasattr(q, "collect_batch") and getattr(q, "action_dist", "categorical") != action_dist:
+            raise ValueError(f"the RingQueue holds {getattr(q, 'action_dist', 'categorical')} actions, "
+                             f"the learner was built for action_dist={action_dist!r}")
         # reward clipping inside the V-trace kernel: checked here, in the launching process
         _cabi.reward_clip_code(reward_clip)
         self.reward_clip = reward_clip
@@ -330,9 +375,9 @@ class Learner:
             # staging ring every rank can DMA its shard from (created before the fork)
             from .ring import RingQueue
 
-            O, A, _, _ = _dims(self.policy, self.value_fn)
-            self._stage_ring = RingQueue(self.hp.max_timesteps, self.hp.batch_size, O, A, slabs=2,
-                                         obs_dtype=self.obs_dtype, frames=self.frames)
+            c = self._cfg()
+            self._stage_ring = RingQueue(self.hp.max_timesteps, self.hp.batch_size, c["O"], c["A"], slabs=2,
+                                         obs_dtype=self.obs_dtype, frames=self.frames, action_dist=self.action_dist)
         self.p.start()
         print(f"[main] Started learner_{self.id} with pid {self.p.pid}")
 
@@ -349,13 +394,15 @@ class Learner:
     # ------------------------------------------------------------------ helpers
     def _cfg(self):
         O, A, H_pi, H_v = _dims(self.policy, self.value_fn)
+        if self.action_dist == "gaussian":
+            A //= 2  # action dimensions; the policy has 2A outputs
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
                     obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics,
                     replay_slabs=self.replay_slabs, replay_columns=self.replay_columns, optimizer=self.optimizer,
                     optimizer_kwargs=self.optimizer_kwargs, popart=self.popart, popart_beta=self.popart_beta,
-                    reward_clip=self.reward_clip)
+                    reward_clip=self.reward_clip, action_dist=self.action_dist)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -369,7 +416,7 @@ class Learner:
                             replay_slabs=c["replay_slabs"], replay_columns=c["replay_columns"],
                             optimizer=c["optimizer"], optimizer_kwargs=c["optimizer_kwargs"],
                             lr_table=self.optim.lr_table, popart=c["popart"], popart_beta=c["popart_beta"],
-                            reward_clip=c["reward_clip"])
+                            reward_clip=c["reward_clip"], action_dist=c["action_dist"])
         eng.load_state(self._init_state(), self._popart_init())
         return eng
 
@@ -418,6 +465,9 @@ class Learner:
         own `utils.test_policy` when this class is deployed inside that repo."""
         if self.evaluator is not None:
             return self.evaluator(policy)
+        if self.action_dist == "gaussian":  # the reference's test_policy refuses continuous environments
+            print(f"[learner_{self.id}] evaluation skipped: a Gaussian policy is evaluated through evaluator= only")
+            return None
         try:
             import utils as ref_utils  # the reference's utils.py, if on sys.path
 

@@ -35,6 +35,29 @@ class MlpPolicy(nn.Module):
         return torch.multinomial(torch.softmax(logits, dim=-1), num_samples=1), logits
 
 
+class GaussianMlpPolicy(nn.Module):
+    """Diagonal Gaussian policy with a state-dependent log-std (Learner(action_dist="gaussian")): the same
+    two-layer MLP with 2 action_dim outputs [mean_0..A-1 | log_std_0..A-1], so the state_dict keys are MlpPolicy's."""
+
+    def __init__(self, obs_dim: int, action_dim: int, hidden_dim: int):
+        super().__init__()
+        self.action_dim = action_dim
+        self.model = _two_layer(obs_dim, hidden_dim, 2 * action_dim)
+
+    def forward(self, x):
+        return self.model(x)
+
+    def select_action(self, obs, deterministic: bool = False):
+        """Returns (action (A,) float64, params (2A,)): the unsquashed sample mean + exp(log_std) eps (the mean when
+        deterministic).  The learner needs the sample itself; clip it to the action space only for env.step."""
+        params = self.forward(obs)
+        mean, log_std = params[..., :self.action_dim], params[..., self.action_dim:]
+        if deterministic:
+            return mean.detach().clone(), params
+        with torch.no_grad():
+            return mean + torch.exp(log_std) * torch.randn_like(mean), params
+
+
 class MlpValueFn(nn.Module):
     def __init__(self, obs_dim: int, hidden_dim: int):
         super().__init__()

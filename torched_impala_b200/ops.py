@@ -134,20 +134,27 @@ def obs_unstack(frames, k: int, out_dtype=None):
 
 
 def batch_compose(store, plan, T: int, B: int, Bf: int, F: int, frames: int, A: int, obs_dtype: str = "float32",
-                  out=None):
+                  out=None, action_dist: str = "categorical"):
     """The B-column training slab (uint8 bytes, _cabi.batch_layout(T, B, ...)) gathered from `store`, a
     (slabs, slab_bytes) uint8 tensor of Bf-column slabs, by `plan` (B, 2) int32 (slab, column), slab < 0 = an
-    empty column (impala_batch_compose).  `out`: a uint8 tensor of the slab's size to write into."""
+    empty column (impala_batch_compose; impala_batch_compose_act for action_dist="gaussian").  `out`: a uint8
+    tensor of the slab's size to write into."""
     _need_cuda(store, plan)
     if store.dtype != torch.uint8 or store.dim() != 2 or plan.dtype != torch.int32 or tuple(plan.shape) != (B, 2):
         raise _cabi.ImpalaCudaError(f"batch_compose takes a (slabs, bytes) uint8 store and a ({B}, 2) int32 plan, got "
                                     f"{tuple(store.shape)} {store.dtype}, {tuple(plan.shape)} {plan.dtype}")
-    _, total = _cabi.batch_layout(T, B, F * frames, A, obs_dtype, frames)
+    _, total = _cabi.batch_layout(T, B, F * frames, A, obs_dtype, frames, action_dist)
     if out is None:
         out = torch.empty(total, dtype=torch.uint8, device=store.device)
     _need_cuda(out)
     if out.dtype != torch.uint8 or out.numel() != total:
         raise _cabi.ImpalaCudaError(f"batch_compose writes a slab of {total} bytes, got {out.numel()} {out.dtype}")
+    if action_dist != "categorical":
+        _cabi.check(_cabi.lib().impala_batch_compose_act(_p(out), _p(store), store.shape[1], _p(plan), T, B, Bf, F,
+                                                         frames, A, _cabi.obs_dtype_code(obs_dtype),
+                                                         _cabi.act_kind_code(action_dist), _st()),
+                    "impala_batch_compose_act")
+        return out
     _cabi.check(_cabi.lib().impala_batch_compose(_p(out), _p(store), store.shape[1], _p(plan), T, B, Bf, F, frames, A,
                                                  _cabi.obs_dtype_code(obs_dtype), _st()), "impala_batch_compose")
     return out
@@ -352,6 +359,46 @@ def vtrace_loss_rclip(cur_logits, beh_logits, actions, rewards, done, lens, v, h
         float(inv_batch), _cabi.MODES[mode], None if diag is None else _p(diag),
         None if popart is None else _p(popart), code, _st()), "impala_vtrace_loss_rclip")
     out = dict(vs=vs, pg_adv=pg, dlogits=dlogits, dv=dv, scalars=scalars)
+    if with_diag:
+        out["diag"] = diag
+    return out
+
+
+def vtrace_loss_gauss(cur_params, beh_params, actions, rewards, done, lens, v, hp, inv_batch, mode="reference",
+                      diagnostics=False, popart=None, reward_clip=None):
+    """The V-trace loss kernel for diagonal Gaussian policies (impala_vtrace_loss_gauss): cur_params / beh_params
+    (T, B, 2A) float32 policy outputs [mean | log std], actions (T, B, A) float32 samples.  Returns vs, pg_adv,
+    dparams (T, B, 2A), dv, scalars and, with diagnostics=True or popart (the statistics tensor), diag."""
+    code = _cabi.reward_clip_code(reward_clip)
+    _need_cuda(cur_params, beh_params, actions, rewards, done, lens, v)
+    if popart is not None:
+        _need_cuda(popart)
+        if popart.dtype != torch.float64 or popart.numel() < 3:
+            raise _cabi.ImpalaCudaError("popart must be a float64 tensor of the statistics (popart_stats)")
+    T, B, A2 = cur_params.shape
+    if A2 % 2 or actions.dtype != torch.float32 or tuple(actions.shape) != (T, B, A2 // 2):
+        raise _cabi.ImpalaCudaError(f"vtrace_loss_gauss takes (T, B, 2A) outputs and (T, B, A) float32 actions, got "
+                                    f"{tuple(cur_params.shape)} and {tuple(actions.shape)} {actions.dtype}")
+    A = A2 // 2
+    with_diag = bool(diagnostics) or popart is not None
+    dev = v.device
+    vs = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    pg = torch.empty(T, B, dtype=torch.float32, device=dev)
+    dparams = torch.empty(T, B, 2 * A, dtype=torch.float32, device=dev)
+    dv = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    scalars = torch.empty(4, dtype=torch.float64, device=dev)
+    diag = torch.empty(8, dtype=torch.float64, device=dev) if with_diag else None
+    lib = _cabi.lib()
+    ws_fn = lib.impala_vtrace_loss_diag_workspace if with_diag else lib.impala_vtrace_loss_workspace
+    ws_bytes = int(ws_fn(T, B, A))
+    ws = torch.zeros(ws_bytes, dtype=torch.uint8, device=dev)
+    _cabi.check(lib.impala_vtrace_loss_gauss(
+        _p(cur_params), _p(beh_params), _p(actions), _p(rewards), _p(done), _p(lens), _p(v), _p(vs),
+        _p(pg), _p(dparams), _p(dv), _p(scalars), _p(ws), ws_bytes, T, B, A, float(hp.gamma),
+        float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c), float(hp.policy_loss_c), float(hp.entropy_c),
+        float(inv_batch), _cabi.MODES[mode], None if diag is None else _p(diag),
+        None if popart is None else _p(popart), code, _st()), "impala_vtrace_loss_gauss")
+    out = dict(vs=vs, pg_adv=pg, dparams=dparams, dv=dv, scalars=scalars)
     if with_diag:
         out["diag"] = diag
     return out

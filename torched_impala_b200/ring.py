@@ -49,15 +49,23 @@ def _pause(t_start: float) -> None:
 _OBS_BYTES = {"float32": 4, "uint8": 1}
 
 
-def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1):
-    """Same 256-byte aligned layout as include/impala_b200.h::impala_batch_layout_frames with F = O / frames
-    (impala_batch_layout_obs at frames = 1; pure python so actor processes do not need the CUDA library)."""
+_ACT_DISTS = ("categorical", "gaussian")
+
+
+def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1,
+            action_dist: str = "categorical"):
+    """Same 256-byte aligned layout as include/impala_b200.h::impala_batch_layout_act with F = O / frames
+    (impala_batch_layout_obs at frames = 1, categorical; pure python so actor processes do not need the CUDA
+    library).  "gaussian": beh_logits (T, B, 2A) f32 and actions (T, B, A) f32 for A action dimensions."""
+    if action_dist not in _ACT_DISTS:
+        raise ValueError(f"action_dist must be one of {list(_ACT_DISTS)}, got {action_dist!r}")
+    g = action_dist == "gaussian"
     if obs_dtype not in _OBS_BYTES:
         raise ValueError(f"obs_dtype must be one of {sorted(_OBS_BYTES)}, got {obs_dtype!r}")
     if frames < 1 or O % frames:
         raise ValueError(f"{O} observation features do not split into {frames} frames")
-    sizes = ((T + frames) * B * (O // frames) * _OBS_BYTES[obs_dtype], T * B * A * 4, T * B * 4, T * B * 4, T * B,
-             B * 4)
+    sizes = ((T + frames) * B * (O // frames) * _OBS_BYTES[obs_dtype], T * B * (2 * A if g else A) * 4,
+             T * B * (A if g else 1) * 4, T * B * 4, T * B, B * 4)
     offs, off = [], 0
     for s in sizes:
         offs.append(off)
@@ -68,17 +76,25 @@ def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: 
 class RingQueue:
     """Drop-in for the `mp.Queue` between actors and learner, backed by shared-memory batch slabs."""
 
-    def __init__(self, T: int, B: int, O: int, A: int, slabs: int = 3, obs_dtype: str = "float32", frames: int = 1):
+    def __init__(self, T: int, B: int, O: int, A: int, slabs: int = 3, obs_dtype: str = "float32", frames: int = 1,
+                 action_dist: str = "categorical"):
         if slabs < 2:
             raise ValueError("need at least two slabs (one filling while one is consumed)")
+        if action_dist == "gaussian" and not 1 <= A <= 16:
+            raise ValueError(f"a Gaussian policy takes 1 to 16 action dimensions, got {A}")
         self.T, self.B, self.O, self.A, self.K = T, B, O, A, slabs
         # "uint8": byte observations (Atari RAM, MinAtar planes), a quarter of the float32 slab bytes
-        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype, frames)
+        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype, frames, action_dist)
+        # "gaussian": A action dimensions; the actors' [mean | log std] (2A) and float32 samples (A) per step
+        self.action_dist = action_dist
+        self.gaussian = action_dist == "gaussian"
         self.obs_dtype = obs_dtype
         # frames > 1: observations are `frames` stacked frames of O / frames features, each frame stored once
         # per column, (T + frames, B, O / frames); the learner rebuilds the stacked rows on the device
         self.frames = frames
         self._fields = (("obs", np.dtype(obs_dtype).type),) + _FIELDS[1:]
+        if self.gaussian:
+            self._fields = self._fields[:2] + (("actions", np.float32),) + self._fields[3:]
         # control block after the slabs: filled u8[K][B] | rsum f64[K][B] | tid i64[K][B] |
         # released i64[K] | next_ticket i64[1]   (8-byte aligned pieces)
         kb = slabs * B
@@ -126,9 +142,10 @@ class RingQueue:
     def views(self, k: int) -> dict:
         """Numpy views of slab k (the six batch tensors, learner layout)."""
         if self._views is None:
-            shapes = {"obs": (self.T + self.frames, self.B, self.O // self.frames), "beh_logits": (self.T, self.B, self.A),
-                      "actions": (self.T, self.B), "rewards": (self.T, self.B), "done": (self.T, self.B),
-                      "lens": (self.B,)}
+            N = 2 * self.A if self.gaussian else self.A
+            shapes = {"obs": (self.T + self.frames, self.B, self.O // self.frames), "beh_logits": (self.T, self.B, N),
+                      "actions": (self.T, self.B, self.A) if self.gaussian else (self.T, self.B),
+                      "rewards": (self.T, self.B), "done": (self.T, self.B), "lens": (self.B,)}
             self._views = []
             for kk in range(self.K):
                 base = kk * self.slab_bytes
@@ -199,6 +216,10 @@ class RingQueue:
         want = (self.T + self.frames, n, self.O // self.frames)
         if self.frames > 1 and tuple(np.shape(block["obs"])) != want:
             raise ValueError(f"obs block of shape {tuple(np.shape(block['obs']))}; this ring takes {want}")
+        if self.gaussian:
+            from .learner import check_gaussian_block
+
+            check_gaussian_block(block, self.T, n, self.A)
         c = self._control()
         end = None if timeout is None else time.monotonic() + timeout
         t_wait = time.monotonic()

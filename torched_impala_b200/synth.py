@@ -135,11 +135,35 @@ def init_params(seed: int, O: int, A: int, H_pi: int, H_v: int | None = None) ->
     }
 
 
+def make_gaussian_batch(seed: int, T: int, B: int, O: int, A: int, ragged: bool = False, params: dict | None = None,
+                        obs_kind: str = "normal", frames: int = 1) -> dict:
+    """A batch of a diagonal Gaussian policy over A action dimensions (action_dist="gaussian"): obs, rewards, done
+    and lens as make_batch(seed, ..., A=1); beh_logits (T, B, 2A) the behaviour outputs [m | s] and actions
+    (T, B, A) float32 samples m + e^s eps.  With `params` (init_params(seed, O, 2A, H) layout) the behaviour is the
+    policy's own output on the (dense) observations, moved 0.1-0.3 per entry (the off-policy lag of an actor);
+    without, m ~ N(0, 1) and s ~ U(-1.5, 0.5).  Padded steps are zero."""
+    b = make_batch(seed, T, B, O, 1, ragged=ragged, obs_kind=obs_kind, frames=frames)
+    rng = np.random.default_rng(seed + 1299709)
+    if params is None:
+        beh = np.concatenate([rng.standard_normal((T, B, A)), rng.uniform(-1.5, 0.5, (T, B, A))], -1)
+    else:
+        x = (stack_frames(b, frames) if frames > 1 else b)["obs"][:-1].astype(np.float64)
+        p = [np.asarray(params["policy"][k], np.float64) for k in ("model.0.weight", "model.0.bias",
+                                                                      "model.3.weight", "model.3.bias")]
+        beh = np.maximum(x @ p[0].T + p[1], 0.0) @ p[2].T + p[3]
+        beh = beh + rng.uniform(0.1, 0.3, beh.shape) * rng.choice([-1.0, 1.0], beh.shape)
+    act = beh[..., :A] + np.exp(beh[..., A:]) * rng.standard_normal((T, B, A))
+    pad = np.arange(T)[:, None] >= b["lens"][None, :]
+    beh[pad], act[pad] = 0.0, 0.0
+    return dict(b, beh_logits=beh.astype(np.float32), actions=act.astype(np.float32))
+
+
 def to_trajectories(batch: dict, torch_dtype=None) -> list:
     """Expand a dense batch into the reference wire format (one Trajectory per b).
 
     Shapes/dtypes follow what actor.py:72-92 appends: obs (O,) f64, a (1,) i64,
-    r () f64, d () bool, logits (A,) f64.
+    r () f64, d () bool, logits (A,) f64.  A Gaussian batch (actions (T, B, A)) gives a (A,) f64 and
+    logits (2A,) f64.
     """
     import torch
 
@@ -148,7 +172,8 @@ def to_trajectories(batch: dict, torch_dtype=None) -> list:
     dt = torch.float64 if torch_dtype is None else torch_dtype
     obs = torch.from_numpy(batch["obs"]).to(dt)
     beh = torch.from_numpy(batch["beh_logits"]).to(dt)
-    act = torch.from_numpy(batch["actions"]).to(torch.int64)
+    gauss = batch["actions"].ndim == 3
+    act = torch.from_numpy(batch["actions"]).to(dt if gauss else torch.int64)
     rew = torch.from_numpy(batch["rewards"]).to(dt)
     don = torch.from_numpy(batch["done"]).to(torch.bool)
     out = []
@@ -156,7 +181,7 @@ def to_trajectories(batch: dict, torch_dtype=None) -> list:
         tr = Trajectory((0, b + 1))
         tr.obs.append(obs[0, b].clone())
         for t in range(L):
-            tr.add(obs[t + 1, b].clone(), act[t, b].reshape(1).clone(), rew[t, b].clone(),
+            tr.add(obs[t + 1, b].clone(), act[t, b].clone() if gauss else act[t, b].reshape(1).clone(), rew[t, b].clone(),
                    don[t, b].clone(), beh[t, b].clone())
         out.append(tr)
     return out
