@@ -204,6 +204,21 @@ int impala_mlp_backward_pair(const float* x, const float* params_pi, const float
                              int64_t workspace_vf_bytes, int M_pi, int M_vf, int O, int H_pi,
                              int H_vf, int A, void* stream);
 
+/* Shared-torso actor-critic: ONE network with N2 = N + 1 outputs [policy | value] on M = (T+1)*B rows,
+ * its outputs split into two buffers so the V-trace kernels read and write them where they do for two
+ * networks.  Head a (the policy) is columns [0, N) of the first M_a = T*B rows, in logits (M_a, N); head b
+ * (the value) is column N of all M rows, in values (M).  The forward does not write rows >= M_a of head a;
+ * the backward reads dz from dlogits (M_a, N) and dv (M), rows >= M_a of head a as 0.  Results are bitwise
+ * equal to impala_mlp_forward / impala_mlp_backward with N2 = N + 1 on the interleaved (M, N + 1) layout.
+ * x_dtype: IMPALA_OBS_F32, or IMPALA_OBS_U8 for byte rows (O > 128 only, as impala_mlp_forward_u8).  The
+ * workspace is sized by impala_mlp_backward_workspace(M, O, H, N + 1).  N < 1, N + 1 > 32, M_a > M, an
+ * unknown x_dtype or a NULL pointer returns IMPALA_ERR_BAD_ARG; shapes as impala_mlp_forward. */
+int impala_mlp_forward_shared(const void* x, int x_dtype, const float* params, float* logits, float* values,
+                              int M_a, int M, int O, int H, int N, void* stream);
+int impala_mlp_backward_shared(const void* x, int x_dtype, const float* params, const float* dlogits,
+                               const float* dv, double* grad, void* workspace, int64_t workspace_bytes, int M_a,
+                               int M, int O, int H, int N, void* stream);
+
 /* V-trace only (learner.py:116-135): from current/behaviour logits, actions,
  * rewards, done, lens and the value estimates v (T+1,B) produce
  * vs (T+1,B) [the reference's `vt` after :131] and pg_adv (T,B).

@@ -24,7 +24,10 @@ before each).
 --compare-reward-clip alternates engines with reward_clip None, "abs_one" and "soft_asymmetric" on the same batch
 (rewards N(0, 5^2), so both transforms act) the same way, and times impala_vtrace_loss against
 impala_vtrace_loss_rclip in both modes alone on the engine's buffers (median of 200 launches each, alternating,
-L2 flushed before each)."""
+L2 flushed before each).
+--compare-shared alternates a two-network engine and a shared-torso engine (shared_torso=True: one hidden layer
+feeding the policy and the value head) on the same batch the same way, and reports both steps' launches.  Byte
+observations for the Atari RAM and MinAtar shapes, as --compare-popart."""
 import argparse
 import os
 import statistics
@@ -70,6 +73,7 @@ ap.add_argument("--compare-diag", action="store_true", help="alternate engines w
 ap.add_argument("--compare-popart", action="store_true", help="alternate engines without / with PopArt")
 ap.add_argument("--compare-replay", action="store_true", help="alternate engines without / with experience replay")
 ap.add_argument("--compare-reward-clip", action="store_true", help="alternate engines without / with reward clipping")
+ap.add_argument("--compare-shared", action="store_true", help="alternate two networks and a shared-torso network")
 ap.add_argument("--replay-slabs", type=int, default=2, help="past fresh batches in the pool of --compare-replay")
 ap.add_argument("--replay-columns", type=int, default=None, help="replayed columns of --compare-replay (default B/2)")
 a = ap.parse_args()
@@ -106,6 +110,11 @@ if a.compare_reward_clip:
             "reward_clip soft_asymmetric": arms["default"]}
     rclip_arm = {name: dict(reward_clip=name.split()[1]) for name in list(arms)[1:]}
     obs_dt = {name: "uint8" if a.config in ("ram", "ram4", "ram8", "minatar", "ram_a6") else "float32" for name in arms}
+shared_arm = {}
+if a.compare_shared:
+    arms = {"two networks": arms["default"], "shared torso": arms["default"]}
+    shared_arm = {"shared torso": dict(shared_torso=True)}
+    obs_dt = {name: "uint8" if a.config in ("ram", "ram4", "ram8", "minatar", "ram_a6") else "float32" for name in arms}
 replay_arm = {}
 if a.compare_replay:
     Br = w["B"] // 2 if a.replay_columns is None else a.replay_columns
@@ -121,10 +130,10 @@ for name, tc in arms.items():
     k = n_frames.get(name, 1)
     eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k,
                         diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}), **popart_arm.get(name, {}),
-                        **rclip_arm.get(name, {}))
+                        **rclip_arm.get(name, {}), **shared_arm.get(name, {}))
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
     byte_obs = (a.compare_obs or ((a.compare_frames or a.compare_replay) and dt == "uint8")
-                or ((a.compare_diag or a.compare_popart or a.compare_reward_clip) and dt == "uint8"))
+                or ((a.compare_diag or a.compare_popart or a.compare_reward_clip or a.compare_shared) and dt == "uint8"))
     if a.compare_replay:
         engines[name] = eng
         continue
@@ -386,3 +395,7 @@ if a.compare_reward_clip:
         m1 = statistics.median(ts[name])
         print(f"{name} overhead {a.config}: {m1 - m0:+.1f} us/step ({100 * (m1 / m0 - 1):+.1f} %), launches "
               f"{engines[name].launches_per_step} against {engines['reward_clip None'].launches_per_step}")
+if a.compare_shared:
+    m0, m1 = statistics.median(ts["two networks"]), statistics.median(ts["shared torso"])
+    print(f"shared torso {a.config}: {m1:.1f} us/step against {m0:.1f} ({m1 - m0:+.1f} us, {100 * (m1 / m0 - 1):+.1f} %), "
+          f"launches {engines['shared torso'].launches_per_step} against {engines['two networks'].launches_per_step}")

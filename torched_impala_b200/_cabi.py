@@ -87,6 +87,8 @@ SIGNATURES = {
     "impala_mlp_backward_workspace": (_i64, [_i, _i, _i, _i]),
     "impala_mlp_backward": (_i, [_p, _p, _p, _p, _p, _i64, _i, _i, _i, _i, _p]),
     "impala_mlp_backward_pair": (_i, [_p] * 8 + [_i64, _p, _i64] + [_i] * 6 + [_p]),
+    "impala_mlp_forward_shared": (_i, [_p, _i, _p, _p, _p] + [_i] * 5 + [_p]),
+    "impala_mlp_backward_shared": (_i, [_p, _i, _p, _p, _p, _p, _p, _i64] + [_i] * 5 + [_p]),
     "impala_peer_alloc": (_i, [_i64, _p, _p]),
     "impala_peer_open": (_i, [_p, _p]),
     "impala_peer_close": (_i, [_p]),

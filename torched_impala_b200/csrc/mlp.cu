@@ -106,7 +106,7 @@ size_t fill_args(MlpArgs* a, const MlpConfig& c, bool bwd, int M, int O, int H, 
     return ((size_t)kRows * c.op + tail) * sizeof(float);
 }
 
-int dispatch(bool bwd, const MlpArgs& a, const MlpConfig& c, size_t smem, cudaStream_t st,
+int dispatch(bool bwd, const MlpSplitArgs& a, const MlpConfig& c, size_t smem, cudaStream_t st,
              int* grid) {
     switch (c.op) {
         case 8: return bwd ? impala_mlp_bwd_op8(a, c, smem, st, grid) : impala_mlp_fwd_op8(a, c, smem, st, grid);
@@ -186,13 +186,14 @@ int route(bool bwd, int M, int O, int H, int N2, bool bytes, bool x_al, bool dou
     return IMPALA_OK;
 }
 
+// out_b != nullptr: split heads (out = head a of M_a rows, out_b = head b; mlp_kernels.cuh split_out)
 int forward(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
-            cudaStream_t st) {
-    if (p.kernel == MlpKernel::Obs) return impala_mlp_fwd_obs(p, x, params, out, M, O, H, N2, st);
-    if (p.kernel != MlpKernel::Fp32) return impala_mlp_fwd_tc(p, x, params, out, M, O, H, N2, st);
-    MlpArgs a{};
+            cudaStream_t st, float* out_b = nullptr, int M_a = 0) {
+    if (p.kernel == MlpKernel::Obs) return impala_mlp_fwd_obs(p, x, params, out, M, O, H, N2, st, out_b, M_a);
+    if (p.kernel != MlpKernel::Fp32) return impala_mlp_fwd_tc(p, x, params, out, M, O, H, N2, st, out_b, M_a);
+    MlpSplitArgs a{};
     const size_t smem = fill_args(&a, p.fp32, false, M, O, H, N2);
-    a.x = x, a.params = params, a.out = out;
+    a.x = x, a.params = params, a.out = out, a.out_b = out_b, a.M_a = M_a;
     int grid = 0;
     return dispatch(false, a, p.fp32, smem, st, &grid);
 }
@@ -201,10 +202,11 @@ int forward(const MlpPlan& p, const float* x, const float* params, float* out, i
 // each summed in float64.
 template <typename XT>
 int backward_obs(const MlpPlan& p, const XT* x, const float* params, const float* dout, double* grad,
-                 void* workspace, int M, int O, int H, int N2, cudaStream_t st) {
+                 void* workspace, int M, int O, int H, int N2, cudaStream_t st, const float* dout_b = nullptr,
+                 int M_a = 0) {
     const ObsBwdLayout L = impala_mlp_obs_bwd_layout(M, O, H, N2);
     char* ws = static_cast<char*>(workspace) + kWsHeader;
-    const int rc = impala_mlp_bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st);
+    const int rc = impala_mlp_bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st, dout_b, M_a);
     if (rc != IMPALA_OK) return rc;
     const MlpLayout lay = impala_make_layout(O, H, N2);
     const int64_t nr = lay.total - lay.ob1;
@@ -216,20 +218,23 @@ int backward_obs(const MlpPlan& p, const XT* x, const float* params, const float
     return impala_launch_status();
 }
 
+// dout_b != nullptr: split heads (dout = head a of M_a rows, dout_b = head b; mlp_kernels.cuh split_dz)
 int backward(const MlpPlan& p, const float* x, const float* params, const float* dout, double* grad, void* workspace,
-             int M, int O, int H, int N2, cudaStream_t st) {
-    if (p.kernel == MlpKernel::Obs) return backward_obs(p, x, params, dout, grad, workspace, M, O, H, N2, st);
+             int M, int O, int H, int N2, cudaStream_t st, const float* dout_b = nullptr, int M_a = 0) {
+    if (p.kernel == MlpKernel::Obs)
+        return backward_obs(p, x, params, dout, grad, workspace, M, O, H, N2, st, dout_b, M_a);
     // workspace = [control words (kWsHeader bytes, zero-filled once by the caller) | partial rows]
     float* ws = reinterpret_cast<float*>(static_cast<char*>(workspace) + kWsHeader);
     if (p.reduce_in_kernel)
-        return impala_mlp_bwd_tc(x, params, dout, ws, grad, static_cast<unsigned int*>(workspace), M, O, H, N2, st);
+        return impala_mlp_bwd_tc(x, params, dout, ws, grad, static_cast<unsigned int*>(workspace), M, O, H, N2, st,
+                                 dout_b, M_a);
     int grid = 0, rc;
     if (p.kernel == MlpKernel::Wide) {
-        rc = impala_mlp_bwd_tcw(p, x, params, dout, ws, M, O, H, N2, st, &grid);
+        rc = impala_mlp_bwd_tcw(p, x, params, dout, ws, M, O, H, N2, st, &grid, dout_b, M_a);
     } else {
-        MlpArgs a{};
+        MlpSplitArgs a{};
         const size_t smem = fill_args(&a, p.fp32, true, M, O, H, N2);
-        a.x = x, a.params = params, a.dout = dout, a.ws = ws;
+        a.x = x, a.params = params, a.dout = dout, a.ws = ws, a.dout_b = dout_b, a.M_a = M_a;
         rc = dispatch(true, a, p.fp32, smem, st, &grid);
     }
     if (rc != IMPALA_OK) return rc;
@@ -275,8 +280,9 @@ cudaError_t impala_resident_ctas(const void* kernel, int threads, size_t smem, i
 }
 
 // Persistent grid = resident CTAs per SM x SM count / slices.
-int impala_mlp_launch(void (*kernel)(MlpArgs), const MlpArgs& a, const MlpConfig& c, size_t smem,
-                      cudaStream_t st, int* grid_out) {
+template <typename Args>
+int launch_persistent(void (*kernel)(Args), const Args& a, const MlpConfig& c, size_t smem, cudaStream_t st,
+                      int* grid_out) {
     int per_sm = 0, sms = 0;
     cudaError_t e;
     if ((e = impala_resident_ctas((const void*)kernel, c.threads, smem, &per_sm)) != cudaSuccess) return (int)e;
@@ -289,6 +295,15 @@ int impala_mlp_launch(void (*kernel)(MlpArgs), const MlpArgs& a, const MlpConfig
     kernel<<<dim3(grid, c.slices), c.threads, smem, st>>>(a);
     *grid_out = grid;
     return impala_launch_status();
+}
+
+int impala_mlp_launch(void (*kernel)(MlpArgs), const MlpArgs& a, const MlpConfig& c, size_t smem,
+                      cudaStream_t st, int* grid_out) {
+    return launch_persistent(kernel, a, c, smem, st, grid_out);
+}
+int impala_mlp_launch(void (*kernel)(MlpSplitArgs), const MlpSplitArgs& a, const MlpConfig& c, size_t smem,
+                      cudaStream_t st, int* grid_out) {
+    return launch_persistent(kernel, a, c, smem, st, grid_out);
 }
 
 extern "C" int impala_mlp_forward(const float* x, const float* params, float* out, int M, int O,
@@ -407,6 +422,48 @@ extern "C" int impala_mlp_backward_pair_push(const float* x, const float* params
         reinterpret_cast<float*>(static_cast<char*>(workspace_vf) + kWsHeader), nullptr, nullptr,
         static_cast<unsigned int*>(workspace_pi), M_pi, M_vf, O, H_pi, H_vf, A, (cudaStream_t)stream, &push, extra,
         n_extra);
+}
+
+// ---- shared-torso network: one MLP with N + 1 outputs [policy | value] over M = (T + 1) B rows, whose
+// outputs (and output gradients) live in two buffers - the policy logits (M_a = T B rows of N) and the
+// values (M rows) - so the V-trace kernel reads and writes them where it does for two networks.
+// Bitwise equal to impala_mlp_forward / impala_mlp_backward with N2 = N + 1 on the interleaved layout.
+namespace {
+
+bool shared_args_ok(int x_dtype, int M_a, int M, int N) {
+    return (x_dtype == IMPALA_OBS_F32 || x_dtype == IMPALA_OBS_U8) && N >= 1 && N + 1 <= 32 && M_a >= 0 && M_a <= M;
+}
+
+}  // namespace
+
+extern "C" int impala_mlp_forward_shared(const void* x, int x_dtype, const float* params, float* logits,
+                                         float* values, int M_a, int M, int O, int H, int N, void* stream) {
+    if (!x || !params || !logits || !values || !shared_args_ok(x_dtype, M_a, M, N)) return IMPALA_ERR_BAD_ARG;
+    const bool bytes = x_dtype == IMPALA_OBS_U8;
+    const cudaStream_t st = (cudaStream_t)stream;
+    MlpPlan p;
+    const int rc = route(false, M, O, H, N + 1, bytes, aligned(x, bytes ? 4 : 16), true, true, 0, &p);
+    if (rc != IMPALA_OK) return rc;
+    if (bytes)
+        return impala_mlp_fwd_obs(p, static_cast<const uint8_t*>(x), params, logits, M, O, H, N + 1, st, values, M_a);
+    return forward(p, static_cast<const float*>(x), params, logits, M, O, H, N + 1, st, values, M_a);
+}
+
+extern "C" int impala_mlp_backward_shared(const void* x, int x_dtype, const float* params, const float* dlogits,
+                                          const float* dv, double* grad, void* workspace, int64_t workspace_bytes,
+                                          int M_a, int M, int O, int H, int N, void* stream) {
+    if (!x || !params || !dlogits || !dv || !grad || !workspace || !shared_args_ok(x_dtype, M_a, M, N))
+        return IMPALA_ERR_BAD_ARG;
+    const bool bytes = x_dtype == IMPALA_OBS_U8;
+    const cudaStream_t st = (cudaStream_t)stream;
+    MlpPlan p;
+    const int rc = route(true, M, O, H, N + 1, bytes, aligned(x, bytes ? 4 : 16), aligned(dlogits, 16) && aligned(dv, 16),
+                         aligned(grad, 16), workspace_bytes, &p);
+    if (rc != IMPALA_OK) return rc;
+    if (bytes)
+        return backward_obs(p, static_cast<const uint8_t*>(x), params, dlogits, grad, workspace, M, O, H, N + 1, st, dv,
+                            M_a);
+    return backward(p, static_cast<const float*>(x), params, dlogits, grad, workspace, M, O, H, N + 1, st, dv, M_a);
 }
 
 // out[i] = x[i] (exact): 4 bytes -> one float4 per thread and iteration when both pointers allow it

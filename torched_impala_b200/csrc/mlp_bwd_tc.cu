@@ -65,6 +65,23 @@ struct BwdTcArgs {
     MlpLayout lay;
 };
 
+// The arguments of the split-head twins (SPLIT kernels): dout is head a, dout_b head b (split_dz).  A
+// struct of its own, so the kernels of the interleaved layout keep their parameter space.
+struct BwdTcSplitArgs : BwdTcArgs {
+    const float* dout_b;
+    int M_a;
+};
+template <bool SPLIT>
+using BwdArgs = std::conditional_t<SPLIT, BwdTcSplitArgs, BwdTcArgs>;
+
+// dz entry (row, n0 + n) of the tile loads: interleaved (M, N2) rows, or the split heads (SPLIT twins).  The dense
+// address is formed as the loads always formed it, row start + n0 + n, so the dense kernels keep their code
+template <bool SPLIT>
+__device__ __forceinline__ float load_dz(const BwdArgs<SPLIT>& a, int row, int n0, int n) {
+    if constexpr (SPLIT) return split_dz(a.dout, a.dout_b, a.M_a, a.N2, row, n0 + n);
+    else return __ldg(a.dout + (size_t)row * a.N2 + n0 + n);
+}
+
 __host__ __device__ constexpr size_t bwd_smem_bytes(int ka, int np) {
     // W1 block hi / lo [KA][128 hidden][128 B] + x hi / lo [KA][RT rows][128 B] + x^T hi / lo
     // [RT / 32 K atoms][32 KA features][128 B] + dz [RT][NPS] + db2 exchange; NP = 32 (layer 2 through
@@ -91,8 +108,8 @@ __device__ __forceinline__ float f4(const float4& v, int e) { return e == 0 ? v.
 // units apart, hit different banks) - and dW2 is formed per tile in chunks of NP / 4 outputs, summed over
 // the quad and kept by lane q for outputs [NP / 4 q, NP / 4 (q + 1)).  dW2 / db1 are accumulated in the
 // first feature half only.
-template <int NP, int KA>
-__device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int cta, const int ncta) {
+template <int NP, int KA, bool SPLIT = false>
+__device__ __forceinline__ uint8_t* bwd_tc_body(const BwdArgs<SPLIT>& a, const int cta, const int ncta) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     constexpr bool X4 = KA == 4;
@@ -147,12 +164,12 @@ __device__ __forceinline__ uint8_t* bwd_tc_body(const BwdTcArgs& a, const int ct
             const int row = tile * RT + tid / NQ, n0 = 4 * (tid % NQ);
 #pragma unroll
             for (int n = 0; n < 4; ++n)
-                z[n] = (tile < a.num_tiles && row < a.M && n0 + n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n0 + n) : 0.f;
+                z[n] = (tile < a.num_tiles && row < a.M && n0 + n < a.N2) ? load_dz<SPLIT>(a, row, n0, n) : 0.f;
         } else {
             const int row = tile * RT + tid;
 #pragma unroll
             for (int n = 0; n < NP; ++n)
-                z[n] = (tid < RT && tile < a.num_tiles && row < a.M && n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
+                z[n] = (tid < RT && tile < a.num_tiles && row < a.M && n < a.N2) ? load_dz<SPLIT>(a, row, 0, n) : 0.f;
         }
     };
     float gb2[NZ];  // db2 = column sums of dout: this thread's dz values, first pass only
@@ -549,8 +566,8 @@ static_assert(kStageBytes % 1024 == 0, "stages stay 1024-byte aligned");
 // the block's entries of partial row r (dW1 rows, db1, dW2 columns; group 0 also db2 and the pads), so
 // that the rows hold every entry exactly once each.  Returns >= 16 KiB of shared memory the caller may
 // use as scratch.
-template <int NP>
-__device__ __forceinline__ uint8_t* bwd_blk_body(const BwdTcArgs& a, const int cta, const int ncta) {
+template <int NP, bool SPLIT = false>
+__device__ __forceinline__ uint8_t* bwd_blk_body(const BwdArgs<SPLIT>& a, const int cta, const int ncta) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     // the warpgroup index broadcast from lane 0: known warp-uniform, so the stage addresses and the
@@ -597,7 +614,7 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdTcArgs& a, const int c
         const int row = tile * kRowsT + lt;
 #pragma unroll
         for (int n = 0; n < NP; ++n)
-            z[n] = (lt < kRowsT && tile < a.num_tiles && row < a.M && n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
+            z[n] = (lt < kRowsT && tile < a.num_tiles && row < a.M && n < a.N2) ? load_dz<SPLIT>(a, row, 0, n) : 0.f;
     };
     float gb2[NP];  // db2 = column sums of dout: this thread's dz values
 #pragma unroll
@@ -911,6 +928,14 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_bwd_tc_kernel(const __grid_co
     grid_depart(a.ctl);
 }
 
+// Its split-head twin (shared-torso networks, NP = 4 only), a kernel of its own name and arguments
+__global__ void __launch_bounds__(kThreads, 1) mlp_bwd_tc_split_kernel(const __grid_constant__ BwdTcSplitArgs a) {
+    uint8_t* scratch = bwd_blk_body<4, true>(a, blockIdx.x, gridDim.x);
+    grid_arrive_and_wait(a.ctl);
+    reduce_rows(a, gridDim.x / (a.H / 64), blockIdx.x, gridDim.x, reinterpret_cast<double*>(scratch));
+    grid_depart(a.ctl);
+}
+
 // Policy and value network of one learner step in ONE launch: CTAs [0, n_pi) take the policy's
 // tiles (partial rows 0 .. n_pi / (H_pi / 64) of its workspace), the rest the value function's.  After
 // the grid barrier every CTA helps reduce both sets of rows (the value function's chunks are dealt from
@@ -948,6 +973,12 @@ __global__ void __launch_bounds__(kThreads) mlp_bwd_tcw_kernel(const __grid_cons
     bwd_tc_body<NP, KA>(a, blockIdx.x, gridDim.x);
 }
 
+// Its split-head twin (shared-torso networks, NP >= 4 only)
+template <int NP, int KA>
+__global__ void __launch_bounds__(kThreads) mlp_bwd_tcw_split_kernel(const __grid_constant__ BwdTcSplitArgs a) {
+    bwd_tc_body<NP, KA, true>(a, blockIdx.x, gridDim.x);
+}
+
 static_assert(kWarps * 64 * sizeof(double) <= 2 * kXAtomBytes, "reduction scratch fits the x stage");
 
 BwdTcArgs make_bwd_args(const float* x, const float* params, const float* dout, float* ws, double* grad,
@@ -975,27 +1006,48 @@ void split_sets(int tiles_a, int tiles_b, int grid, int ga, int gb, int64_t wa, 
     }
 }
 
+// Persistent grid of a Wide plan's backward: resident CTAs, at most one per tile and kMaxParts.
+template <typename Args>
+int launch_tcw(void (*kernel)(Args), const MlpPlan& p, const Args& a, cudaStream_t st, int* nparts) {
+    const size_t smem = bwd_smem_bytes(p.ka, p.np);
+    cudaError_t e;
+    int sms = 0, per_sm = 0;
+    if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
+    if ((e = impala_resident_ctas((const void*)kernel, kThreads, smem, &per_sm)) != cudaSuccess) return (int)e;
+    if (per_sm < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
+    int grid = per_sm * sms;
+    if (grid > a.num_tiles) grid = a.num_tiles;
+    if (grid > kMaxParts) grid = kMaxParts;
+    if ((e = impala_launch(kernel, grid, kThreads, smem, st, true, a)) != cudaSuccess) return (int)e;
+    *nparts = grid;
+    return impala_launch_status();
+}
+
 }  // namespace
 
 // Per-CTA partial gradient rows go to ws (same layout as the FP32 kernel), their float64 sum to
 // grad; ctl = two zeroed control words (see the grid barrier in the kernel).
 int impala_mlp_bwd_tc(const float* x, const float* params, const float* dout, float* ws,
-                      double* grad, unsigned int* ctl, int M, int O, int H, int N2, cudaStream_t st) {
-    const BwdTcArgs a = make_bwd_args(x, params, dout, ws, grad, ctl, M, O, H, N2);
+                      double* grad, unsigned int* ctl, int M, int O, int H, int N2, cudaStream_t st,
+                      const float* dout_b, int M_a) {
+    const BwdTcSplitArgs a{make_bwd_args(x, params, dout, ws, grad, ctl, M, O, H, N2), dout_b, M_a};
     const size_t smem = kBlkSmemBytes;
     cudaError_t e;
     int sms = 0;
     if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
     auto kernel = N2 == 1 ? mlp_bwd_tc_kernel<1> : mlp_bwd_tc_kernel<4>;
+    const void* kfn = dout_b ? (const void*)mlp_bwd_tc_split_kernel : (const void*)kernel;  // split: N2 >= 2
     int per_sm = 0;  // unused: the cooperative launch fails when the grid cannot be resident
-    if ((e = impala_resident_ctas((const void*)kernel, kThreads, smem, &per_sm)) != cudaSuccess) return (int)e;
+    if ((e = impala_resident_ctas(kfn, kThreads, smem, &per_sm)) != cudaSuccess) return (int)e;
     // every hidden block gets the same number of CTAs, no more than there are tiles (= partial rows the
     // workspace holds); grid <= SM count: the grid barrier needs residency
     const int nblk = H / 64;
     int cpg = (sms < kMaxParts ? sms : kMaxParts) / nblk;
     if (cpg > a.num_tiles) cpg = a.num_tiles;
     if (cpg < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    if ((e = impala_launch_ex(kernel, nblk * cpg, kThreads, smem, st, true, true, a)) != cudaSuccess) return (int)e;
+    e = dout_b ? impala_launch_ex(mlp_bwd_tc_split_kernel, nblk * cpg, kThreads, smem, st, true, true, a)
+               : impala_launch_ex(kernel, nblk * cpg, kThreads, smem, st, true, true, static_cast<const BwdTcArgs&>(a));
+    if (e != cudaSuccess) return (int)e;
     return impala_launch_status();
 }
 
@@ -1037,23 +1089,18 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
 // Wide plans: per-CTA float32 partial gradient rows into ws (row stride = layout total); *nparts = rows
 // written.  At four K atoms (GEMM2 in 64-feature halves) the tiles are 32 rows high.
 int impala_mlp_bwd_tcw(const MlpPlan& p, const float* x, const float* params, const float* dout, float* ws, int M,
-                       int O, int H, int N2, cudaStream_t st, int* nparts) {
-    BwdTcArgs a = make_bwd_args(x, params, dout, ws, nullptr, nullptr, M, O, H, N2);
+                       int O, int H, int N2, cudaStream_t st, int* nparts, const float* dout_b, int M_a) {
+    BwdTcSplitArgs a{make_bwd_args(x, params, dout, ws, nullptr, nullptr, M, O, H, N2), dout_b, M_a};
     a.num_tiles = (M + p.rows - 1) / p.rows;
     const int np = p.np;
+    if (dout_b) {  // split heads: N2 >= 2, so np >= 4
+        auto kernel = p.ka == 1   ? (np == 4 ? mlp_bwd_tcw_split_kernel<4, 1> : mlp_bwd_tcw_split_kernel<16, 1>)
+                      : p.ka == 2 ? (np == 4 ? mlp_bwd_tcw_split_kernel<4, 2> : mlp_bwd_tcw_split_kernel<16, 2>)
+                                  : (np == 4 ? mlp_bwd_tcw_split_kernel<4, 4> : mlp_bwd_tcw_split_kernel<32, 4>);
+        return launch_tcw(kernel, p, a, st, nparts);
+    }
     auto kernel = p.ka == 1   ? (np == 1 ? mlp_bwd_tcw_kernel<1, 1> : np == 4 ? mlp_bwd_tcw_kernel<4, 1> : mlp_bwd_tcw_kernel<16, 1>)
                   : p.ka == 2 ? (np == 1 ? mlp_bwd_tcw_kernel<1, 2> : np == 4 ? mlp_bwd_tcw_kernel<4, 2> : mlp_bwd_tcw_kernel<16, 2>)
                               : (np == 1 ? mlp_bwd_tcw_kernel<1, 4> : np == 4 ? mlp_bwd_tcw_kernel<4, 4> : mlp_bwd_tcw_kernel<32, 4>);
-    const size_t smem = bwd_smem_bytes(p.ka, np);
-    cudaError_t e;
-    int sms = 0, per_sm = 0;
-    if ((e = impala_sm_count(&sms)) != cudaSuccess) return (int)e;
-    if ((e = impala_resident_ctas((const void*)kernel, kThreads, smem, &per_sm)) != cudaSuccess) return (int)e;
-    if (per_sm < 1) return IMPALA_ERR_UNSUPPORTED_SHAPE;
-    int grid = per_sm * sms;
-    if (grid > a.num_tiles) grid = a.num_tiles;
-    if (grid > kMaxParts) grid = kMaxParts;
-    if ((e = impala_launch(kernel, grid, kThreads, smem, st, true, a)) != cudaSuccess) return (int)e;
-    *nparts = grid;
-    return impala_launch_status();
+    return launch_tcw(kernel, p, static_cast<const BwdTcArgs&>(a), st, nparts);
 }

@@ -108,8 +108,8 @@ __device__ __forceinline__ void stage_weights(const FwdTcArgs& a, int p, uint8_t
 // The 32-unit slices go to the tensor cores two at a time, as one m64n64 MMA chain into one
 // 32-register accumulator (see `issue`): a tile waits on 4 batches instead of 8, and issues 9 MMAs per
 // batch instead of 18.
-template <int NP, int KA>
-__device__ __forceinline__ void fwd_rs_body(const FwdTcArgs& a, const int cta, const int ncta) {
+template <int NP, int KA, bool SPLIT = false>
+__device__ __forceinline__ void fwd_rs_body(const FwdArgs<SPLIT>& a, const int cta, const int ncta) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     const int HB = a.hb;
@@ -211,15 +211,15 @@ __device__ __forceinline__ void fwd_rs_body(const FwdTcArgs& a, const int cta, c
                 tc::fence_acc(d);
                 slice_epilogue<NP>(d, nc, q, b1s, w2s, p0, p1);
             }
-            write_rows<NP>(a, p, tile, warp, g, q, p0, p1);
+            write_rows<NP, SPLIT>(a, p, tile, warp, g, q, p0, p1);
         }
     }
 }
 
 // x tile staged in shared memory (four K atoms): each warpgroup splits it into its own hi / lo
 // swizzled tiles, and every slice waits for its MMAs before its epilogue.
-template <int NP, int KA>
-__device__ __forceinline__ void fwd_ss_body(const FwdTcArgs& a, const int cta, const int ncta) {
+template <int NP, int KA, bool SPLIT = false>
+__device__ __forceinline__ void fwd_ss_body(const FwdArgs<SPLIT>& a, const int cta, const int ncta) {
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment (SWIZZLE_128B atoms) by OFFSETTING the __shared__ array
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -305,7 +305,7 @@ __device__ __forceinline__ void fwd_ss_body(const FwdTcArgs& a, const int cta, c
                 tc::fence_acc(d);
                 slice_epilogue<NP>(d, nc, q, b1s, w2s, p0, p1);
             }
-            write_rows<NP>(a, p, tile, warp, g, q, p0, p1);
+            write_rows<NP, SPLIT>(a, p, tile, warp, g, q, p0, p1);
         }
     }
 }
@@ -314,6 +314,14 @@ template <int NP, int KA>
 __global__ void __launch_bounds__(kThreads) mlp_fwd_tc_kernel(const __grid_constant__ FwdTcArgs a) {
     if constexpr (x_in_regs(KA)) fwd_rs_body<NP, KA>(a, blockIdx.x, gridDim.x);
     else fwd_ss_body<NP, KA>(a, blockIdx.x, gridDim.x);
+}
+
+// Its split-head twin (shared-torso networks, NP >= 4 only): a kernel of its own name and arguments, so the
+// kernels of the interleaved layout keep theirs
+template <int NP, int KA>
+__global__ void __launch_bounds__(kThreads) mlp_fwd_tc_split_kernel(const __grid_constant__ FwdTcSplitArgs a) {
+    if constexpr (x_in_regs(KA)) fwd_rs_body<NP, KA, true>(a, blockIdx.x, gridDim.x);
+    else fwd_ss_body<NP, KA, true>(a, blockIdx.x, gridDim.x);
 }
 
 // Policy and value network of one learner step in ONE launch: CTAs [0, n_pi) run the policy
@@ -358,19 +366,26 @@ int resident_grid(const void* kernel, size_t smem, int* grid) {
     return IMPALA_OK;
 }
 
-template <int NP, int KA>
-int launch_fwd(const FwdTcArgs& a, cudaStream_t st) {
+template <int NP, int KA, bool SPLIT = false>
+int launch_fwd(const FwdArgs<SPLIT>& a, cudaStream_t st) {
     const size_t smem = fwd_smem_bytes(a.hb, KA, NP);
+    const void* kernel;
+    if constexpr (SPLIT) kernel = (const void*)mlp_fwd_tc_split_kernel<NP, KA>;
+    else kernel = (const void*)mlp_fwd_tc_kernel<NP, KA>;
     int grid = 0;
-    const int rc = resident_grid((const void*)mlp_fwd_tc_kernel<NP, KA>, smem, &grid);
+    const int rc = resident_grid(kernel, smem, &grid);
     if (rc != IMPALA_OK) return rc;
     const int want = (a.num_tiles + kWG - 1) / kWG;
-    mlp_fwd_tc_kernel<NP, KA><<<want < grid ? want : grid, kThreads, smem, st>>>(a);
+    if constexpr (SPLIT) mlp_fwd_tc_split_kernel<NP, KA><<<want < grid ? want : grid, kThreads, smem, st>>>(a);
+    else mlp_fwd_tc_kernel<NP, KA><<<want < grid ? want : grid, kThreads, smem, st>>>(a);
     return impala_launch_status();
 }
 
 template <int KA>
-int launch_fwd_ka(int np, const FwdTcArgs& a, cudaStream_t st) {
+int launch_fwd_ka(int np, const FwdTcSplitArgs& a, cudaStream_t st) {
+    if (a.out_b)  // split heads: N2 >= 2, so np >= 4
+        return np == 4 ? launch_fwd<4, KA, true>(a, st) : np == 16 ? launch_fwd<16, KA, true>(a, st)
+                                                        : launch_fwd<32, KA, true>(a, st);
     return np == 1 ? launch_fwd<1, KA>(a, st) : np == 4 ? launch_fwd<4, KA>(a, st)
                    : np == 16 ? launch_fwd<16, KA>(a, st) : launch_fwd<32, KA>(a, st);
 }
@@ -378,8 +393,8 @@ int launch_fwd_ka(int np, const FwdTcArgs& a, cudaStream_t st) {
 }  // namespace
 
 int impala_mlp_fwd_tc(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
-                      cudaStream_t st) {
-    const FwdTcArgs a = make_fwd_args(x, params, out, M, O, H, N2, p.hb);
+                      cudaStream_t st, float* out_b, int M_a) {
+    const FwdTcSplitArgs a{make_fwd_args(x, params, out, M, O, H, N2, p.hb), out_b, M_a};
     return p.ka == 1 ? launch_fwd_ka<1>(p.np, a, st) : p.ka == 2 ? launch_fwd_ka<2>(p.np, a, st)
                                                      : launch_fwd_ka<4>(p.np, a, st);
 }

@@ -2,6 +2,8 @@
 // layer on the fp32 accumulator of a 32-unit hidden slice, and the pass rule that writes an output row.
 #pragma once
 
+#include <type_traits>
+
 #include "mlp_kernels.cuh"
 
 namespace {
@@ -16,6 +18,15 @@ struct FwdTcArgs {
     int hb;  // hidden units per pass (multiple of 32, <= 256, divides H)
     MlpLayout lay;
 };
+
+// The arguments of the split-head twins (SPLIT kernels): out is head a, out_b head b (split_out).  A
+// struct of its own, so the kernels of the interleaved layout keep their parameter space.
+struct FwdTcSplitArgs : FwdTcArgs {
+    float* out_b;
+    int M_a;
+};
+template <bool SPLIT>
+using FwdArgs = std::conditional_t<SPLIT, FwdTcSplitArgs, FwdTcArgs>;
 
 // W2 rows in shared memory are padded to NP + 4 at NP = 16 and 32: the lanes of a quad read hidden units
 // two apart, and with 64- or 128-byte rows their 16-byte loads would fall into one bank group
@@ -55,9 +66,9 @@ __device__ __forceinline__ void slice_epilogue(const float (&d)[ND], int nc, int
 }
 
 // The quad's four column sets meet (fixed order), lane q == 0 writes (pass 0: b2 + z_0) or adds to
-// what it wrote in the previous pass the two rows of this tile
-template <int NP>
-__device__ __forceinline__ void write_rows(const FwdTcArgs& a, int p, int tile, int warp, int g, int q, float (&p0)[NP],
+// what it wrote in the previous pass the two rows of this tile (SPLIT: at the split-head addresses)
+template <int NP, bool SPLIT = false>
+__device__ __forceinline__ void write_rows(const FwdArgs<SPLIT>& a, int p, int tile, int warp, int g, int q, float (&p0)[NP],
                                            float (&p1)[NP]) {
     const float* __restrict__ b2 = a.params + a.lay.ob2;
 #pragma unroll
@@ -72,10 +83,18 @@ __device__ __forceinline__ void write_rows(const FwdTcArgs& a, int p, int tile, 
         for (int h = 0; h < 2; ++h) {
             const int row = tile * kTileM + 16 * warp + g + 8 * h;
             if (row < a.M) {
-                float* o = a.out + (size_t)row * a.N2;
+                if constexpr (SPLIT) {
 #pragma unroll
-                for (int n = 0; n < NP; ++n)
-                    if (n < a.N2) o[n] = (p == 0 ? __ldg(b2 + n) : o[n]) + (h ? p1[n] : p0[n]);
+                    for (int n = 0; n < NP; ++n) {
+                        float* o = n < a.N2 ? split_out(a.out, a.out_b, a.M_a, a.N2, row, n) : nullptr;
+                        if (o) *o = (p == 0 ? __ldg(b2 + n) : *o) + (h ? p1[n] : p0[n]);
+                    }
+                } else {
+                    float* o = a.out + (size_t)row * a.N2;
+#pragma unroll
+                    for (int n = 0; n < NP; ++n)
+                        if (n < a.N2) o[n] = (p == 0 ? __ldg(b2 + n) : o[n]) + (h ? p1[n] : p0[n]);
+                }
             }
         }
     }

@@ -3,6 +3,8 @@
 // (-DIMPALA_OP=..) and direction (-DIMPALA_BWD=0/1) so the instantiations build in parallel.
 #pragma once
 
+#include <type_traits>
+
 #include "common.cuh"
 
 struct MlpArgs {
@@ -16,6 +18,28 @@ struct MlpArgs {
     MlpLayout lay;
 };
 
+// The arguments of the FP32 split-head twins (SPLIT kernels): out / dout is head a, out_b / dout_b head b (see
+// split_out).  A struct of its own, so the kernels of the interleaved layout keep their parameter space.
+struct MlpSplitArgs : MlpArgs {
+    float* out_b;
+    const float* dout_b;
+    int M_a;
+};
+template <bool SPLIT>
+using MlpArgsT = std::conditional_t<SPLIT, MlpSplitArgs, MlpArgs>;
+
+// Split heads of a shared-torso network (impala_mlp_forward_shared / impala_mlp_backward_shared): the
+// N2 = N + 1 outputs of M rows are head a, columns [0, N) of rows [0, M_a) at `a` (row stride N), and head b,
+// column N of every row at `b` (stride 1).  Rows >= M_a of head a are not written and read as 0.  The
+// kernels take this as a compile-time SPLIT flag, instantiated for N2 >= 2 only; SPLIT = false is the
+// interleaved (M, N2) layout, unchanged.
+__device__ __forceinline__ float* split_out(float* a, float* b, int M_a, int N2, int row, int n) {
+    return n == N2 - 1 ? b + row : row < M_a ? a + (size_t)row * (N2 - 1) + n : nullptr;
+}
+__device__ __forceinline__ float split_dz(const float* a, const float* b, int M_a, int N2, int row, int n) {
+    return n == N2 - 1 ? __ldg(b + row) : row < M_a ? __ldg(a + (size_t)row * (N2 - 1) + n) : 0.f;
+}
+
 struct MlpConfig {
     int jpt, maxt, op, np, threads, slices;
     int ks;  // backward: threads per hidden unit (2 / 4 = the observation features are split over a lane pair / quad)
@@ -28,6 +52,8 @@ constexpr int kMaxParts = 1024;  // upper bound on persistent CTAs (= per-CTA pa
 // Defined in mlp.cu: caches occupancy per (kernel, device, block, smem) and launches a
 // persistent grid of min(tiles, resident CTAs) x slices blocks.
 int impala_mlp_launch(void (*kernel)(MlpArgs), const MlpArgs& a, const MlpConfig& c, size_t smem,
+                      cudaStream_t st, int* grid_out);
+int impala_mlp_launch(void (*kernel)(MlpSplitArgs), const MlpSplitArgs& a, const MlpConfig& c, size_t smem,
                       cudaStream_t st, int* grid_out);
 
 // Which kernels run one MLP call: decided by the route in mlp.cu, carried out by the launchers below.
@@ -48,8 +74,9 @@ struct MlpPlan {
 };
 
 // Tensor-core (wgmma, 3xTF32) forward of the Narrow and Wide plans, defined in mlp_fwd_tc.cu.
+// out_b != nullptr: split heads (out = head a, out_b = head b, see split_out), the SPLIT kernels.
 int impala_mlp_fwd_tc(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
-                      cudaStream_t st);
+                      cudaStream_t st, float* out_b = nullptr, int M_a = 0);
 
 // Policy + value network in one launch (CTA ranges per network); A in 2..4, both nets on Narrow plans.
 int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* params_vf, float* logits,
@@ -57,8 +84,10 @@ int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* 
                            cudaStream_t st);
 
 // Tensor-core backward of a Narrow plan (mlp_bwd_tc.cu): per-CTA partial rows into ws, reduced in-kernel to grad.
+// dout_b != nullptr (here and below): split heads (dout = head a, dout_b = head b, see split_dz).
 int impala_mlp_bwd_tc(const float* x, const float* params, const float* dout, float* ws,
-                      double* grad, unsigned int* ctl, int M, int O, int H, int N2, cudaStream_t st);
+                      double* grad, unsigned int* ctl, int M, int O, int H, int N2, cudaStream_t st,
+                      const float* dout_b = nullptr, int M_a = 0);
 
 int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* params_vf,
                            const float* dlogits, const float* dv, float* ws_pi, float* ws_vf,
@@ -69,14 +98,15 @@ int impala_mlp_bwd_tc_pair(const float* x, const float* params_pi, const float* 
 // Tensor-core backward of a Wide plan (mlp_bwd_tc.cu): *nparts float32 partial rows in ws for
 // reduce_partials_kernel.
 int impala_mlp_bwd_tcw(const MlpPlan& p, const float* x, const float* params, const float* dout, float* ws, int M,
-                       int O, int H, int N2, cudaStream_t st, int* nparts);
+                       int O, int H, int N2, cudaStream_t st, int* nparts, const float* dout_b = nullptr,
+                       int M_a = 0);
 
 // Obs plans (mlp_obs_tc.cu): 128 < O <= 1024, K streamed.  Byte observations (values 0..255) enter the
 // network as they are.
 int impala_mlp_fwd_obs(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
-                       cudaStream_t st);
+                       cudaStream_t st, float* out_b = nullptr, int M_a = 0);
 int impala_mlp_fwd_obs(const MlpPlan& p, const uint8_t* x, const float* params, float* out, int M, int O, int H,
-                       int N2, cudaStream_t st);
+                       int N2, cudaStream_t st, float* out_b = nullptr, int M_a = 0);
 // Backward workspace past the control header: byte offsets of DP^T and of the two sets of float32 partial
 // rows (r1 rows of layout entries [ob1, total), p2 rows of [0, ob1)) for reduce_partials_kernel.
 struct ObsBwdLayout {
@@ -85,14 +115,17 @@ struct ObsBwdLayout {
 };
 ObsBwdLayout impala_mlp_obs_bwd_layout(int M, int O, int H, int N2);
 int impala_mlp_bwd_obs(const MlpPlan& p, const float* x, const float* params, const float* dout, void* ws,
-                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st);
+                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st,
+                       const float* dout_b = nullptr, int M_a = 0);
 int impala_mlp_bwd_obs(const MlpPlan& p, const uint8_t* x, const float* params, const float* dout, void* ws,
-                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st);
+                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st,
+                       const float* dout_b = nullptr, int M_a = 0);
 
-// One per padded observation width / direction, defined in mlp_inst.cu.
+// One per padded observation width / direction, defined in mlp_inst.cu; out_b / dout_b != nullptr selects the
+// split-head twin.
 #define IMPALA_DECL_DISPATCH(OPV)                                                             \
-    int impala_mlp_fwd_op##OPV(const MlpArgs&, const MlpConfig&, size_t, cudaStream_t, int*); \
-    int impala_mlp_bwd_op##OPV(const MlpArgs&, const MlpConfig&, size_t, cudaStream_t, int*);
+    int impala_mlp_fwd_op##OPV(const MlpSplitArgs&, const MlpConfig&, size_t, cudaStream_t, int*); \
+    int impala_mlp_bwd_op##OPV(const MlpSplitArgs&, const MlpConfig&, size_t, cudaStream_t, int*);
 IMPALA_DECL_DISPATCH(8)
 IMPALA_DECL_DISPATCH(24)
 IMPALA_DECL_DISPATCH(32)
@@ -170,8 +203,9 @@ __device__ __forceinline__ void bfly_step(float (&vals)[32], int lane) {
 
 // The wide-shape instantiations ask for one resident CTA per SM: without it ptxas caps the OP = 64,
 // NP = 32 kernel at 128 registers and spills.
-template <int JPT, int OP, int NP, int MAXT>
-__global__ void __launch_bounds__(MAXT, (OP == 128 || NP == 32) ? 1 : 0) mlp_fwd_kernel(MlpArgs a) {
+// SPLIT: the split-head twin (shared-torso networks, NP >= 4 only)
+template <int JPT, int OP, int NP, int MAXT, bool SPLIT = false>
+__global__ void __launch_bounds__(MAXT, (OP == 128 || NP == 32) ? 1 : 0) mlp_fwd_kernel(MlpArgsT<SPLIT> a) {
     static_assert(kGroup * NP == 32 || NP != 4, "butterfly chunk must be 32 values");
     // the instantiations of the wide shapes (O > 64 or N2 > 16) keep the butterfly in registers
     constexpr bool kSelp = OP == 128 || NP == 32;
@@ -274,7 +308,11 @@ __global__ void __launch_bounds__(MAXT, (OP == 128 || NP == 32) ? 1 : 0) mlp_fwd
             if (n < a.N2 && row < a.M) {
                 float s = __ldg(b2 + n);
                 for (int ww = 0; ww < nwarps; ++ww) s += part[ww * (kRows * NP) + idx];
-                a.out[(size_t)row * a.N2 + n] = s;
+                if constexpr (SPLIT) {
+                    if (float* o = split_out(a.out, a.out_b, a.M_a, a.N2, row, n)) *o = s;
+                } else {
+                    a.out[(size_t)row * a.N2 + n] = s;
+                }
             }
         }
     }
@@ -296,8 +334,8 @@ __device__ __forceinline__ void zero_range(float* p, int64_t lo, int64_t hi) {
 // four broadcast loads of a row hit four different bank groups.
 // NP = 32 (and NP = 16 at KS = 4): the W2 column of a unit and its gradient are split over the KS lanes
 // as well (NP / KS outputs per lane); the partial dh of the lanes meet through log2(KS) shuffles per row.
-template <int JPT, int OP, int NP, int MAXT, int KS = 1>
-__global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgs a) {
+template <int JPT, int OP, int NP, int MAXT, int KS = 1, bool SPLIT = false>
+__global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgsT<SPLIT> a) {
     extern __shared__ __align__(16) float smem[];
     constexpr int OPH = OP / KS;  // features held by this thread
     constexpr bool SPLITN = NP > 16 || (KS == 4 && NP == 16);
@@ -344,7 +382,10 @@ __global__ void __launch_bounds__(MAXT) mlp_bwd_kernel(MlpArgs a) {
         for (int idx = tid; idx < kRows * NP; idx += nt) {
             const int r = idx / NP, n = idx - r * NP;
             const int row = row0 + r;
-            dzs[idx] = (row < a.M && n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
+            if constexpr (SPLIT)
+                dzs[idx] = (row < a.M && n < a.N2) ? split_dz(a.dout, a.dout_b, a.M_a, a.N2, row, n) : 0.f;
+            else
+                dzs[idx] = (row < a.M && n < a.N2) ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
         }
         __syncthreads();
 #pragma unroll 1

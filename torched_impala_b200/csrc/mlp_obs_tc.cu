@@ -254,6 +254,38 @@ __global__ void __launch_bounds__(kT) mlp_fwd_obs_kernel(const __grid_constant__
     }
 }
 
+// Its split-head twin (shared-torso networks, NP >= 4 only): the same body with the split-head write_rows, as a
+// kernel of its own name and arguments.  The body is repeated, not shared through a device function: with the
+// body in one, ptxas scheduled the dense kernel differently (other registers and instruction order).
+template <int NP, typename XT>
+__global__ void __launch_bounds__(kT) mlp_fwd_obs_split_kernel(const __grid_constant__ FwdTcSplitArgs a,
+                                                               const XT* __restrict__ x) {
+    constexpr int NPS = w2s_stride(NP);
+    uint8_t* stage = aligned_smem();
+    float* b1s = reinterpret_cast<float*>(stage + kStageBytes);  // [64]
+    float* w2s = b1s + kHBlk;                                     // [64][NPS]
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
+    const int tile = blockIdx.x;
+    const Mat<XT> X{x, a.O, a.M};
+    const Mat<float> W1{a.params + a.lay.oW1, a.O, a.H};
+    for (int p = 0; p < a.H / kHBlk; ++p) {
+        __syncthreads();  // the previous pass's epilogue is done with b1s / w2s
+        for (int j = tid; j < kHBlk; j += kT) b1s[j] = __ldg(a.params + a.lay.ob1 + p * kHBlk + j);
+        for (int idx = tid; idx < kHBlk * NP; idx += kT) {
+            const int j = idx / NP, n = idx - j * NP;
+            w2s[j * NPS + n] = n < a.N2 ? __ldg(a.params + a.lay.oW2 + (size_t)n * a.H + p * kHBlk + j) : 0.f;
+        }
+        float run[2][16] = {};
+        kstream<false>(X, tile * kTileM, W1, p * kHBlk, 0, 0, a.O, stage, run);
+        float p0[NP], p1[NP];
+#pragma unroll
+        for (int n = 0; n < NP; ++n) p0[n] = 0.f, p1[n] = 0.f;
+        slice_epilogue<NP>(run[0], 0, q, b1s, w2s, p0, p1);
+        slice_epilogue<NP>(run[1], 1, q, b1s, w2s, p0, p1);
+        write_rows<NP, true>(a, p, tile, warp, g, q, p0, p1);
+    }
+}
+
 // ------------------------------------------------------------------ backward
 struct ObsBwdArgs {
     const void* x;  // float or uint8_t rows (the kernels' XT)
@@ -264,6 +296,8 @@ struct ObsBwdArgs {
     float* ws_w;    // partial rows [p2][lay.ob1]: entries [0, ob1) (dW1, pads)
     int M, O, H, N2, num_tiles, mp, r1, p2;
     MlpLayout lay;
+    const float* dout_b;  // SPLIT kernels: dout is head a, dout_b head b (split_dz)
+    int M_a;
 };
 
 // Backward 1: CTA (r, blk) recomputes PRE of hidden block blk for tiles r, r + r1, ... and runs the
@@ -271,8 +305,8 @@ struct ObsBwdArgs {
 // block, 16 batch rows): h = relu(PRE + b1), dh = W2^T dz, dW2 += dz h, DP = PRE + b1 > 0 ? dh : 0,
 // db1 += DP; DP goes to DP^T.  dW2 / db1 of the block (and db2 and the pads: blk 0) go to partial row r.
 // NP = 32: dW2 in chunks of 8 outputs that the quad sums and lane q keeps (as bwd_tc_body).
-template <int NP, typename XT>
-__global__ void __launch_bounds__(kT) mlp_bwd_obs_pre_kernel(const __grid_constant__ ObsBwdArgs a) {
+template <int NP, typename XT, bool SPLIT = false>
+__device__ __forceinline__ void bwd_obs_pre_body(const ObsBwdArgs& a) {
     constexpr bool L2S = NP > 4;
     constexpr int NPS = w2s_stride(NP);
     uint8_t* stage = aligned_smem();
@@ -311,7 +345,9 @@ __global__ void __launch_bounds__(kT) mlp_bwd_obs_pre_kernel(const __grid_consta
         __syncthreads();  // the previous tile's epilogue is done with dzs
         for (int idx = tid; idx < kTileM * NP; idx += kT) {
             const int m = idx / NP, n = idx - m * NP, row = tile * kTileM + m;
-            const float z = row < a.M && n < a.N2 ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
+            float z;
+            if constexpr (SPLIT) z = row < a.M && n < a.N2 ? split_dz(a.dout, a.dout_b, a.M_a, a.N2, row, n) : 0.f;
+            else z = row < a.M && n < a.N2 ? __ldg(a.dout + (size_t)row * a.N2 + n) : 0.f;
             dzs[m * NPS + n] = z;
             gb2 += z;
         }
@@ -439,6 +475,17 @@ __global__ void __launch_bounds__(kT) mlp_bwd_obs_pre_kernel(const __grid_consta
     }
 }
 
+template <int NP, typename XT>
+__global__ void __launch_bounds__(kT) mlp_bwd_obs_pre_kernel(const __grid_constant__ ObsBwdArgs a) {
+    bwd_obs_pre_body<NP, XT>(a);
+}
+
+// Its split-head twin (shared-torso networks, NP >= 4 only)
+template <int NP, typename XT>
+__global__ void __launch_bounds__(kT) mlp_bwd_obs_pre_split_kernel(const __grid_constant__ ObsBwdArgs a) {
+    bwd_obs_pre_body<NP, XT, true>(a);
+}
+
 // Backward 2: CTA (r, fb, hb) forms dW1 of hidden block hb x feature block fb over the batch-row chunks
 // [r nc / p2, (r + 1) nc / p2) (nc = mp / 32) and writes it (and, CTA (r, 0, 0), the W1 pads) to
 // partial row r.
@@ -486,24 +533,28 @@ int launch(void (*kernel)(KArgs...), dim3 grid, size_t smem, cudaStream_t st, Ar
 
 template <typename XT>
 int fwd_obs(const MlpPlan& p, const XT* x, const float* params, float* out, int M, int O, int H, int N2,
-            cudaStream_t st) {
-    FwdTcArgs a{};
+            cudaStream_t st, float* out_b, int M_a) {
+    FwdTcSplitArgs a{};
     a.x = sizeof(XT) == 4 ? reinterpret_cast<const float*>(x) : nullptr, a.params = params, a.out = out;
     a.M = M, a.O = O, a.H = H, a.N2 = N2;
     a.num_tiles = (M + kTileM - 1) / kTileM;
     a.hb = kHBlk;
     a.lay = impala_make_layout(O, H, N2);
+    a.out_b = out_b, a.M_a = M_a;
     const dim3 grid(a.num_tiles);
+    if (out_b)  // split heads: N2 >= 2, so np >= 4
+        return p.np == 4 ? launch(mlp_fwd_obs_split_kernel<4, XT>, grid, kFwdSmem(4), st, a, x)
+                         : launch(mlp_fwd_obs_split_kernel<32, XT>, grid, kFwdSmem(32), st, a, x);
     switch (p.np) {
-        case 1: return launch(mlp_fwd_obs_kernel<1, XT>, grid, kFwdSmem(1), st, a, x);
-        case 4: return launch(mlp_fwd_obs_kernel<4, XT>, grid, kFwdSmem(4), st, a, x);
-        default: return launch(mlp_fwd_obs_kernel<32, XT>, grid, kFwdSmem(32), st, a, x);
+        case 1: return launch(mlp_fwd_obs_kernel<1, XT>, grid, kFwdSmem(1), st, static_cast<const FwdTcArgs&>(a), x);
+        case 4: return launch(mlp_fwd_obs_kernel<4, XT>, grid, kFwdSmem(4), st, static_cast<const FwdTcArgs&>(a), x);
+        default: return launch(mlp_fwd_obs_kernel<32, XT>, grid, kFwdSmem(32), st, static_cast<const FwdTcArgs&>(a), x);
     }
 }
 
 template <typename XT>
 int bwd_obs(const MlpPlan& p, const XT* x, const float* params, const float* dout, void* ws, const ObsBwdLayout& L,
-            int M, int O, int H, int N2, cudaStream_t st) {
+            int M, int O, int H, int N2, cudaStream_t st, const float* dout_b, int M_a) {
     ObsBwdArgs a{};
     a.x = x, a.params = params, a.dout = dout;
     a.dpt = reinterpret_cast<float*>(static_cast<char*>(ws) + L.dpt_off);
@@ -513,9 +564,13 @@ int bwd_obs(const MlpPlan& p, const XT* x, const float* params, const float* dou
     a.num_tiles = (M + kTileM - 1) / kTileM;
     a.mp = L.mp, a.r1 = L.r1, a.p2 = L.p2;
     a.lay = impala_make_layout(O, H, N2);
+    a.dout_b = dout_b, a.M_a = M_a;
     const dim3 g1(L.r1, H / kHBlk);
     int rc;
-    switch (p.np) {
+    if (dout_b)  // split heads: N2 >= 2, so np >= 4
+        rc = p.np == 4 ? launch(mlp_bwd_obs_pre_split_kernel<4, XT>, g1, kPreSmem(4), st, a)
+                       : launch(mlp_bwd_obs_pre_split_kernel<32, XT>, g1, kPreSmem(32), st, a);
+    else switch (p.np) {
         case 1: rc = launch(mlp_bwd_obs_pre_kernel<1, XT>, g1, kPreSmem(1), st, a); break;
         case 4: rc = launch(mlp_bwd_obs_pre_kernel<4, XT>, g1, kPreSmem(4), st, a); break;
         default: rc = launch(mlp_bwd_obs_pre_kernel<32, XT>, g1, kPreSmem(32), st, a); break;
@@ -527,12 +582,12 @@ int bwd_obs(const MlpPlan& p, const XT* x, const float* params, const float* dou
 }  // namespace
 
 int impala_mlp_fwd_obs(const MlpPlan& p, const float* x, const float* params, float* out, int M, int O, int H, int N2,
-                       cudaStream_t st) {
-    return fwd_obs(p, x, params, out, M, O, H, N2, st);
+                       cudaStream_t st, float* out_b, int M_a) {
+    return fwd_obs(p, x, params, out, M, O, H, N2, st, out_b, M_a);
 }
 int impala_mlp_fwd_obs(const MlpPlan& p, const uint8_t* x, const float* params, float* out, int M, int O, int H,
-                       int N2, cudaStream_t st) {
-    return fwd_obs(p, x, params, out, M, O, H, N2, st);
+                       int N2, cudaStream_t st, float* out_b, int M_a) {
+    return fwd_obs(p, x, params, out, M, O, H, N2, st, out_b, M_a);
 }
 
 // Workspace past the control header: DP^T [H][mp] | r1 partial rows of [ob1, total) | p2 partial rows of
@@ -555,10 +610,12 @@ ObsBwdLayout impala_mlp_obs_bwd_layout(int M, int O, int H, int N2) {
 }
 
 int impala_mlp_bwd_obs(const MlpPlan& p, const float* x, const float* params, const float* dout, void* ws,
-                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st) {
-    return bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st);
+                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st, const float* dout_b,
+                       int M_a) {
+    return bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st, dout_b, M_a);
 }
 int impala_mlp_bwd_obs(const MlpPlan& p, const uint8_t* x, const float* params, const float* dout, void* ws,
-                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st) {
-    return bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st);
+                       const ObsBwdLayout& L, int M, int O, int H, int N2, cudaStream_t st, const float* dout_b,
+                       int M_a) {
+    return bwd_obs(p, x, params, dout, ws, L, M, O, H, N2, st, dout_b, M_a);
 }

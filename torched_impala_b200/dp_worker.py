@@ -40,7 +40,8 @@ def main():
                             diagnostics=c.get("diagnostics", False), optimizer=c.get("optimizer", "adam"),
                             optimizer_kwargs=c.get("optimizer_kwargs"), lr_table=lr_table,
                             popart=c.get("popart", False), popart_beta=c.get("popart_beta", 3e-4),
-                            reward_clip=c.get("reward_clip"), action_dist=c.get("action_dist", "categorical"))
+                            reward_clip=c.get("reward_clip"), action_dist=c.get("action_dist", "categorical"),
+                            shared_torso=c.get("shared_torso", False))
         popart = state.pop("popart", None)  # rank 0's statistics: every rank starts identical
         eng.load_state(state, {k: float(v) for k, v in popart.items()} if popart else None)
         shm = dp.attach_untracked(spec["slab_shm"])

@@ -31,6 +31,14 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       transforms every reward where it enters V-trace, so the slabs, the replay store and the transport keep raw
       rewards; the logged batch_mean_reward stays raw, the losses, diagnostics and PopArt statistics are in
       clipped-reward units.  No launch is added.
+    shared_torso=True (shared-torso actor-critic): ONE network with N + 1 outputs [policy | value] in one parameter
+      block in place of the two: impala_mlp_forward_shared / impala_mlp_backward_shared replace the pair entry
+      points (and the u8 calls), writing and reading the same logits / values / dlogits / dv buffers, so every
+      V-trace launch above runs unchanged.  One clip norm over the whole block (the optimizer's value range is all
+      of it, its policy range empty; the norm is logged as norm_policy and norm_value is 0), and PopArt's value
+      head is row N of W2 and b2[N].  Data-parallel steps push the
+      flat gradient with impala_peer_push.  launches_per_step counts the kernels this route takes (a Wide-plan
+      backward adds its reduction launch, where the two networks' paired Narrow backward had none).
     action_dist="gaussian" (continuous actions): A counts action dimensions (at most 16) and the policy has 2A
       outputs [mean | log std] of a diagonal Gaussian.  The slabs hold the behaviour outputs (T, B, 2A) and the
       float32 samples (T, B, A) (impala_batch_layout_act); impala_vtrace_loss_gauss takes the V-trace slot of the
@@ -110,6 +118,18 @@ def popart_sigma(mu: float, nu: float) -> float:
     return min(max(max(nu - mu * mu, 0.0) ** 0.5, 1e-4), 1e6)
 
 
+def check_shared_torso(shared_torso: bool, H_pi: int, H_v: int, n_policy: int) -> bool:
+    """The shared-torso setting, checked before any device work: one hidden layer of H_pi == H_v units and
+    n_policy + 1 <= 32 outputs (categorical A <= 31, Gaussian A <= 15)."""
+    if not shared_torso:
+        return False
+    if H_pi != H_v:
+        raise ValueError(f"a shared torso has one hidden layer: H_pi ({H_pi}) must equal H_v ({H_v})")
+    if n_policy + 1 > 32:
+        raise ValueError(f"a shared torso takes at most 31 policy outputs (+ 1 value), got {n_policy}")
+    return True
+
+
 def _ptr(t: torch.Tensor) -> C.c_void_p:
     return C.c_void_p(t.data_ptr())
 
@@ -133,7 +153,7 @@ class LearnerEngine:
                  replay_slabs: int = 0, replay_columns: int = 0, replay_seed: int = 0,
                  optimizer: str = "adam", optimizer_kwargs: dict | None = None, lr_lambda=None, lr_table=None,
                  popart: bool = False, popart_beta: float = POPART_BETA, reward_clip: str | None = None,
-                 action_dist: str = "categorical"):
+                 action_dist: str = "categorical", shared_torso: bool = False):
         # update rule and learning-rate schedule, checked before any device work (optim.optim_config); the
         # default - Adam at 0.95 * hp.lr - keeps impala_clip_adam with the rate as a launch argument
         self.optim = optim_config(hp, optimizer, optimizer_kwargs, lr_lambda, lr_table)
@@ -148,6 +168,7 @@ class LearnerEngine:
         if self.gaussian and not 1 <= A <= _cabi.MAX_GAUSSIAN_DIMS:
             raise ValueError(f"a Gaussian policy takes 1 to {_cabi.MAX_GAUSSIAN_DIMS} action dimensions, got {A}")
         self.N_pi = 2 * A if self.gaussian else A  # policy outputs
+        self.shared_torso = check_shared_torso(shared_torso, H_pi, H_v, self.N_pi)
         if not torch.cuda.is_available():
             raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
         self.lib = _cabi.lib()
@@ -184,10 +205,18 @@ class LearnerEngine:
         self.copy_stream = torch.cuda.Stream(device=self.dev)
         self.launches_per_step = 0
 
-        # ---- parameter blocks: [policy | value_fn], float32, 128-byte aligned tensors
-        self.pi_off, self.n_pi = _cabi.param_layout(O, H_pi, self.N_pi)
-        self.vf_off, self.n_vf = _cabi.param_layout(O, H_v, 1)
+        # ---- parameter blocks: [policy | value_fn], float32, 128-byte aligned tensors.  Shared torso: one block of
+        # N_pi + 1 outputs, n_pi = n_total (n_clip below sets how the optimizer clips it)
+        if self.shared_torso:
+            self.pi_off, self.n_pi = _cabi.param_layout(O, H_pi, self.N_pi + 1)
+            self.vf_off, self.n_vf = None, 0
+        else:
+            self.pi_off, self.n_pi = _cabi.param_layout(O, H_pi, self.N_pi)
+            self.vf_off, self.n_vf = _cabi.param_layout(O, H_v, 1)
         self.n_total = self.n_pi + self.n_vf
+        # the optimizer clips [0, n_clip) and [n_clip, n_total) separately.  Shared torso: one range, the whole
+        # block, as the value range (PopArt's value head must lie in it); its norm is logged as norm_policy
+        self.n_clip = 0 if self.shared_torso else self.n_pi
         f32 = dict(dtype=torch.float32, device=self.dev)
         self.params = torch.zeros(self.n_total, **f32)
         self.adam_m = torch.zeros(self.n_total, **f32)
@@ -205,8 +234,11 @@ class LearnerEngine:
             self.lr_table = torch.tensor([self.optim.lr_scalar], dtype=torch.float32, device=self.dev)
         # PopArt statistics {mu, nu, sigma, mu_loss, sigma_loss} (IMPALA_POPART_STATS), a fresh run at mu 0, nu 1
         self.popart_buf = torch.tensor([0.0, 1.0, 1.0, 0.0, 1.0], dtype=torch.float64, device=self.dev)
-        # the value head inside `params`: W2 (1 x H_v) and b2
-        self.w2_at, self.b2_at = self.n_pi + self.vf_off[2], self.n_pi + self.vf_off[3]
+        # the value head inside `params`: W2 (1 x H_v) and b2 (shared torso: row N_pi of W2 and b2[N_pi])
+        if self.shared_torso:
+            self.w2_at, self.b2_at = self.pi_off[2] + self.N_pi * H_pi, self.pi_off[3] + self.N_pi
+        else:
+            self.w2_at, self.b2_at = self.n_pi + self.vf_off[2], self.n_pi + self.vf_off[3]
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts (replay: the host slabs
         # hold the B_fresh columns that cross the host link, the device slabs the B columns trained on)
@@ -257,8 +289,12 @@ class LearnerEngine:
         self.dlogits = torch.zeros(T, B_local, self.N_pi, **f32)
         self.dv = torch.zeros(T + 1, B_local, **f32)
         self.M_pi, self.M_vf = T * B_local, (T + 1) * B_local
-        self.ws_pi_bytes = self._ws_bytes(self.M_pi, O, H_pi, self.N_pi)
-        self.ws_vf_bytes = self._ws_bytes(self.M_vf, O, H_v, 1)
+        if self.shared_torso:  # one backward over the (T + 1) B rows; ws_pi is its workspace
+            self.ws_pi_bytes = self._ws_bytes(self.M_vf, O, H_pi, self.N_pi + 1)
+            self.ws_vf_bytes = 0
+        else:
+            self.ws_pi_bytes = self._ws_bytes(self.M_pi, O, H_pi, self.N_pi)
+            self.ws_vf_bytes = self._ws_bytes(self.M_vf, O, H_v, 1)
         self.ws_pi = torch.zeros(self.ws_pi_bytes, dtype=torch.uint8, device=self.dev)
         self.ws_vf = torch.zeros(self.ws_vf_bytes, dtype=torch.uint8, device=self.dev)
         # byte observations: O > 128 runs the networks on the bytes (impala_mlp_{forward,backward}_u8); narrower
@@ -341,8 +377,9 @@ class LearnerEngine:
                               "using the NCCL all-reduce between backward and optimizer")
             return
         i64 = dict(dtype=torch.int64, device=self.dev)
-        fused = bool(lib.impala_mlp_backward_pair_push_supported(self.M_pi, self.M_vf, self.O, self.H_pi, self.H_v,
-                                                                  self.N_pi))
+        # the fused push is the paired backward's; a shared torso pushes `comm` after its backward
+        fused = not self.shared_torso and bool(lib.impala_mlp_backward_pair_push_supported(
+            self.M_pi, self.M_vf, self.O, self.H_pi, self.H_v, self.N_pi))
         if os.environ.get("IMPALA_PUSH_FUSED", "1") == "0":
             fused = False
         self.peer = dict(gather=mine["gather"][0], opened=opened, gather_ptrs=torch.tensor(ptrs["gather"], **i64),
@@ -365,8 +402,17 @@ class LearnerEngine:
         return int(n)
 
     def _segments(self):
-        """(group, key, flat offset, shape) of every parameter tensor in `self.params`."""
+        """(group, key, flat offset, shape) of every parameter tensor in `self.params`.  Shared torso: the
+        policy view (W1, b1, W2[:N], b2[:N]) and the value view (W1, b1, W2[N:], b2[N:]) of the one block; the
+        two views share W1 and b1."""
         O, N = self.O, self.N_pi
+        if self.shared_torso:
+            H, o = self.H_pi, self.pi_off
+            for key, off, shp in zip(PKEYS, o, ((H, O), (H,), (N, H), (N,))):
+                yield "policy", key, off, shp
+            for key, off, shp in zip(PKEYS, (o[0], o[1], o[2] + N * H, o[3] + N), ((H, O), (H,), (1, H), (1,))):
+                yield "value_fn", key, off, shp
+            return
         shp_pi = ((self.H_pi, O), (self.H_pi,), (N, self.H_pi), (N,))
         shp_vf = ((self.H_v, O), (self.H_v,), (1, self.H_v), (1,))
         for key, off, shp in zip(PKEYS, self.pi_off, shp_pi):
@@ -379,13 +425,19 @@ class LearnerEngine:
 
         With PopArt the value function is taken FOLDED, in reward units (what `state()` returns): popart =
         {"mu": mu, "nu": nu} sets the statistics and unfolds W2 / sigma, (b2 - mu) / sigma (in float64) into the
-        normalized head; popart=None starts from mu = 0, nu = 1, where the folded head is the normalized one."""
+        normalized head; popart=None starts from mu = 0, nu = 1, where the folded head is the normalized one.
+
+        Shared torso: the torso (W1, b1) and the policy head come from "policy", the value head (W2 of one row,
+        b2 of one entry) from "value_fn"; the value function's first layer is ignored, so a two-network state
+        loads with the policy's torso.  load_state(state()) restores the block exactly."""
         if popart is not None and not self.popart:
             raise ValueError("PopArt statistics given to an engine built with popart=False")
         mu, nu = (0.0, 1.0) if popart is None else (float(popart["mu"]), float(popart["nu"]))
         sigma = popart_sigma(mu, nu)
         flat = torch.zeros(self.n_total, dtype=torch.float32)
         for grp, key, off, shp in self._segments():
+            if self.shared_torso and grp == "value_fn" and key in PKEYS[:2]:
+                continue
             t = torch.as_tensor(np.asarray(state[grp][key]) if not torch.is_tensor(state[grp][key])
                                 else state[grp][key].detach().cpu())
             if tuple(t.shape) != tuple(shp):
@@ -556,7 +608,12 @@ class LearnerEngine:
             _cabi.check(lib.impala_obs_u8_to_f32(obs, _ptr(self.obs_f32), self.obs_f32.numel(), st),
                         "impala_obs_u8_to_f32")
             obs = _ptr(self.obs_f32)
-        if self.obs_u8_native:
+        x_code = _cabi.OBS_U8 if self.obs_u8_native else _cabi.OBS_F32
+        if self.shared_torso:  # one network, its two heads written into logits and values
+            _cabi.check(lib.impala_mlp_forward_shared(obs, x_code, p_pi, _ptr(self.logits), _ptr(self.values),
+                                                      self.M_pi, self.M_vf, O, self.H_pi, A, st),
+                        "impala_mlp_forward_shared")
+        elif self.obs_u8_native:
             # the pair entry point runs the two networks one after the other at these widths: same launches
             for p, out, M, H, N2 in ((p_pi, self.logits, self.M_pi, self.H_pi, A),
                                      (p_vf, self.values, self.M_vf, self.H_v, 1)):
@@ -599,7 +656,11 @@ class LearnerEngine:
                 _ptr(pr["gather_ptrs"]), _ptr(pr["seq"]), pr["slot"], pr["buf"], pr["rank"], self.world, st),
                 "impala_mlp_backward_pair_push")
         else:
-            if self.obs_u8_native:
+            if self.shared_torso:  # dz from dlogits (rows < T B) and dv: the gradient of the whole block
+                _cabi.check(lib.impala_mlp_backward_shared(obs, x_code, p_pi, _ptr(self.dlogits), _ptr(self.dv), g_pi,
+                                                           _ptr(self.ws_pi), self.ws_pi_bytes, self.M_pi, self.M_vf, O,
+                                                           self.H_pi, A, st), "impala_mlp_backward_shared")
+            elif self.obs_u8_native:
                 for p, dout, g, ws, nbytes, M, H, N2 in (
                         (p_pi, self.dlogits, g_pi, self.ws_pi, self.ws_pi_bytes, self.M_pi, self.H_pi, A),
                         (p_vf, self.dv, g_vf, self.ws_vf, self.ws_vf_bytes, self.M_vf, self.H_v, 1)):
@@ -629,12 +690,12 @@ class LearnerEngine:
             _cabi.check(self.lib.impala_gather_clip_adam(
                 _ptr(self.params), _ptr(self.comm), C.c_void_p(pr["gather"]), _ptr(pr["seq"]),
                 pr["slot"], pr["buf"], self.world, self.n_extra, _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step),
-                self.n_pi, self.n_total, float(hp.max_norm), float(0.95 * hp.lr), 0.9, 0.999, 1e-8,
+                self.n_clip, self.n_total, float(hp.max_norm), float(0.95 * hp.lr), 0.9, 0.999, 1e-8,
                 _ptr(self.norms), _ptr(pr["err"]), pr["timeout_s"], st), "impala_gather_clip_adam")
             return 1
         _cabi.check(self.lib.impala_clip_adam(
             _ptr(self.params), _ptr(self.comm), _ptr(self.adam_m), _ptr(self.adam_v),
-            _ptr(self.adam_step), self.n_pi, self.n_total, float(hp.max_norm),
+            _ptr(self.adam_step), self.n_clip, self.n_total, float(hp.max_norm),
             float(0.95 * hp.lr),  # LambdaLR(lambda e: 0.95): constant factor, learner.py:42
             0.9, 0.999, 1e-8, _ptr(self.norms), st), "impala_clip_adam")
         return 1
@@ -650,11 +711,11 @@ class LearnerEngine:
             _cabi.check(self.lib.impala_gather_clip_optim(
                 _ptr(self.params), _ptr(self.comm), C.c_void_p(pr["gather"]), _ptr(pr["seq"]),
                 pr["slot"], pr["buf"], self.world, self.n_extra, _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step),
-                self.n_pi, self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), _ptr(pr["err"]), pr["timeout_s"],
+                self.n_clip, self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), _ptr(pr["err"]), pr["timeout_s"],
                 st), "impala_gather_clip_optim")
             return 1
         _cabi.check(self.lib.impala_clip_optim(
-            _ptr(self.params), _ptr(self.comm), _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step), self.n_pi,
+            _ptr(self.params), _ptr(self.comm), _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step), self.n_clip,
             self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), st), "impala_clip_optim")
         return 1
 
@@ -667,11 +728,11 @@ class LearnerEngine:
             _cabi.check(self.lib.impala_gather_clip_optim_popart(
                 _ptr(self.params), _ptr(self.comm), C.c_void_p(pr["gather"]), _ptr(pr["seq"]),
                 pr["slot"], pr["buf"], self.world, self.n_extra, _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step),
-                self.n_pi, self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), _ptr(pr["err"]), pr["timeout_s"],
+                self.n_clip, self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), _ptr(pr["err"]), pr["timeout_s"],
                 *pop, st), "impala_gather_clip_optim_popart")
             return 1
         _cabi.check(self.lib.impala_clip_optim_popart(
-            _ptr(self.params), _ptr(self.comm), _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step), self.n_pi,
+            _ptr(self.params), _ptr(self.comm), _ptr(self.adam_m), _ptr(self.adam_v), _ptr(self.adam_step), self.n_clip,
             self.n_total, float(hp.max_norm), *rule, _ptr(self.norms), *pop, st), "impala_clip_optim_popart")
         return 1
 
@@ -781,7 +842,7 @@ class LearnerEngine:
         out = dict(zip(SCALAR_NAMES, s[:4]))
         out["total_loss"] = (hp.v_loss_c * out["value_fn_loss"] + hp.policy_loss_c * out["policy_loss"]
                              - hp.entropy_c * out["policy_entropy"])  # learner.py:154-159
-        out["norm_policy"], out["norm_value"] = s[4], s[5]
+        out["norm_policy"], out["norm_value"] = (s[5], 0.0) if self.shared_torso else (s[4], s[5])
         if self.popart:
             out["popart_mu"], out["popart_sigma"] = s[16], s[18]
         if self.diagnostics:

@@ -290,7 +290,8 @@ class Learner:
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
                  evaluator=None, obs_dtype="float32", frames=1, diagnostics=False,
                  replay_slabs=0, replay_columns=0, optimizer="adam", optimizer_kwargs=None, lr_lambda=None,
-                 popart=False, popart_beta=POPART_BETA, reward_clip=None, action_dist="categorical"):
+                 popart=False, popart_beta=POPART_BETA, reward_clip=None, action_dist="categorical",
+                 shared_torso=False):
         self.id = id
         # action distribution: "gaussian" = a diagonal Gaussian policy with 2A outputs [mean | log std]
         _cabi.act_kind_code(action_dist)
@@ -303,6 +304,11 @@ class Learner:
         if hasattr(q, "collect_batch") and getattr(q, "action_dist", "categorical") != action_dist:
             raise ValueError(f"the RingQueue holds {getattr(q, 'action_dist', 'categorical')} actions, "
                              f"the learner was built for action_dist={action_dist!r}")
+        # shared torso (one hidden layer feeding both heads; engine.py): checked here, in the launching process
+        from .engine import check_shared_torso
+
+        _, n_out, H_pi, H_v = _dims(policy, value_fn)
+        self.shared_torso = check_shared_torso(shared_torso, H_pi, H_v, n_out)
         # reward clipping inside the V-trace kernel: checked here, in the launching process
         _cabi.reward_clip_code(reward_clip)
         self.reward_clip = reward_clip
@@ -402,7 +408,7 @@ class Learner:
                     obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics,
                     replay_slabs=self.replay_slabs, replay_columns=self.replay_columns, optimizer=self.optimizer,
                     optimizer_kwargs=self.optimizer_kwargs, popart=self.popart, popart_beta=self.popart_beta,
-                    reward_clip=self.reward_clip, action_dist=self.action_dist)
+                    reward_clip=self.reward_clip, action_dist=self.action_dist, shared_torso=self.shared_torso)
 
     def _make_engine(self, process_group=None, world=1):
         from .engine import LearnerEngine
@@ -416,7 +422,8 @@ class Learner:
                             replay_slabs=c["replay_slabs"], replay_columns=c["replay_columns"],
                             optimizer=c["optimizer"], optimizer_kwargs=c["optimizer_kwargs"],
                             lr_table=self.optim.lr_table, popart=c["popart"], popart_beta=c["popart_beta"],
-                            reward_clip=c["reward_clip"], action_dist=c["action_dist"])
+                            reward_clip=c["reward_clip"], action_dist=c["action_dist"],
+                            shared_torso=c["shared_torso"])
         eng.load_state(self._init_state(), self._popart_init())
         return eng
 
@@ -729,12 +736,19 @@ class Learner:
 
     # ------------------------------------------------------ checkpoints (learner.py:277-295)
     def save(self, path):
+        """Reference checkpoint keys.  Shared torso: the two state dicts are the policy and value views of the one
+        network (both hold the torso) and "shared_torso" is True; the policy view is an MlpPolicy state dict."""
         ckpt = {"policy_state_dict": self.policy.state_dict(), "value_fn_state_dict": self.value_fn.state_dict()}
+        if self.shared_torso:
+            ckpt["shared_torso"] = True
         if self.popart:  # value_fn is folded (reward units); the statistics that unfold it
             ckpt["popart"] = dict(self.popart_init or {"mu": 0.0, "nu": 1.0})
         torch.save(ckpt, path)
 
     def load(self, path):
+        """Restores a checkpoint of either kind into the two modules.  A shared-torso learner builds its network
+        from the policy's torso and heads and the value function's head (engine.load_state), so a two-network
+        checkpoint starts it from the policy's torso."""
         checkpoint = torch.load(path)
         self.policy.load_state_dict(checkpoint["policy_state_dict"])
         self.value_fn.load_state_dict(checkpoint["value_fn_state_dict"])
