@@ -9,7 +9,8 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "libimpala_b200.so")
+# IMPALA_LIB_DIR: a library built elsewhere (build.py honours the same variable)
+LIB_PATH = os.path.join(os.environ.get("IMPALA_LIB_DIR", os.path.join(_HERE, "lib")), "libimpala_b200.so")
 
 MODE_REFERENCE = 0
 MODE_PAPER = 1

@@ -18,6 +18,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # IMPALA_LIB_DIR: build somewhere else (compile checks while a snapshot of the tree is in flight)
 _LIB_DIR = os.environ.get("IMPALA_LIB_DIR", os.path.join(HERE, "lib"))
+# IMPALA_PHASE_CLOCKS=1: compile the phase clocks of the narrow tensor-core MLP kernels in
+# (csrc/phase_clocks.cuh, scripts/phase_mlp.py); build such a library into an IMPALA_LIB_DIR of its own
+_DEFS = ["-DIMPALA_PHASE_CLOCKS"] if os.environ.get("IMPALA_PHASE_CLOCKS") == "1" else []
 OBJ = os.path.join(_LIB_DIR, "obj")
 LIB = os.path.join(_LIB_DIR, "libimpala_b200.so")
 
@@ -59,7 +62,7 @@ def _compile(nvcc, name, src, defs, stamp):
     log = os.path.join(OBJ, name + ".ptxas.log")
     if os.path.exists(obj) and os.path.getmtime(obj) >= stamp:
         return name, 0, "cached"
-    cmd = [nvcc, *ARCH, *COMMON, *defs, "-c", os.path.join(CSRC, src), "-o", obj]
+    cmd = [nvcc, *ARCH, *COMMON, *_DEFS, *defs, "-c", os.path.join(CSRC, src), "-o", obj]
     res = subprocess.run(cmd, capture_output=True, text=True)
     with open(log, "w") as f:
         f.write(res.stderr)
@@ -70,6 +73,15 @@ def build(verbose: bool = False, jobs: int | None = None) -> str:
     nvcc = _nvcc()
     os.makedirs(OBJ, exist_ok=True)
     stamp = _newest_source_mtime()
+    # the objects of a directory were built with one set of defines, recorded beside them: other (or unknown)
+    # defines rebuild every unit, so a default and an IMPALA_PHASE_CLOCKS build never share an object
+    defs_file = os.path.join(OBJ, "defines.txt")
+    defs = " ".join(_DEFS)
+    built_with = open(defs_file).read() if os.path.exists(defs_file) else None
+    if built_with != defs:
+        stamp = float("inf")
+        if built_with is not None:
+            os.remove(defs_file)
     units = _units()
     jobs = jobs or min(len(units), os.cpu_count() or 4)
     with cf.ThreadPoolExecutor(jobs) as ex:
@@ -79,6 +91,8 @@ def build(verbose: bool = False, jobs: int | None = None) -> str:
             raise RuntimeError(f"nvcc failed on {name}:\n{msg}")
         if verbose:
             print(f"[build] {name}: {msg}")
+    with open(defs_file, "w") as f:
+        f.write(defs)
     objs = [os.path.join(OBJ, u[0] + ".o") for u in units]
     if (not os.path.exists(LIB)) or any(os.path.getmtime(o) > os.path.getmtime(LIB) for o in objs):
         cmd = [nvcc, *ARCH, "-shared", "-cudart", "static", "-o", LIB, *objs]

@@ -34,7 +34,8 @@
 // 64-unit hidden block of one network for the whole launch, so W1 of the block is loaded once and held
 // in registers as GEMM1's A operand (only the x tile is read from shared memory).  Its two warpgroups
 // are independent - each takes alternate tiles of the CTA's share, with its own x stage and named
-// barrier - so one warpgroup's MMAs overlap the other's CUDA-core epilogue.  The warpgroups meet once,
+// barrier - so one warpgroup's MMAs overlap the other's CUDA-core epilogue (their GEMM2s are issued in
+// turn, see the ping-pong comment in the body).  The warpgroups meet once,
 // at the end (fixed order), and the rows are summed in-kernel after a grid barrier (paired launch,
 // optional peer push).  GEMM1 covers the tile's 64 batch rows with one m64n64 MMA per product (the
 // accumulator is the two 32-row halves side by side, so every entry takes the same products in the same
@@ -43,6 +44,7 @@
 // Wide shapes (bwd_tc_body): one CTA = 2 warpgroups = 128 hidden units per pass, wider layers walked
 // in passes (x is re-read once per pass); reduce_partials_kernel sums the rows.
 #include "mlp_kernels.cuh"
+#include "phase_clocks.cuh"
 #include "tc_common.cuh"
 
 namespace {
@@ -651,10 +653,25 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdArgs<SPLIT>& a, const 
     const uint64_t dxt_hi = tc::smem_desc_k_sw128(xt_hi, 0), dxt_lo = tc::smem_desc_k_sw128(xt_lo, 0);
 
     const int bar = 1 + wg, tstride = 2 * cpg;  // this warpgroup's named barrier and tile stride
+    // Ping-pong: the warpgroups take turns to issue GEMM2, the larger of a tile's two MMA batches: warpgroup
+    // 0's, warpgroup 1's, warpgroup 0's, ..., so that their GEMM2s reach the tensor pipe one after the other
+    // instead of together, each while the other warpgroup runs its epilogue or staging.  Turn barrier 3 + w
+    // (256 threads) is warpgroup w's: it syncs on its own before the issue and arrives on the other's after
+    // the commit.  Warpgroup 0 takes n0 turns and warpgroup 1 as many (n0 - n1 <= 1: one empty turn after its
+    // last tile), and every arrival is awaited: warpgroup 0 skips the sync of its first turn, warpgroup 1 the
+    // arrival of its last, so both barriers are back at zero before the closing __syncthreads
+    // (tests/test_pingpong_protocol_cpu.py models the sequence: bwd_ops there restates the three turn
+    // conditions below - the G2 sync, the G2 arrival and the empty turn - and changes with them).  GEMM1
+    // takes no turn: a token per GEMM measured the same step rate with twice the barriers (chosen by step rate,
+    // not by the phase clocks).  Only the issue order changes, not the arithmetic.
+    const int own = 3 + wg, other = 4 - wg;
+    PHASE_BEGIN(wg);
     load(r + cpg * wg);
     for (int tile = r + cpg * wg; tile < a.num_tiles; tile += tstride) {
+        PHASE_TILE(wg);
         // ---- stage the tile: x row-major (B of GEMM1) and transposed (B of GEMM2), hi / lo; dz
         tc::named_bar(bar, 128);  // every MMA of the warpgroup that read the previous tile has retired
+        PHASE_MARK(wg, 0);
 #pragma unroll
         for (int k = 0; k < kLd; ++k) {
             if (k >= ksteps) continue;  // features GEMM1 does not read; GEMM2's columns of them are dropped
@@ -681,7 +698,7 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdArgs<SPLIT>& a, const 
         }
         tc::fence_proxy_async();
         tc::named_bar(bar, 128);
-        load(tile + tstride);  // in flight during this tile's MMAs and epilogue
+        PHASE_MARK(wg, 1);
 
         // ---- GEMM1: PRE = W1_blk * X^T (one m64n64 MMA per product over the tile's 64 batch rows), A
         // from registers; descriptors = the stage's plus the operand's offset in 16-byte units (start
@@ -694,6 +711,7 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdArgs<SPLIT>& a, const 
         for (int i = 0; i < 32; ++i) d[i] = 0.f;
         // zeroed accumulators defined before the warpgroup fence (see bwd_tc_body)
         tc::fence_acc(d);
+        PHASE_GEMM_ON(wg);
         tc::wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
@@ -708,8 +726,14 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdArgs<SPLIT>& a, const 
             if (kk < ksteps) tc::wgmma_n64_rs(d, wh[kk], bx_hi + ((kk * 32) >> 4), true);
         }
         tc::wgmma_commit();
+        // the next tile's loads go out after GEMM1 is issued, not before: their address arithmetic and
+        // bounds checks run while the MMAs execute instead of delaying the issue; they are in flight during
+        // this tile's MMAs and epilogue
+        load(tile + tstride);
         tc::wgmma_wait<0>();
         tc::fence_acc(d);
+        PHASE_GEMM_OFF(wg);
+        PHASE_MARK(wg, 2);
 
         // ---- epilogue: d <- DP in place (thread: hidden units j0 / j1, batch columns 8 i + 2 q + e)
 #pragma unroll
@@ -749,6 +773,10 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdArgs<SPLIT>& a, const 
         }
         uint64_t bxt_hi = dxt_hi, bxt_lo = dxt_lo;
         asm volatile("" : "+l"(bxt_hi), "+l"(bxt_lo));
+        PHASE_MARK(wg, 3);
+        tc::named_bar_if(wg == 1 || tile != r, own, 256);  // G2 turn
+        PHASE_MARK(wg, 5);
+        PHASE_GEMM_ON(wg);
         tc::wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < 8; ++kk) {
@@ -761,12 +789,20 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdArgs<SPLIT>& a, const 
             tc::wgmma_n32_rs(acc_hh, ah, bxt_hi + xo, true);
         }
         tc::wgmma_commit();
+        tc::named_bar_arrive_if(wg == 0 || tile + cpg < a.num_tiles, other, 256);  // 1: warpgroup 0 has a next tile
         tc::wgmma_wait<0>();
         // the A registers are read asynchronously: keep them (and the accumulators) untouched until here
         tc::fence_acc(d);
 #pragma unroll
         for (int i = 0; i < 32; ++i) asm volatile("" : "+r"(lo[i])::"memory");
         tc::fence_acc(acc_hh), tc::fence_acc(acc_c);
+        PHASE_GEMM_OFF(wg);
+        PHASE_MARK(wg, 4);
+    }
+    // an odd number of tiles in the CTA (r, r + cpg, ... alternate between the warpgroups): warpgroup 1 has
+    // one fewer and takes the empty turn of warpgroup 0's last tile
+    if (wg == 1 && (r < a.num_tiles ? (a.num_tiles - 1 - r) / cpg + 1 : 0) % 2 == 1) {
+        tc::named_bar(own, 256);
     }
 
     // ---- end of the launch: the quad's column sets meet, then warpgroup 0 + warpgroup 1 (fixed order)
@@ -834,6 +870,7 @@ __device__ __forceinline__ uint8_t* bwd_blk_body(const BwdArgs<SPLIT>& a, const 
     }
     __threadfence();  // this thread's partial-row stores are visible device-wide
     __syncthreads();
+    PHASE_END(wg);
     return smem;
 }
 
@@ -1104,3 +1141,15 @@ int impala_mlp_bwd_tcw(const MlpPlan& p, const float* x, const float* params, co
                               : (np == 1 ? mlp_bwd_tcw_kernel<1, 4> : np == 4 ? mlp_bwd_tcw_kernel<4, 4> : mlp_bwd_tcw_kernel<32, 4>);
     return launch_tcw(kernel, p, static_cast<const BwdTcArgs&>(a), st, nparts);
 }
+
+#ifdef IMPALA_PHASE_CLOCKS
+IMPALA_PHASE_READER(impala_phase_read_bwd)
+
+// The phase counters of the narrow backward body (out[0, kSlots)) and forward body (out[kSlots, 2 kSlots)),
+// summed over every launch since the last reset; reset != 0 zeroes them after the copy.  Only in a build
+// with IMPALA_PHASE_CLOCKS (scripts/phase_mlp.py).
+extern "C" int impala_phase_read(unsigned long long* out, int reset) {
+    const int e = impala_phase_read_bwd(out, reset);
+    return e ? e : impala_phase_read_fwd(out + phase::kSlots, reset);
+}
+#endif

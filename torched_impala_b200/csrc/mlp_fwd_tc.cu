@@ -19,14 +19,16 @@
 // up to 256 hidden units (a "block") sit in shared memory and are shared.  At one K atom (O <= 32)
 // the x tile is wgmma's A operand straight from registers: each thread loads the x elements of its
 // own fragment slots from global memory and splits them, so nothing is staged and the tile loop has
-// no barrier (fwd_rs_body).  With two or four K atoms the tile is split into per-warpgroup hi / lo
-// stages in shared memory instead (fwd_ss_body).  While one
+// no barrier but the ping-pong turns of the two warpgroups' MMA batches (fwd_rs_body).  With two or
+// four K atoms the tile is split into per-warpgroup hi / lo stages in shared memory instead
+// (fwd_ss_body).  While one
 // warpgroup runs its epilogue the other warpgroups' MMAs keep the tensor cores busy, and every
 // warpgroup has the next tile's x in flight in registers while it computes the current one.  Wider hidden
 // layers walk their blocks in passes: out[row] = ((b2 + z_0) + z_1) + ...  where the thread that
 // owns a row adds the block's partial second-layer sum to what the SAME thread wrote in the
 // previous pass (fixed order, bitwise reproducible, no workspace).
 #include "mlp_fwd_tc.cuh"
+#include "phase_clocks.cuh"
 #include "tc_common.cuh"
 
 namespace {
@@ -102,9 +104,10 @@ __device__ __forceinline__ void stage_weights(const FwdTcArgs& a, int p, uint8_t
 // x fragments in registers (one K atom).  Thread (warp, g, q) owns rows 16 warp + g and + 8
 // of the tile in both the A fragment and the accumulator, so it loads its own features 8 kk + q and
 // 8 kk + q + 4 of those two rows straight from global memory: nothing is staged, and a warpgroup
-// never waits for another thread.  The next tile's raw values are in flight in xr while the current
-// tile computes; they are split into hi / lo after the tile's last MMA batch has retired.  Only W1
-// is read from shared memory (1 KB per MMA instead of 3 KB), and the tile loop has no barrier.
+// waits for the other only for its turn to issue.  The next tile's raw values are in flight in xr while
+// the current tile computes; they are split into hi / lo after the tile's last MMA batch has retired.  Only W1
+// is read from shared memory (1 KB per MMA instead of 3 KB), and the tile loop has no barrier but the
+// ping-pong turns below.
 // The 32-unit slices go to the tensor cores two at a time, as one m64n64 MMA chain into one
 // 32-register accumulator (see `issue`): a tile waits on 4 batches instead of 8, and issues 9 MMAs per
 // batch instead of 18.
@@ -117,7 +120,10 @@ __device__ __forceinline__ void fwd_rs_body(const FwdArgs<SPLIT>& a, const int c
     uint8_t* w_lo = w_hi + KA * HB * 128;
     float* b1s = reinterpret_cast<float*>(smem + 2 * KA * HB * 128);  // [HB]
     float* w2s = b1s + HB;                                             // [HB][NPS]
-    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    // the warpgroup index broadcast from lane 0: known warp-uniform, or ptxas takes the turn barriers for
+    // divergent code and serializes every wgmma (C7520)
+    const int wg = __shfl_sync(IMPALA_FULL_MASK, (int)threadIdx.x >> 7, 0);
+    const int tid = threadIdx.x, warp = (tid >> 5) & 3, lane = tid & 31;
     const int g = lane >> 2, q = lane & 3;
     const int O = a.O, ksteps = (O + 7) >> 3, nslices = HB / 32;
     const int unit = cta * kWG + wg, nunits = ncta * kWG;
@@ -170,6 +176,20 @@ __device__ __forceinline__ void fwd_rs_body(const FwdArgs<SPLIT>& a, const int c
         tc::wgmma_commit();
     };
 
+    // Ping-pong: the warpgroups take turns to issue an MMA batch, batch 0 of warpgroup 0, batch 0 of
+    // warpgroup 1, batch 1 of 0, ..., so that one warpgroup's epilogue runs while the other's MMAs execute.
+    // Turn barrier 3 + w (256 threads) is warpgroup w's: it syncs on its own before the issue and arrives on
+    // the other's after the commit.  Within a pass warpgroup 0 takes nb turns per tile and warpgroup 1 as many
+    // (one tile fewer: it takes that tile's nb turns empty); warpgroup 0 skips the sync of its first turn,
+    // warpgroup 1 the arrival of its last, so both barriers are back at zero at the pass's closing
+    // __syncthreads (tests/test_pingpong_protocol_cpu.py models the sequence: fwd_ops there restates `turn`,
+    // `pass_turn` and the empty turns after the tile loop, and changes with them).
+    const int nb = (nslices + 1) / 2;  // MMA batches per tile
+    auto turn = [&](bool first) { tc::named_bar_if(wg == 1 || !first, 3 + wg, 256); };
+    auto pass_turn = [&](bool last, int tile) {  // after the commit; last: the tile's last batch
+        tc::named_bar_arrive_if(wg == 0 || !last || tile - 1 + nunits < a.num_tiles, 4 - wg, 256);
+    };
+    PHASE_BEGIN(wg);
     const int npass = a.H / HB;
     for (int p = 0; p < npass; ++p) {
         load(unit);       // in flight during the weight staging
@@ -177,8 +197,11 @@ __device__ __forceinline__ void fwd_rs_body(const FwdArgs<SPLIT>& a, const int c
         stage_weights<NP, KA>(a, p, w_hi, w_lo, b1s, w2s);
         tc::fence_proxy_async();
         __syncthreads();
+        PHASE_MARK(wg, 5);
 
-        for (int tile = unit; tile < a.num_tiles; tile += nunits) {
+        int tile = unit;
+        for (; tile < a.num_tiles; tile += nunits) {
+            PHASE_TILE(wg);
             // the previous tile's MMAs have all retired: its fragments may be overwritten
 #pragma unroll
             for (int kk = 0; kk < KS; ++kk) {
@@ -192,6 +215,7 @@ __device__ __forceinline__ void fwd_rs_body(const FwdArgs<SPLIT>& a, const int c
                 tc::fence_frag(xl[kk]);
             }
             load(tile + nunits);  // in flight during this tile's MMAs and epilogue
+            PHASE_MARK(wg, 2);
 
             float p0[NP], p1[NP];
 #pragma unroll
@@ -199,21 +223,45 @@ __device__ __forceinline__ void fwd_rs_body(const FwdArgs<SPLIT>& a, const int c
             int nc = 0;
             for (; nc + 2 <= nslices; nc += 2) {
                 float d[32];
+                turn(tile == unit && nc == 0);
+                PHASE_MARK(wg, 4);
+                PHASE_GEMM_ON(wg);
                 issue(d, nc);
+                pass_turn(nc + 2 >= nslices, tile);
                 tc::wgmma_wait<0>();
                 tc::fence_acc(d);
+                PHASE_GEMM_OFF(wg);
+                PHASE_MARK(wg, 0);
                 slice_epilogue<NP>(d, nc, q, b1s, w2s, p0, p1);
+                PHASE_MARK(wg, 1);
             }
             if (nc < nslices) {  // odd number of slices (H = 32, 96, 160, 224)
                 float d[16];
+                turn(tile == unit && nc == 0);
+                PHASE_MARK(wg, 4);
+                PHASE_GEMM_ON(wg);
                 issue(d, nc);
+                pass_turn(true, tile);
                 tc::wgmma_wait<0>();
                 tc::fence_acc(d);
+                PHASE_GEMM_OFF(wg);
+                PHASE_MARK(wg, 0);
                 slice_epilogue<NP>(d, nc, q, b1s, w2s, p0, p1);
+                PHASE_MARK(wg, 1);
             }
             write_rows<NP, SPLIT>(a, p, tile, warp, g, q, p0, p1);
+            PHASE_MARK(wg, 3);
+        }
+        // warpgroup 1 with one tile fewer in the pass (tile - 1: warpgroup 0's next): its empty turns
+        if (wg == 1 && tile - 1 < a.num_tiles) {
+            for (int b = 0; b < nb; ++b) {
+                tc::named_bar(4, 256);
+                if (b + 1 < nb) tc::named_bar_arrive(3, 256);
+            }
         }
     }
+    PHASE_SYNC();
+    PHASE_END(wg);
 }
 
 // x tile staged in shared memory (four K atoms): each warpgroup splits it into its own hi / lo
@@ -422,3 +470,7 @@ int impala_mlp_fwd_tc_pair(const float* x, const float* params_pi, const float* 
     mlp_fwd_tc_pair_kernel<<<grid, kThreads, smem, st>>>(a_pi, a_vf, n_pi);
     return impala_launch_status();
 }
+
+#ifdef IMPALA_PHASE_CLOCKS
+IMPALA_PHASE_READER(impala_phase_read_fwd)
+#endif

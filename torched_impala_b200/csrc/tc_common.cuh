@@ -28,6 +28,23 @@ __device__ __forceinline__ void fence_proxy_async() {
 __device__ __forceinline__ void named_bar(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// arrive at named barrier `id` without waiting: with `nthreads` = 2 x 128, the other warpgroup's bar.sync
+// on it returns once this one has arrived (a token handed from one warpgroup to the other).  Two arrivals
+// of the same warpgroup before the other's sync would complete the barrier on their own: a protocol built
+// on it alternates arrivals and syncs.
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// the same two, executed only where `pred` holds (warp-uniform), as predicated instructions: no branch in
+// the code around the wgmmas
+__device__ __forceinline__ void named_bar_if(bool pred, int id, int nthreads) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p bar.sync %0, %1;\n\t}" ::"r"(id), "r"(nthreads),
+                 "r"((int)pred) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive_if(bool pred, int id, int nthreads) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p bar.arrive %0, %1;\n\t}" ::"r"(id), "r"(nthreads),
+                 "r"((int)pred) : "memory");
+}
 
 // ------------------------------------------------------------------ wgmma
 // K-major operand tile, rows of 128 bytes (32 tf32), SWIZZLE_128B, 8-row groups 1024 B apart.
