@@ -22,8 +22,7 @@ def main():
     import torch.distributed as dist
 
     from . import dp
-    from .engine import LearnerEngine
-    from .utils import Hyperparameters
+    from .engine import engine_from_cfg
 
     rank, world, dev = spec["rank"], spec["world"], spec["device"]
     ctl = dp.ShardControl(spec["ctl"])
@@ -32,16 +31,8 @@ def main():
         dist.init_process_group("nccl", init_method=f"tcp://127.0.0.1:{spec['port']}", rank=rank, world_size=world,
                                 device_id=torch.device(dev))
         c = spec["cfg"]
-        hp = Hyperparameters(**c["hp"])
         state, lr_table = dp.read_init_state(spec["state"])
-        eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], hp, global_batch=c["B"],
-                            device=dev, mode=c["mode"], process_group=dist.group.WORLD,
-                            obs_dtype=c.get("obs_dtype", "float32"), frames=c.get("frames", 1),
-                            diagnostics=c.get("diagnostics", False), optimizer=c.get("optimizer", "adam"),
-                            optimizer_kwargs=c.get("optimizer_kwargs"), lr_table=lr_table,
-                            popart=c.get("popart", False), popart_beta=c.get("popart_beta", 3e-4),
-                            reward_clip=c.get("reward_clip"), action_dist=c.get("action_dist", "categorical"),
-                            shared_torso=c.get("shared_torso", False))
+        eng = engine_from_cfg(c, world, dev, dist.group.WORLD, lr_table)
         popart = state.pop("popart", None)  # rank 0's statistics: every rank starts identical
         eng.load_state(state, {k: float(v) for k, v in popart.items()} if popart else None)
         shm = dp.attach_untracked(spec["slab_shm"])

@@ -72,10 +72,15 @@ the event the step waits on, so the captured graphs keep fixed pointers.  R + 2 
 the slot that receives update n + 1 is in nobody's pool, so the DMA still runs under the kernels.  The kernels
 after the compose launch are unchanged; the logged `batch_mean_reward` scalar is the composed batch's (sum of
 all B columns' rewards / B), the mean over the fresh trajectories is the caller's (Learner logs that one).
+
+The keyword options above (obs_dtype, frames, diagnostics, replay_slabs, replay_columns, optimizer, optimizer_kwargs,
+popart, popart_beta, reward_clip, action_dist, shared_torso) are the fields of `LearnerOptions`.
 """
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -130,6 +135,69 @@ def check_shared_torso(shared_torso: bool, H_pi: int, H_v: int, n_policy: int) -
     return True
 
 
+class CheckedOptions(NamedTuple):
+    """What `LearnerOptions.check` derives from the options and the shapes."""
+    B_fresh: int           # columns of an update that arrive from the host (B without replay)
+    N_pi: int              # policy outputs: A, or 2A [mean | log std] for a Gaussian policy
+    obs_code: int          # IMPALA_OBS_*
+    act_kind: int          # IMPALA_ACT_*
+    reward_clip_code: int  # IMPALA_REWARD_CLIP_*, 0 = none
+
+
+@dataclasses.dataclass(frozen=True)
+class LearnerOptions:
+    """The learner's feature options (module docstring): `Learner` and `LearnerEngine` keywords, JSON for the worker
+    ranks of a data-parallel learner.  The schedule is not one: a lambda is not JSON, its table travels apart."""
+    obs_dtype: str = "float32"
+    frames: int = 1
+    diagnostics: bool = False
+    replay_slabs: int = 0
+    replay_columns: int = 0
+    optimizer: str = "adam"
+    optimizer_kwargs: dict = dataclasses.field(default_factory=dict)
+    popart: bool = False
+    popart_beta: float = POPART_BETA
+    reward_clip: str | None = None
+    action_dist: str = "categorical"
+    shared_torso: bool = False
+
+    def __post_init__(self):
+        object.__setattr__(self, "optimizer_kwargs", dict(self.optimizer_kwargs or {}))
+
+    def check(self, B: int, O: int, A: int, H_pi: int, H_v: int, world: int = 1) -> CheckedOptions:
+        """Refuse options that B columns per update, O features, A actions (Gaussian: action dimensions), hidden
+        widths H_pi, H_v and `world` devices cannot take.  optim_config checks the optimizer and its keywords."""
+        obs_code = _cabi.obs_dtype_code(self.obs_dtype)
+        if self.frames < 1 or O % self.frames:
+            raise ValueError(f"{O} observation features do not split into {self.frames} stacked frames")
+        act_kind = _cabi.act_kind_code(self.action_dist)
+        gaussian = act_kind == _cabi.ACT_GAUSSIAN
+        if gaussian and not 1 <= A <= _cabi.MAX_GAUSSIAN_DIMS:
+            raise ValueError(f"a Gaussian policy takes 1 to {_cabi.MAX_GAUSSIAN_DIMS} action dimensions (2A outputs "
+                             f"[mean | log std]), got A = {A}")
+        N_pi = 2 * A if gaussian else A
+        check_shared_torso(self.shared_torso, H_pi, H_v, N_pi)
+        reward_clip_code = _cabi.reward_clip_code(self.reward_clip)
+        check_popart_args(self.popart, self.popart_beta)
+        B_fresh = check_replay_args(B, self.replay_slabs, self.replay_columns)
+        if self.replay_slabs and world > 1:
+            raise ValueError(f"experience replay runs on one device, not {world}: the store is not sharded")
+        return CheckedOptions(B_fresh, N_pi, obs_code, act_kind, reward_clip_code)
+
+
+def engine_from_cfg(cfg: dict, world: int, device, process_group=None, lr_table=None) -> LearnerEngine:
+    """The engine of one of `world` ranks from a Learner's JSON config (`Learner._cfg`) and learning-rate table:
+    rank 0 and every data-parallel worker rank build theirs here, so all of them train with the same options."""
+    from .utils import Hyperparameters
+
+    if cfg["B"] % world:
+        raise ValueError(f"batch_size {cfg['B']} does not divide over {world} devices")
+    return LearnerEngine(cfg["T"], cfg["B"] // world, cfg["O"], cfg["A"], cfg["H_pi"], cfg["H_v"],
+                         Hyperparameters(**cfg["hp"]), global_batch=cfg["B"], device=device, mode=cfg["mode"],
+                         process_group=process_group, lr_table=lr_table,
+                         **{f.name: cfg[f.name] for f in dataclasses.fields(LearnerOptions)})
+
+
 def _ptr(t: torch.Tensor) -> C.c_void_p:
     return C.c_void_p(t.data_ptr())
 
@@ -148,56 +216,36 @@ _NO_CTX = _NoCtx()
 class LearnerEngine:
     def __init__(self, T: int, B_local: int, O: int, A: int, H_pi: int, H_v: int, hp,
                  global_batch: int | None = None, device: str | torch.device = "cuda:0",
-                 mode: str = "reference", process_group=None, use_graph: bool = True,
-                 slabs: int = 2, obs_dtype: str = "float32", frames: int = 1, diagnostics: bool = False,
-                 replay_slabs: int = 0, replay_columns: int = 0, replay_seed: int = 0,
-                 optimizer: str = "adam", optimizer_kwargs: dict | None = None, lr_lambda=None, lr_table=None,
-                 popart: bool = False, popart_beta: float = POPART_BETA, reward_clip: str | None = None,
-                 action_dist: str = "categorical", shared_torso: bool = False):
-        # update rule and learning-rate schedule, checked before any device work (optim.optim_config); the
-        # default - Adam at 0.95 * hp.lr - keeps impala_clip_adam with the rate as a launch argument
-        self.optim = optim_config(hp, optimizer, optimizer_kwargs, lr_lambda, lr_table)
-        self.popart_beta = check_popart_args(popart, popart_beta)
-        self.popart = bool(popart)
-        # reward transform inside the V-trace kernel (IMPALA_REWARD_CLIP_*; 0 = none), checked before device work
-        self.reward_clip_code = _cabi.reward_clip_code(reward_clip)
-        # action distribution (IMPALA_ACT_*): the policy has A outputs (categorical) or 2A (Gaussian over A dimensions)
-        self.act_kind = _cabi.act_kind_code(action_dist)
-        self.action_dist = action_dist
-        self.gaussian = self.act_kind == _cabi.ACT_GAUSSIAN
-        if self.gaussian and not 1 <= A <= _cabi.MAX_GAUSSIAN_DIMS:
-            raise ValueError(f"a Gaussian policy takes 1 to {_cabi.MAX_GAUSSIAN_DIMS} action dimensions, got {A}")
-        self.N_pi = 2 * A if self.gaussian else A  # policy outputs
-        self.shared_torso = check_shared_torso(shared_torso, H_pi, H_v, self.N_pi)
-        if not torch.cuda.is_available():
-            raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
-        self.lib = _cabi.lib()
-        # "uint8": byte observations in the slabs (Atari RAM, MinAtar), entering the networks unscaled
-        self.obs_code = _cabi.obs_dtype_code(obs_dtype)
-        self.obs_dtype = obs_dtype
-        if frames < 1 or O % frames:
-            raise ValueError(f"{O} observation features do not split into {frames} stacked frames")
-        self.frames, self.F = frames, O // frames
-        self.dev = torch.device(device)
-        torch.cuda.set_device(self.dev)
-        self.T, self.B, self.O, self.A, self.H_pi, self.H_v = T, B_local, O, A, H_pi, H_v
-        self.hp = hp
-        # experience replay: B_fresh of the B columns of an update arrive from the host, the rest from the store
-        self.B_fresh = check_replay_args(B_local, replay_slabs, replay_columns)
-        self.replay_slabs, self.replay_columns = int(replay_slabs), int(replay_columns)
-        if self.replay_slabs and process_group is not None:
-            raise ValueError("experience replay runs on one device: the store is not sharded over a process group")
-        # off-policy diagnostics of every update (impala_vtrace_loss_diag); every rank must agree on it
-        self.diagnostics = bool(diagnostics)
-        # logged float64 values after the gradient in `comm`; PopArt forms its statistics from the eight sums
-        self.n_extra = 12 if self.diagnostics or self.popart else 4
-        self.mode = _cabi.MODES[mode]
+                 mode: str = "reference", process_group=None, use_graph: bool = True, slabs: int = 2,
+                 replay_seed: int = 0, lr_lambda=None, lr_table=None, **options):
+        # the options, the update rule and the schedule, checked before any device work; the default rule - Adam at
+        # 0.95 * hp.lr - keeps impala_clip_adam with the rate as a launch argument
+        o = self.options = LearnerOptions(**options)
+        self.optim = optim_config(hp, o.optimizer, o.optimizer_kwargs, lr_lambda, lr_table)
         self.pg = process_group
         self.world = 1
         if process_group is not None:
             import torch.distributed as dist
 
             self.world = dist.get_world_size(process_group)
+        # B_fresh of the B columns of an update arrive from the host (the rest from the replay store)
+        self.B_fresh, self.N_pi, self.obs_code, self.act_kind, self.reward_clip_code = o.check(
+            B_local, O, A, H_pi, H_v, self.world)
+        if not torch.cuda.is_available():
+            raise _cabi.ImpalaCudaError("LearnerEngine needs a CUDA device; there is no CPU path")
+        self.lib = _cabi.lib()
+        # the options the step reads; every rank must agree on diagnostics and PopArt (the length of `comm`)
+        self.gaussian = self.act_kind == _cabi.ACT_GAUSSIAN
+        self.shared_torso, self.popart, self.diagnostics = bool(o.shared_torso), bool(o.popart), bool(o.diagnostics)
+        self.popart_beta, self.replay_slabs = float(o.popart_beta), int(o.replay_slabs)
+        self.frames, self.F = o.frames, O // o.frames
+        self.dev = torch.device(device)
+        torch.cuda.set_device(self.dev)
+        self.T, self.B, self.O, self.A, self.H_pi, self.H_v = T, B_local, O, A, H_pi, H_v
+        self.hp = hp
+        # logged float64 values after the gradient in `comm`; PopArt forms its statistics from the eight sums
+        self.n_extra = 12 if o.diagnostics or o.popart else 4
+        self.mode = _cabi.MODES[mode]
         self.global_batch = int(global_batch if global_batch is not None else B_local * self.world)
         self.inv_batch = 1.0 / self.global_batch
         self.use_graph = use_graph
@@ -242,11 +290,12 @@ class LearnerEngine:
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts (replay: the host slabs
         # hold the B_fresh columns that cross the host link, the device slabs the B columns trained on)
-        train_off, train_bytes = _cabi.batch_layout(T, B_local, O, A, obs_dtype, frames, action_dist)
+        train_off, train_bytes = _cabi.batch_layout(T, B_local, O, A, o.obs_dtype, o.frames, o.action_dist)
         self.slab_off, self.slab_bytes = train_off, train_bytes
         if self.replay_slabs:
-            self.slab_off, self.slab_bytes = _cabi.batch_layout(T, self.B_fresh, O, A, obs_dtype, frames, action_dist)
-        self.fields = ((("obs", np.uint8 if obs_dtype == "uint8" else np.float32),) + _BATCH_FIELDS[1:])
+            self.slab_off, self.slab_bytes = _cabi.batch_layout(T, self.B_fresh, O, A, o.obs_dtype, o.frames,
+                                                                o.action_dist)
+        self.fields = ((("obs", np.uint8 if o.obs_dtype == "uint8" else np.float32),) + _BATCH_FIELDS[1:])
         if self.gaussian:  # float32 action samples
             self.fields = self.fields[:2] + (("actions", np.float32),) + self.fields[3:]
         self.n_slabs = slabs
@@ -272,7 +321,7 @@ class LearnerEngine:
         self.slab_free = [torch.cuda.Event() for _ in range(slabs)]   # last consumer of slab done
         self._slab_used = [False] * slabs
         if self.replay_slabs:
-            self.sampler = ReplaySampler(replay_seed, self.replay_slabs, self.B_fresh, self.replay_columns)
+            self.sampler = ReplaySampler(replay_seed, self.replay_slabs, self.B_fresh, o.replay_columns)
             self.store = torch.zeros(self.replay_slabs + 2, self.slab_bytes, dtype=torch.uint8, device=self.dev)
             self.d_plans = [torch.zeros(B_local, 2, dtype=torch.int32, device=self.dev) for _ in range(slabs)]
             self.h_plans = [torch.zeros(B_local, 2, dtype=torch.int32).pin_memory() for _ in range(slabs)]
@@ -299,12 +348,12 @@ class LearnerEngine:
         self.ws_vf = torch.zeros(self.ws_vf_bytes, dtype=torch.uint8, device=self.dev)
         # byte observations: O > 128 runs the networks on the bytes (impala_mlp_{forward,backward}_u8); narrower
         # observations are widened once per step into this float32 copy for the float kernels
-        self.obs_u8_native = obs_dtype == "uint8" and O > 128
-        self.obs_f32 = (torch.zeros((T + 1) * B_local * O, **f32) if obs_dtype == "uint8" and not self.obs_u8_native
+        self.obs_u8_native = o.obs_dtype == "uint8" and O > 128
+        self.obs_f32 = (torch.zeros((T + 1) * B_local * O, **f32) if o.obs_dtype == "uint8" and not self.obs_u8_native
                         else None)
         # frames > 1: the dense rows the kernels read, rebuilt from the slab's frames once per step
         self.obs_dense = None
-        if frames > 1:
+        if o.frames > 1:
             self.obs_dense = self.obs_f32 if self.obs_f32 is not None else torch.zeros(
                 (T + 1) * B_local * O, dtype=torch.uint8 if self.obs_u8_native else torch.float32, device=self.dev)
         ws_fn = (self.lib.impala_vtrace_loss_diag_workspace if self.n_extra == 12
@@ -313,7 +362,7 @@ class LearnerEngine:
         self.ws_vt = torch.zeros(self.ws_vt_bytes, dtype=torch.uint8, device=self.dev)  # zeroed once
         # ring of 4 tickets: [4 scalars | 2 norms | peer error | pad (| 8 off-policy sums) (| 5 PopArt statistics |
         # pad)]
-        self.h_scalars = torch.zeros(4, 24 if self.popart else 16 if self.diagnostics else 8,
+        self.h_scalars = torch.zeros(4, 24 if o.popart else 16 if o.diagnostics else 8,
                                      dtype=torch.float64).pin_memory()
         self._scalar_events = [torch.cuda.Event() for _ in range(4)]
         self._ticket = 0
@@ -498,7 +547,7 @@ class LearnerEngine:
 
     def fill_host(self, batch: dict, slot: int = 0) -> None:
         for name, _ in self.fields:
-            if name == "obs" and self.obs_dtype == "uint8" and np.asarray(batch["obs"]).dtype != np.uint8:
+            if name == "obs" and self.options.obs_dtype == "uint8" and np.asarray(batch["obs"]).dtype != np.uint8:
                 raise ValueError("a uint8-observation engine takes uint8 obs arrays")
             np.copyto(self.h_views[slot][name], batch[name])
 

@@ -58,6 +58,7 @@ swapping the class therefore changes training dynamics, not only speed (INTEGRAT
 from __future__ import annotations
 
 import copy
+import dataclasses
 import queue
 import sys
 import threading
@@ -68,9 +69,8 @@ import numpy as np
 import torch
 import torch.multiprocessing as mp
 
-from . import _cabi
-from .optim import POPART_BETA, check_popart_args, optim_config
-from .replay import check_replay_args
+from .engine import LearnerOptions, engine_from_cfg
+from .optim import optim_config
 
 PKEYS = ("model.0.weight", "model.0.bias", "model.3.weight", "model.3.bias")
 
@@ -182,13 +182,31 @@ def pack_trajectory(views: dict, b: int, traj, T: int, obs=None) -> float:
     return float(r.sum(dtype=torch.float64))  # summed as received (float64 from actor.py), like learner.py:108
 
 
-def _dims(policy, value_fn):
-    """(O, policy outputs, H_pi, H_v) of the two modules."""
+def _dims(policy, value_fn, action_dist):
+    """(O, A, H_pi, H_v) of the two modules: A actions, or the action dimensions of a Gaussian policy, whose 2A outputs
+    are [mean | log std]."""
     sd_p, sd_v = policy.state_dict(), value_fn.state_dict()
     H_pi, O = sd_p[PKEYS[0]].shape
-    A = sd_p[PKEYS[2]].shape[0]
+    A = int(sd_p[PKEYS[2]].shape[0])
     H_v = sd_v[PKEYS[0]].shape[0]
-    return int(O), int(A), int(H_pi), int(H_v)
+    if action_dist == "gaussian":
+        if A % 2:
+            raise ValueError(f"a Gaussian policy has 2A outputs [mean | log std]; this policy has {A}")
+        A //= 2
+    return int(O), A, int(H_pi), int(H_v)
+
+
+def _check_ring(q, options, B_fresh: int) -> None:
+    """A RingQueue (the queue with `collect_batch`) fills slabs the engine DMAs as they are, so it must hold what the
+    options and B_fresh describe.  A plain queue carries reference trajectories, which the learner packs itself."""
+    if not hasattr(q, "collect_batch"):
+        return
+    for want, have, what in ((options.action_dist, q.action_dist, "{} actions"),
+                             (options.obs_dtype, q.obs_dtype, "{} observations"),
+                             (options.frames, q.frames, "{} frames per observation"),
+                             (B_fresh, q.B, "{} trajectories per update (batch_size - replay_columns)")):
+        if want != have:
+            raise ValueError(f"the learner takes {what.format(want)}, the RingQueue was built for {what.format(have)}")
 
 
 class _Publisher:
@@ -288,71 +306,26 @@ class _Publisher:
 class Learner:
     def __init__(self, id, hparams, policy, value_fn, q, update_counter, log_path=None,
                  timeout=200, device="cuda:0", mode="reference", devices=None, publish_every=1,
-                 evaluator=None, obs_dtype="float32", frames=1, diagnostics=False,
-                 replay_slabs=0, replay_columns=0, optimizer="adam", optimizer_kwargs=None, lr_lambda=None,
-                 popart=False, popart_beta=POPART_BETA, reward_clip=None, action_dist="categorical",
-                 shared_torso=False):
+                 evaluator=None, lr_lambda=None, **options):
         self.id = id
-        # action distribution: "gaussian" = a diagonal Gaussian policy with 2A outputs [mean | log std]
-        _cabi.act_kind_code(action_dist)
-        self.action_dist = action_dist
-        if action_dist == "gaussian":
-            n_out = _dims(policy, value_fn)[1]
-            if n_out % 2 or not 2 <= n_out <= 2 * _cabi.MAX_GAUSSIAN_DIMS:
-                raise ValueError(f"a Gaussian policy has 2A outputs [mean | log std] for 1 <= A <= "
-                                 f"{_cabi.MAX_GAUSSIAN_DIMS}; this policy has {n_out}")
-        if hasattr(q, "collect_batch") and getattr(q, "action_dist", "categorical") != action_dist:
-            raise ValueError(f"the RingQueue holds {getattr(q, 'action_dist', 'categorical')} actions, "
-                             f"the learner was built for action_dist={action_dist!r}")
-        # shared torso (one hidden layer feeding both heads; engine.py): checked here, in the launching process
-        from .engine import check_shared_torso
-
-        _, n_out, H_pi, H_v = _dims(policy, value_fn)
-        self.shared_torso = check_shared_torso(shared_torso, H_pi, H_v, n_out)
-        # reward clipping inside the V-trace kernel: checked here, in the launching process
-        _cabi.reward_clip_code(reward_clip)
-        self.reward_clip = reward_clip
-        # PopArt value normalization: checked here, in the launching process
-        self.popart_beta = check_popart_args(popart, popart_beta)
-        self.popart = bool(popart)
-        self.popart_init = None  # {"mu", "nu"} of the folded value_fn (load() of a PopArt checkpoint sets it)
-        # update rule and learning-rate schedule: checked and tabulated here, in the launching process (a lambda
-        # need not pickle; data-parallel worker ranks receive the table)
-        self.optimizer, self.optimizer_kwargs = optimizer, dict(optimizer_kwargs or {})
-        self.optim = optim_config(hparams, optimizer, optimizer_kwargs, lr_lambda)
-        if obs_dtype not in ("float32", "uint8"):
-            raise ValueError(f"obs_dtype must be 'float32' or 'uint8', got {obs_dtype!r}")
-        if hasattr(q, "collect_batch") and getattr(q, "obs_dtype", "float32") != obs_dtype:
-            raise ValueError(f"the RingQueue holds {getattr(q, 'obs_dtype', 'float32')} observations, "
-                             f"the learner was built for {obs_dtype}")
-        if frames != 1 and (frames < 1 or _dims(policy, value_fn)[0] % frames):
-            raise ValueError(f"{_dims(policy, value_fn)[0]} observation features do not split into {frames} "
-                             "stacked frames")
-        if hasattr(q, "collect_batch") and getattr(q, "frames", 1) != frames:
-            raise ValueError(f"the RingQueue stores observations as {getattr(q, 'frames', 1)} frames, "
-                             f"the learner was built for frames={frames}")
+        self.devices = [str(d) for d in devices] if devices else [str(device)]
+        # the options, checked here, in the launching process, as every engine checks them; the schedule is
+        # tabulated here (a lambda need not pickle; data-parallel worker ranks receive the table)
+        o = self.options = LearnerOptions(**options)
+        self.optim = optim_config(hparams, o.optimizer, o.optimizer_kwargs, lr_lambda)
         # experience replay: B_fresh trajectories per update come off the queue, replay_columns out of HBM
-        self.B_fresh = check_replay_args(hparams.batch_size, replay_slabs, replay_columns)
-        self.replay_slabs, self.replay_columns = int(replay_slabs), int(replay_columns)
-        if self.replay_slabs and devices and len(devices) > 1:
-            raise ValueError(f"experience replay runs on one device, got devices={list(devices)}")
-        if hasattr(q, "collect_batch") and self.replay_slabs and q.B != self.B_fresh:
-            raise ValueError(f"with replay_columns={replay_columns} an update takes batch_size - replay_columns = "
-                             f"{self.B_fresh} trajectories from the queue; the RingQueue was built for {q.B}")
-        self.obs_dtype = obs_dtype  # "uint8": byte observations end to end (ring / slabs / MLP kernels)
-        self.frames = frames  # > 1: each of the stacked frames stored once (ring / slabs), unstacked on the device
+        self.B_fresh = o.check(hparams.batch_size, *_dims(policy, value_fn, o.action_dist), len(self.devices)).B_fresh
+        _check_ring(q, o, self.B_fresh)
+        self.popart_init = None  # {"mu", "nu"} of the folded value_fn (load() of a PopArt checkpoint sets it)
         self.hp = hparams
         self.policy = policy
         self.value_fn = value_fn
         self.timeout = timeout
         self.q = q
         self.update_counter = update_counter
-        self.devices = [str(d) for d in devices] if devices else [str(device)]
         self.device = self.devices[0]
         self.mode = mode
         self.publish_every = max(1, int(publish_every))
-        # off-policy diagnostics of every update (ratio clipping, behaviour KL, value explained variance)
-        self.diagnostics = bool(diagnostics)
         for name, mod in (("policy", policy), ("value_fn", value_fn)):
             if any(p.is_cuda for p in mod.parameters()):
                 raise ValueError(
@@ -381,9 +354,9 @@ class Learner:
             # staging ring every rank can DMA its shard from (created before the fork)
             from .ring import RingQueue
 
-            c = self._cfg()
+            c, o = self._cfg(), self.options
             self._stage_ring = RingQueue(self.hp.max_timesteps, self.hp.batch_size, c["O"], c["A"], slabs=2,
-                                         obs_dtype=self.obs_dtype, frames=self.frames, action_dist=self.action_dist)
+                                         obs_dtype=o.obs_dtype, frames=o.frames, action_dist=o.action_dist)
         self.p.start()
         print(f"[main] Started learner_{self.id} with pid {self.p.pid}")
 
@@ -399,37 +372,22 @@ class Learner:
 
     # ------------------------------------------------------------------ helpers
     def _cfg(self):
-        O, A, H_pi, H_v = _dims(self.policy, self.value_fn)
-        if self.action_dist == "gaussian":
-            A //= 2  # action dimensions; the policy has 2A outputs
+        """The JSON every rank builds its engine from (engine.engine_from_cfg): shapes, mode, hp and the fields of
+        LearnerOptions.  The learning-rate table travels apart, in the init-state file (dp.write_init_state)."""
+        O, A, H_pi, H_v = _dims(self.policy, self.value_fn, self.options.action_dist)
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
-                    obs_dtype=self.obs_dtype, frames=self.frames, diagnostics=self.diagnostics,
-                    replay_slabs=self.replay_slabs, replay_columns=self.replay_columns, optimizer=self.optimizer,
-                    optimizer_kwargs=self.optimizer_kwargs, popart=self.popart, popart_beta=self.popart_beta,
-                    reward_clip=self.reward_clip, action_dist=self.action_dist, shared_torso=self.shared_torso)
+                    **dataclasses.asdict(self.options))
 
     def _make_engine(self, process_group=None, world=1):
-        from .engine import LearnerEngine
-
-        c = self._cfg()
-        if c["B"] % world:
-            raise ValueError(f"batch_size {c['B']} does not divide over {world} devices")
-        eng = LearnerEngine(c["T"], c["B"] // world, c["O"], c["A"], c["H_pi"], c["H_v"], self.hp,
-                            global_batch=c["B"], device=self.device, mode=self.mode, process_group=process_group,
-                            obs_dtype=c["obs_dtype"], frames=c["frames"], diagnostics=c["diagnostics"],
-                            replay_slabs=c["replay_slabs"], replay_columns=c["replay_columns"],
-                            optimizer=c["optimizer"], optimizer_kwargs=c["optimizer_kwargs"],
-                            lr_table=self.optim.lr_table, popart=c["popart"], popart_beta=c["popart_beta"],
-                            reward_clip=c["reward_clip"], action_dist=c["action_dist"],
-                            shared_torso=c["shared_torso"])
+        eng = engine_from_cfg(self._cfg(), world, self.device, process_group, self.optim.lr_table)
         eng.load_state(self._init_state(), self._popart_init())
         return eng
 
     def _popart_init(self):
         """The statistics the folded value_fn goes with: those of a loaded checkpoint, else None (mu 0, nu 1)."""
-        return dict(self.popart_init) if self.popart and self.popart_init is not None else None
+        return dict(self.popart_init) if self.options.popart and self.popart_init is not None else None
 
     def _init_state(self):
         return {"policy": {k: v.detach().cpu() for k, v in self.policy.state_dict().items()},
@@ -440,7 +398,7 @@ class Learner:
         weights (checkpoints, end of run).  The per-update path is `_Publisher.post`."""
         pub.drain()
         st = eng.state()  # the value function folded into reward units under PopArt
-        if self.popart:
+        if self.options.popart:
             s = eng.popart_stats()
             self.popart_init = {"mu": s["mu"], "nu": s["nu"]}  # what save() writes next to the folded value_fn
         with torch.no_grad():
@@ -472,7 +430,7 @@ class Learner:
         own `utils.test_policy` when this class is deployed inside that repo."""
         if self.evaluator is not None:
             return self.evaluator(policy)
-        if self.action_dist == "gaussian":  # the reference's test_policy refuses continuous environments
+        if self.options.action_dist == "gaussian":  # the reference's test_policy refuses continuous environments
             print(f"[learner_{self.id}] evaluation skipped: a Gaussian policy is evaluated through evaluator= only")
             return None
         try:
@@ -531,7 +489,7 @@ class Learner:
         diagnostics when they are on)."""
         if self.hp.verbose >= 1:
             diag = (f", rho clipped {100.0 * sc['rho_clip_fraction']:.1f} %, kl {sc['kl_behaviour_current']:.4f}"
-                    if self.diagnostics else "")
+                    if self.options.diagnostics else "")
             print(f"[learner_{self.id}] update {n}: batch mean reward {reward:.2f}, "
                   f"loss {sc['total_loss']:.2f}{diag}")
         if writer is None:
@@ -542,11 +500,11 @@ class Learner:
                           ("loss/policy_entropy", sc["policy_entropy"]),
                           ("loss/total_loss", sc["total_loss"])):
             writer.add_scalar(f"{tag}/{name}", val, n)
-        if self.diagnostics:
+        if self.options.diagnostics:
             for name in ("log_ratio_mean", "rho_clip_fraction", "c_clip_fraction", "kl_behaviour_current"):
                 writer.add_scalar(f"{tag}/offpolicy/{name}", sc[name], n)
             writer.add_scalar(f"{tag}/value/explained_variance", sc["value_explained_variance"], n)
-        if self.popart:
+        if self.options.popart:
             writer.add_scalar(f"{tag}/popart/mu", sc["popart_mu"], n)
             writer.add_scalar(f"{tag}/popart/sigma", sc["popart_sigma"], n)
 
@@ -739,9 +697,9 @@ class Learner:
         """Reference checkpoint keys.  Shared torso: the two state dicts are the policy and value views of the one
         network (both hold the torso) and "shared_torso" is True; the policy view is an MlpPolicy state dict."""
         ckpt = {"policy_state_dict": self.policy.state_dict(), "value_fn_state_dict": self.value_fn.state_dict()}
-        if self.shared_torso:
+        if self.options.shared_torso:
             ckpt["shared_torso"] = True
-        if self.popart:  # value_fn is folded (reward units); the statistics that unfold it
+        if self.options.popart:  # value_fn is folded (reward units); the statistics that unfold it
             ckpt["popart"] = dict(self.popart_init or {"mu": 0.0, "nu": 1.0})
         torch.save(ckpt, path)
 
