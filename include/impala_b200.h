@@ -86,13 +86,18 @@ int impala_batch_layout_frames(int T, int B, int F, int frames, int A, int obs_d
  *   IMPALA_ACT_CATEGORICAL: A actions; beh_logits (T,B,A) f32, actions (T,B) i32 (indices).
  *   IMPALA_ACT_GAUSSIAN: diagonal Gaussian over A action dimensions; the behaviour record is the actor's
  *     policy output [m | s] (means, then log standard deviations), beh_logits (T,B,2A) f32, and the action the
- *     unsquashed sample m + e^s eps, actions (T,B,A) f32. */
+ *     unsquashed sample m + e^s eps, actions (T,B,A) f32.
+ *   IMPALA_ACT_MULTI_DISCRETE(K): K independent categorical heads (a gym MultiDiscrete space), 1 <= K <= 16, of
+ *     n_k >= 2 actions each; A = N = sum_k n_k policy outputs, head k owning [s_k, s_k + n_k) with s_k = sum_{i<k} n_i.
+ *     beh_logits (T,B,N) f32, actions (T,B,K) i32 (one index per head).  K = 1 is the categorical layout. */
 #define IMPALA_ACT_CATEGORICAL 0
 #define IMPALA_ACT_GAUSSIAN 1
+#define IMPALA_ACT_MULTI_DISCRETE(K) (0x100 | (K))
 
 /* impala_batch_layout_frames for the action distribution act_kind: IMPALA_ACT_CATEGORICAL is exactly
- * impala_batch_layout_frames, IMPALA_ACT_GAUSSIAN widens beh_logits to (T,B,2A) f32 and actions to (T,B,A) f32.
- * An unknown act_kind returns IMPALA_ERR_BAD_ARG. */
+ * impala_batch_layout_frames, IMPALA_ACT_GAUSSIAN widens beh_logits to (T,B,2A) f32 and actions to (T,B,A) f32,
+ * IMPALA_ACT_MULTI_DISCRETE(K) widens actions to (T,B,K) i32.  An unknown act_kind, K outside 1..16 or A < 2K
+ * returns IMPALA_ERR_BAD_ARG. */
 int impala_batch_layout_act(int T, int B, int F, int frames, int A, int obs_dtype, int act_kind, int64_t offsets[6],
                             int64_t* total_bytes);
 
@@ -327,6 +332,26 @@ int impala_vtrace_loss_gauss(const float* cur_params, const float* beh_params, c
                              int64_t workspace_bytes, int T, int B, int A, float gamma, float rho_bar, float c_bar,
                              float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch, int mode,
                              double* diag, const double* popart, int reward_clip, void* stream);
+
+/* The V-trace loss kernel of impala_vtrace_loss_rclip for multi-discrete policies (IMPALA_ACT_MULTI_DISCRETE(K)):
+ * K <= 16 independent softmax heads over A = N = sum_k n_k <= 32 policy outputs, host_heads[k] = n_k >= 2 (read at
+ * call time and passed to the kernel by value, so a captured graph keeps them).  cur_logits / beh_logits / dlogits
+ * (T,B,N); actions (T,B,K) i32, a_k in [0, n_k).  With p the softmax within a head (z[s_k : s_k + n_k]):
+ *   log pi(a) = sum_k log p_k(a_k), the same for mu with the behaviour logits; ratio, clipping, V-trace, vs and
+ *   pg_adv as for categorical policies.  policy_loss = sum -log pi(a) pg_adv, policy_entropy = sum_k H_k, each
+ *   sum_b .. inv_batch.  For j in head k:
+ *   dz_j = inv_batch [policy_loss_c pg_adv (p_j - [j = s_k + a_k]) + entropy_c p_j (log p_j + H_k)]; zero at padded
+ *   steps.  diag[4] = sum KL(mu || pi) = sum_k KL_k.  K = 1 is impala_vtrace_loss_rclip's categorical policy.
+ * diag, popart, reward_clip and the workspace as impala_vtrace_loss_gauss (impala_vtrace_loss[_diag]_workspace(T, B,
+ * N)).  K > 16 or N > 32 returns IMPALA_ERR_UNSUPPORTED_SHAPE; a NULL host_heads, K < 1, an n_k < 2, sum_k n_k != A,
+ * a popart without diag, an unknown reward_clip and what impala_vtrace_loss refuses return IMPALA_ERR_BAD_ARG. */
+int impala_vtrace_loss_md(const float* cur_logits, const float* beh_logits, const int32_t* actions,
+                          const float* rewards, const uint8_t* done, const int32_t* lens, const float* v, float* vs,
+                          float* pg_adv, float* dlogits, float* dv, double* scalars, void* workspace,
+                          int64_t workspace_bytes, int T, int B, int A, float gamma, float rho_bar, float c_bar,
+                          float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch, int mode,
+                          double* diag, const double* popart, int reward_clip, const int32_t* host_heads, int K,
+                          void* stream);
 
 /* Per-group gradient clipping + Adam in one launch (learner.py:176-183).
  *   params/m/v: f32 [n_total]; grad: f64 [n_total] (the possibly all-reduced sum);

@@ -27,7 +27,11 @@ impala_vtrace_loss_rclip in both modes alone on the engine's buffers (median of 
 L2 flushed before each).
 --compare-shared alternates a two-network engine and a shared-torso engine (shared_torso=True: one hidden layer
 feeding the policy and the value head) on the same batch the same way, and reports both steps' launches.  Byte
-observations for the Atari RAM and MinAtar shapes, as --compare-popart."""
+observations for the Atari RAM and MinAtar shapes, as --compare-popart.
+--compare-heads (configs md_c4, md_ram) alternates a categorical engine at A = N and a multi-discrete engine
+(action_dist="multi_discrete" with the config's heads, N = sum of them) on batches of the same shapes the same way,
+and times impala_vtrace_loss against impala_vtrace_loss_md alone on each engine's buffers (median of 200 launches
+each, alternating, L2 flushed before each)."""
 import argparse
 import os
 import statistics
@@ -41,7 +45,10 @@ from torched_impala_b200 import synth  # noqa: E402
 from torched_impala_b200.engine import LearnerEngine  # noqa: E402
 from torched_impala_b200.utils import default_hparams  # noqa: E402
 
-CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256), "c5": dict(T=100, B=8192, O=64, A=4, H=512),
+CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256),
+       # multi-discrete policies (--compare-heads): A = N = sum(heads) policy outputs
+       "md_c4": dict(T=20, B=4096, O=24, A=8, H=256, heads=(3, 3, 2)),
+       "md_ram": dict(T=20, B=4096, O=128, A=20, H=256, heads=(3, 3, 2, 2, 5, 5)), "c5": dict(T=100, B=8192, O=64, A=4, H=512),
        "c3": dict(T=20, B=1024, O=24, A=4, H=256), "c2": dict(T=20, B=256, O=4, A=2, H=32),
        # c4 with 512 hidden units: the wide forward at one K atom (two passes of 256) and the wide backward
        "c4h512": dict(T=20, B=4096, O=24, A=4, H=512),
@@ -74,6 +81,8 @@ ap.add_argument("--compare-popart", action="store_true", help="alternate engines
 ap.add_argument("--compare-replay", action="store_true", help="alternate engines without / with experience replay")
 ap.add_argument("--compare-reward-clip", action="store_true", help="alternate engines without / with reward clipping")
 ap.add_argument("--compare-shared", action="store_true", help="alternate two networks and a shared-torso network")
+ap.add_argument("--compare-heads", action="store_true",
+                help="alternate a categorical engine at A = N and a multi-discrete engine (configs md_c4, md_ram)")
 ap.add_argument("--replay-slabs", type=int, default=2, help="past fresh batches in the pool of --compare-replay")
 ap.add_argument("--replay-columns", type=int, default=None, help="replayed columns of --compare-replay (default B/2)")
 a = ap.parse_args()
@@ -115,6 +124,13 @@ if a.compare_shared:
     arms = {"two networks": arms["default"], "shared torso": arms["default"]}
     shared_arm = {"shared torso": dict(shared_torso=True)}
     obs_dt = {name: "uint8" if a.config in ("ram", "ram4", "ram8", "minatar", "ram_a6") else "float32" for name in arms}
+heads_arm = {}
+if a.compare_heads:
+    if "heads" not in w:
+        raise SystemExit(f"--compare-heads takes a multi-discrete config (md_c4, md_ram), not {a.config}")
+    md_name = f"multi-discrete heads {w['heads']}"
+    arms = {f"categorical A={w['A']}": arms["default"], md_name: arms["default"]}
+    heads_arm = {md_name: dict(action_dist="multi_discrete", action_heads=w["heads"])}
 replay_arm = {}
 if a.compare_replay:
     Br = w["B"] // 2 if a.replay_columns is None else a.replay_columns
@@ -130,7 +146,7 @@ for name, tc in arms.items():
     k = n_frames.get(name, 1)
     eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k,
                         diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}), **popart_arm.get(name, {}),
-                        **rclip_arm.get(name, {}), **shared_arm.get(name, {}))
+                        **rclip_arm.get(name, {}), **shared_arm.get(name, {}), **heads_arm.get(name, {}))
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
     byte_obs = (a.compare_obs or ((a.compare_frames or a.compare_replay) and dt == "uint8")
                 or ((a.compare_diag or a.compare_popart or a.compare_reward_clip or a.compare_shared) and dt == "uint8"))
@@ -142,6 +158,8 @@ for name, tc in arms.items():
                                  frames=a.frames)
         if k == 1:
             batch = synth.stack_frames(batch, a.frames)
+    elif name in heads_arm:
+        batch = synth.make_md_batch(1, w["T"], w["B"], w["O"], w["heads"])
     else:
         batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if byte_obs else "normal")
     if dt == "float32":
@@ -364,6 +382,41 @@ if a.compare_reward_clip:  # the V-trace + loss kernel alone, without and with e
         k1 = statistics.median(tk[name])
         print(f", {name} {k1:.1f} us ({k1 - k0:+.1f} us, {100 * (k1 / k0 - 1):+.1f} %)", end="")
     print()
+if a.compare_heads:  # the V-trace + loss kernel alone, categorical against multi-discrete, each on its engine's buffers
+    import ctypes
+
+    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    tail = (w["T"], w["B"], w["A"], hp.gamma, hp.rho_bar, hp.c_bar, hp.v_loss_c, hp.policy_loss_c, hp.entropy_c,
+            1.0 / w["B"], 0)
+
+    def _ins(e):
+        d = e.d_views[0]
+        return (P(e.logits), P(d["beh_logits"]), P(d["actions"]), P(d["rewards"]), P(d["done"]), P(d["lens"]),
+                P(e.values), P(e.vs), P(e.pg_adv), P(e.dlogits), P(e.dv), ctypes.c_void_p(e.comm.data_ptr() + 8 * e.n_total),
+                P(e.ws_vt), e.ws_vt_bytes)
+
+    ec, em = engines[list(arms)[0]], engines[md_name]
+    hh = (ctypes.c_int32 * len(w["heads"]))(*w["heads"])
+    calls = {"impala_vtrace_loss": lambda st: ec.lib.impala_vtrace_loss(*_ins(ec), *tail, st),
+             "impala_vtrace_loss_md": lambda st: em.lib.impala_vtrace_loss_md(*_ins(em), *tail[:-1], tail[-1], None,
+                                                                              None, 0, hh, len(w["heads"]), st)}
+    tk = {name: [] for name in calls}
+    with torch.cuda.stream(em.stream):
+        st = ctypes.c_void_p(em.stream.cuda_stream)
+        for i in range(220):
+            for name, fn in calls.items():
+                flush.zero_()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(em.stream)
+                rc = fn(st)
+                e1.record(em.stream)
+                e1.synchronize()
+                assert rc == 0, (name, rc)
+                if i >= 20:
+                    tk[name].append(e0.elapsed_time(e1) * 1e3)
+    k0, k1 = statistics.median(tk["impala_vtrace_loss"]), statistics.median(tk["impala_vtrace_loss_md"])
+    print(f"V-trace + loss kernel {a.config}: impala_vtrace_loss (A={w['A']}) {k0:.1f} us, impala_vtrace_loss_md "
+          f"(heads {w['heads']}) {k1:.1f} us ({k1 - k0:+.1f} us, {100 * (k1 / k0 - 1):+.1f} %)")
 q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
                     "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 print(f"GPU (nvidia-smi): {q}")
@@ -399,3 +452,7 @@ if a.compare_shared:
     m0, m1 = statistics.median(ts["two networks"]), statistics.median(ts["shared torso"])
     print(f"shared torso {a.config}: {m1:.1f} us/step against {m0:.1f} ({m1 - m0:+.1f} us, {100 * (m1 / m0 - 1):+.1f} %), "
           f"launches {engines['shared torso'].launches_per_step} against {engines['two networks'].launches_per_step}")
+if a.compare_heads:
+    m0, m1 = statistics.median(ts[list(arms)[0]]), statistics.median(ts[md_name])
+    print(f"multi-discrete {a.config}: {m1:.1f} us/step against {m0:.1f} ({m1 - m0:+.1f} us, {100 * (m1 / m0 - 1):+.1f} %), "
+          f"launches {engines[md_name].launches_per_step} against {engines[list(arms)[0]].launches_per_step}")

@@ -6,6 +6,7 @@ missing, or a call returns non-zero, an exception is raised.
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -47,13 +48,36 @@ def reward_clip_code(reward_clip) -> int:
 
 ACT_CATEGORICAL = 0
 ACT_GAUSSIAN = 1
+ACT_MULTI_DISCRETE = 0x100  # IMPALA_ACT_MULTI_DISCRETE(K) = ACT_MULTI_DISCRETE | K
 ACT_DISTS = {"categorical": ACT_CATEGORICAL, "gaussian": ACT_GAUSSIAN}  # action distributions (IMPALA_ACT_*)
 MAX_GAUSSIAN_DIMS = 16  # action dimensions of impala_vtrace_loss_gauss (2A <= 32 policy outputs)
+MAX_HEADS = 16  # heads of impala_vtrace_loss_md (sum n_k <= 32 policy outputs)
+MAX_OUTPUTS = 32  # policy outputs of the MLP kernels
 
 
-def act_kind_code(action_dist: str) -> int:
+def check_heads(action_heads) -> tuple:
+    """The head sizes (n_0, .., n_K-1) of a multi-discrete policy as a tuple of ints: 1 <= K <= 16 heads of at least
+    two actions each, at most 32 outputs in all; anything else raises ValueError."""
+    heads = tuple(action_heads)
+    if not all(isinstance(n, numbers.Integral) and not isinstance(n, bool) for n in heads):
+        raise ValueError(f"action_heads must be integers, got {heads!r}")
+    heads = tuple(int(n) for n in heads)
+    if not 1 <= len(heads) <= MAX_HEADS:
+        raise ValueError(f"a multi-discrete policy takes 1 to {MAX_HEADS} heads, got {len(heads)}")
+    if min(heads) < 2:
+        raise ValueError(f"every head of a multi-discrete policy has at least 2 actions, got {heads}")
+    if sum(heads) > MAX_OUTPUTS:
+        raise ValueError(f"a multi-discrete policy takes at most {MAX_OUTPUTS} outputs in all, got sum{heads} = "
+                         f"{sum(heads)}")
+    return heads
+
+
+def act_kind_code(action_dist: str, action_heads=()) -> int:
+    """The IMPALA_ACT_* code of `action_dist`; "multi_discrete" carries its head count (check_heads)."""
+    if action_dist == "multi_discrete":
+        return ACT_MULTI_DISCRETE | len(check_heads(action_heads))
     if not isinstance(action_dist, str) or action_dist not in ACT_DISTS:
-        raise ValueError(f"action_dist must be one of {sorted(ACT_DISTS)}, got {action_dist!r}")
+        raise ValueError(f"action_dist must be one of {sorted(ACT_DISTS) + ['multi_discrete']}, got {action_dist!r}")
     return ACT_DISTS[action_dist]
 
 
@@ -107,6 +131,7 @@ SIGNATURES = {
     "impala_vtrace_loss_popart": (_i, [_p] * 14 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p]),
     "impala_vtrace_loss_rclip": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p]),
     "impala_vtrace_loss_gauss": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p]),
+    "impala_vtrace_loss_md": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p, _i, _p]),
     "impala_batch_layout_act": (_i, [_i] * 7 + [C.POINTER(_i64), C.POINTER(_i64)]),
     "impala_ingest_shard_act": (_i, [_p, _p] + [_i] * 9 + [_p]),
     "impala_batch_compose_act": (_i, [_p, _p, _i64, _p] + [_i] * 8 + [_p]),
@@ -163,17 +188,18 @@ def param_layout(O: int, H: int, N2: int):
 
 
 def batch_layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1,
-                 action_dist: str = "categorical"):
+                 action_dist: str = "categorical", action_heads=()):
     """Slab layout for networks of O observation features; frames > 1 stores the O / frames features of
     each stacked frame once (impala_batch_layout_frames); action_dist="gaussian" holds (T, B, 2A) behaviour
-    outputs and (T, B, A) float32 actions (impala_batch_layout_act)."""
+    outputs and (T, B, A) float32 actions, "multi_discrete" (T, B, A = sum action_heads) behaviour logits and
+    (T, B, K) int32 actions (impala_batch_layout_act)."""
     offs = (_i64 * 6)()
     total = _i64()
     if action_dist != "categorical":
         if frames < 1 or O % frames:
             raise ValueError(f"{O} observation features do not split into {frames} frames")
         check(lib().impala_batch_layout_act(T, B, O // frames, frames, A, obs_dtype_code(obs_dtype),
-                                            act_kind_code(action_dist), offs, C.byref(total)),
+                                            act_kind_code(action_dist, action_heads), offs, C.byref(total)),
               "impala_batch_layout_act")
     elif frames == 1:
         check(lib().impala_batch_layout_obs(T, B, O, A, obs_dtype_code(obs_dtype), offs, C.byref(total)),

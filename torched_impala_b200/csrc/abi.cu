@@ -24,12 +24,17 @@ static int64_t obs_bytes(int obs_dtype) {
     return obs_dtype == IMPALA_OBS_F32 ? 4 : obs_dtype == IMPALA_OBS_U8 ? 1 : 0;
 }
 
-static bool act_kind_ok(int act_kind) { return act_kind == IMPALA_ACT_CATEGORICAL || act_kind == IMPALA_ACT_GAUSSIAN; }
+// multi-discrete: 1 <= K <= 16 heads of at least two actions each among the A outputs
+static bool act_kind_ok(int act_kind, int A) {
+    if (act_kind == IMPALA_ACT_CATEGORICAL || act_kind == IMPALA_ACT_GAUSSIAN) return true;
+    const int K = impala_md_heads(act_kind);
+    return K >= 1 && K <= 16 && A >= 2 * K;
+}
 
 extern "C" int impala_batch_layout_act(int T, int B, int F, int frames, int A, int obs_dtype, int act_kind,
                                        int64_t offsets[6], int64_t* total_bytes) {
     const int64_t ob = obs_bytes(obs_dtype);
-    if (T < 1 || B < 1 || F < 1 || frames < 1 || A < 1 || ob == 0 || !act_kind_ok(act_kind) || !offsets ||
+    if (T < 1 || B < 1 || F < 1 || frames < 1 || A < 1 || ob == 0 || !act_kind_ok(act_kind, A) || !offsets ||
         !total_bytes)
         return IMPALA_ERR_BAD_ARG;
     const int64_t al = 256;

@@ -96,6 +96,13 @@ using VtArgsB = typename std::conditional<POPART, VtPopArgs,
                                           typename std::conditional<DIAG, VtDiagArgs, VtArgs>::type>::type;
 template <bool DIAG, bool POPART = false, bool RCLIP = false>
 using VtArgsT = typename std::conditional<RCLIP, VtClipArgs<VtArgsB<DIAG, POPART>>, VtArgsB<DIAG, POPART>>::type;
+// MD instantiations (on top of any of the above) take the multi-discrete heads as well, by value.
+template <class Base>
+struct VtMdArgs : Base {
+    unsigned head_mask;  // bit j set: policy output j is the first of a head (bit 0 always set)
+};
+template <bool DIAG, bool POPART = false, bool RCLIP = false, bool MD = false>
+using VtArgsM = typename std::conditional<MD, VtMdArgs<VtArgsT<DIAG, POPART, RCLIP>>, VtArgsT<DIAG, POPART, RCLIP>>::type;
 
 // The reward transform of the RCLIP instantiations (DeepMind's IMPALA `reward_clipping`), with compares and
 // selects rather than fminf / fmaxf so that a NaN reward stays NaN (as torch.clamp keeps it): abs_one is
@@ -249,6 +256,176 @@ __device__ __forceinline__ void gauss_terms(const float* __restrict__ pc, const 
     *kl2 = kl * kLog2e;
 }
 
+// ---- MD: multi-discrete (factorised categorical) policies.  Head k owns the policy outputs [s_k, s_k + n_k) of a
+// step's A = N outputs (bit s_k of the head mask hm), its action row holds K = popc(hm) indices a_k.  Head boundaries
+// are runtime values, so every sweep below walks the unrolled entries j with the head mask as a predicate (uniform
+// over the grid) and never indexes a register array with a runtime value: a head's log-sum-exp is an online one,
+// reset at the head's first entry, and the per-head values come back to the head's entries through a sweep in the
+// other direction.  Each head is shifted by its own first logit, x_j = z_j log2(e) - z_s log2(e) (one rounding), and
+// the shift cancels in log2 p_j = x_j - lse_k; the online maximum keeps every 2^(x - m) in (0, 1].  The sweeps read
+// the rows four logits at a time (md_chunk; step 4's second sweep re-reads, an L1 hit).  At AP = 32 the kernel is
+// bounded at 256 threads (255 registers): under the 512-thread bound of the other widths it spills.
+template <int AP, bool VEC>
+__device__ __forceinline__ void md_chunk(const float* __restrict__ p, unsigned elem, int A, int j0,
+                                         float (&q)[AP < 4 ? AP : 4]) {
+    if constexpr (VEC && AP == 2) {
+        const float2 v = __ldg(reinterpret_cast<const float2*>(p + elem * 2));
+        q[0] = v.x, q[1] = v.y;
+    } else if constexpr (VEC) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(p + elem * AP + j0));
+        q[0] = v.x, q[1] = v.y, q[2] = v.z, q[3] = v.w;
+    } else {
+#pragma unroll
+        for (int u = 0; u < (AP < 4 ? AP : 4); ++u) q[u] = j0 + u < A ? __ldg(p + elem * A + j0 + u) : 0.f;
+    }
+}
+// one entry x of a head's online log-sum-exp (base 2): m the running maximum, s = sum 2^(x_i - m); returns the
+// factor 2^-|x - m| and whether the maximum moved (the KL weight of the behaviour row rescales with them)
+__device__ __forceinline__ bool md_online(float x, float& m, float& s, float* e) {
+    const float d = x - m;
+    *e = ex2f(-fabsf(d));
+    const bool up = d > 0.f;
+    s = up ? fmaf(s, *e, 1.f) : s + *e, m = fmaxf(m, x);
+    return up;
+}
+// Step 2, reduced as the two rows and the K indices load (base 2, like the categorical terms):
+//   *lp2 = log2 pi(a) = sum_k (x_{s_k + a_k} - lse_k),
+//   *lr2 = log2 pi(a) - log2 mu(a) = sum_k [d_{s_k + a_k} - log2 sum_j mu_j 2^d_j],
+//   *kl2 (DIAG) = sum_k KL_k / ln 2 = sum_k [log2 sum_j mu_j 2^d_j - sum_j mu_j d_j],
+// with d_j = ((z_j - zb_j) - (z_s - zb_s)) log2(e) measured from the head's first entry s (both terms are invariant to
+// it): a head the current policy shifts as a whole against the behaviour (softmax-invariant) gives d = 0, so 2^d
+// overflows only where the logit differences within one head spread over ~88 nats.
+// The ratio and KL come from the per-entry differences d_j (the behaviour perturbs the policy by little, so they are
+// small and exact to a rounding of their own size), not from two log-sum-exps of shifted logits of magnitude ~10 per
+// head: K heads of those would add K such roundings to the log ratio.  The sums over a head are online ones under the
+// behaviour row's maximum; a closed head folds into a product (each sum in [1, n_k] or near 1), so a row costs few lg2.
+// Returns the taken mask: bit s_k + a_k for every head (an index outside its head sets no bit).
+constexpr int kMaxHeads = 16;
+template <int AP, bool VEC, bool DIAG>
+__device__ __forceinline__ unsigned md_terms(const float* __restrict__ pc, const float* __restrict__ pb,
+                                             const int32_t* __restrict__ pa, unsigned elem, int A, unsigned hm,
+                                             float* lp2, float* lr2, float* kl2) {
+    constexpr int W = AP < 4 ? AP : 4;
+    const int K = __popc(hm);
+    unsigned taken = 0u, rest = hm;
+#pragma unroll
+    for (int k = 0; k < kMaxHeads; ++k) {
+        if (k < K) {
+            const int ak = __ldg(pa + elem * (unsigned)K + k), s = __ffs(rest) - 1;
+            rest &= rest - 1u;
+            const int n = (rest ? __ffs(rest) - 1 : A) - s;
+            if ((unsigned)ak < (unsigned)n) taken |= 1u << (s + ak);
+        }
+    }
+    // current row: shift sh, maximum m, sum s; behaviour row: shb, mb, sb; ub = sum 2^(xb - mb) 2^d,
+    // wb = sum 2^(xb - mb) (-d).  Closed heads: msc = sum of the maxima, prc / prb / pru = products of the sums
+    float shc = 0.f, shb = 0.f, rs = 0.f, mc = 0.f, sc = 1.f, mb = 0.f, sb = 1.f, ub = 1.f, wb = 0.f;
+    float msc = 0.f, prc = 1.f, prb = 1.f, pru = 1.f, klw = 0.f, za = 0.f, da = 0.f;
+#pragma unroll
+    for (int j0 = 0; j0 < AP; j0 += W) {
+        float zc[W], zb[W];
+        md_chunk<AP, VEC>(pc, elem, A, j0, zc);
+        md_chunk<AP, VEC>(pb, elem, A, j0, zb);
+#pragma unroll
+        for (int u = 0; u < W; ++u) {
+            const int j = j0 + u;
+            if (j < A) {
+                const bool st = (hm >> j) & 1u;
+                if (st) {
+                    if (j > 0) {  // close the previous head
+                        msc += mc, prc *= sc, prb *= sb, pru *= ub;
+                        if constexpr (DIAG) klw += __fdividef(wb, sb);
+                    }
+                    shc = -zc[u] * kLog2e, shb = -zb[u] * kLog2e, rs = zc[u] - zb[u];
+                }
+                const float xc = fmaf(zc[u], kLog2e, shc), xb = fmaf(zb[u], kLog2e, shb);
+                const float d = ((zc[u] - zb[u]) - rs) * kLog2e, ed = ex2f(d);
+                if (st) {
+                    mc = xc, sc = 1.f, mb = xb, sb = 1.f, ub = ed, wb = -d;
+                } else {
+                    float ec, eb;
+                    md_online(xc, mc, sc, &ec);
+                    const bool up = md_online(xb, mb, sb, &eb);
+                    ub = up ? fmaf(ub, eb, ed) : fmaf(eb, ed, ub);
+                    if constexpr (DIAG) wb = up ? fmaf(wb, eb, -d) : fmaf(eb, -d, wb);
+                }
+                if ((taken >> j) & 1u) za += xc, da += d;
+            }
+        }
+    }
+    msc += mc, prc *= sc, prb *= sb, pru *= ub;
+    if constexpr (DIAG) klw += __fdividef(wb, sb);
+    const float lrs = lg2f(pru / prb);  // sum_k log2 sum_j mu_j 2^d_j
+    *lp2 = za - (msc + lg2f(prc));
+    *lr2 = da - lrs;
+    *kl2 = klw + lrs;
+    return taken;
+}
+// Step 4: the current row re-read into its entropy sum_k H_k (returned) and the N gradients
+//   dz_j = inv_batch [cp (p_j - [j taken]) + entropy_c p_j (ln p_j + H_k)],  cp = policy_loss_c pg_adv, zero if !valid,
+// in two sweeps that each read the row and keep only dz:
+//   forward:  each head's online lse and t = sum_j 2^(x_j - m) x_j, so that H_k / ln 2 = lse_k - t / s; its offset
+//             c_k = sh_k - lse_k (log2 p_j = z_j log2(e) + c_k, one rounding) is left at its last entry and H_k at the
+//             entry before (n_k >= 2);
+//   backward: the gradient, with c_k and H_k picked up at the head's last entry.
+template <int AP, bool VEC>
+__device__ __forceinline__ float md_grad(const float* __restrict__ pc, unsigned elem, int A, unsigned hm,
+                                         unsigned taken, bool valid, float cp, float entropy_c, float inv_batch,
+                                         float (&dz)[AP]) {
+    constexpr int W = AP < 4 ? AP : 4;
+    const unsigned em = (hm >> 1) | (1u << (A - 1));  // bit j: output j is the last of its head
+    float sh = 0.f, m = 0.f, s = 1.f, t = 0.f, ent = 0.f;
+#pragma unroll
+    for (int j0 = 0; j0 < AP; j0 += W) {
+        float z[W];
+        md_chunk<AP, VEC>(pc, elem, A, j0, z);
+#pragma unroll
+        for (int u = 0; u < W; ++u) {
+            const int j = j0 + u;
+            if (j < A) {
+                const bool st = (hm >> j) & 1u;
+                if (st) sh = -z[u] * kLog2e;
+                const float x = fmaf(z[u], kLog2e, sh);
+                if (st) {
+                    m = x, s = 1.f, t = x;
+                } else {
+                    float e;
+                    t = md_online(x, m, s, &e) ? fmaf(t, e, x) : fmaf(e, x, t);
+                }
+                if ((em >> j) & 1u) {
+                    const float lse = m + lg2f(s), h = (lse - __fdividef(t, s)) * kLn2;
+                    ent += h;
+                    dz[j] = sh - lse;
+                    if (j > 0) dz[j > 0 ? j - 1 : 0] = h;
+                }
+            }
+        }
+    }
+    float c = 0.f, H = 0.f;
+#pragma unroll
+    for (int j0 = AP - W; j0 >= 0; j0 -= W) {
+        float z[W];
+        md_chunk<AP, VEC>(pc, elem, A, j0, z);
+#pragma unroll
+        for (int u = W - 1; u >= 0; --u) {
+            const int j = j0 + u;
+            if (j < A) {
+                if ((em >> j) & 1u) {
+                    c = dz[j];
+                    if (j > 0) H = dz[j > 0 ? j - 1 : 0];
+                }
+                const float lp = fmaf(z[u], kLog2e, c), p = ex2f(lp);  // log2 p_j, p_j
+                const float onehot = ((taken >> j) & 1u) ? 1.f : 0.f;
+                const float d = inv_batch * (cp * (p - onehot) + entropy_c * p * (lp * kLn2 + H));
+                dz[j] = valid ? d : 0.f;
+            } else {
+                dz[j] = 0.f;
+            }
+        }
+    }
+    return ent;
+}
+
 // POPART: {mu, sigma, 1 / sigma} as float32 in shared memory, read through a volatile pointer at every use so
 // that the three values take no register across the unroll (the DIAG twins are at their register limit).
 struct PopVals {
@@ -308,15 +485,21 @@ struct PopVals {
 // sums scaled by 1 / sigma: the loss is that of the normalized targets, 0.5 sum ((v - vs) / sigma)^2, and
 // the advantage pg / sigma.  mu = 0, sigma = 1 leaves every value as it is (FMA with 1 and 0, products by 1).
 // ------------------------------------------------------------------------------------------------
-// The body is one device function; vtrace_lane_kernel (softmax policies) and vtrace_gauss_kernel (GAUSS) are its
-// two thin __global__ entries, so the categorical instantiations keep their names and their code.
-template <int AP, int S, bool WITH_LOSS, bool VEC, bool DIAG, bool POPART, bool RCLIP, bool GAUSS>
-__device__ __forceinline__ void vtrace_lane_body(const VtArgsT<DIAG, POPART, RCLIP>& a) {
-    constexpr bool STREAM = !GAUSS && AP > 16;
-    constexpr bool HELD = !STREAM && !GAUSS;  // the logit rows of a chunk are held in registers
+// MD (with WITH_LOSS): the multi-discrete policy terms (md_terms, md_grad) in place of the softmax ones, AP = the
+// padded output count N.  As on the GAUSS path no row is held across the chunk: step 2 reduces the current and
+// behaviour rows and the K action indices of a step as they load, and keeps the step's taken mask in the action slot
+// of the rows; step 4 re-reads the current row for the entropy and the N gradients.
+// ------------------------------------------------------------------------------------------------
+// The body is one device function; vtrace_lane_kernel (softmax policies), vtrace_gauss_kernel (GAUSS) and
+// vtrace_md_kernel (MD) are its thin __global__ entries, so the categorical instantiations keep their names and code.
+template <int AP, int S, bool WITH_LOSS, bool VEC, bool DIAG, bool POPART, bool RCLIP, bool GAUSS, bool MD = false>
+__device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCLIP, MD>& a) {
+    constexpr bool STREAM = !GAUSS && !MD && AP > 16;
+    constexpr bool HELD = !STREAM && !GAUSS && !MD;  // the logit rows of a chunk are held in registers
     constexpr int SR = HELD ? S : 1, AR = HELD ? AP : 1;  // extent of the held logit rows
     static_assert(!STREAM || S == 1, "the streaming rows keep one step per thread");
     static_assert(!GAUSS || (WITH_LOSS && AP <= 16), "Gaussian policies: the loss kernel, up to 16 action dimensions");
+    static_assert(!MD || (WITH_LOSS && !GAUSS), "multi-discrete policies: the loss kernel");
     // GAUSS: the (T, B, A) float32 action samples (the categorical kernels read int32 indices there)
     const float* const gact = reinterpret_cast<const float*>(a.actions);
     static_assert(!DIAG || WITH_LOSS, "the off-policy sums ride the loss reduction");
@@ -374,7 +557,7 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsT<DIAG, POPART, RCL
                 load_logits<AP, VEC>(a.beh_logits, e, A, R.zb[i]);
             }
             R.r[i] = __ldg(a.rewards + e);
-            if constexpr (!GAUSS) R.act[i] = __ldg(a.actions + e);
+            if constexpr (!GAUSS && !MD) R.act[i] = __ldg(a.actions + e);
             R.dn[i] = __ldg(a.done + e);
         }
 #pragma unroll
@@ -396,6 +579,14 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsT<DIAG, POPART, RCL
                 const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
                 float kl2;
                 gauss_terms<AP, VEC, DIAG>(a.cur_logits, a.beh_logits, gact, e, A, &lp2a[i], &lr2, &kl2);
+                if constexpr (DIAG) {
+                    if (valid) d_kl += kl2;
+                }
+            } else if constexpr (MD) {
+                const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
+                float kl2;
+                R.act[i] = (int)md_terms<AP, VEC, DIAG>(a.cur_logits, a.beh_logits, a.actions, e, A, a.head_mask,
+                                                        &lp2a[i], &lr2, &kl2);
                 if constexpr (DIAG) {
                     if (valid) d_kl += kl2;
                 }
@@ -546,6 +737,10 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsT<DIAG, POPART, RCL
                         dz[AP + k] = valid ? a.inv_batch * (cp * fmaf(-d, du, 1.f) - a.entropy_c) : 0.f;
                     }
                     ent = fmaf((float)A, kHalfLog2PiE, ent);
+                } else if constexpr (MD) {
+                    ent = md_grad<AP, VEC>(a.cur_logits, (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl, A,
+                                           a.head_mask, (unsigned)R.act[i], valid, a.policy_loss_c * pg, a.entropy_c,
+                                           a.inv_batch, dz);
                 } else if constexpr (STREAM) {
                     // re-read the row; dz holds log2 pi(k), then the gradient (one row of registers)
                     load_logits<AP, VEC>(a.cur_logits, (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl, A, dz);
@@ -711,6 +906,10 @@ template <int AP, int S, int MAXT, int MINB, bool VEC, bool DIAG, bool POPART, b
 __global__ void __launch_bounds__(MAXT, MINB) vtrace_gauss_kernel(const VtArgsT<DIAG, POPART, RCLIP> a) {
     vtrace_lane_body<AP, S, true, VEC, DIAG, POPART, RCLIP, true>(a);
 }
+template <int AP, int S, int MAXT, int MINB, bool VEC, bool DIAG, bool POPART, bool RCLIP>
+__global__ void __launch_bounds__(MAXT, MINB) vtrace_md_kernel(const VtArgsM<DIAG, POPART, RCLIP, true> a) {
+    vtrace_lane_body<AP, S, true, VEC, DIAG, POPART, RCLIP, false, true>(a);
+}
 
 int pick_ap(int A) {
     if (A <= 2) return 2;
@@ -723,10 +922,14 @@ int pick_ap(int A) {
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool DIAG, bool POPART, bool RCLIP, bool GAUSS = false>
-int launch_s(const VtArgsT<DIAG, POPART, RCLIP>& a, bool vec, unsigned groups, int nw, int cl, cudaStream_t st) {
+template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool DIAG, bool POPART, bool RCLIP, bool GAUSS = false,
+          bool MD = false>
+int launch_s(const VtArgsM<DIAG, POPART, RCLIP, MD>& a, bool vec, unsigned groups, int nw, int cl, cudaStream_t st) {
     cudaError_t e;
-    if constexpr (GAUSS)
+    if constexpr (MD)
+        e = vec ? impala_launch_cl(vtrace_md_kernel<AP, S, MAXT, MINB, true, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
+                : impala_launch_cl(vtrace_md_kernel<AP, S, MAXT, MINB, false, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
+    else if constexpr (GAUSS)
         e = vec ? impala_launch_cl(vtrace_gauss_kernel<AP, S, MAXT, MINB, true, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
                 : impala_launch_cl(vtrace_gauss_kernel<AP, S, MAXT, MINB, false, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
     else
@@ -747,9 +950,11 @@ constexpr int kMaxCluster = 8;  // portable cluster size
 // GAUSS: a.A action dimensions (rows of 2A policy outputs), AP = the padded dimension count, at most 16; S = 2 up
 // to AP = 4 and S = 1 from AP = 8 on, where the five rows of two steps in flight would spill (IMPALA_VTRACE_S
 // does not apply).
+// MD: a.A = N policy outputs, AP = the padded N; S as the categorical twin at that AP (IMPALA_VTRACE_S does not apply),
+// at most 8 warps per CTA at AP = 32 (the 256-thread bound of those instantiations).
 constexpr int kMaxGaussA = 16;
-template <bool WITH_LOSS, bool DIAG = false, bool POPART = false, bool RCLIP = false, bool GAUSS = false>
-int launch(VtArgsT<DIAG, POPART, RCLIP>& a, cudaStream_t st) {
+template <bool WITH_LOSS, bool DIAG = false, bool POPART = false, bool RCLIP = false, bool GAUSS = false, bool MD = false>
+int launch(VtArgsM<DIAG, POPART, RCLIP, MD>& a, cudaStream_t st) {
     if (a.T < 1 || a.B < 1 || a.A < 1) return IMPALA_ERR_BAD_ARG;
     const int AP = (GAUSS && a.A > kMaxGaussA) ? 0 : pick_ap(a.A);
     if (!AP) return IMPALA_ERR_UNSUPPORTED_SHAPE;
@@ -759,7 +964,7 @@ int launch(VtArgsT<DIAG, POPART, RCLIP>& a, cudaStream_t st) {
     const bool vec = a.A == AP && aligned16(a.cur_logits) && aligned16(a.beh_logits) &&
                      (!WITH_LOSS || aligned16(a.dlogits)) && (!GAUSS || aligned16(a.actions));
     int S = AP >= (GAUSS ? 8 : 16) ? 1 : 2;
-    const int s_env = GAUSS ? 0 : impala_env_int("IMPALA_VTRACE_S", 0);
+    const int s_env = (GAUSS || MD) ? 0 : impala_env_int("IMPALA_VTRACE_S", 0);
     if (AP <= 4 && (s_env == 1 || s_env == 2 || s_env == 5)) S = s_env;
     const int max_w = S == 5 ? 10 : (AP <= 4 && S == 1 ? kMaxSeg : 16);
     const int nseg = (a.T + S - 1) / S;
@@ -770,7 +975,13 @@ int launch(VtArgsT<DIAG, POPART, RCLIP>& a, cudaStream_t st) {
     if (nw > max_w) nw = max_w;
     const int n_env = impala_env_int("IMPALA_VTRACE_NSEG", 0);
     if (n_env >= 1 && n_env <= max_w) nw = n_env;
-    if constexpr (GAUSS) {
+    if constexpr (MD) {
+        if (AP == 2) return launch_s<2, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, nw, cl, st);
+        if (AP == 4) return launch_s<4, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, nw, cl, st);
+        if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, nw, cl, st);
+        if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, nw, cl, st);
+        return launch_s<32, 1, 256, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, 8 < nw ? 8 : nw, cl, st);
+    } else if constexpr (GAUSS) {
         if (AP == 2) return launch_s<2, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
         if (AP == 4) return launch_s<4, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
         if (AP == 8) return launch_s<8, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);

@@ -43,6 +43,11 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       outputs [mean | log std] of a diagonal Gaussian.  The slabs hold the behaviour outputs (T, B, 2A) and the
       float32 samples (T, B, A) (impala_batch_layout_act); impala_vtrace_loss_gauss takes the V-trace slot of the
       step with the same flags (diagnostics, PopArt, reward clip) and the same workspace.  No launch is added.
+    action_dist="multi_discrete", action_heads=(n_0, .., n_K-1) (a gym MultiDiscrete space): K <= 16 independent
+      softmax heads over the A = sum n_k <= 32 policy outputs, head k owning [s_k, s_k + n_k).  The slabs hold the
+      behaviour logits (T, B, A) and K int32 indices per step, actions (T, B, K) (impala_batch_layout_act with
+      IMPALA_ACT_MULTI_DISCRETE(K)); impala_vtrace_loss_md takes the V-trace slot of the step with the same flags and
+      workspace, the head sizes passed by value.  No launch is added.
 
 obs_dtype="uint8" (byte observations): the slabs hold obs as uint8 (impala_batch_layout_obs).  For
 O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one after the other as the
@@ -74,7 +79,7 @@ after the compose launch are unchanged; the logged `batch_mean_reward` scalar is
 all B columns' rewards / B), the mean over the fresh trajectories is the caller's (Learner logs that one).
 
 The keyword options above (obs_dtype, frames, diagnostics, replay_slabs, replay_columns, optimizer, optimizer_kwargs,
-popart, popart_beta, reward_clip, action_dist, shared_torso) are the fields of `LearnerOptions`.
+popart, popart_beta, reward_clip, action_dist, action_heads, shared_torso) are the fields of `LearnerOptions`.
 """
 from __future__ import annotations
 
@@ -138,9 +143,9 @@ def check_shared_torso(shared_torso: bool, H_pi: int, H_v: int, n_policy: int) -
 class CheckedOptions(NamedTuple):
     """What `LearnerOptions.check` derives from the options and the shapes."""
     B_fresh: int           # columns of an update that arrive from the host (B without replay)
-    N_pi: int              # policy outputs: A, or 2A [mean | log std] for a Gaussian policy
+    N_pi: int              # policy outputs: A, or 2A [mean | log std] for a Gaussian policy (multi-discrete: A)
     obs_code: int          # IMPALA_OBS_*
-    act_kind: int          # IMPALA_ACT_*
+    act_kind: int          # IMPALA_ACT_* (multi-discrete: IMPALA_ACT_MULTI_DISCRETE(K))
     reward_clip_code: int  # IMPALA_REWARD_CLIP_*, 0 = none
 
 
@@ -159,10 +164,24 @@ class LearnerOptions:
     popart_beta: float = POPART_BETA
     reward_clip: str | None = None
     action_dist: str = "categorical"
+    # multi_discrete: the head sizes (n_0, .., n_K-1), sum = A, a tuple whatever sequence came in (a JSON list on the
+    # worker ranks: Learner._cfg carries it and engine_from_cfg passes it on).  Init-only rather than a field, so that
+    # dataclasses.asdict / fields list the options every action distribution has; compared by __eq__ like a field.
+    # dataclasses.replace does not carry it: pass action_heads= again.
+    action_heads: dataclasses.InitVar[tuple] = ()
     shared_torso: bool = False
 
-    def __post_init__(self):
+    def __post_init__(self, action_heads):
         object.__setattr__(self, "optimizer_kwargs", dict(self.optimizer_kwargs or {}))
+        # a tuple whatever sequence came in; check() refuses bad entries
+        heads = tuple(action_heads) if isinstance(action_heads, (list, tuple)) else action_heads
+        object.__setattr__(self, "action_heads", heads)
+
+    def __eq__(self, other):
+        if other.__class__ is not self.__class__:
+            return NotImplemented
+        return self.action_heads == other.action_heads and all(
+            getattr(self, f.name) == getattr(other, f.name) for f in dataclasses.fields(self))
 
     def check(self, B: int, O: int, A: int, H_pi: int, H_v: int, world: int = 1) -> CheckedOptions:
         """Refuse options that B columns per update, O features, A actions (Gaussian: action dimensions), hidden
@@ -170,7 +189,16 @@ class LearnerOptions:
         obs_code = _cabi.obs_dtype_code(self.obs_dtype)
         if self.frames < 1 or O % self.frames:
             raise ValueError(f"{O} observation features do not split into {self.frames} stacked frames")
-        act_kind = _cabi.act_kind_code(self.action_dist)
+        if self.action_dist == "multi_discrete":
+            if not isinstance(self.action_heads, tuple):
+                raise ValueError(f"action_heads must be a sequence of head sizes, got {self.action_heads!r}")
+            heads = _cabi.check_heads(self.action_heads)
+            if sum(heads) != A:
+                raise ValueError(f"the heads {heads} of a multi-discrete policy have {sum(heads)} outputs; the policy "
+                                 f"has A = {A}")
+        elif self.action_heads != ():
+            raise ValueError(f"action_heads is for action_dist='multi_discrete', not {self.action_dist!r}")
+        act_kind = _cabi.act_kind_code(self.action_dist, self.action_heads)
         gaussian = act_kind == _cabi.ACT_GAUSSIAN
         if gaussian and not 1 <= A <= _cabi.MAX_GAUSSIAN_DIMS:
             raise ValueError(f"a Gaussian policy takes 1 to {_cabi.MAX_GAUSSIAN_DIMS} action dimensions (2A outputs "
@@ -195,7 +223,8 @@ def engine_from_cfg(cfg: dict, world: int, device, process_group=None, lr_table=
     return LearnerEngine(cfg["T"], cfg["B"] // world, cfg["O"], cfg["A"], cfg["H_pi"], cfg["H_v"],
                          Hyperparameters(**cfg["hp"]), global_batch=cfg["B"], device=device, mode=cfg["mode"],
                          process_group=process_group, lr_table=lr_table,
-                         **{f.name: cfg[f.name] for f in dataclasses.fields(LearnerOptions)})
+                         **{f.name: cfg[f.name] for f in dataclasses.fields(LearnerOptions)},
+                         **({"action_heads": tuple(cfg["action_heads"])} if cfg.get("action_heads") else {}))
 
 
 def _ptr(t: torch.Tensor) -> C.c_void_p:
@@ -236,6 +265,9 @@ class LearnerEngine:
         self.lib = _cabi.lib()
         # the options the step reads; every rank must agree on diagnostics and PopArt (the length of `comm`)
         self.gaussian = self.act_kind == _cabi.ACT_GAUSSIAN
+        # multi-discrete: the head sizes (K = len), passed by value to every impala_vtrace_loss_md call
+        self.heads = tuple(int(n) for n in o.action_heads) if o.action_dist == "multi_discrete" else ()
+        self.md_heads = (C.c_int32 * len(self.heads))(*self.heads) if self.heads else None
         self.shared_torso, self.popart, self.diagnostics = bool(o.shared_torso), bool(o.popart), bool(o.diagnostics)
         self.popart_beta, self.replay_slabs = float(o.popart_beta), int(o.replay_slabs)
         self.frames, self.F = o.frames, O // o.frames
@@ -290,11 +322,12 @@ class LearnerEngine:
 
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts (replay: the host slabs
         # hold the B_fresh columns that cross the host link, the device slabs the B columns trained on)
-        train_off, train_bytes = _cabi.batch_layout(T, B_local, O, A, o.obs_dtype, o.frames, o.action_dist)
+        train_off, train_bytes = _cabi.batch_layout(T, B_local, O, A, o.obs_dtype, o.frames, o.action_dist,
+                                                    o.action_heads)
         self.slab_off, self.slab_bytes = train_off, train_bytes
         if self.replay_slabs:
             self.slab_off, self.slab_bytes = _cabi.batch_layout(T, self.B_fresh, O, A, o.obs_dtype, o.frames,
-                                                                o.action_dist)
+                                                                o.action_dist, o.action_heads)
         self.fields = ((("obs", np.uint8 if o.obs_dtype == "uint8" else np.float32),) + _BATCH_FIELDS[1:])
         if self.gaussian:  # float32 action samples
             self.fields = self.fields[:2] + (("actions", np.float32),) + self.fields[3:]
@@ -442,7 +475,8 @@ class LearnerEngine:
         """Shapes of the six batch tensors in a slab of B columns."""
         T, A = self.T, self.A
         return {"obs": (T + self.frames, B, self.F), "beh_logits": (T, B, self.N_pi),
-                "actions": (T, B, A) if self.gaussian else (T, B), "rewards": (T, B), "done": (T, B), "lens": (B,)}
+                "actions": (T, B, A) if self.gaussian else (T, B, len(self.heads)) if self.heads else (T, B),
+                "rewards": (T, B), "done": (T, B), "lens": (B,)}
 
     def _ws_bytes(self, M, O, H, N2):
         n = self.lib.impala_mlp_backward_workspace(M, O, H, N2)
@@ -605,7 +639,7 @@ class LearnerEngine:
         cs = self.copy_stream
         if self._slab_used[slot]:
             cs.wait_event(self.slab_free[slot])
-        if self.gaussian:
+        if self.gaussian or self.heads:
             _cabi.check(self.lib.impala_ingest_shard_act(_ptr(self.d_slabs[slot]), C.c_void_p(host_address), self.T,
                                                          B_total, self.F, self.frames, self.A, self.obs_code,
                                                          self.act_kind, b0, self.B, C.c_void_p(cs.cuda_stream)),
@@ -629,7 +663,7 @@ class LearnerEngine:
         launched = lib.impala_launch_count()
         d = self.d_views[slot]
         T, B, O, A = self.T, self.B, self.O, self.N_pi  # A: the policy's outputs from here on
-        if self.replay_slabs and self.gaussian:
+        if self.replay_slabs and (self.gaussian or self.heads):
             _cabi.check(lib.impala_batch_compose_act(_ptr(self.d_slabs[slot]), _ptr(self.store), self.slab_bytes,
                                                      _ptr(self.d_plans[slot]), T, B, self.B_fresh, self.F, self.frames,
                                                      self.A, self.obs_code, self.act_kind, st),
@@ -681,6 +715,12 @@ class LearnerEngine:
             _cabi.check(lib.impala_vtrace_loss_gauss(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, T, B, self.A,
                                                      *vt_hp[3:-1], sums, _ptr(self.popart_buf) if self.popart else None,
                                                      self.reward_clip_code, st), "impala_vtrace_loss_gauss")
+        elif self.heads:  # the same flags through the multi-discrete policy terms; A = sum of the heads
+            sums = C.c_void_p(gbase + 8 * (self.n_total + 4)) if self.n_extra == 12 else None
+            _cabi.check(lib.impala_vtrace_loss_md(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp[:-1], sums,
+                                                  _ptr(self.popart_buf) if self.popart else None,
+                                                  self.reward_clip_code, self.md_heads, len(self.heads), st),
+                        "impala_vtrace_loss_md")
         elif self.reward_clip_code:  # the same kernel as below with the reward transform
             sums = C.c_void_p(gbase + 8 * (self.n_total + 4)) if self.n_extra == 12 else None
             _cabi.check(lib.impala_vtrace_loss_rclip(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp[:-1], sums,

@@ -150,28 +150,83 @@ def check_gaussian_block(block: dict, T: int, n: int, A: int) -> None:
             raise ValueError(f"Gaussian block: non-finite {name} (column {int(np.argwhere(~np.isfinite(v))[0, 1])})")
 
 
-def pack_trajectory(views: dict, b: int, traj, T: int, obs=None) -> float:
+def _is_int(x) -> bool:
+    return not (x.is_floating_point() or x.is_complex() or x.dtype == torch.bool)
+
+
+def md_steps(traj, L: int, heads):
+    """A multi-discrete trajectory's actions (L, K) int32 and behaviour logits (L, N) float32, N = sum(heads).  Raises
+    ValueError, naming the trajectory, the step and the head, for a step of another shape, a non-integer action or
+    an index a_k outside [0, n_k): such an index would train the logit of another head's action without an error."""
+    tid = getattr(traj, "id", "?")
+    K, N = len(heads), sum(heads)
+    acts = [torch.as_tensor(x) for x in traj.a]
+    logits = [torch.as_tensor(x) for x in traj.logits]
+    for t, x in enumerate(acts):
+        if tuple(x.shape) != (K,):
+            raise ValueError(f"trajectory {tid}: step {t} action has shape {tuple(x.shape)}, a multi-discrete policy "
+                             f"of {K} heads takes ({K},)")
+        if not _is_int(x):
+            raise ValueError(f"trajectory {tid}: step {t} action has dtype {x.dtype}; the head indices must be integers")
+    for t, x in enumerate(logits):
+        if tuple(x.shape) != (N,):
+            raise ValueError(f"trajectory {tid}: step {t} behaviour logits have shape {tuple(x.shape)}, the heads "
+                             f"{tuple(heads)} take ({N},)")
+    a = torch.stack(acts).to(torch.int64).numpy() if acts else np.zeros((0, K), np.int64)
+    bad = np.argwhere((a < 0) | (a >= np.asarray(heads)))
+    if bad.size:
+        t, k = (int(v) for v in bad[0])
+        raise ValueError(f"trajectory {tid}: step {t} head {k} action {int(a[t, k])} is outside [0, {heads[k]})")
+    z = _np(torch.stack(logits), torch.float32) if logits else np.zeros((0, N), np.float32)
+    return a.astype(np.int32), z
+
+
+def check_md_block(block: dict, T: int, n: int, heads) -> None:
+    """put_block's checks of a multi-discrete block: (T, n, K) integer actions with a_k in [0, n_k) and (T, n, N)
+    behaviour logits."""
+    K, N = len(heads), sum(heads)
+    a, z = np.asarray(block["actions"]), np.asarray(block["beh_logits"])
+    if a.shape != (T, n, K):
+        raise ValueError(f"multi-discrete block actions of shape {a.shape}; this ring takes {(T, n, K)}")
+    if not np.issubdtype(a.dtype, np.integer):
+        raise ValueError(f"multi-discrete block actions of dtype {a.dtype}; the head indices must be integers")
+    if z.shape != (T, n, N):
+        raise ValueError(f"multi-discrete block beh_logits of shape {z.shape}; this ring takes {(T, n, N)}")
+    bad = np.argwhere((a < 0) | (a >= np.asarray(heads)))
+    if bad.size:
+        t, col, k = (int(v) for v in bad[0])
+        raise ValueError(f"multi-discrete block: column {col} step {t} head {k} action {int(a[t, col, k])} is outside "
+                         f"[0, {heads[k]})")
+
+
+def pack_trajectory(views: dict, b: int, traj, T: int, obs=None, heads=()) -> float:
     """Write one reference-format trajectory into column `b` of a host batch slab.
 
     Replaces learner.py:104-109,117 (five torch.stack calls + `disc`): float64 -> float32 (or the
     checked uint8 of obs_array for a byte-observation slab), int64 -> int32, bool -> u8, zero padding
     past the trajectory's length.  `obs`: obs_array's result if the caller already has it.  A frame slab
     (obs (T+k, B, F), k > 1) receives obs_frames' L+k frames.  A Gaussian slab (actions (T, B, A)) takes
-    (A,) actions and (2A,) behaviour outputs per step (gaussian_steps).  Returns the trajectory's reward sum
+    (A,) actions and (2A,) behaviour outputs per step (gaussian_steps); a multi-discrete slab (`heads`: the head
+    sizes, actions (T, B, K)) (K,) integer actions and (N,) logits (md_steps).  Returns the trajectory's reward sum
     (learner.py:108)."""
     L = check_trajectory(traj, T)
-    gauss = views["actions"].ndim == 3
+    multi = bool(heads)
+    if multi and tuple(views["actions"].shape[2:]) != (len(heads),):
+        raise ValueError(f"a slab of actions {tuple(views['actions'].shape)} does not hold the heads {tuple(heads)}")
+    gauss = views["actions"].ndim == 3 and not multi
     if gauss:
         act, beh = gaussian_steps(traj, L, views["actions"].shape[2])
+    elif multi:
+        act, beh = md_steps(traj, L, heads)
     obs = obs_array(traj, views["obs"].dtype) if obs is None else obs
     k = views["obs"].shape[0] - T
     if k > 1:
         obs = obs_frames(obs, k, traj)
     views["obs"][:L + k, b] = obs
     views["obs"][L + k:, b] = 0
-    views["beh_logits"][:L, b] = beh if gauss else _np(torch.stack(traj.logits), torch.float32)
+    views["beh_logits"][:L, b] = beh if gauss or multi else _np(torch.stack(traj.logits), torch.float32)
     views["beh_logits"][L:, b] = 0
-    views["actions"][:L, b] = act if gauss else _np(torch.stack(traj.a).reshape(L), torch.int32)
+    views["actions"][:L, b] = act if gauss or multi else _np(torch.stack(traj.a).reshape(L), torch.int32)
     views["actions"][L:, b] = 0
     r = torch.stack(traj.r)
     views["rewards"][:L, b] = _np(r, torch.float32)
@@ -183,8 +238,8 @@ def pack_trajectory(views: dict, b: int, traj, T: int, obs=None) -> float:
 
 
 def _dims(policy, value_fn, action_dist):
-    """(O, A, H_pi, H_v) of the two modules: A actions, or the action dimensions of a Gaussian policy, whose 2A outputs
-    are [mean | log std]."""
+    """(O, A, H_pi, H_v) of the two modules: A actions (a multi-discrete policy: its N = sum n_k outputs), or the action
+    dimensions of a Gaussian policy, whose 2A outputs are [mean | log std]."""
     sd_p, sd_v = policy.state_dict(), value_fn.state_dict()
     H_pi, O = sd_p[PKEYS[0]].shape
     A = int(sd_p[PKEYS[2]].shape[0])
@@ -202,6 +257,7 @@ def _check_ring(q, options, B_fresh: int) -> None:
     if not hasattr(q, "collect_batch"):
         return
     for want, have, what in ((options.action_dist, q.action_dist, "{} actions"),
+                             (tuple(options.action_heads), tuple(getattr(q, "action_heads", ())), "action heads {}"),
                              (options.obs_dtype, q.obs_dtype, "{} observations"),
                              (options.frames, q.frames, "{} frames per observation"),
                              (B_fresh, q.B, "{} trajectories per update (batch_size - replay_columns)")):
@@ -356,7 +412,8 @@ class Learner:
 
             c, o = self._cfg(), self.options
             self._stage_ring = RingQueue(self.hp.max_timesteps, self.hp.batch_size, c["O"], c["A"], slabs=2,
-                                         obs_dtype=o.obs_dtype, frames=o.frames, action_dist=o.action_dist)
+                                         obs_dtype=o.obs_dtype, frames=o.frames, action_dist=o.action_dist,
+                                         action_heads=o.action_heads)
         self.p.start()
         print(f"[main] Started learner_{self.id} with pid {self.p.pid}")
 
@@ -377,8 +434,9 @@ class Learner:
         O, A, H_pi, H_v = _dims(self.policy, self.value_fn, self.options.action_dist)
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
+        # action_heads is an init-only option (engine.LearnerOptions), so it rides next to the fields
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
-                    **dataclasses.asdict(self.options))
+                    action_heads=list(self.options.action_heads), **dataclasses.asdict(self.options))
 
     def _make_engine(self, process_group=None, world=1):
         eng = engine_from_cfg(self._cfg(), world, self.device, process_group, self.optim.lr_table)
@@ -433,6 +491,9 @@ class Learner:
         if self.options.action_dist == "gaussian":  # the reference's test_policy refuses continuous environments
             print(f"[learner_{self.id}] evaluation skipped: a Gaussian policy is evaluated through evaluator= only")
             return None
+        if self.options.action_dist == "multi_discrete":  # test_policy steps one Discrete index per action
+            print(f"[learner_{self.id}] evaluation skipped: a multi-discrete policy is evaluated through evaluator= only")
+            return None
         try:
             import utils as ref_utils  # the reference's utils.py, if on sys.path
 
@@ -480,7 +541,7 @@ class Learner:
                 raise
             if hp.verbose >= 2:
                 print(f"[learner_{self.id}] packing traj_{traj.id} into column {b}")
-            reward += pack_trajectory(views, b, traj, hp.max_timesteps) / self.B_fresh
+            reward += pack_trajectory(views, b, traj, hp.max_timesteps, heads=self.options.action_heads) / self.B_fresh
             del traj  # drop the shared-memory handles of its ~5T tensors right away
         return reward
 

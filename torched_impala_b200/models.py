@@ -58,6 +58,31 @@ class GaussianMlpPolicy(nn.Module):
             return mean + torch.exp(log_std) * torch.randn_like(mean), params
 
 
+class MultiDiscreteMlpPolicy(nn.Module):
+    """Factorised categorical policy over a MultiDiscrete([n_0, .., n_K-1]) space (Learner(action_dist=
+    "multi_discrete", action_heads=...) or LearnerEngine): the same two-layer MLP with N = sum n_k outputs, head k owning
+    [s_k, s_k + n_k), so the state_dict keys are MlpPolicy's."""
+
+    def __init__(self, obs_dim: int, action_heads, hidden_dim: int):
+        super().__init__()
+        self.action_heads = tuple(int(n) for n in action_heads)
+        self.model = _two_layer(obs_dim, hidden_dim, sum(self.action_heads))
+
+    def forward(self, x):
+        return self.model(x)
+
+    def select_action(self, obs, deterministic: bool = False):
+        """Returns (actions (K,) int64, logits (N,)): one index per head, sampled from the softmax of its slice (the
+        per-head argmax when deterministic)."""
+        logits = self.forward(obs)
+        out = []
+        with torch.no_grad():
+            for z in torch.split(logits, self.action_heads, dim=-1):
+                out.append(z.argmax(-1) if deterministic else
+                           torch.multinomial(torch.softmax(z, dim=-1).reshape(-1, z.shape[-1]), 1).reshape(z.shape[:-1]))
+        return torch.stack(out, -1).to(torch.int64), logits
+
+
 class MlpValueFn(nn.Module):
     def __init__(self, obs_dim: int, hidden_dim: int):
         super().__init__()

@@ -49,23 +49,25 @@ def _pause(t_start: float) -> None:
 _OBS_BYTES = {"float32": 4, "uint8": 1}
 
 
-_ACT_DISTS = ("categorical", "gaussian")
+_ACT_DISTS = ("categorical", "gaussian", "multi_discrete")
 
 
 def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1,
-            action_dist: str = "categorical"):
+            action_dist: str = "categorical", action_heads=()):
     """Same 256-byte aligned layout as include/impala_b200.h::impala_batch_layout_act with F = O / frames
     (impala_batch_layout_obs at frames = 1, categorical; pure python so actor processes do not need the CUDA
-    library).  "gaussian": beh_logits (T, B, 2A) f32 and actions (T, B, A) f32 for A action dimensions."""
+    library).  "gaussian": beh_logits (T, B, 2A) f32 and actions (T, B, A) f32 for A action dimensions.
+    "multi_discrete": beh_logits (T, B, A) f32 for A = sum(action_heads) outputs and actions (T, B, K) i32."""
     if action_dist not in _ACT_DISTS:
         raise ValueError(f"action_dist must be one of {list(_ACT_DISTS)}, got {action_dist!r}")
     g = action_dist == "gaussian"
+    K = len(action_heads) if action_dist == "multi_discrete" else 1
     if obs_dtype not in _OBS_BYTES:
         raise ValueError(f"obs_dtype must be one of {sorted(_OBS_BYTES)}, got {obs_dtype!r}")
     if frames < 1 or O % frames:
         raise ValueError(f"{O} observation features do not split into {frames} frames")
     sizes = ((T + frames) * B * (O // frames) * _OBS_BYTES[obs_dtype], T * B * (2 * A if g else A) * 4,
-             T * B * (A if g else 1) * 4, T * B * 4, T * B, B * 4)
+             T * B * (A if g else K) * 4, T * B * 4, T * B, B * 4)
     offs, off = [], 0
     for s in sizes:
         offs.append(off)
@@ -77,14 +79,24 @@ class RingQueue:
     """Drop-in for the `mp.Queue` between actors and learner, backed by shared-memory batch slabs."""
 
     def __init__(self, T: int, B: int, O: int, A: int, slabs: int = 3, obs_dtype: str = "float32", frames: int = 1,
-                 action_dist: str = "categorical"):
+                 action_dist: str = "categorical", action_heads=()):
         if slabs < 2:
             raise ValueError("need at least two slabs (one filling while one is consumed)")
         if action_dist == "gaussian" and not 1 <= A <= 16:
             raise ValueError(f"a Gaussian policy takes 1 to 16 action dimensions, got {A}")
+        # "multi_discrete": K heads of action_heads[k] actions, A = sum(action_heads) outputs; K int32 indices per step
+        if action_dist == "multi_discrete":
+            from ._cabi import check_heads  # pure python: no library load
+
+            action_heads = check_heads(action_heads)
+            if sum(action_heads) != A:
+                raise ValueError(f"the heads {action_heads} have {sum(action_heads)} outputs; this ring takes A = {A}")
+        elif tuple(action_heads) != ():
+            raise ValueError(f"action_heads is for action_dist='multi_discrete', not {action_dist!r}")
+        self.action_heads = tuple(action_heads)
         self.T, self.B, self.O, self.A, self.K = T, B, O, A, slabs
         # "uint8": byte observations (Atari RAM, MinAtar planes), a quarter of the float32 slab bytes
-        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype, frames, action_dist)
+        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype, frames, action_dist, self.action_heads)
         # "gaussian": A action dimensions; the actors' [mean | log std] (2A) and float32 samples (A) per step
         self.action_dist = action_dist
         self.gaussian = action_dist == "gaussian"
@@ -144,7 +156,8 @@ class RingQueue:
         if self._views is None:
             N = 2 * self.A if self.gaussian else self.A
             shapes = {"obs": (self.T + self.frames, self.B, self.O // self.frames), "beh_logits": (self.T, self.B, N),
-                      "actions": (self.T, self.B, self.A) if self.gaussian else (self.T, self.B),
+                      "actions": ((self.T, self.B, self.A) if self.gaussian else
+                                  (self.T, self.B, len(self.action_heads)) if self.action_heads else (self.T, self.B)),
                       "rewards": (self.T, self.B), "done": (self.T, self.B), "lens": (self.B,)}
             self._views = []
             for kk in range(self.K):
@@ -167,6 +180,10 @@ class RingQueue:
 
         check_trajectory(traj, self.T)  # BEFORE a column is taken: a malformed trajectory must not leave a hole
         obs = obs_array(traj, self.obs_dtype)  # the same: raises on obs a uint8 ring cannot hold
+        if self.action_heads:  # the same: wrong widths, non-integer or out-of-range head indices
+            from .learner import md_steps
+
+            md_steps(traj, len(traj.r), self.action_heads)
         c = self._control()
         end = None if (timeout is None or not block) else time.monotonic() + timeout
         t_wait = time.monotonic()
@@ -181,7 +198,7 @@ class RingQueue:
                 raise queue.Full  # like mp.Queue.put on a full queue; actor.py:120 retries
             _pause(t_wait)
         try:
-            rsum = pack_trajectory(self.views(k), b, traj, self.T, obs=obs)
+            rsum = pack_trajectory(self.views(k), b, traj, self.T, obs=obs, heads=self.action_heads)
         except BaseException:
             # never leave the column unfilled (the learner would stall on it until its timeout):
             # publish it as an empty trajectory - neutral padding for the update - and re-raise
@@ -220,6 +237,10 @@ class RingQueue:
             from .learner import check_gaussian_block
 
             check_gaussian_block(block, self.T, n, self.A)
+        if self.action_heads:
+            from .learner import check_md_block
+
+            check_md_block(block, self.T, n, self.action_heads)
         c = self._control()
         end = None if timeout is None else time.monotonic() + timeout
         t_wait = time.monotonic()

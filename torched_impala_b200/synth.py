@@ -158,12 +158,45 @@ def make_gaussian_batch(seed: int, T: int, B: int, O: int, A: int, ragged: bool 
     return dict(b, beh_logits=beh.astype(np.float32), actions=act.astype(np.float32))
 
 
+def make_md_batch(seed: int, T: int, B: int, O: int, heads, ragged: bool = False, params: dict | None = None,
+                  obs_kind: str = "normal", frames: int = 1) -> dict:
+    """A batch of a multi-discrete policy with head sizes `heads` (action_dist="multi_discrete"): obs, rewards, done
+    and lens as make_batch(seed, ..., A=2); beh_logits (T, B, N = sum heads) and actions (T, B, K) int32, one index per
+    head sampled from the softmax of its slice.  With `params` (init_params(seed, O, N, H) layout) the behaviour is the
+    policy's own output on the (dense) observations, moved 0.1-0.3 per entry (the off-policy lag of an actor);
+    without, N(0, 1) logits.  Padded steps are zero."""
+    heads = tuple(int(n) for n in heads)
+    N, K = sum(heads), len(heads)
+    b = make_batch(seed, T, B, O, 2, ragged=ragged, obs_kind=obs_kind, frames=frames)
+    rng = np.random.default_rng(seed + 7919)
+    if params is None:
+        beh = rng.standard_normal((T, B, N))
+    else:
+        x = (stack_frames(b, frames) if frames > 1 else b)["obs"][:-1].astype(np.float64)
+        p = [np.asarray(params["policy"][k], np.float64) for k in ("model.0.weight", "model.0.bias",
+                                                                      "model.3.weight", "model.3.bias")]
+        beh = np.maximum(x @ p[0].T + p[1], 0.0) @ p[2].T + p[3]
+        beh = beh + rng.uniform(0.1, 0.3, beh.shape) * rng.choice([-1.0, 1.0], beh.shape)
+    beh = beh.astype(np.float32)
+    act = np.zeros((T, B, K), np.int32)
+    s = 0
+    for k, n in enumerate(heads):
+        z = beh[..., s:s + n].astype(np.float64)
+        q = np.exp(z - z.max(-1, keepdims=True))
+        q /= q.sum(-1, keepdims=True)
+        act[..., k] = np.minimum((np.cumsum(q, -1) < rng.random((T, B, 1))).sum(-1), n - 1)
+        s += n
+    pad = np.arange(T)[:, None] >= b["lens"][None, :]
+    beh[pad], act[pad] = 0.0, 0
+    return dict(b, beh_logits=beh, actions=act)
+
+
 def to_trajectories(batch: dict, torch_dtype=None) -> list:
     """Expand a dense batch into the reference wire format (one Trajectory per b).
 
     Shapes/dtypes follow what actor.py:72-92 appends: obs (O,) f64, a (1,) i64,
     r () f64, d () bool, logits (A,) f64.  A Gaussian batch (actions (T, B, A)) gives a (A,) f64 and
-    logits (2A,) f64.
+    logits (2A,) f64; a multi-discrete batch (int32 actions (T, B, K)) a (K,) i64 and logits (N,) f64.
     """
     import torch
 
@@ -172,7 +205,9 @@ def to_trajectories(batch: dict, torch_dtype=None) -> list:
     dt = torch.float64 if torch_dtype is None else torch_dtype
     obs = torch.from_numpy(batch["obs"]).to(dt)
     beh = torch.from_numpy(batch["beh_logits"]).to(dt)
-    gauss = batch["actions"].ndim == 3
+    # (T, B, A) float actions: Gaussian samples; (T, B, K) integer actions: multi-discrete indices
+    gauss = batch["actions"].ndim == 3 and np.issubdtype(batch["actions"].dtype, np.floating)
+    multi = batch["actions"].ndim == 3 and not gauss
     act = torch.from_numpy(batch["actions"]).to(dt if gauss else torch.int64)
     rew = torch.from_numpy(batch["rewards"]).to(dt)
     don = torch.from_numpy(batch["done"]).to(torch.bool)
@@ -181,7 +216,7 @@ def to_trajectories(batch: dict, torch_dtype=None) -> list:
         tr = Trajectory((0, b + 1))
         tr.obs.append(obs[0, b].clone())
         for t in range(L):
-            tr.add(obs[t + 1, b].clone(), act[t, b].clone() if gauss else act[t, b].reshape(1).clone(), rew[t, b].clone(),
+            tr.add(obs[t + 1, b].clone(), act[t, b].clone() if gauss or multi else act[t, b].reshape(1).clone(), rew[t, b].clone(),
                    don[t, b].clone(), beh[t, b].clone())
         out.append(tr)
     return out
