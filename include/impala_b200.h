@@ -89,15 +89,30 @@ int impala_batch_layout_frames(int T, int B, int F, int frames, int A, int obs_d
  *     unsquashed sample m + e^s eps, actions (T,B,A) f32.
  *   IMPALA_ACT_MULTI_DISCRETE(K): K independent categorical heads (a gym MultiDiscrete space), 1 <= K <= 16, of
  *     n_k >= 2 actions each; A = N = sum_k n_k policy outputs, head k owning [s_k, s_k + n_k) with s_k = sum_{i<k} n_i.
- *     beh_logits (T,B,N) f32, actions (T,B,K) i32 (one index per head).  K = 1 is the categorical layout. */
+ *     beh_logits (T,B,N) f32, actions (T,B,K) i32 (one index per head).  K = 1 is the categorical layout.
+ *   IMPALA_ACT_MASKED, OR-ed onto IMPALA_ACT_CATEGORICAL or IMPALA_ACT_MULTI_DISCRETE(K): invalid-action masking.
+ *     Each step carries one 32-bit legal word, as one more int32 column of the actions: (T,B,2) [a, legal] and
+ *     (T,B,K+1) [a_0 .. a_{K-1}, legal].  Bit j set: policy output j is legal (A, N <= 32).
+ *       - Bits >= A are ignored.  A head with no legal bit (categorical: the whole row) is all-legal, so padded
+ *         steps and the empty columns of replay (every byte 0) need no special case.
+ *       - pi and mu are the softmaxes of the current and behaviour logits renormalised over the legal entries
+ *         (within each head); log pi(a), the ratio, V-trace, vs, pg_adv, the entropy -sum_{j legal} p_j log p_j
+ *         and KL(mu || pi) come from them, and dz_j = 0 exactly at an illegal j.
+ *       - The logit values at illegal entries, current or behaviour, reach no output (raw logits, -inf, -1e30 or
+ *         NaN give identical results).
+ *       - A taken action must be legal: that is the caller's responsibility, like an in-range index.
+ *       - With every legal bit set, every output is bitwise that of the unmasked kernel with the same flags.
+ *     IMPALA_ACT_GAUSSIAN | IMPALA_ACT_MASKED is refused (IMPALA_ERR_BAD_ARG). */
 #define IMPALA_ACT_CATEGORICAL 0
 #define IMPALA_ACT_GAUSSIAN 1
 #define IMPALA_ACT_MULTI_DISCRETE(K) (0x100 | (K))
+#define IMPALA_ACT_MASKED 0x200
 
 /* impala_batch_layout_frames for the action distribution act_kind: IMPALA_ACT_CATEGORICAL is exactly
  * impala_batch_layout_frames, IMPALA_ACT_GAUSSIAN widens beh_logits to (T,B,2A) f32 and actions to (T,B,A) f32,
- * IMPALA_ACT_MULTI_DISCRETE(K) widens actions to (T,B,K) i32.  An unknown act_kind, K outside 1..16 or A < 2K
- * returns IMPALA_ERR_BAD_ARG. */
+ * IMPALA_ACT_MULTI_DISCRETE(K) widens actions to (T,B,K) i32, IMPALA_ACT_MASKED adds one i32 column (the legal word)
+ * to the actions of either.  An unknown act_kind, K outside 1..16, A < 2K, a masked Gaussian or a masked kind with
+ * A > 32 returns IMPALA_ERR_BAD_ARG. */
 int impala_batch_layout_act(int T, int B, int F, int frames, int A, int obs_dtype, int act_kind, int64_t offsets[6],
                             int64_t* total_bytes);
 
@@ -352,6 +367,20 @@ int impala_vtrace_loss_md(const float* cur_logits, const float* beh_logits, cons
                           float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch, int mode,
                           double* diag, const double* popart, int reward_clip, const int32_t* host_heads, int K,
                           void* stream);
+
+/* Invalid-action masking (IMPALA_ACT_MASKED, see above) in the V-trace loss kernel of impala_vtrace_loss_rclip.  The
+ * arguments are those of impala_vtrace_loss_md, with actions in the widened layout: host_heads == NULL selects one
+ * categorical softmax over the A <= 32 outputs, actions (T,B,2) [a, legal]; otherwise the K heads of
+ * impala_vtrace_loss_md, actions (T,B,K+1) [a_0 .. a_{K-1}, legal].  actions must be 8-byte aligned (host_heads ==
+ * NULL).  diag, popart, reward_clip and the workspace (impala_vtrace_loss[_diag]_workspace(T, B, A)) as
+ * impala_vtrace_loss_md; A > 32 returns IMPALA_ERR_UNSUPPORTED_SHAPE, the rest what impala_vtrace_loss_md refuses. */
+int impala_vtrace_loss_mask(const float* cur_logits, const float* beh_logits, const int32_t* actions,
+                            const float* rewards, const uint8_t* done, const int32_t* lens, const float* v, float* vs,
+                            float* pg_adv, float* dlogits, float* dv, double* scalars, void* workspace,
+                            int64_t workspace_bytes, int T, int B, int A, float gamma, float rho_bar, float c_bar,
+                            float v_loss_c, float policy_loss_c, float entropy_c, float inv_batch, int mode,
+                            double* diag, const double* popart, int reward_clip, const int32_t* host_heads, int K,
+                            void* stream);
 
 /* Per-group gradient clipping + Adam in one launch (learner.py:176-183).
  *   params/m/v: f32 [n_total]; grad: f64 [n_total] (the possibly all-reduced sum);

@@ -31,7 +31,12 @@ observations for the Atari RAM and MinAtar shapes, as --compare-popart.
 --compare-heads (configs md_c4, md_ram) alternates a categorical engine at A = N and a multi-discrete engine
 (action_dist="multi_discrete" with the config's heads, N = sum of them) on batches of the same shapes the same way,
 and times impala_vtrace_loss against impala_vtrace_loss_md alone on each engine's buffers (median of 200 launches
-each, alternating, L2 flushed before each)."""
+each, alternating, L2 flushed before each).
+--compare-mask (configs mask_c4, mask_ram, md_mask_c4) alternates the unmasked engine and the masked one
+(action_mask=True: legal words in the actions, about half the entries legal) on batches of the same shapes the same
+way, and times the unmasked V-trace + loss kernel (impala_vtrace_loss, or impala_vtrace_loss_md for md_mask_c4)
+against impala_vtrace_loss_mask alone on each engine's buffers (median of 200 launches each, alternating, L2 flushed
+before each)."""
 import argparse
 import os
 import statistics
@@ -49,6 +54,9 @@ CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256),
        # multi-discrete policies (--compare-heads): A = N = sum(heads) policy outputs
        "md_c4": dict(T=20, B=4096, O=24, A=8, H=256, heads=(3, 3, 2)),
        "md_ram": dict(T=20, B=4096, O=128, A=20, H=256, heads=(3, 3, 2, 2, 5, 5)), "c5": dict(T=100, B=8192, O=64, A=4, H=512),
+       # invalid-action masks (--compare-mask): categorical at c4 and Atari-RAM shapes (byte observations), and md_c4's heads
+       "mask_c4": dict(T=20, B=4096, O=24, A=8, H=256, mask=()), "mask_ram": dict(T=20, B=4096, O=128, A=18, H=256, mask=()),
+       "md_mask_c4": dict(T=20, B=4096, O=24, A=8, H=256, mask=(3, 3, 2)),
        "c3": dict(T=20, B=1024, O=24, A=4, H=256), "c2": dict(T=20, B=256, O=4, A=2, H=32),
        # c4 with 512 hidden units: the wide forward at one K atom (two passes of 256) and the wide backward
        "c4h512": dict(T=20, B=4096, O=24, A=4, H=512),
@@ -83,6 +91,8 @@ ap.add_argument("--compare-reward-clip", action="store_true", help="alternate en
 ap.add_argument("--compare-shared", action="store_true", help="alternate two networks and a shared-torso network")
 ap.add_argument("--compare-heads", action="store_true",
                 help="alternate a categorical engine at A = N and a multi-discrete engine (configs md_c4, md_ram)")
+ap.add_argument("--compare-mask", action="store_true",
+                help="alternate an unmasked and a masked engine (configs mask_c4, mask_ram, md_mask_c4)")
 ap.add_argument("--replay-slabs", type=int, default=2, help="past fresh batches in the pool of --compare-replay")
 ap.add_argument("--replay-columns", type=int, default=None, help="replayed columns of --compare-replay (default B/2)")
 a = ap.parse_args()
@@ -131,6 +141,16 @@ if a.compare_heads:
     md_name = f"multi-discrete heads {w['heads']}"
     arms = {f"categorical A={w['A']}": arms["default"], md_name: arms["default"]}
     heads_arm = {md_name: dict(action_dist="multi_discrete", action_heads=w["heads"])}
+mask_arm = {}
+if a.compare_mask:
+    if "mask" not in w:
+        raise SystemExit(f"--compare-mask takes a masked config (mask_c4, mask_ram, md_mask_c4), not {a.config}")
+    md_kw = dict(action_dist="multi_discrete", action_heads=w["mask"]) if w["mask"] else {}
+    mask_name = "masked"
+    arms = {"unmasked": arms["default"], mask_name: arms["default"]}
+    heads_arm = {name: md_kw for name in arms} if md_kw else {}
+    mask_arm = {mask_name: dict(action_mask=True)}
+    obs_dt = {name: "uint8" if a.config == "mask_ram" else "float32" for name in arms}
 replay_arm = {}
 if a.compare_replay:
     Br = w["B"] // 2 if a.replay_columns is None else a.replay_columns
@@ -146,10 +166,12 @@ for name, tc in arms.items():
     k = n_frames.get(name, 1)
     eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k,
                         diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}), **popart_arm.get(name, {}),
-                        **rclip_arm.get(name, {}), **shared_arm.get(name, {}), **heads_arm.get(name, {}))
+                        **rclip_arm.get(name, {}), **shared_arm.get(name, {}), **heads_arm.get(name, {}),
+                        **mask_arm.get(name, {}))
     eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
     byte_obs = (a.compare_obs or ((a.compare_frames or a.compare_replay) and dt == "uint8")
-                or ((a.compare_diag or a.compare_popart or a.compare_reward_clip or a.compare_shared) and dt == "uint8"))
+                or ((a.compare_diag or a.compare_popart or a.compare_reward_clip or a.compare_shared or a.compare_mask)
+                    and dt == "uint8"))
     if a.compare_replay:
         engines[name] = eng
         continue
@@ -158,8 +180,13 @@ for name, tc in arms.items():
                                  frames=a.frames)
         if k == 1:
             batch = synth.stack_frames(batch, a.frames)
+    elif name in mask_arm:
+        batch = synth.make_masked_batch(1, w["T"], w["B"], w["O"], w["A"], w["mask"], density=0.5,
+                                        obs_kind="bytes" if byte_obs else "normal")
+        batch.pop("legal")
     elif name in heads_arm:
-        batch = synth.make_md_batch(1, w["T"], w["B"], w["O"], w["heads"])
+        batch = (synth.make_md_batch(1, w["T"], w["B"], w["O"], w["heads"]) if "heads" in w else
+                 synth.make_md_batch(1, w["T"], w["B"], w["O"], w["mask"]))
     else:
         batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if byte_obs else "normal")
     if dt == "float32":
@@ -417,6 +444,45 @@ if a.compare_heads:  # the V-trace + loss kernel alone, categorical against mult
     k0, k1 = statistics.median(tk["impala_vtrace_loss"]), statistics.median(tk["impala_vtrace_loss_md"])
     print(f"V-trace + loss kernel {a.config}: impala_vtrace_loss (A={w['A']}) {k0:.1f} us, impala_vtrace_loss_md "
           f"(heads {w['heads']}) {k1:.1f} us ({k1 - k0:+.1f} us, {100 * (k1 / k0 - 1):+.1f} %)")
+if a.compare_mask:  # the V-trace + loss kernel alone, unmasked against masked, each on its engine's buffers
+    import ctypes
+
+    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    tail = (w["T"], w["B"], w["A"], hp.gamma, hp.rho_bar, hp.c_bar, hp.v_loss_c, hp.policy_loss_c, hp.entropy_c,
+            1.0 / w["B"], 0)
+
+    def _ins(e):
+        d = e.d_views[0]
+        return (P(e.logits), P(d["beh_logits"]), P(d["actions"]), P(d["rewards"]), P(d["done"]), P(d["lens"]),
+                P(e.values), P(e.vs), P(e.pg_adv), P(e.dlogits), P(e.dv), ctypes.c_void_p(e.comm.data_ptr() + 8 * e.n_total),
+                P(e.ws_vt), e.ws_vt_bytes)
+
+    eu, em = engines["unmasked"], engines[mask_name]
+    K = len(w["mask"])
+    hh = (ctypes.c_int32 * K)(*w["mask"]) if K else None
+    plain_name = "impala_vtrace_loss_md" if K else "impala_vtrace_loss"
+    calls = {plain_name: (lambda st: eu.lib.impala_vtrace_loss_md(*_ins(eu), *tail[:-1], tail[-1], None, None, 0, hh, K,
+                                                                  st)) if K else
+             (lambda st: eu.lib.impala_vtrace_loss(*_ins(eu), *tail, st)),
+             "impala_vtrace_loss_mask": lambda st: em.lib.impala_vtrace_loss_mask(*_ins(em), *tail[:-1], tail[-1], None,
+                                                                                  None, 0, hh, K, st)}
+    tk = {name: [] for name in calls}
+    with torch.cuda.stream(em.stream):
+        st = ctypes.c_void_p(em.stream.cuda_stream)
+        for i in range(220):
+            for name, fn in calls.items():
+                flush.zero_()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(em.stream)
+                rc = fn(st)
+                e1.record(em.stream)
+                e1.synchronize()
+                assert rc == 0, (name, rc)
+                if i >= 20:
+                    tk[name].append(e0.elapsed_time(e1) * 1e3)
+    k0, k1 = statistics.median(tk[plain_name]), statistics.median(tk["impala_vtrace_loss_mask"])
+    print(f"V-trace + loss kernel {a.config}: {plain_name} {k0:.1f} us, impala_vtrace_loss_mask {k1:.1f} us "
+          f"({k1 - k0:+.1f} us, {100 * (k1 / k0 - 1):+.1f} %)")
 q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
                     "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 print(f"GPU (nvidia-smi): {q}")
@@ -456,3 +522,7 @@ if a.compare_heads:
     m0, m1 = statistics.median(ts[list(arms)[0]]), statistics.median(ts[md_name])
     print(f"multi-discrete {a.config}: {m1:.1f} us/step against {m0:.1f} ({m1 - m0:+.1f} us, {100 * (m1 / m0 - 1):+.1f} %), "
           f"launches {engines[md_name].launches_per_step} against {engines[list(arms)[0]].launches_per_step}")
+if a.compare_mask:
+    m0, m1 = statistics.median(ts["unmasked"]), statistics.median(ts[mask_name])
+    print(f"masked {a.config}: {m1:.1f} us/step against {m0:.1f} ({m1 - m0:+.1f} us, {100 * (m1 / m0 - 1):+.1f} %), "
+          f"launches {engines[mask_name].launches_per_step} against {engines['unmasked'].launches_per_step}")

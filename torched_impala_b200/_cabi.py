@@ -49,6 +49,7 @@ def reward_clip_code(reward_clip) -> int:
 ACT_CATEGORICAL = 0
 ACT_GAUSSIAN = 1
 ACT_MULTI_DISCRETE = 0x100  # IMPALA_ACT_MULTI_DISCRETE(K) = ACT_MULTI_DISCRETE | K
+ACT_MASKED = 0x200  # IMPALA_ACT_MASKED: OR-ed onto categorical or multi-discrete, one int32 legal word per step
 ACT_DISTS = {"categorical": ACT_CATEGORICAL, "gaussian": ACT_GAUSSIAN}  # action distributions (IMPALA_ACT_*)
 MAX_GAUSSIAN_DIMS = 16  # action dimensions of impala_vtrace_loss_gauss (2A <= 32 policy outputs)
 MAX_HEADS = 16  # heads of impala_vtrace_loss_md (sum n_k <= 32 policy outputs)
@@ -72,13 +73,20 @@ def check_heads(action_heads) -> tuple:
     return heads
 
 
-def act_kind_code(action_dist: str, action_heads=()) -> int:
-    """The IMPALA_ACT_* code of `action_dist`; "multi_discrete" carries its head count (check_heads)."""
+def act_kind_code(action_dist: str, action_heads=(), action_mask: bool = False) -> int:
+    """The IMPALA_ACT_* code of `action_dist`; "multi_discrete" carries its head count (check_heads), action_mask=True
+    adds IMPALA_ACT_MASKED (categorical and multi-discrete only)."""
+    if not isinstance(action_mask, bool):
+        raise ValueError(f"action_mask must be a bool, got {action_mask!r}")
     if action_dist == "multi_discrete":
-        return ACT_MULTI_DISCRETE | len(check_heads(action_heads))
-    if not isinstance(action_dist, str) or action_dist not in ACT_DISTS:
+        code = ACT_MULTI_DISCRETE | len(check_heads(action_heads))
+    elif not isinstance(action_dist, str) or action_dist not in ACT_DISTS:
         raise ValueError(f"action_dist must be one of {sorted(ACT_DISTS) + ['multi_discrete']}, got {action_dist!r}")
-    return ACT_DISTS[action_dist]
+    else:
+        code = ACT_DISTS[action_dist]
+    if action_mask and code == ACT_GAUSSIAN:
+        raise ValueError("action_mask is for categorical and multi-discrete policies, not action_dist='gaussian'")
+    return code | ACT_MASKED if action_mask else code
 
 
 _ERRORS = {-1: "IMPALA_ERR_BAD_ARG", -2: "IMPALA_ERR_UNSUPPORTED_SHAPE",
@@ -132,6 +140,7 @@ SIGNATURES = {
     "impala_vtrace_loss_rclip": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p]),
     "impala_vtrace_loss_gauss": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p]),
     "impala_vtrace_loss_md": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p, _i, _p]),
+    "impala_vtrace_loss_mask": (_i, [_p] * 13 + [_i64, _i, _i, _i] + [_f] * 7 + [_i, _p, _p, _i, _p, _i, _p]),
     "impala_batch_layout_act": (_i, [_i] * 7 + [C.POINTER(_i64), C.POINTER(_i64)]),
     "impala_ingest_shard_act": (_i, [_p, _p] + [_i] * 9 + [_p]),
     "impala_batch_compose_act": (_i, [_p, _p, _i64, _p] + [_i] * 8 + [_p]),
@@ -188,18 +197,20 @@ def param_layout(O: int, H: int, N2: int):
 
 
 def batch_layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1,
-                 action_dist: str = "categorical", action_heads=()):
+                 action_dist: str = "categorical", action_heads=(), action_mask: bool = False):
     """Slab layout for networks of O observation features; frames > 1 stores the O / frames features of
     each stacked frame once (impala_batch_layout_frames); action_dist="gaussian" holds (T, B, 2A) behaviour
     outputs and (T, B, A) float32 actions, "multi_discrete" (T, B, A = sum action_heads) behaviour logits and
-    (T, B, K) int32 actions (impala_batch_layout_act)."""
+    (T, B, K) int32 actions (impala_batch_layout_act); action_mask=True adds the legal word to the actions, (T, B, 2)
+    or (T, B, K + 1) int32."""
     offs = (_i64 * 6)()
     total = _i64()
-    if action_dist != "categorical":
+    if action_dist != "categorical" or action_mask:
         if frames < 1 or O % frames:
             raise ValueError(f"{O} observation features do not split into {frames} frames")
         check(lib().impala_batch_layout_act(T, B, O // frames, frames, A, obs_dtype_code(obs_dtype),
-                                            act_kind_code(action_dist, action_heads), offs, C.byref(total)),
+                                            act_kind_code(action_dist, action_heads, action_mask), offs,
+                                            C.byref(total)),
               "impala_batch_layout_act")
     elif frames == 1:
         check(lib().impala_batch_layout_obs(T, B, O, A, obs_dtype_code(obs_dtype), offs, C.byref(total)),

@@ -40,6 +40,7 @@ def _units():
     units = [("mlp", "mlp.cu", []), ("vtrace_loss", "vtrace_loss.cu", []),
              ("vtrace_loss_rclip", "vtrace_loss_rclip.cu", []), ("vtrace_loss_gauss", "vtrace_loss_gauss.cu", []),
              ("vtrace_loss_md", "vtrace_loss_md.cu", []),
+             ("vtrace_loss_mask", "vtrace_loss_mask.cu", []),
              ("optim", "optim.cu", []), ("abi", "abi.cu", []),
              ("mlp_fwd_tc", "mlp_fwd_tc.cu", []), ("mlp_bwd_tc", "mlp_bwd_tc.cu", []),
              ("loss_terms", "loss_terms.cu", []), ("mlp_obs_tc", "mlp_obs_tc.cu", []),

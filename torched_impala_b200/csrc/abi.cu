@@ -24,8 +24,13 @@ static int64_t obs_bytes(int obs_dtype) {
     return obs_dtype == IMPALA_OBS_F32 ? 4 : obs_dtype == IMPALA_OBS_U8 ? 1 : 0;
 }
 
-// multi-discrete: 1 <= K <= 16 heads of at least two actions each among the A outputs
+// multi-discrete: 1 <= K <= 16 heads of at least two actions each among the A outputs; masked: categorical or
+// multi-discrete, at most 32 outputs (one legal word)
 static bool act_kind_ok(int act_kind, int A) {
+    if (act_kind & IMPALA_ACT_MASKED) {
+        const int base = act_kind & ~IMPALA_ACT_MASKED;
+        return A <= 32 && (base == IMPALA_ACT_CATEGORICAL || (impala_md_heads(base) && act_kind_ok(base, A)));
+    }
     if (act_kind == IMPALA_ACT_CATEGORICAL || act_kind == IMPALA_ACT_GAUSSIAN) return true;
     const int K = impala_md_heads(act_kind);
     return K >= 1 && K <= 16 && A >= 2 * K;

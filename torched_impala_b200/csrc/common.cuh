@@ -15,11 +15,16 @@ static inline int64_t impala_round_up(int64_t x, int64_t a) { return (x + a - 1)
 static inline int64_t impala_beh_width(int A, int act_kind) {
     return (int64_t)(act_kind == IMPALA_ACT_GAUSSIAN ? 2 * A : A) * 4;
 }
-// the head count K of an IMPALA_ACT_MULTI_DISCRETE(K) kind, 0 for the other kinds
-static inline int impala_md_heads(int act_kind) { return (act_kind & ~0xff) == 0x100 ? (act_kind & 0xff) : 0; }
+// the head count K of an IMPALA_ACT_MULTI_DISCRETE(K) kind, masked or not, 0 for the other kinds
+static inline int impala_md_heads(int act_kind) {
+    const int k = act_kind & ~IMPALA_ACT_MASKED;
+    return (k & ~0xff) == 0x100 ? (k & 0xff) : 0;
+}
+// IMPALA_ACT_MASKED: one more int32 per step, the legal word
 static inline int64_t impala_act_width(int A, int act_kind) {
-    if (const int K = impala_md_heads(act_kind)) return (int64_t)K * 4;
-    return act_kind == IMPALA_ACT_GAUSSIAN ? (int64_t)A * 4 : 4;
+    const int64_t legal = (act_kind & IMPALA_ACT_MASKED) ? 4 : 0;
+    if (const int K = impala_md_heads(act_kind)) return (int64_t)K * 4 + legal;
+    return act_kind == IMPALA_ACT_GAUSSIAN ? (int64_t)A * 4 : 4 + legal;
 }
 
 struct MlpLayout {

@@ -3,8 +3,9 @@
 //
 // The kernel body and its launcher; vtrace_loss.cu holds the entry points of the plain, diag and PopArt
 // kernels, vtrace_loss_rclip.cu those of the reward-clipping ones and vtrace_loss_gauss.cu those of the
-// diagonal-Gaussian policies (three translation units, so the parallel build compiles the sets of
-// instantiations side by side).
+// diagonal-Gaussian policies, vtrace_loss_md.cu those of the multi-discrete ones and vtrace_loss_mask.cu those of
+// the masked categorical and multi-discrete ones (separate translation units, so the parallel build compiles the
+// sets of instantiations side by side).
 //
 // Lane = trajectory, warp = time segment (vtrace_lane_kernel below): every tensor of the
 // time-major (T, B[, A]) batch is read and written as fully coalesced row segments straight from /
@@ -56,6 +57,25 @@ __device__ __forceinline__ float selp_f32(bool p, float x, float y) {
     asm("{\n\t.reg .pred q;\n\tsetp.ne.s32 q, %3, 0;\n\tselp.f32 %0, %1, %2, q;\n\t}" : "=f"(d) : "f"(x), "f"(y), "r"((int)p));
     return d;
 }
+
+// MASK: a step's legal word with the bits >= A dropped; no legal bit makes the whole row legal (padded steps, the
+// empty columns of replay)
+__device__ __forceinline__ unsigned legal_row(unsigned w, int A) {
+    const unsigned all = A >= 32 ? ~0u : (1u << A) - 1u;
+    w &= all;
+    return w ? w : all;
+}
+
+// MASK: the illegal entries of a row (lg: legal_row) set to -inf by selects, so that whatever the row held there (raw
+// logits, -inf, NaN) is gone: the maximum and log-sum-exp of the legal entries follow with the unmasked arithmetic
+// (2^-inf = 0 adds exactly zero), and every later use tests the entry against -inf.  With every bit set nothing changes.
+template <int AP>
+__device__ __forceinline__ void mask_row(unsigned lg, float (&z)[AP]) {
+#pragma unroll
+    for (int k = 0; k < AP; ++k) z[k] = ((lg >> k) & 1u) ? z[k] : -INFINITY;
+}
+// legal entry test of a masked row (log2 pi or a shifted logit: -inf exactly where mask_row put it)
+__device__ __forceinline__ bool is_legal(float x) { return x != -INFINITY; }
 
 constexpr int kMaxSeg = 32;  // time segments (= warps) per CTA
 
@@ -155,11 +175,13 @@ __device__ __forceinline__ void store_logits(float* __restrict__ p, unsigned ele
 // whole-row register arrays of the other instantiations no longer fit: the row is loaded, reduced
 // and dropped.  Returns the base-2 shift -max * log2(e) and lse2 = log2 sum_k 2^(z_k log2(e) - max
 // log2(e)), so log2 pi(k) = fmaf(z_k, log2(e), shift) - lse2; *za is the shifted logit of `act`.
-template <int AP, bool VEC>
+// MASK: over the entries of the legal word lg only (mask_row: the illegal ones are -inf, 2^-inf adds exactly 0).
+template <int AP, bool VEC, bool MASK = false>
 __device__ __forceinline__ void row_lse2(const float* __restrict__ p, unsigned elem, int A, int act, float* shift,
-                                         float* lse2, float* za) {
+                                         float* lse2, float* za, unsigned lg = 0u) {
     float z[AP];
     load_logits<AP, VEC>(p, elem, A, z);
+    if constexpr (MASK) mask_row<AP>(lg, z);
     float mx = z[0];
 #pragma unroll
     for (int k = 1; k < AP; ++k)
@@ -176,10 +198,10 @@ __device__ __forceinline__ void row_lse2(const float* __restrict__ p, unsigned e
 }
 
 // KL(mu || pi) / ln 2 of one streaming row pair (VEC rows), from the shifts and log-sum-exps row_lse2 returned:
-// both rows are read again four logits at a time (L1 / L2 hits), so no whole row is held.
-template <int AP>
+// both rows are read again four logits at a time (L1 / L2 hits), so no whole row is held.  MASK: the legal entries only.
+template <int AP, bool MASK = false>
 __device__ __forceinline__ float row_kl2(const float* __restrict__ pc, const float* __restrict__ pb, unsigned elem,
-                                         float shc, float lsec, float shb, float lseb) {
+                                         float shc, float lsec, float shb, float lseb, unsigned lg = 0u) {
     float kl = 0.f;
 #pragma unroll
     for (int k = 0; k < AP; k += 4) {
@@ -189,7 +211,7 @@ __device__ __forceinline__ float row_kl2(const float* __restrict__ pc, const flo
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const float lpi = fmaf(zc[j], kLog2e, shc) - lsec, lmu = fmaf(zb[j], kLog2e, shb) - lseb;
-            kl = fmaf(ex2f(lmu), lmu - lpi, kl);
+            if (!MASK || ((lg >> (k + j)) & 1u)) kl = fmaf(ex2f(lmu), lmu - lpi, kl);
         }
     }
     return kl;
@@ -426,6 +448,145 @@ __device__ __forceinline__ float md_grad(const float* __restrict__ pc, unsigned 
     return ent;
 }
 
+// md_terms for MASK (the unmasked kernels keep md_terms above, and its code): the action row is [a_0 .. a_{K-1}, legal];
+// *lgo receives the legal word (legal_row, then every head without a legal bit made all-legal).  The sweep skips the
+// illegal entries: a head's differences d_j and online sums start at its first legal entry, which takes the place of
+// s_k.  With every bit set it is md_terms, operation for operation.
+template <int AP, bool VEC, bool DIAG>
+__device__ __forceinline__ unsigned md_terms_masked(const float* __restrict__ pc, const float* __restrict__ pb,
+                                             const int32_t* __restrict__ pa, unsigned elem, int A, unsigned hm,
+                                             float* lp2, float* lr2, float* kl2, unsigned* lgo) {
+    constexpr int W = AP < 4 ? AP : 4;
+    const int K = __popc(hm);
+    const unsigned KW = (unsigned)K + 1u;  // int32 per action row: the K indices, the legal word
+    const unsigned lg0 = legal_row((unsigned)__ldg(pa + elem * KW + K), A);
+    unsigned taken = 0u, rest = hm, lg = lg0;
+#pragma unroll
+    for (int k = 0; k < kMaxHeads; ++k) {
+        if (k < K) {
+            const int ak = __ldg(pa + elem * KW + k), s = __ffs(rest) - 1;
+            rest &= rest - 1u;
+            const int n = (rest ? __ffs(rest) - 1 : A) - s;
+            if ((unsigned)ak < (unsigned)n) taken |= 1u << (s + ak);
+            const unsigned hb = (unsigned)(((1ull << n) - 1ull) << s);  // an empty head is all-legal
+            if (!(lg0 & hb)) lg |= hb;
+        }
+    }
+    *lgo = lg;
+    bool fresh = false, any = false;  // no legal entry of the open head seen yet; a head opened
+    // current row: shift sh, maximum m, sum s; behaviour row: shb, mb, sb; ub = sum 2^(xb - mb) 2^d,
+    // wb = sum 2^(xb - mb) (-d).  Closed heads: msc = sum of the maxima, prc / prb / pru = products of the sums
+    float shc = 0.f, shb = 0.f, rs = 0.f, mc = 0.f, sc = 1.f, mb = 0.f, sb = 1.f, ub = 1.f, wb = 0.f;
+    float msc = 0.f, prc = 1.f, prb = 1.f, pru = 1.f, klw = 0.f, za = 0.f, da = 0.f;
+#pragma unroll
+    for (int j0 = 0; j0 < AP; j0 += W) {
+        float zc[W], zb[W];
+        md_chunk<AP, VEC>(pc, elem, A, j0, zc);
+        md_chunk<AP, VEC>(pb, elem, A, j0, zb);
+#pragma unroll
+        for (int u = 0; u < W; ++u) {
+            const int j = j0 + u;
+            fresh = fresh || ((hm >> j) & 1u);
+            if (j < A && ((lg >> j) & 1u)) {
+                const bool st = fresh;  // the head's first legal entry
+                fresh = false;
+                if (st) {
+                    if (any) {  // close the previous head
+                        msc += mc, prc *= sc, prb *= sb, pru *= ub;
+                        if constexpr (DIAG) klw += __fdividef(wb, sb);
+                    }
+                    any = true;
+                    shc = -zc[u] * kLog2e, shb = -zb[u] * kLog2e, rs = zc[u] - zb[u];
+                }
+                const float xc = fmaf(zc[u], kLog2e, shc), xb = fmaf(zb[u], kLog2e, shb);
+                const float d = ((zc[u] - zb[u]) - rs) * kLog2e, ed = ex2f(d);
+                if (st) {
+                    mc = xc, sc = 1.f, mb = xb, sb = 1.f, ub = ed, wb = -d;
+                } else {
+                    float ec, eb;
+                    md_online(xc, mc, sc, &ec);
+                    const bool up = md_online(xb, mb, sb, &eb);
+                    ub = up ? fmaf(ub, eb, ed) : fmaf(eb, ed, ub);
+                    if constexpr (DIAG) wb = up ? fmaf(wb, eb, -d) : fmaf(eb, -d, wb);
+                }
+                if ((taken >> j) & 1u) za += xc, da += d;
+            }
+        }
+    }
+    msc += mc, prc *= sc, prb *= sb, pru *= ub;
+    if constexpr (DIAG) klw += __fdividef(wb, sb);
+    const float lrs = lg2f(pru / prb);  // sum_k log2 sum_j mu_j 2^d_j
+    *lp2 = za - (msc + lg2f(prc));
+    *lr2 = da - lrs;
+    *kl2 = klw + lrs;
+    return taken;
+}
+// md_grad for MASK (lg: md_terms_masked's *lgo): the forward sweep skips the illegal entries, each head's sums
+// starting at its first legal entry; the head's last entry still parks c_k and H_k, legal or not (n_k >= 2 is the head
+// size); the gradient is exactly zero at illegal entries.
+template <int AP, bool VEC>
+__device__ __forceinline__ float md_grad_masked(const float* __restrict__ pc, unsigned elem, int A, unsigned hm,
+                                         unsigned taken, bool valid, float cp, float entropy_c, float inv_batch,
+                                         float (&dz)[AP], unsigned lg) {
+    constexpr int W = AP < 4 ? AP : 4;
+    const unsigned em = (hm >> 1) | (1u << (A - 1));  // bit j: output j is the last of its head
+    float sh = 0.f, m = 0.f, s = 1.f, t = 0.f, ent = 0.f;
+    bool fresh = false;  // no legal entry of the open head seen yet
+#pragma unroll
+    for (int j0 = 0; j0 < AP; j0 += W) {
+        float z[W];
+        md_chunk<AP, VEC>(pc, elem, A, j0, z);
+#pragma unroll
+        for (int u = 0; u < W; ++u) {
+            const int j = j0 + u;
+            fresh = fresh || ((hm >> j) & 1u);
+            if (j < A) {
+                if ((lg >> j) & 1u) {
+                    const bool st = fresh;  // the head's first legal entry
+                    fresh = false;
+                    if (st) sh = -z[u] * kLog2e;
+                    const float x = fmaf(z[u], kLog2e, sh);
+                    if (st) {
+                        m = x, s = 1.f, t = x;
+                    } else {
+                        float e;
+                        t = md_online(x, m, s, &e) ? fmaf(t, e, x) : fmaf(e, x, t);
+                    }
+                }
+                if ((em >> j) & 1u) {
+                    const float lse = m + lg2f(s), h = (lse - __fdividef(t, s)) * kLn2;
+                    ent += h;
+                    dz[j] = sh - lse;
+                    if (j > 0) dz[j > 0 ? j - 1 : 0] = h;
+                }
+            }
+        }
+    }
+    float c = 0.f, H = 0.f;
+#pragma unroll
+    for (int j0 = AP - W; j0 >= 0; j0 -= W) {
+        float z[W];
+        md_chunk<AP, VEC>(pc, elem, A, j0, z);
+#pragma unroll
+        for (int u = W - 1; u >= 0; --u) {
+            const int j = j0 + u;
+            if (j < A) {
+                if ((em >> j) & 1u) {
+                    c = dz[j];
+                    if (j > 0) H = dz[j > 0 ? j - 1 : 0];
+                }
+                const float lp = fmaf(z[u], kLog2e, c), p = ex2f(lp);  // log2 p_j, p_j
+                const float onehot = ((taken >> j) & 1u) ? 1.f : 0.f;
+                const float d = inv_batch * (cp * (p - onehot) + entropy_c * p * (lp * kLn2 + H));
+                dz[j] = (valid && ((lg >> j) & 1u)) ? d : 0.f;
+            } else {
+                dz[j] = 0.f;
+            }
+        }
+    }
+    return ent;
+}
+
 // POPART: {mu, sigma, 1 / sigma} as float32 in shared memory, read through a volatile pointer at every use so
 // that the three values take no register across the unroll (the DIAG twins are at their register limit).
 struct PopVals {
@@ -490,9 +651,18 @@ struct PopVals {
 // behaviour rows and the K action indices of a step as they load, and keeps the step's taken mask in the action slot
 // of the rows; step 4 re-reads the current row for the entropy and the N gradients.
 // ------------------------------------------------------------------------------------------------
-// The body is one device function; vtrace_lane_kernel (softmax policies), vtrace_gauss_kernel (GAUSS) and
-// vtrace_md_kernel (MD) are its thin __global__ entries, so the categorical instantiations keep their names and code.
-template <int AP, int S, bool WITH_LOSS, bool VEC, bool DIAG, bool POPART, bool RCLIP, bool GAUSS, bool MD = false>
+// MASK (categorical or MD): invalid-action masking.  The action row carries one more int32, the step's legal word
+// (categorical: [a, legal], read with the index in one 64-bit load; MD: [a_0 .. a_{K-1}, legal], read by md_terms),
+// kept as one register per step (legal_row: bits >= A dropped, an empty head all-legal).  Every sum over a row's
+// entries (maxima, log-sum-exps, KL, entropy) takes the legal entries only, the maxima folding from -inf, and the
+// gradient is selected to exactly zero at illegal entries, so no illegal logit reaches an output.  With every bit set
+// the predicates are all true and the arithmetic and its order are those of the unmasked twin.
+// ------------------------------------------------------------------------------------------------
+// The body is one device function; vtrace_lane_kernel (softmax policies), vtrace_gauss_kernel (GAUSS),
+// vtrace_md_kernel (MD), vtrace_mask_kernel (MASK) and vtrace_md_mask_kernel (MD and MASK) are its thin __global__
+// entries, so the categorical instantiations keep their names and code.
+template <int AP, int S, bool WITH_LOSS, bool VEC, bool DIAG, bool POPART, bool RCLIP, bool GAUSS, bool MD = false,
+          bool MASK = false>
 __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCLIP, MD>& a) {
     constexpr bool STREAM = !GAUSS && !MD && AP > 16;
     constexpr bool HELD = !STREAM && !GAUSS && !MD;  // the logit rows of a chunk are held in registers
@@ -500,6 +670,7 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCL
     static_assert(!STREAM || S == 1, "the streaming rows keep one step per thread");
     static_assert(!GAUSS || (WITH_LOSS && AP <= 16), "Gaussian policies: the loss kernel, up to 16 action dimensions");
     static_assert(!MD || (WITH_LOSS && !GAUSS), "multi-discrete policies: the loss kernel");
+    static_assert(!MASK || (WITH_LOSS && !GAUSS), "action masks: categorical and multi-discrete loss kernels");
     // GAUSS: the (T, B, A) float32 action samples (the categorical kernels read int32 indices there)
     const float* const gact = reinterpret_cast<const float*>(a.actions);
     static_assert(!DIAG || WITH_LOSS, "the off-policy sums ride the loss reduction");
@@ -545,6 +716,7 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCL
     struct Rows {
         float zc[SR][AR], zb[SR][AR], r[S], vv[S + 1];
         int act[S];
+        unsigned lg[MASK ? S : 1];  // MASK: the legal words (legal_row)
         unsigned char dn[S];  // raw: compared where it is used, so the load is not waited for at issue
     };
     auto load_rows = [&](Rows& R, const int c) {
@@ -557,7 +729,12 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCL
                 load_logits<AP, VEC>(a.beh_logits, e, A, R.zb[i]);
             }
             R.r[i] = __ldg(a.rewards + e);
-            if constexpr (!GAUSS && !MD) R.act[i] = __ldg(a.actions + e);
+            if constexpr (MASK && !MD) {
+                const int2 q = __ldg(reinterpret_cast<const int2*>(a.actions) + e);  // [a, legal]
+                R.act[i] = q.x, R.lg[i] = legal_row((unsigned)q.y, A);
+            } else if constexpr (!GAUSS && !MD) {
+                R.act[i] = __ldg(a.actions + e);
+            }
             R.dn[i] = __ldg(a.done + e);
         }
 #pragma unroll
@@ -585,8 +762,12 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCL
             } else if constexpr (MD) {
                 const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
                 float kl2;
-                R.act[i] = (int)md_terms<AP, VEC, DIAG>(a.cur_logits, a.beh_logits, a.actions, e, A, a.head_mask,
-                                                        &lp2a[i], &lr2, &kl2);
+                if constexpr (MASK)
+                    R.act[i] = (int)md_terms_masked<AP, VEC, DIAG>(a.cur_logits, a.beh_logits, a.actions, e, A,
+                                                                   a.head_mask, &lp2a[i], &lr2, &kl2, &R.lg[MASK ? i : 0]);
+                else
+                    R.act[i] = (int)md_terms<AP, VEC, DIAG>(a.cur_logits, a.beh_logits, a.actions, e, A, a.head_mask,
+                                                            &lp2a[i], &lr2, &kl2);
                 if constexpr (DIAG) {
                     if (valid) d_kl += kl2;
                 }
@@ -596,17 +777,20 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCL
                 if constexpr (STREAM) {
                     const unsigned e = (unsigned)min(tb + i, T - 1) * (unsigned)B + (unsigned)bl;
                     float shb;
-                    row_lse2<AP, VEC>(a.cur_logits, e, A, R.act[i], &shc[i], &lsec[i], &z_a);
-                    row_lse2<AP, VEC>(a.beh_logits, e, A, R.act[i], &shb, &lseb, &zb_a);
+                    const unsigned lg = MASK ? R.lg[MASK ? i : 0] : 0u;
+                    row_lse2<AP, VEC, MASK>(a.cur_logits, e, A, R.act[i], &shc[i], &lsec[i], &z_a, lg);
+                    row_lse2<AP, VEC, MASK>(a.beh_logits, e, A, R.act[i], &shb, &lseb, &zb_a, lg);
                     lse = lsec[i];
                     if constexpr (DIAG && VEC) {
-                        if (valid) d_kl += row_kl2<AP>(a.cur_logits, a.beh_logits, e, shc[i], lsec[i], shb, lseb);
+                        if (valid)
+                            d_kl += row_kl2<AP, MASK>(a.cur_logits, a.beh_logits, e, shc[i], lsec[i], shb, lseb, lg);
                     } else if constexpr (DIAG) {
                         // non-VEC rows: KL in step 4 next to the current row's re-read (row_kl2 here spills); the
                         // behaviour row's shift and lse2 are parked in the row slots the streaming path leaves unused
                         R.zb[i][0] = shb, R.zc[i][0] = lseb;
                     }
                 } else {
+                    if constexpr (MASK) mask_row<AP>(R.lg[MASK ? i : 0], R.zc[i]), mask_row<AP>(R.lg[MASK ? i : 0], R.zb[i]);
                     float mx = R.zc[i][0], mxb = R.zb[i][0];
 #pragma unroll
                     for (int k = 1; k < AP; ++k)
@@ -619,7 +803,8 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCL
                         R.zb[i][k] = fmaf(R.zb[i][k], kLog2e, mxbl);
                         if (k < A) se += ex2f(R.zc[i][k]), seb += ex2f(R.zb[i][k]);
                         if constexpr (DIAG) {
-                            if (k < A) klw = fmaf(ex2f(R.zb[i][k]), R.zb[i][k] - R.zc[i][k], klw);  // same ex2 as seb's
+                            if (k < A && (!MASK || is_legal(R.zb[i][k])))
+                                klw = fmaf(ex2f(R.zb[i][k]), R.zb[i][k] - R.zc[i][k], klw);  // same ex2 as seb's
                         }
                     }
                     lse = lg2f(se), lseb = lg2f(seb);
@@ -738,16 +923,27 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCL
                     }
                     ent = fmaf((float)A, kHalfLog2PiE, ent);
                 } else if constexpr (MD) {
-                    ent = md_grad<AP, VEC>(a.cur_logits, (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl, A,
-                                           a.head_mask, (unsigned)R.act[i], valid, a.policy_loss_c * pg, a.entropy_c,
-                                           a.inv_batch, dz);
+                    if constexpr (MASK)
+                        ent = md_grad_masked<AP, VEC>(a.cur_logits, (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl,
+                                                      A, a.head_mask, (unsigned)R.act[i], valid, a.policy_loss_c * pg,
+                                                      a.entropy_c, a.inv_batch, dz, R.lg[MASK ? i : 0]);
+                    else
+                        ent = md_grad<AP, VEC>(a.cur_logits, (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl, A,
+                                               a.head_mask, (unsigned)R.act[i], valid, a.policy_loss_c * pg, a.entropy_c,
+                                               a.inv_batch, dz);
                 } else if constexpr (STREAM) {
                     // re-read the row; dz holds log2 pi(k), then the gradient (one row of registers)
                     load_logits<AP, VEC>(a.cur_logits, (unsigned)min(t, T - 1) * (unsigned)B + (unsigned)bl, A, dz);
+                    if constexpr (MASK) mask_row<AP>(R.lg[MASK ? i : 0], dz);
 #pragma unroll
                     for (int k = 0; k < AP; ++k) {
                         dz[k] = fmaf(dz[k], kLog2e, shc[i]) - lsec[i];
-                        if (k < A) ent -= ex2f(dz[k]) * (dz[k] * kLn2);
+                        // MASK: the twin's form - VEC, the unconditional FMA with a zero factor at an illegal entry
+                        // (2^-inf = 0); otherwise the predicated one
+                        if constexpr (MASK && VEC)
+                            ent -= ex2f(dz[k]) * (is_legal(dz[k]) ? dz[k] * kLn2 : 0.f);
+                        else if (k < A && (!MASK || is_legal(dz[k])))
+                            ent -= ex2f(dz[k]) * (dz[k] * kLn2);
                     }
                     if constexpr (DIAG && !VEC) {
                         // KL(mu || pi) / ln 2 against the log2 pi(k) in dz: the behaviour row again
@@ -758,33 +954,37 @@ __device__ __forceinline__ void vtrace_lane_body(const VtArgsM<DIAG, POPART, RCL
                             for (int k = 0; k < AP; ++k) {
                                 const float zb = k < A ? __ldg(a.beh_logits + eb * A + k) : 0.f;
                                 const float lmu = fmaf(zb, kLog2e, R.zb[i][0]) - R.zc[i][0];  // log2 mu(k)
-                                if (k < A) kl = fmaf(ex2f(lmu), lmu - dz[k], kl);
+                                if (k < A && (!MASK || is_legal(dz[k]))) kl = fmaf(ex2f(lmu), lmu - dz[k], kl);
                             }
                             d_kl += kl;
                         }
                     }
 #pragma unroll
                     for (int k = 0; k < AP; ++k) {
+                        // MASK: pk = 2^-inf = 0 at an illegal entry already; its gradient (0 * -inf) is selected away
+                        const bool ok = k < A && (!MASK || is_legal(dz[k]));
                         const float lz = dz[k] * kLn2, pk = (k < A) ? ex2f(dz[k]) : 0.f;
                         const float onehot = (k == R.act[i]) ? 1.f : 0.f;
                         const float d = a.inv_batch * (a.policy_loss_c * pg * (pk - onehot) +
                                                        a.entropy_c * pk * (lz + ent));
-                        dz[k] = (valid && k < A) ? d : 0.f;
+                        dz[k] = (valid && ok) ? d : 0.f;
                     }
                 } else {
                     float pk[AP], lz[AP];
 #pragma unroll
                     for (int k = 0; k < AP; ++k) {
+                        const bool ok = k < A && (!MASK || is_legal(R.zc[i][k]));
                         lz[k] = R.zc[i][k] * kLn2;
-                        pk[k] = (k < A) ? ex2f(R.zc[i][k]) : 0.f;
-                        if (k < A) ent -= pk[k] * lz[k];                           // :310-314, :153
+                        pk[k] = ok ? ex2f(R.zc[i][k]) : 0.f;
+                        if (ok) ent -= pk[k] * lz[k];                           // :310-314, :153
                     }
 #pragma unroll
                     for (int k = 0; k < AP; ++k) {
+                        const bool ok = k < A && (!MASK || is_legal(R.zc[i][k]));
                         const float onehot = (k == R.act[i]) ? 1.f : 0.f;
                         const float d = a.inv_batch * (a.policy_loss_c * pg * (pk[k] - onehot) +
                                                        a.entropy_c * pk[k] * (lz[k] + ent));
-                        dz[k] = (valid && k < A) ? d : 0.f;
+                        dz[k] = (valid && ok) ? d : 0.f;
                     }
                 }
                 if (live && t < T) {
@@ -910,6 +1110,14 @@ template <int AP, int S, int MAXT, int MINB, bool VEC, bool DIAG, bool POPART, b
 __global__ void __launch_bounds__(MAXT, MINB) vtrace_md_kernel(const VtArgsM<DIAG, POPART, RCLIP, true> a) {
     vtrace_lane_body<AP, S, true, VEC, DIAG, POPART, RCLIP, false, true>(a);
 }
+template <int AP, int S, int MAXT, int MINB, bool VEC, bool DIAG, bool POPART, bool RCLIP>
+__global__ void __launch_bounds__(MAXT, MINB) vtrace_mask_kernel(const VtArgsT<DIAG, POPART, RCLIP> a) {
+    vtrace_lane_body<AP, S, true, VEC, DIAG, POPART, RCLIP, false, false, true>(a);
+}
+template <int AP, int S, int MAXT, int MINB, bool VEC, bool DIAG, bool POPART, bool RCLIP>
+__global__ void __launch_bounds__(MAXT, MINB) vtrace_md_mask_kernel(const VtArgsM<DIAG, POPART, RCLIP, true> a) {
+    vtrace_lane_body<AP, S, true, VEC, DIAG, POPART, RCLIP, false, true, true>(a);
+}
 
 int pick_ap(int A) {
     if (A <= 2) return 2;
@@ -923,10 +1131,16 @@ int pick_ap(int A) {
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 template <int AP, int S, int MAXT, int MINB, bool WITH_LOSS, bool DIAG, bool POPART, bool RCLIP, bool GAUSS = false,
-          bool MD = false>
+          bool MD = false, bool MASK = false>
 int launch_s(const VtArgsM<DIAG, POPART, RCLIP, MD>& a, bool vec, unsigned groups, int nw, int cl, cudaStream_t st) {
     cudaError_t e;
-    if constexpr (MD)
+    if constexpr (MD && MASK)
+        e = vec ? impala_launch_cl(vtrace_md_mask_kernel<AP, S, MAXT, MINB, true, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
+                : impala_launch_cl(vtrace_md_mask_kernel<AP, S, MAXT, MINB, false, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
+    else if constexpr (MASK)
+        e = vec ? impala_launch_cl(vtrace_mask_kernel<AP, S, MAXT, MINB, true, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
+                : impala_launch_cl(vtrace_mask_kernel<AP, S, MAXT, MINB, false, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
+    else if constexpr (MD)
         e = vec ? impala_launch_cl(vtrace_md_kernel<AP, S, MAXT, MINB, true, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a)
                 : impala_launch_cl(vtrace_md_kernel<AP, S, MAXT, MINB, false, DIAG, POPART, RCLIP>, groups * cl, 32 * nw, 0, st, true, false, cl, a);
     else if constexpr (GAUSS)
@@ -952,8 +1166,13 @@ constexpr int kMaxCluster = 8;  // portable cluster size
 // does not apply).
 // MD: a.A = N policy outputs, AP = the padded N; S as the categorical twin at that AP (IMPALA_VTRACE_S does not apply),
 // at most 8 warps per CTA at AP = 32 (the 256-thread bound of those instantiations).
+// MASK: the launch shapes of the unmasked twin (categorical or MD), so a full mask gives its results bit for bit.
+// IMPALA_VTRACE_S does not apply (the S = 1 and S = 5 overrides of AP <= 4 spill with the legal words), and the
+// categorical AP = 32 kernels are bounded at 320 threads, the most the launcher picks there (IMPALA_VTRACE_NSEG is
+// clamped to 10 warps): under 512 they spilled.
 constexpr int kMaxGaussA = 16;
-template <bool WITH_LOSS, bool DIAG = false, bool POPART = false, bool RCLIP = false, bool GAUSS = false, bool MD = false>
+template <bool WITH_LOSS, bool DIAG = false, bool POPART = false, bool RCLIP = false, bool GAUSS = false, bool MD = false,
+          bool MASK = false>
 int launch(VtArgsM<DIAG, POPART, RCLIP, MD>& a, cudaStream_t st) {
     if (a.T < 1 || a.B < 1 || a.A < 1) return IMPALA_ERR_BAD_ARG;
     const int AP = (GAUSS && a.A > kMaxGaussA) ? 0 : pick_ap(a.A);
@@ -964,7 +1183,7 @@ int launch(VtArgsM<DIAG, POPART, RCLIP, MD>& a, cudaStream_t st) {
     const bool vec = a.A == AP && aligned16(a.cur_logits) && aligned16(a.beh_logits) &&
                      (!WITH_LOSS || aligned16(a.dlogits)) && (!GAUSS || aligned16(a.actions));
     int S = AP >= (GAUSS ? 8 : 16) ? 1 : 2;
-    const int s_env = (GAUSS || MD) ? 0 : impala_env_int("IMPALA_VTRACE_S", 0);
+    const int s_env = (GAUSS || MD || MASK) ? 0 : impala_env_int("IMPALA_VTRACE_S", 0);
     if (AP <= 4 && (s_env == 1 || s_env == 2 || s_env == 5)) S = s_env;
     const int max_w = S == 5 ? 10 : (AP <= 4 && S == 1 ? kMaxSeg : 16);
     const int nseg = (a.T + S - 1) / S;
@@ -976,29 +1195,32 @@ int launch(VtArgsM<DIAG, POPART, RCLIP, MD>& a, cudaStream_t st) {
     const int n_env = impala_env_int("IMPALA_VTRACE_NSEG", 0);
     if (n_env >= 1 && n_env <= max_w) nw = n_env;
     if constexpr (MD) {
-        if (AP == 2) return launch_s<2, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, nw, cl, st);
-        if (AP == 4) return launch_s<4, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, nw, cl, st);
-        if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, nw, cl, st);
-        if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, nw, cl, st);
-        return launch_s<32, 1, 256, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true>(a, vec, groups, 8 < nw ? 8 : nw, cl, st);
+        if (AP == 2) return launch_s<2, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true, MASK>(a, vec, groups, nw, cl, st);
+        if (AP == 4) return launch_s<4, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true, MASK>(a, vec, groups, nw, cl, st);
+        if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true, MASK>(a, vec, groups, nw, cl, st);
+        if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true, MASK>(a, vec, groups, nw, cl, st);
+        return launch_s<32, 1, 256, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, true, MASK>(a, vec, groups, 8 < nw ? 8 : nw, cl, st);
     } else if constexpr (GAUSS) {
         if (AP == 2) return launch_s<2, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
         if (AP == 4) return launch_s<4, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
         if (AP == 8) return launch_s<8, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
         return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, true>(a, vec, groups, nw, cl, st);
     } else {
-#define VT_AP(APV)                                                                                      \
-    if (AP == APV) {                                                                                    \
-        if (S == 5) return launch_s<APV, 5, 320, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st); \
-        if (S == 1) return launch_s<APV, 1, 1024, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);\
-        return launch_s<APV, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);             \
+#define VT_AP(APV)                                                                                                    \
+    if (AP == APV) {                                                                                                  \
+        if constexpr (!MASK) {                                                                                        \
+            if (S == 5) return launch_s<APV, 5, 320, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st); \
+            if (S == 1) return launch_s<APV, 1, 1024, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);\
+        }                                                                                                             \
+        return launch_s<APV, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, false, MASK>(a, vec, groups, nw, cl, st); \
     }
     VT_AP(2)
     VT_AP(4)
 #undef VT_AP
-    if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);
-    if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);
-    return launch_s<32, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);
+    if (AP == 8) return launch_s<8, 2, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, false, MASK>(a, vec, groups, nw, cl, st);
+    if (AP == 16) return launch_s<16, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, false, MASK>(a, vec, groups, nw, cl, st);
+    if constexpr (MASK) return launch_s<32, 1, 320, 1, WITH_LOSS, DIAG, POPART, RCLIP, false, false, true>(a, vec, groups, 10 < nw ? 10 : nw, cl, st);
+    else return launch_s<32, 1, 512, 1, WITH_LOSS, DIAG, POPART, RCLIP>(a, vec, groups, nw, cl, st);
     }
 }
 

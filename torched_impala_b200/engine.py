@@ -48,6 +48,10 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       behaviour logits (T, B, A) and K int32 indices per step, actions (T, B, K) (impala_batch_layout_act with
       IMPALA_ACT_MULTI_DISCRETE(K)); impala_vtrace_loss_md takes the V-trace slot of the step with the same flags and
       workspace, the head sizes passed by value.  No launch is added.
+    action_mask=True (categorical or multi-discrete; invalid-action masking): every step's actions end in one more
+      int32, the legal word (bit j: output j is legal), (T, B, 2) or (T, B, K + 1) (impala_batch_layout_act with
+      IMPALA_ACT_MASKED); impala_vtrace_loss_mask takes the V-trace slot with the same flags and workspace, pi and mu
+      renormalised over the legal entries.  No launch is added.
 
 obs_dtype="uint8" (byte observations): the slabs hold obs as uint8 (impala_batch_layout_obs).  For
 O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one after the other as the
@@ -79,7 +83,8 @@ after the compose launch are unchanged; the logged `batch_mean_reward` scalar is
 all B columns' rewards / B), the mean over the fresh trajectories is the caller's (Learner logs that one).
 
 The keyword options above (obs_dtype, frames, diagnostics, replay_slabs, replay_columns, optimizer, optimizer_kwargs,
-popart, popart_beta, reward_clip, action_dist, action_heads, shared_torso) are the fields of `LearnerOptions`.
+popart, popart_beta, reward_clip, action_dist, action_heads, shared_torso, action_mask) are the fields of
+`LearnerOptions`.
 """
 from __future__ import annotations
 
@@ -170,17 +175,21 @@ class LearnerOptions:
     # dataclasses.replace does not carry it: pass action_heads= again.
     action_heads: dataclasses.InitVar[tuple] = ()
     shared_torso: bool = False
+    # invalid-action masking (categorical and multi-discrete): every step carries a legal word in its actions.
+    # Init-only like action_heads (Learner._cfg carries it, engine_from_cfg passes it when true).
+    action_mask: dataclasses.InitVar[bool] = False
 
-    def __post_init__(self, action_heads):
+    def __post_init__(self, action_heads, action_mask):
         object.__setattr__(self, "optimizer_kwargs", dict(self.optimizer_kwargs or {}))
         # a tuple whatever sequence came in; check() refuses bad entries
         heads = tuple(action_heads) if isinstance(action_heads, (list, tuple)) else action_heads
         object.__setattr__(self, "action_heads", heads)
+        object.__setattr__(self, "action_mask", action_mask)
 
     def __eq__(self, other):
         if other.__class__ is not self.__class__:
             return NotImplemented
-        return self.action_heads == other.action_heads and all(
+        return self.action_heads == other.action_heads and self.action_mask is other.action_mask and all(
             getattr(self, f.name) == getattr(other, f.name) for f in dataclasses.fields(self))
 
     def check(self, B: int, O: int, A: int, H_pi: int, H_v: int, world: int = 1) -> CheckedOptions:
@@ -198,7 +207,10 @@ class LearnerOptions:
                                  f"has A = {A}")
         elif self.action_heads != ():
             raise ValueError(f"action_heads is for action_dist='multi_discrete', not {self.action_dist!r}")
-        act_kind = _cabi.act_kind_code(self.action_dist, self.action_heads)
+        act_kind = _cabi.act_kind_code(self.action_dist, self.action_heads, self.action_mask)
+        if self.action_mask and A > _cabi.MAX_OUTPUTS:
+            raise ValueError(f"action_mask takes at most {_cabi.MAX_OUTPUTS} policy outputs (one 32-bit legal word), "
+                             f"got A = {A}")
         gaussian = act_kind == _cabi.ACT_GAUSSIAN
         if gaussian and not 1 <= A <= _cabi.MAX_GAUSSIAN_DIMS:
             raise ValueError(f"a Gaussian policy takes 1 to {_cabi.MAX_GAUSSIAN_DIMS} action dimensions (2A outputs "
@@ -224,7 +236,8 @@ def engine_from_cfg(cfg: dict, world: int, device, process_group=None, lr_table=
                          Hyperparameters(**cfg["hp"]), global_batch=cfg["B"], device=device, mode=cfg["mode"],
                          process_group=process_group, lr_table=lr_table,
                          **{f.name: cfg[f.name] for f in dataclasses.fields(LearnerOptions)},
-                         **({"action_heads": tuple(cfg["action_heads"])} if cfg.get("action_heads") else {}))
+                         **({"action_heads": tuple(cfg["action_heads"])} if cfg.get("action_heads") else {}),
+                         **({"action_mask": True} if cfg.get("action_mask") else {}))
 
 
 def _ptr(t: torch.Tensor) -> C.c_void_p:
@@ -268,6 +281,8 @@ class LearnerEngine:
         # multi-discrete: the head sizes (K = len), passed by value to every impala_vtrace_loss_md call
         self.heads = tuple(int(n) for n in o.action_heads) if o.action_dist == "multi_discrete" else ()
         self.md_heads = (C.c_int32 * len(self.heads))(*self.heads) if self.heads else None
+        # action_mask: one more int32 per step in the actions, the legal word (impala_vtrace_loss_mask)
+        self.masked = bool(o.action_mask)
         self.shared_torso, self.popart, self.diagnostics = bool(o.shared_torso), bool(o.popart), bool(o.diagnostics)
         self.popart_beta, self.replay_slabs = float(o.popart_beta), int(o.replay_slabs)
         self.frames, self.F = o.frames, O // o.frames
@@ -323,11 +338,11 @@ class LearnerEngine:
         # ---- batch slab (device) and pinned staging slabs (host), identical layouts (replay: the host slabs
         # hold the B_fresh columns that cross the host link, the device slabs the B columns trained on)
         train_off, train_bytes = _cabi.batch_layout(T, B_local, O, A, o.obs_dtype, o.frames, o.action_dist,
-                                                    o.action_heads)
+                                                    o.action_heads, o.action_mask)
         self.slab_off, self.slab_bytes = train_off, train_bytes
         if self.replay_slabs:
             self.slab_off, self.slab_bytes = _cabi.batch_layout(T, self.B_fresh, O, A, o.obs_dtype, o.frames,
-                                                                o.action_dist, o.action_heads)
+                                                                o.action_dist, o.action_heads, o.action_mask)
         self.fields = ((("obs", np.uint8 if o.obs_dtype == "uint8" else np.float32),) + _BATCH_FIELDS[1:])
         if self.gaussian:  # float32 action samples
             self.fields = self.fields[:2] + (("actions", np.float32),) + self.fields[3:]
@@ -474,8 +489,9 @@ class LearnerEngine:
     def _shapes(self, B: int) -> dict:
         """Shapes of the six batch tensors in a slab of B columns."""
         T, A = self.T, self.A
+        K = (len(self.heads) or 1) + 1 if self.masked else len(self.heads)  # the indices, then the legal word
         return {"obs": (T + self.frames, B, self.F), "beh_logits": (T, B, self.N_pi),
-                "actions": (T, B, A) if self.gaussian else (T, B, len(self.heads)) if self.heads else (T, B),
+                "actions": (T, B, A) if self.gaussian else (T, B, K) if self.heads or self.masked else (T, B),
                 "rewards": (T, B), "done": (T, B), "lens": (B,)}
 
     def _ws_bytes(self, M, O, H, N2):
@@ -639,7 +655,7 @@ class LearnerEngine:
         cs = self.copy_stream
         if self._slab_used[slot]:
             cs.wait_event(self.slab_free[slot])
-        if self.gaussian or self.heads:
+        if self.gaussian or self.heads or self.masked:
             _cabi.check(self.lib.impala_ingest_shard_act(_ptr(self.d_slabs[slot]), C.c_void_p(host_address), self.T,
                                                          B_total, self.F, self.frames, self.A, self.obs_code,
                                                          self.act_kind, b0, self.B, C.c_void_p(cs.cuda_stream)),
@@ -663,7 +679,7 @@ class LearnerEngine:
         launched = lib.impala_launch_count()
         d = self.d_views[slot]
         T, B, O, A = self.T, self.B, self.O, self.N_pi  # A: the policy's outputs from here on
-        if self.replay_slabs and (self.gaussian or self.heads):
+        if self.replay_slabs and (self.gaussian or self.heads or self.masked):
             _cabi.check(lib.impala_batch_compose_act(_ptr(self.d_slabs[slot]), _ptr(self.store), self.slab_bytes,
                                                      _ptr(self.d_plans[slot]), T, B, self.B_fresh, self.F, self.frames,
                                                      self.A, self.obs_code, self.act_kind, st),
@@ -715,6 +731,12 @@ class LearnerEngine:
             _cabi.check(lib.impala_vtrace_loss_gauss(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, T, B, self.A,
                                                      *vt_hp[3:-1], sums, _ptr(self.popart_buf) if self.popart else None,
                                                      self.reward_clip_code, st), "impala_vtrace_loss_gauss")
+        elif self.masked:  # the same flags with the legal words (categorical, or the heads of a multi-discrete policy)
+            sums = C.c_void_p(gbase + 8 * (self.n_total + 4)) if self.n_extra == 12 else None
+            _cabi.check(lib.impala_vtrace_loss_mask(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp[:-1], sums,
+                                                    _ptr(self.popart_buf) if self.popart else None,
+                                                    self.reward_clip_code, self.md_heads, len(self.heads), st),
+                        "impala_vtrace_loss_mask")
         elif self.heads:  # the same flags through the multi-discrete policy terms; A = sum of the heads
             sums = C.c_void_p(gbase + 8 * (self.n_total + 4)) if self.n_extra == 12 else None
             _cabi.check(lib.impala_vtrace_loss_md(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp[:-1], sums,

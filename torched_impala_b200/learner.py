@@ -199,7 +199,80 @@ def check_md_block(block: dict, T: int, n: int, heads) -> None:
                          f"[0, {heads[k]})")
 
 
-def pack_trajectory(views: dict, b: int, traj, T: int, obs=None, heads=()) -> float:
+def _mask_word_errors(m, a, heads):
+    """The first problem of legal masks m (L, N) against action indices a (L, K) over `heads` as (step, head, what),
+    or None: values other than 0 / 1, a head without a legal entry, an illegal taken action."""
+    m = np.asarray(m)
+    if m.dtype != bool:
+        bad = np.argwhere((m != 0) & (m != 1))
+        if bad.size:
+            t, j = (int(v) for v in bad[0])
+            return t, None, f"mask value {m[t, j]!r} at output {j} is not 0 / 1"
+    m = m.astype(bool)
+    s = 0
+    for k, n in enumerate(heads):
+        empty = np.argwhere(~m[:, s:s + n].any(-1))
+        if empty.size:
+            return int(empty[0, 0]), k, "has no legal action"
+        off = np.argwhere(~np.take_along_axis(m[:, s:s + n], a[:, k:k + 1].astype(np.int64), -1)[:, 0])
+        if off.size:
+            t = int(off[0, 0])
+            return t, k, f"action {int(a[t, k])} is illegal under its mask"
+        s += n
+    return None
+
+
+def mask_steps(traj, L: int, heads, actions) -> np.ndarray:
+    """The (L,) int32 legal words of a masked trajectory: traj.action_mask holds L masks of shape (N,), N = sum(heads)
+    (a categorical policy: heads = (A,)), bool or 0 / 1, true meaning legal, as the mask that held when a_t was
+    chosen; `actions` (L, K) the indices taken.  Raises ValueError, naming the trajectory, the step and the head, for a
+    missing mask, a wrong width, values other than 0 / 1, a head without a legal entry or an illegal taken action."""
+    tid = getattr(traj, "id", "?")
+    N = sum(heads)
+    masks = getattr(traj, "action_mask", None)
+    if masks is None or len(masks) != L:
+        raise ValueError(f"trajectory {tid}: a masked learner takes one action_mask per step, got "
+                         f"{'none' if masks is None else len(masks)} for {L} steps")
+    ms = [torch.as_tensor(x) for x in masks]
+    for t, x in enumerate(ms):
+        if tuple(x.shape) != (N,):
+            raise ValueError(f"trajectory {tid}: step {t} action_mask has shape {tuple(x.shape)}, this policy takes "
+                             f"({N},)")
+    m = torch.stack(ms).numpy() if ms else np.zeros((0, N), bool)
+    err = _mask_word_errors(m, np.asarray(actions).reshape(L, len(heads)), heads)
+    if err is not None:
+        t, k, what = err
+        raise ValueError(f"trajectory {tid}: step {t}{'' if k is None else f' head {k}'} {what}")
+    from .synth import legal_words
+
+    return legal_words(m.astype(bool))
+
+
+def check_mask_block(block: dict, T: int, n: int, heads) -> np.ndarray:
+    """put_block's checks of a masked block: block["action_mask"] (T, n, N) legal masks against block["actions"]
+    ((T, n) categorical, (T, n, K) multi-discrete) over the valid steps of each column; returns the (T, n) int32 legal
+    words (0 on padded steps)."""
+    N = sum(heads)
+    if "action_mask" not in block:
+        raise ValueError("a masked ring takes block['action_mask'] of shape (T, n, N)")
+    m = np.asarray(block["action_mask"])
+    if m.shape != (T, n, N):
+        raise ValueError(f"block action_mask of shape {m.shape}; this ring takes {(T, n, N)}")
+    a = np.asarray(block["actions"]).reshape(T, n, len(heads))
+    lens = np.asarray(block["lens"])
+    for col in range(n):
+        L = int(lens[col])
+        err = _mask_word_errors(m[:L, col], a[:L, col], heads)
+        if err is not None:
+            t, k, what = err
+            raise ValueError(f"masked block: column {col} step {t}{'' if k is None else f' head {k}'} {what}")
+    valid = np.arange(T)[:, None] < lens[None, :]
+    from .synth import legal_words
+
+    return np.where(valid, legal_words(m.astype(bool)), 0).astype(np.int32)
+
+
+def pack_trajectory(views: dict, b: int, traj, T: int, obs=None, heads=(), masked: bool = False) -> float:
     """Write one reference-format trajectory into column `b` of a host batch slab.
 
     Replaces learner.py:104-109,117 (five torch.stack calls + `disc`): float64 -> float32 (or the
@@ -207,17 +280,23 @@ def pack_trajectory(views: dict, b: int, traj, T: int, obs=None, heads=()) -> fl
     past the trajectory's length.  `obs`: obs_array's result if the caller already has it.  A frame slab
     (obs (T+k, B, F), k > 1) receives obs_frames' L+k frames.  A Gaussian slab (actions (T, B, A)) takes
     (A,) actions and (2A,) behaviour outputs per step (gaussian_steps); a multi-discrete slab (`heads`: the head
-    sizes, actions (T, B, K)) (K,) integer actions and (N,) logits (md_steps).  Returns the trajectory's reward sum
-    (learner.py:108)."""
+    sizes, actions (T, B, K)) (K,) integer actions and (N,) logits (md_steps).  A masked slab (`masked`, actions
+    (T, B, 2) or (T, B, K + 1)) takes traj.action_mask as well and stores its legal words last (mask_steps).
+    Returns the trajectory's reward sum (learner.py:108)."""
     L = check_trajectory(traj, T)
     multi = bool(heads)
-    if multi and tuple(views["actions"].shape[2:]) != (len(heads),):
+    if multi and tuple(views["actions"].shape[2:]) != (len(heads) + masked,):
         raise ValueError(f"a slab of actions {tuple(views['actions'].shape)} does not hold the heads {tuple(heads)}")
-    gauss = views["actions"].ndim == 3 and not multi
+    gauss = views["actions"].ndim == 3 and not multi and not masked
     if gauss:
         act, beh = gaussian_steps(traj, L, views["actions"].shape[2])
     elif multi:
         act, beh = md_steps(traj, L, heads)
+    if masked:
+        if not multi:
+            act = _np(torch.stack(traj.a).reshape(L), torch.int32) if L else np.zeros(0, np.int32)
+        words = mask_steps(traj, L, heads or (views["beh_logits"].shape[2],), act)
+        act = np.concatenate([act.reshape(L, -1), words[:, None]], -1)
     obs = obs_array(traj, views["obs"].dtype) if obs is None else obs
     k = views["obs"].shape[0] - T
     if k > 1:
@@ -226,7 +305,7 @@ def pack_trajectory(views: dict, b: int, traj, T: int, obs=None, heads=()) -> fl
     views["obs"][L + k:, b] = 0
     views["beh_logits"][:L, b] = beh if gauss or multi else _np(torch.stack(traj.logits), torch.float32)
     views["beh_logits"][L:, b] = 0
-    views["actions"][:L, b] = act if gauss or multi else _np(torch.stack(traj.a).reshape(L), torch.int32)
+    views["actions"][:L, b] = act if gauss or multi or masked else _np(torch.stack(traj.a).reshape(L), torch.int32)
     views["actions"][L:, b] = 0
     r = torch.stack(traj.r)
     views["rewards"][:L, b] = _np(r, torch.float32)
@@ -258,6 +337,7 @@ def _check_ring(q, options, B_fresh: int) -> None:
         return
     for want, have, what in ((options.action_dist, q.action_dist, "{} actions"),
                              (tuple(options.action_heads), tuple(getattr(q, "action_heads", ())), "action heads {}"),
+                             (options.action_mask, getattr(q, "action_mask", False), "action_mask={}"),
                              (options.obs_dtype, q.obs_dtype, "{} observations"),
                              (options.frames, q.frames, "{} frames per observation"),
                              (B_fresh, q.B, "{} trajectories per update (batch_size - replay_columns)")):
@@ -413,7 +493,7 @@ class Learner:
             c, o = self._cfg(), self.options
             self._stage_ring = RingQueue(self.hp.max_timesteps, self.hp.batch_size, c["O"], c["A"], slabs=2,
                                          obs_dtype=o.obs_dtype, frames=o.frames, action_dist=o.action_dist,
-                                         action_heads=o.action_heads)
+                                         action_heads=o.action_heads, action_mask=o.action_mask)
         self.p.start()
         print(f"[main] Started learner_{self.id} with pid {self.p.pid}")
 
@@ -434,9 +514,10 @@ class Learner:
         O, A, H_pi, H_v = _dims(self.policy, self.value_fn, self.options.action_dist)
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
-        # action_heads is an init-only option (engine.LearnerOptions), so it rides next to the fields
+        # action_heads and action_mask are init-only options (engine.LearnerOptions), so they ride next to the fields
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
-                    action_heads=list(self.options.action_heads), **dataclasses.asdict(self.options))
+                    action_heads=list(self.options.action_heads), action_mask=self.options.action_mask,
+                    **dataclasses.asdict(self.options))
 
     def _make_engine(self, process_group=None, world=1):
         eng = engine_from_cfg(self._cfg(), world, self.device, process_group, self.optim.lr_table)
@@ -494,6 +575,9 @@ class Learner:
         if self.options.action_dist == "multi_discrete":  # test_policy steps one Discrete index per action
             print(f"[learner_{self.id}] evaluation skipped: a multi-discrete policy is evaluated through evaluator= only")
             return None
+        if self.options.action_mask:  # test_policy steps the environment without its legal-action masks
+            print(f"[learner_{self.id}] evaluation skipped: a masked policy is evaluated through evaluator= only")
+            return None
         try:
             import utils as ref_utils  # the reference's utils.py, if on sys.path
 
@@ -541,7 +625,8 @@ class Learner:
                 raise
             if hp.verbose >= 2:
                 print(f"[learner_{self.id}] packing traj_{traj.id} into column {b}")
-            reward += pack_trajectory(views, b, traj, hp.max_timesteps, heads=self.options.action_heads) / self.B_fresh
+            reward += pack_trajectory(views, b, traj, hp.max_timesteps, heads=self.options.action_heads,
+                                      masked=self.options.action_mask) / self.B_fresh
             del traj  # drop the shared-memory handles of its ~5T tensors right away
         return reward
 

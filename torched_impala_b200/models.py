@@ -19,6 +19,14 @@ def _two_layer(obs_dim: int, hidden_dim: int, out_dim: int) -> nn.Sequential:
                          nn.Linear(hidden_dim, out_dim)).to(torch.float64)
 
 
+def _masked(z, action_mask):
+    """z with -inf at the illegal entries of action_mask (true = legal)."""
+    m = torch.as_tensor(action_mask).to(torch.bool)
+    if m.shape != z.shape[-1:]:
+        raise ValueError(f"action_mask of shape {tuple(m.shape)} for {z.shape[-1]} policy outputs")
+    return z.masked_fill(~m, -torch.inf)
+
+
 class MlpPolicy(nn.Module):
     def __init__(self, obs_dim: int, action_dim: int, hidden_dim: int):
         super().__init__()
@@ -27,12 +35,15 @@ class MlpPolicy(nn.Module):
     def forward(self, x):
         return self.model(x)
 
-    def select_action(self, obs, deterministic: bool = False):
-        """Actor-side sampling (reference models.py:27-34): returns (action, logits)."""
+    def select_action(self, obs, deterministic: bool = False, action_mask=None):
+        """Actor-side sampling (reference models.py:27-34): returns (action, logits).  action_mask (A,) bool or 0 / 1,
+        true meaning legal (Learner(action_mask=True)): the sample (or argmax) is taken over the legal actions only;
+        the logits returned are the raw ones - the learner applies the mask it is given with the step."""
         logits = self.forward(obs)
+        z = logits if action_mask is None else _masked(logits.detach(), action_mask)
         if deterministic:
-            return torch.argmax(logits), logits
-        return torch.multinomial(torch.softmax(logits, dim=-1), num_samples=1), logits
+            return torch.argmax(z), logits
+        return torch.multinomial(torch.softmax(z, dim=-1), num_samples=1), logits
 
 
 class GaussianMlpPolicy(nn.Module):
@@ -71,13 +82,15 @@ class MultiDiscreteMlpPolicy(nn.Module):
     def forward(self, x):
         return self.model(x)
 
-    def select_action(self, obs, deterministic: bool = False):
+    def select_action(self, obs, deterministic: bool = False, action_mask=None):
         """Returns (actions (K,) int64, logits (N,)): one index per head, sampled from the softmax of its slice (the
-        per-head argmax when deterministic)."""
+        per-head argmax when deterministic).  action_mask (N,), true meaning legal: each head samples over its legal
+        entries only; the logits returned are the raw ones."""
         logits = self.forward(obs)
         out = []
         with torch.no_grad():
-            for z in torch.split(logits, self.action_heads, dim=-1):
+            zm = logits if action_mask is None else _masked(logits, action_mask)
+            for z in torch.split(zm, self.action_heads, dim=-1):
                 out.append(z.argmax(-1) if deterministic else
                            torch.multinomial(torch.softmax(z, dim=-1).reshape(-1, z.shape[-1]), 1).reshape(z.shape[:-1]))
         return torch.stack(out, -1).to(torch.int64), logits

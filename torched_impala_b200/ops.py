@@ -134,25 +134,27 @@ def obs_unstack(frames, k: int, out_dtype=None):
 
 
 def batch_compose(store, plan, T: int, B: int, Bf: int, F: int, frames: int, A: int, obs_dtype: str = "float32",
-                  out=None, action_dist: str = "categorical", action_heads=()):
+                  out=None, action_dist: str = "categorical", action_heads=(), action_mask: bool = False):
     """The B-column training slab (uint8 bytes, _cabi.batch_layout(T, B, ...)) gathered from `store`, a
     (slabs, slab_bytes) uint8 tensor of Bf-column slabs, by `plan` (B, 2) int32 (slab, column), slab < 0 = an
     empty column (impala_batch_compose; impala_batch_compose_act for action_dist="gaussian" and "multi_discrete",
-    whose action_heads give the K int32 actions per step).  `out`: a uint8 tensor of the slab's size to write into."""
+    whose action_heads give the K int32 actions per step, and for action_mask=True, whose actions end in the legal
+    word).  `out`: a uint8 tensor of the slab's size to write into."""
     _need_cuda(store, plan)
     if store.dtype != torch.uint8 or store.dim() != 2 or plan.dtype != torch.int32 or tuple(plan.shape) != (B, 2):
         raise _cabi.ImpalaCudaError(f"batch_compose takes a (slabs, bytes) uint8 store and a ({B}, 2) int32 plan, got "
                                     f"{tuple(store.shape)} {store.dtype}, {tuple(plan.shape)} {plan.dtype}")
-    _, total = _cabi.batch_layout(T, B, F * frames, A, obs_dtype, frames, action_dist, action_heads)
+    _, total = _cabi.batch_layout(T, B, F * frames, A, obs_dtype, frames, action_dist, action_heads, action_mask)
     if out is None:
         out = torch.empty(total, dtype=torch.uint8, device=store.device)
     _need_cuda(out)
     if out.dtype != torch.uint8 or out.numel() != total:
         raise _cabi.ImpalaCudaError(f"batch_compose writes a slab of {total} bytes, got {out.numel()} {out.dtype}")
-    if action_dist != "categorical":
+    if action_dist != "categorical" or action_mask:
         _cabi.check(_cabi.lib().impala_batch_compose_act(_p(out), _p(store), store.shape[1], _p(plan), T, B, Bf, F,
                                                          frames, A, _cabi.obs_dtype_code(obs_dtype),
-                                                         _cabi.act_kind_code(action_dist, action_heads), _st()),
+                                                         _cabi.act_kind_code(action_dist, action_heads, action_mask),
+                                                         _st()),
                     "impala_batch_compose_act")
         return out
     _cabi.check(_cabi.lib().impala_batch_compose(_p(out), _p(store), store.shape[1], _p(plan), T, B, Bf, F, frames, A,
@@ -441,6 +443,50 @@ def vtrace_loss_md(cur_logits, beh_logits, actions, rewards, done, lens, v, hp, 
         float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c), float(hp.policy_loss_c), float(hp.entropy_c),
         float(inv_batch), _cabi.MODES[mode], None if diag is None else _p(diag),
         None if popart is None else _p(popart), code, h, K, _st()), "impala_vtrace_loss_md")
+    out = dict(vs=vs, pg_adv=pg, dlogits=dlogits, dv=dv, scalars=scalars)
+    if with_diag:
+        out["diag"] = diag
+    return out
+
+
+def vtrace_loss_mask(cur_logits, beh_logits, actions, rewards, done, lens, v, hp, inv_batch, heads=(),
+                     mode="reference", diagnostics=False, popart=None, reward_clip=None):
+    """The V-trace loss kernel with invalid-action masks (impala_vtrace_loss_mask): cur_logits / beh_logits (T, B, N)
+    float32, N <= 32; actions (T, B, 2) int32 [a, legal] for a categorical policy (heads=()) or (T, B, K + 1)
+    [a_0 .. a_{K-1}, legal] for the multi-discrete heads `heads` (sum = N).  Bit j of the legal word: output j is
+    legal.  Returns vs, pg_adv, dlogits (T, B, N), dv, scalars and, with diagnostics=True or popart, diag."""
+    code = _cabi.reward_clip_code(reward_clip)
+    heads = _cabi.check_heads(heads) if len(heads) else ()
+    _need_cuda(cur_logits, beh_logits, actions, rewards, done, lens, v)
+    if popart is not None:
+        _need_cuda(popart)
+        if popart.dtype != torch.float64 or popart.numel() < 3:
+            raise _cabi.ImpalaCudaError("popart must be a float64 tensor of the statistics (popart_stats)")
+    T, B, N = cur_logits.shape
+    K = len(heads)
+    if (heads and N != sum(heads)) or actions.dtype != torch.int32 or tuple(actions.shape) != (T, B, K + 1 if K else 2):
+        raise _cabi.ImpalaCudaError(f"vtrace_loss_mask takes (T, B, N) logits and (T, B, {K + 1 if K else 2}) int32 "
+                                    f"actions ending in the legal word for heads {heads}, got {tuple(cur_logits.shape)}"
+                                    f" and {tuple(actions.shape)} {actions.dtype}")
+    with_diag = bool(diagnostics) or popart is not None
+    dev = v.device
+    vs = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    pg = torch.empty(T, B, dtype=torch.float32, device=dev)
+    dlogits = torch.empty(T, B, N, dtype=torch.float32, device=dev)
+    dv = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    scalars = torch.empty(4, dtype=torch.float64, device=dev)
+    diag = torch.empty(8, dtype=torch.float64, device=dev) if with_diag else None
+    lib = _cabi.lib()
+    ws_fn = lib.impala_vtrace_loss_diag_workspace if with_diag else lib.impala_vtrace_loss_workspace
+    ws_bytes = int(ws_fn(T, B, N))
+    ws = torch.zeros(ws_bytes, dtype=torch.uint8, device=dev)
+    h = (C.c_int32 * K)(*heads) if K else None
+    _cabi.check(lib.impala_vtrace_loss_mask(
+        _p(cur_logits), _p(beh_logits), _p(actions), _p(rewards), _p(done), _p(lens), _p(v), _p(vs),
+        _p(pg), _p(dlogits), _p(dv), _p(scalars), _p(ws), ws_bytes, T, B, N, float(hp.gamma),
+        float(hp.rho_bar), float(hp.c_bar), float(hp.v_loss_c), float(hp.policy_loss_c), float(hp.entropy_c),
+        float(inv_batch), _cabi.MODES[mode], None if diag is None else _p(diag),
+        None if popart is None else _p(popart), code, h, K, _st()), "impala_vtrace_loss_mask")
     out = dict(vs=vs, pg_adv=pg, dlogits=dlogits, dv=dv, scalars=scalars)
     if with_diag:
         out["diag"] = diag

@@ -53,11 +53,12 @@ _ACT_DISTS = ("categorical", "gaussian", "multi_discrete")
 
 
 def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: int = 1,
-            action_dist: str = "categorical", action_heads=()):
+            action_dist: str = "categorical", action_heads=(), action_mask: bool = False):
     """Same 256-byte aligned layout as include/impala_b200.h::impala_batch_layout_act with F = O / frames
     (impala_batch_layout_obs at frames = 1, categorical; pure python so actor processes do not need the CUDA
     library).  "gaussian": beh_logits (T, B, 2A) f32 and actions (T, B, A) f32 for A action dimensions.
-    "multi_discrete": beh_logits (T, B, A) f32 for A = sum(action_heads) outputs and actions (T, B, K) i32."""
+    "multi_discrete": beh_logits (T, B, A) f32 for A = sum(action_heads) outputs and actions (T, B, K) i32.
+    action_mask=True (categorical, multi_discrete): one more int32 per step in the actions, the legal word."""
     if action_dist not in _ACT_DISTS:
         raise ValueError(f"action_dist must be one of {list(_ACT_DISTS)}, got {action_dist!r}")
     g = action_dist == "gaussian"
@@ -67,7 +68,7 @@ def _layout(T: int, B: int, O: int, A: int, obs_dtype: str = "float32", frames: 
     if frames < 1 or O % frames:
         raise ValueError(f"{O} observation features do not split into {frames} frames")
     sizes = ((T + frames) * B * (O // frames) * _OBS_BYTES[obs_dtype], T * B * (2 * A if g else A) * 4,
-             T * B * (A if g else K) * 4, T * B * 4, T * B, B * 4)
+             T * B * (A if g else K + bool(action_mask)) * 4, T * B * 4, T * B, B * 4)
     offs, off = [], 0
     for s in sizes:
         offs.append(off)
@@ -79,7 +80,7 @@ class RingQueue:
     """Drop-in for the `mp.Queue` between actors and learner, backed by shared-memory batch slabs."""
 
     def __init__(self, T: int, B: int, O: int, A: int, slabs: int = 3, obs_dtype: str = "float32", frames: int = 1,
-                 action_dist: str = "categorical", action_heads=()):
+                 action_dist: str = "categorical", action_heads=(), action_mask: bool = False):
         if slabs < 2:
             raise ValueError("need at least two slabs (one filling while one is consumed)")
         if action_dist == "gaussian" and not 1 <= A <= 16:
@@ -94,9 +95,17 @@ class RingQueue:
         elif tuple(action_heads) != ():
             raise ValueError(f"action_heads is for action_dist='multi_discrete', not {action_dist!r}")
         self.action_heads = tuple(action_heads)
+        # action_mask: the actors' legal-action masks (traj.action_mask, block["action_mask"]) travel as one int32
+        # legal word per step after the action indices
+        if not isinstance(action_mask, bool):
+            raise ValueError(f"action_mask must be a bool, got {action_mask!r}")
+        if action_mask and (action_dist == "gaussian" or A > 32):
+            raise ValueError("action_mask is for categorical and multi-discrete policies of at most 32 outputs")
+        self.action_mask = action_mask
         self.T, self.B, self.O, self.A, self.K = T, B, O, A, slabs
         # "uint8": byte observations (Atari RAM, MinAtar planes), a quarter of the float32 slab bytes
-        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype, frames, action_dist, self.action_heads)
+        self.offsets, self.slab_bytes = _layout(T, B, O, A, obs_dtype, frames, action_dist, self.action_heads,
+                                                action_mask)
         # "gaussian": A action dimensions; the actors' [mean | log std] (2A) and float32 samples (A) per step
         self.action_dist = action_dist
         self.gaussian = action_dist == "gaussian"
@@ -155,9 +164,10 @@ class RingQueue:
         """Numpy views of slab k (the six batch tensors, learner layout)."""
         if self._views is None:
             N = 2 * self.A if self.gaussian else self.A
+            Ka = (len(self.action_heads) or 1) + 1 if self.action_mask else len(self.action_heads)  # indices, legal word
             shapes = {"obs": (self.T + self.frames, self.B, self.O // self.frames), "beh_logits": (self.T, self.B, N),
                       "actions": ((self.T, self.B, self.A) if self.gaussian else
-                                  (self.T, self.B, len(self.action_heads)) if self.action_heads else (self.T, self.B)),
+                                  (self.T, self.B, Ka) if Ka else (self.T, self.B)),
                       "rewards": (self.T, self.B), "done": (self.T, self.B), "lens": (self.B,)}
             self._views = []
             for kk in range(self.K):
@@ -184,6 +194,13 @@ class RingQueue:
             from .learner import md_steps
 
             md_steps(traj, len(traj.r), self.action_heads)
+        if self.action_mask:  # the same: missing, malformed or empty masks, illegal taken actions
+            from .learner import mask_steps, md_steps
+
+            L = len(traj.r)
+            a = (md_steps(traj, L, self.action_heads)[0] if self.action_heads else
+                 np.asarray([int(np.asarray(x).reshape(-1)[0]) for x in traj.a], np.int64).reshape(L, 1))
+            mask_steps(traj, L, self.action_heads or (self.A,), a)
         c = self._control()
         end = None if (timeout is None or not block) else time.monotonic() + timeout
         t_wait = time.monotonic()
@@ -198,7 +215,8 @@ class RingQueue:
                 raise queue.Full  # like mp.Queue.put on a full queue; actor.py:120 retries
             _pause(t_wait)
         try:
-            rsum = pack_trajectory(self.views(k), b, traj, self.T, obs=obs, heads=self.action_heads)
+            rsum = pack_trajectory(self.views(k), b, traj, self.T, obs=obs, heads=self.action_heads,
+                                   masked=self.action_mask)
         except BaseException:
             # never leave the column unfilled (the learner would stall on it until its timeout):
             # publish it as an empty trajectory - neutral padding for the update - and re-raise
@@ -241,6 +259,11 @@ class RingQueue:
             from .learner import check_md_block
 
             check_md_block(block, self.T, n, self.action_heads)
+        words = None
+        if self.action_mask:
+            from .learner import check_mask_block
+
+            words = check_mask_block(block, self.T, n, self.action_heads or (self.A,))
         c = self._control()
         end = None if timeout is None else time.monotonic() + timeout
         t_wait = time.monotonic()
@@ -257,8 +280,13 @@ class RingQueue:
                 raise queue.Full
             _pause(t_wait)
         v = self.views(k)
-        for name in ("obs", "beh_logits", "actions", "rewards", "done"):
+        for name in ("obs", "beh_logits", "rewards", "done"):
             v[name][:, b:b + n] = block[name]
+        if words is None:
+            v["actions"][:, b:b + n] = block["actions"]
+        else:  # the indices, then the legal word
+            v["actions"][:, b:b + n, :-1] = np.asarray(block["actions"]).reshape(self.T, n, -1)
+            v["actions"][:, b:b + n, -1] = words
         v["lens"][b:b + n] = block["lens"]
         rs = block["rewards"].sum(0, dtype=np.float64) if block_rsum is None else block_rsum
         c["rsum"][k, b:b + n] = rs

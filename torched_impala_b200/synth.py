@@ -191,12 +191,86 @@ def make_md_batch(seed: int, T: int, B: int, O: int, heads, ragged: bool = False
     return dict(b, beh_logits=beh, actions=act)
 
 
+def draw_legal(rng, T: int, B: int, heads, density: float = 0.5, single: float = 0.1):
+    """(T, B, N) bool legal-action masks over the heads (categorical: one head of N): each entry legal with probability
+    `density`, at least one legal entry per head, and a fraction `single` of the steps with one legal entry per head."""
+    heads = tuple(int(n) for n in heads)
+    legal = rng.random((T, B, sum(heads))) < density
+    one = rng.random((T, B)) < single
+    s = 0
+    for n in heads:
+        h = legal[..., s:s + n]
+        pick = rng.integers(0, n, (T, B))
+        sole = np.arange(n) == pick[..., None]
+        h[...] = np.where(one[..., None], sole, h | (~h.any(-1, keepdims=True) & sole))
+        s += n
+    return legal
+
+
+def legal_words(legal) -> np.ndarray:
+    """(..., N) bool legal masks -> (...) int32 legal words, bit j = entry j (the slab's last action column)."""
+    legal = np.asarray(legal, bool)
+    w = (legal.astype(np.uint64) << np.arange(legal.shape[-1], dtype=np.uint64)).sum(-1)
+    return w.astype(np.uint32).view(np.int32)
+
+
+def make_masked_batch(seed: int, T: int, B: int, O: int, A: int, heads=(), density: float = 0.5, ragged: bool = False,
+                      params: dict | None = None, obs_kind: str = "normal", frames: int = 1) -> dict:
+    """A batch of a masked policy (action_mask=True): categorical over A actions (heads=()) or multi-discrete with
+    `heads` (sum = A).  obs, rewards, done and lens as make_batch; legal masks per step (draw_legal: `density`, at
+    least one legal entry per head, some single-legal steps); behaviour logits as make_batch / make_md_batch, the
+    actions drawn from the behaviour softmax renormalised over the legal entries, and garbage (+-1e30, -inf, NaN) in
+    the illegal behaviour logits, as an actor may record.  actions (T, B, 2) [a, legal] or (T, B, K + 1)
+    [a_0 .. a_{K-1}, legal] int32 (a multi-discrete batch of one head has the categorical layout); `legal` (T, B, A)
+    bool rides along.  Padded steps are zero (legal word 0)."""
+    md = bool(len(heads))
+    heads = tuple(int(n) for n in heads) or (A,)
+    if sum(heads) != A:
+        raise ValueError(f"the heads {heads} do not have A = {A} outputs")
+    b = make_batch(seed, T, B, O, 2, ragged=ragged, obs_kind=obs_kind, frames=frames)
+    rng = np.random.default_rng(seed + 15485863)
+    if params is None:
+        beh = rng.standard_normal((T, B, A))
+    else:
+        x = (stack_frames(b, frames) if frames > 1 else b)["obs"][:-1].astype(np.float64)
+        p = [np.asarray(params["policy"][k], np.float64) for k in ("model.0.weight", "model.0.bias",
+                                                                      "model.3.weight", "model.3.bias")]
+        beh = np.maximum(x @ p[0].T + p[1], 0.0) @ p[2].T + p[3]
+        beh = beh + rng.uniform(0.1, 0.3, beh.shape) * rng.choice([-1.0, 1.0], beh.shape)
+    legal = draw_legal(rng, T, B, heads, density)
+    K = len(heads)
+    act = np.zeros((T, B, K), np.int32)
+    s = 0
+    for k, n in enumerate(heads):
+        z = np.where(legal[..., s:s + n], beh[..., s:s + n], -np.inf)
+        q = np.exp(z - z.max(-1, keepdims=True))
+        q /= q.sum(-1, keepdims=True)
+        a = np.minimum((np.cumsum(q, -1) < 1.0 - rng.random((T, B, 1))).sum(-1), n - 1)
+        while True:  # the cumulative sum may end a rounding short of 1: step back onto a legal entry
+            off = ~np.take_along_axis(legal[..., s:s + n], a[..., None], -1)[..., 0]
+            if not off.any():
+                break
+            a = np.where(off, a - 1, a)
+        act[..., k] = a
+        s += n
+    beh = beh.astype(np.float32)
+    garbage = np.array([1e30, -1e30, -np.inf, np.nan], np.float32)
+    beh = np.where(legal, beh, garbage[rng.integers(0, 4, beh.shape)]).astype(np.float32)
+    pad = np.arange(T)[:, None] >= b["lens"][None, :]
+    beh[pad], act[pad], legal[pad] = 0.0, 0, False
+    words = legal_words(legal)
+    actions = np.concatenate([act, words[..., None]], -1).astype(np.int32)
+    return dict(b, beh_logits=beh, actions=actions, legal=legal)
+
+
 def to_trajectories(batch: dict, torch_dtype=None) -> list:
     """Expand a dense batch into the reference wire format (one Trajectory per b).
 
     Shapes/dtypes follow what actor.py:72-92 appends: obs (O,) f64, a (1,) i64,
     r () f64, d () bool, logits (A,) f64.  A Gaussian batch (actions (T, B, A)) gives a (A,) f64 and
-    logits (2A,) f64; a multi-discrete batch (int32 actions (T, B, K)) a (K,) i64 and logits (N,) f64.
+    logits (2A,) f64; a multi-discrete batch (int32 actions (T, B, K)) a (K,) i64 and logits (N,) f64.  A masked
+    batch (make_masked_batch: `legal` present, the legal word last in the actions) gives the indices without the word
+    and traj.action_mask, (N,) bool per step.
     """
     import torch
 
@@ -208,7 +282,9 @@ def to_trajectories(batch: dict, torch_dtype=None) -> list:
     # (T, B, A) float actions: Gaussian samples; (T, B, K) integer actions: multi-discrete indices
     gauss = batch["actions"].ndim == 3 and np.issubdtype(batch["actions"].dtype, np.floating)
     multi = batch["actions"].ndim == 3 and not gauss
-    act = torch.from_numpy(batch["actions"]).to(dt if gauss else torch.int64)
+    masked = "legal" in batch
+    act = torch.from_numpy(batch["actions"][..., :-1] if masked else batch["actions"]).to(dt if gauss else torch.int64)
+    legal = torch.from_numpy(batch["legal"]) if masked else None
     rew = torch.from_numpy(batch["rewards"]).to(dt)
     don = torch.from_numpy(batch["done"]).to(torch.bool)
     out = []
@@ -218,5 +294,7 @@ def to_trajectories(batch: dict, torch_dtype=None) -> list:
         for t in range(L):
             tr.add(obs[t + 1, b].clone(), act[t, b].clone() if gauss or multi else act[t, b].reshape(1).clone(), rew[t, b].clone(),
                    don[t, b].clone(), beh[t, b].clone())
+        if masked:
+            tr.action_mask = [legal[t, b].clone() for t in range(L)]
         out.append(tr)
     return out

@@ -45,11 +45,14 @@ class Trajectory:
     0-d float64, `d` 0-d bool, `logits` (A,) float64 behaviour logits.
     """
 
-    __slots__ = ("id", "obs", "a", "r", "d", "logits")
+    __slots__ = ("id", "obs", "a", "r", "d", "logits", "action_mask")
 
     def __init__(self, id, observations=None, actions=None, rewards=None, dones=None,
                  logits=None):
         self.id = id
+        # masked policies (Learner(action_mask=True)): the legal-action mask (A,) / (N,) of each step, true = legal,
+        # appended by the actor next to the step; None for the others
+        self.action_mask = None
         self.obs = [] if observations is None else observations
         self.a = [] if actions is None else actions
         self.r = [] if rewards is None else rewards
