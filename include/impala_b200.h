@@ -466,6 +466,15 @@ int impala_mlp_backward_pair_push(const float* x, const float* params_pi, const 
                                   int H_vf, int A, const double* extra, int n_extra,
                                   void* const* peer_gather, const long long* seq, int64_t slot_stride,
                                   int64_t buf_stride, int rank, int world, void* stream);
+/* impala_mlp_backward_pair_push for an observation-normalizing engine: `extra` holds the n_extra (<= 32) logged
+ * extras followed by impala_obs_normalize's 2 O + 1 sums, and all n_extra + 2 O + 1 of them are pushed (the slot
+ * must hold them).  O > IMPALA_OBS_NORM_MAX_FEATURES returns IMPALA_ERR_BAD_ARG. */
+int impala_mlp_backward_pair_push_obs_norm(const float* x, const float* params_pi, const float* params_vf,
+                                           const float* dlogits, const float* dv, void* workspace_pi,
+                                           int64_t workspace_pi_bytes, void* workspace_vf, int64_t workspace_vf_bytes,
+                                           int M_pi, int M_vf, int O, int H_pi, int H_vf, int A, const double* extra,
+                                           int n_extra, void* const* peer_gather, const long long* seq,
+                                           int64_t slot_stride, int64_t buf_stride, int rank, int world, void* stream);
 int impala_gather_clip_adam(float* params, double* reduced, const void* gather, long long* seq,
                             int64_t slot_stride, int64_t buf_stride, int world, int n_extra, float* m,
                             float* v, int64_t* state, int64_t n_policy, int64_t n_total,
@@ -508,6 +517,49 @@ int impala_gather_clip_optim_popart(float* params, double* reduced, const void* 
                                     const float* lr_table, int64_t n_lr, int rule, float h0, float h1, float eps,
                                     double* norms_out, int* err, double timeout_s, double* popart, int64_t sums_at,
                                     int64_t w2_off, int64_t w2_len, int64_t b2_off, float beta, void* stream);
+
+/* ---- Observation normalization (obs_norm): running per-feature statistics of the raw observations.
+ * Statistics, float64 [count | mean (O) | var (O)]: a fresh run is {0, 0.., 1..}.  The kernels read them as
+ * norm, float32 [mu_f (O) | r_f (O)] with mu_f = (float)mean, r_f = (float)(1 / sqrt(var + eps)).
+ * Sums of a batch, float64 [sum x (O) | sum x^2 (O) | rows]: over the valid rows t < lens[b] (t < T) only. */
+#define IMPALA_OBS_NORM_MAX_FEATURES 1024
+
+/* Bytes of the workspace of impala_obs_normalize for T steps, B columns and O features (O up to
+ * IMPALA_OBS_NORM_MAX_FEATURES, else IMPALA_ERR_BAD_ARG).  Its first bytes are counters the caller zeroes ONCE;
+ * every launch leaves them zeroed. */
+int64_t impala_obs_normalize_workspace(int T, int B, int O);
+
+/* The step's first launch with obs_norm on, in place of impala_obs_unstack / impala_obs_u8_to_f32: reads the
+ * slab's observations - dense (T+1, B, F) when k = 1, frames (T+k, B, F) otherwise (impala_batch_layout_frames),
+ * float32 or uint8 (in_dtype) - and writes
+ *   out (T+1, B, O = k F) float32:  out[r, o] = (x[r, o] - mu_f[o]) * r_f[o]  (float32, every row),
+ *   sums (2 O + 1) float64:          the batch's sums over its valid rows.
+ * The sums are deterministic: per feature, the rows are split into at most 1024 chunks of a size fixed by
+ * (T+1) B alone; eight row lanes each add every eighth row of a chunk in row order, the chunk's partial adds the
+ * lanes in order, eight lanes add every eighth chunk's partial in order and the total adds those in order.  No
+ * float atomics: the same batch gives the same bits.  O > IMPALA_OBS_NORM_MAX_FEATURES returns
+ * IMPALA_ERR_UNSUPPORTED_SHAPE, a short workspace IMPALA_ERR_WORKSPACE_TOO_SMALL. */
+int impala_obs_normalize(const void* obs, int in_dtype, int T, int B, int F, int k, const int32_t* lens,
+                         const float* norm, float* out, double* sums, void* workspace, int64_t workspace_bytes,
+                         void* stream);
+
+/* One launch after the optimizer: merges the batch (sums, summed over the ranks) into the statistics with
+ * Chan's parallel merge in float64,
+ *   n = n_a + n_b,  d = mean_b - mean_a,  mean = mean_a + d n_b / n,
+ *   var = (var_a n_a + max(S2 - S1 mean_b, 0) + d^2 n_a n_b / n) / n     (n_b = 0 leaves them),
+ * rewrites norm from them and writes `folded`: params with the W1 block(s) and b1 of each network folded into
+ * raw-observation coordinates, W1' = W1 diag(r_f) (float32), b1' = b1 - W1' mu_f (float64 sum), every other entry
+ * copied.  Network 0 is (w1_off0, b1_off0, H0); H1 = 0 means one network (shared torso).  ctl: two uint32 the
+ * caller zeroes once (every launch leaves them zeroed).
+ * gather != NULL (data-parallel, peer route): the sums are entries [sums_at, sums_at + 2 O + 1) of every rank's
+ * slot of this rank's gather buffer for the step *seq (the gather optimizer has advanced it), added in rank order;
+ * *err != 0 (the optimizer timed out) leaves everything untouched.  A timeout here sets *err and leaves the
+ * statistics untouched; `folded` is then incomplete (the host raises on *err, as for the optimizer). */
+int impala_obs_norm_update(double* stats, float* norm, const double* sums, double eps, const float* params,
+                           float* folded, int64_t n_total, int O, int64_t w1_off0, int64_t b1_off0, int H0,
+                           int64_t w1_off1, int64_t b1_off1, int H1, unsigned* ctl, const void* gather,
+                           const long long* seq, int64_t slot_stride, int64_t buf_stride, int world, int64_t sums_at,
+                           int* err, double timeout_s, void* stream);
 
 /* Pieces of the reference's module-level loss helpers (learner.py:298-321) for callers that use
  * them individually instead of impala_vtrace_loss.  logits (M,A) f32 row-major, actions (M) i32.

@@ -36,7 +36,11 @@ each, alternating, L2 flushed before each).
 (action_mask=True: legal words in the actions, about half the entries legal) on batches of the same shapes the same
 way, and times the unmasked V-trace + loss kernel (impala_vtrace_loss, or impala_vtrace_loss_md for md_mask_c4)
 against impala_vtrace_loss_mask alone on each engine's buffers (median of 200 launches each, alternating, L2 flushed
-before each)."""
+before each).
+--compare-obs-norm alternates an obs_norm=False and an obs_norm=True engine (observation normalization) on the same
+batch the same way (--obs-dtype for the slab; the halfcheetah config is a Gaussian policy), reports both steps'
+launches, and times impala_obs_normalize alone on the engine's buffers (median of 200 launches, L2 flushed before
+each) against its HBM floor (slab observations read + float32 rows written at 3.35 TB/s)."""
 import argparse
 import os
 import statistics
@@ -75,7 +79,9 @@ CFG = {"c4": dict(T=20, B=4096, O=24, A=4, H=256),
        # 16-output tensor-core epilogue.  ram_a9h512 has no FP32 arm (that forward refuses H > 256 at O > 64)
        "ram_a6": dict(T=20, B=4096, O=128, A=6, H=256),
        "c4a6": dict(T=20, B=4096, O=24, A=6, H=256),
-       "ram_a9h512": dict(T=20, B=4096, O=128, A=9, H=512)}
+       "ram_a9h512": dict(T=20, B=4096, O=128, A=9, H=512),
+       # MuJoCo HalfCheetah-shaped continuous control (--compare-obs-norm): 17 features, 6 action dimensions
+       "halfcheetah": dict(T=20, B=4096, O=17, A=6, H=256, gaussian=True)}
 ap = argparse.ArgumentParser()
 ap.add_argument("--config", default="c5")
 ap.add_argument("--steps", type=int, default=30)
@@ -93,6 +99,8 @@ ap.add_argument("--compare-heads", action="store_true",
                 help="alternate a categorical engine at A = N and a multi-discrete engine (configs md_c4, md_ram)")
 ap.add_argument("--compare-mask", action="store_true",
                 help="alternate an unmasked and a masked engine (configs mask_c4, mask_ram, md_mask_c4)")
+ap.add_argument("--compare-obs-norm", action="store_true",
+                help="alternate engines without / with observation normalization (--obs-dtype for the slab)")
 ap.add_argument("--replay-slabs", type=int, default=2, help="past fresh batches in the pool of --compare-replay")
 ap.add_argument("--replay-columns", type=int, default=None, help="replayed columns of --compare-replay (default B/2)")
 a = ap.parse_args()
@@ -151,6 +159,13 @@ if a.compare_mask:
     heads_arm = {name: md_kw for name in arms} if md_kw else {}
     mask_arm = {mask_name: dict(action_mask=True)}
     obs_dt = {name: "uint8" if a.config == "mask_ram" else "float32" for name in arms}
+obs_norm_arm = {}
+if a.compare_obs_norm:
+    arms = {"obs_norm off": arms["default"], "obs_norm on": arms["default"]}
+    obs_norm_arm = {"obs_norm on": dict(obs_norm=True)}
+    obs_dt = {name: a.obs_dtype for name in arms}
+    if w.get("gaussian"):
+        heads_arm = {name: dict(action_dist="gaussian") for name in arms}
 replay_arm = {}
 if a.compare_replay:
     Br = w["B"] // 2 if a.replay_columns is None else a.replay_columns
@@ -167,8 +182,8 @@ for name, tc in arms.items():
     eng = LearnerEngine(w["T"], w["B"], w["O"], w["A"], w["H"], w["H"], hp, obs_dtype=dt, frames=k,
                         diagnostics=diag_arm.get(name, False), **replay_arm.get(name, {}), **popart_arm.get(name, {}),
                         **rclip_arm.get(name, {}), **shared_arm.get(name, {}), **heads_arm.get(name, {}),
-                        **mask_arm.get(name, {}))
-    eng.load_state(synth.init_params(0, w["O"], w["A"], w["H"]))
+                        **mask_arm.get(name, {}), **obs_norm_arm.get(name, {}))
+    eng.load_state(synth.init_params(0, w["O"], 2 * w["A"] if w.get("gaussian") else w["A"], w["H"]))
     byte_obs = (a.compare_obs or ((a.compare_frames or a.compare_replay) and dt == "uint8")
                 or ((a.compare_diag or a.compare_popart or a.compare_reward_clip or a.compare_shared or a.compare_mask)
                     and dt == "uint8"))
@@ -184,6 +199,10 @@ for name, tc in arms.items():
         batch = synth.make_masked_batch(1, w["T"], w["B"], w["O"], w["A"], w["mask"], density=0.5,
                                         obs_kind="bytes" if byte_obs else "normal")
         batch.pop("legal")
+    elif w.get("gaussian"):
+        batch = synth.make_gaussian_batch(1, w["T"], w["B"], w["O"], w["A"])
+    elif a.compare_obs_norm:
+        batch = synth.make_batch(1, w["T"], w["B"], w["O"], w["A"], obs_kind="bytes" if dt == "uint8" else "normal")
     elif name in heads_arm:
         batch = (synth.make_md_batch(1, w["T"], w["B"], w["O"], w["heads"]) if "heads" in w else
                  synth.make_md_batch(1, w["T"], w["B"], w["O"], w["mask"]))
@@ -483,6 +502,34 @@ if a.compare_mask:  # the V-trace + loss kernel alone, unmasked against masked, 
     k0, k1 = statistics.median(tk[plain_name]), statistics.median(tk["impala_vtrace_loss_mask"])
     print(f"V-trace + loss kernel {a.config}: {plain_name} {k0:.1f} us, impala_vtrace_loss_mask {k1:.1f} us "
           f"({k1 - k0:+.1f} us, {100 * (k1 / k0 - 1):+.1f} %)")
+if a.compare_obs_norm:  # the normalize launch alone, on the engine's slab and buffers
+    import ctypes
+
+    from torched_impala_b200 import _cabi
+
+    eng = engines["obs_norm on"]
+    d = eng.d_views[0]
+    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    sums = ctypes.c_void_p(eng.comm.data_ptr() + 8 * eng.obs_sums_at)
+    with torch.cuda.stream(eng.stream):
+        st = ctypes.c_void_p(eng.stream.cuda_stream)
+        tu = []
+        for i in range(220):
+            flush.zero_()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(eng.stream)
+            _cabi.check(eng.lib.impala_obs_normalize(P(d["obs"]), eng.obs_code, w["T"], w["B"], eng.F, eng.frames,
+                                                     P(d["lens"]), P(eng.obs_norm_dev), P(eng.obs_normed), sums,
+                                                     P(eng.obs_norm_ws), eng.obs_norm_ws.numel(), st),
+                        "impala_obs_normalize")
+            e1.record(eng.stream)
+            e1.synchronize()
+            if i >= 20:
+                tu.append(e0.elapsed_time(e1) * 1e3)
+    us = statistics.median(tu)
+    nbytes = d["obs"].numel() * d["obs"].element_size() + eng.obs_normed.numel() * 4
+    print(f"impala_obs_normalize {a.config} {a.obs_dtype}: {us:.1f} us, {nbytes / 1e6:.1f} MB moved, HBM floor "
+          f"{nbytes / 3.35e12 * 1e6:.1f} us at 3.35 TB/s ({nbytes / 3.35e12 * 1e6 / us:.0%} of it)")
 q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
                     "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 print(f"GPU (nvidia-smi): {q}")
@@ -526,3 +573,9 @@ if a.compare_mask:
     m0, m1 = statistics.median(ts["unmasked"]), statistics.median(ts[mask_name])
     print(f"masked {a.config}: {m1:.1f} us/step against {m0:.1f} ({m1 - m0:+.1f} us, {100 * (m1 / m0 - 1):+.1f} %), "
           f"launches {engines[mask_name].launches_per_step} against {engines['unmasked'].launches_per_step}")
+if a.compare_obs_norm:
+    m0, m1 = statistics.median(ts["obs_norm off"]), statistics.median(ts["obs_norm on"])
+    st = engines["obs_norm on"].obs_norm_stats()
+    print(f"obs_norm {a.config} {a.obs_dtype}: {m1:.1f} us/step against {m0:.1f} ({m1 - m0:+.1f} us, "
+          f"{100 * (m1 / m0 - 1):+.1f} %), launches {engines['obs_norm on'].launches_per_step} against "
+          f"{engines['obs_norm off'].launches_per_step}; rows counted {st['count']:.0f}")

@@ -20,6 +20,7 @@ MODES = {"reference": MODE_REFERENCE, "paper": MODE_PAPER}
 OBS_F32 = 0
 OBS_U8 = 1
 OBS_DTYPES = {"float32": OBS_F32, "uint8": OBS_U8}  # batch-slab observation types (impala_batch_layout_obs)
+OBS_NORM_MAX_FEATURES = 1024  # observation features of impala_obs_normalize (IMPALA_OBS_NORM_MAX_FEATURES)
 
 OPT_ADAM = 0
 OPT_RMSPROP = 1
@@ -112,6 +113,10 @@ SIGNATURES = {
     "impala_obs_unstack": (_i, [_p, _i, _p, _i, _i, _i, _i, _i, _p]),
     "impala_batch_compose": (_i, [_p, _p, _i64, _p] + [_i] * 7 + [_p]),
     "impala_obs_u8_to_f32": (_i, [_p, _p, _i64, _p]),
+    "impala_obs_normalize_workspace": (_i64, [_i, _i, _i]),
+    "impala_obs_normalize": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _i64, _p]),
+    "impala_obs_norm_update": (_i, [_p, _p, _p, C.c_double, _p, _p, _i64, _i, _i64, _i64, _i, _i64, _i64, _i, _p, _p,
+                                    _p, _i64, _i64, _i, _i64, _p, C.c_double, _p]),
     "impala_mlp_forward": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
     "impala_mlp_forward_u8": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
     "impala_mlp_backward_u8": (_i, [_p, _p, _p, _p, _p, _i64, _i, _i, _i, _i, _p]),
@@ -129,6 +134,8 @@ SIGNATURES = {
     "impala_peer_push": (_i, [_p, _i64, _p, _p, _i64, _i64, _i, _i, _p]),
     "impala_mlp_backward_pair_push_supported": (_i, [_i] * 6),
     "impala_mlp_backward_pair_push": (_i, [_p] * 6 + [_i64, _p, _i64] + [_i] * 6 + [_p, _i, _p, _p, _i64, _i64, _i, _i, _p]),
+    "impala_mlp_backward_pair_push_obs_norm": (_i, [_p] * 6 + [_i64, _p, _i64] + [_i] * 6
+                                               + [_p, _i, _p, _p, _i64, _i64, _i, _i, _p]),
     "impala_gather_clip_adam": (_i, [_p] * 4 + [_i64, _i64, _i, _i, _p, _p, _p, _i64, _i64] + [_f] * 5
                                 + [_p, _p, C.c_double, _p]),
     "impala_vtrace": (_i, [_p] * 9 + [_i, _i, _i, _f, _f, _f, _i, _p]),

@@ -44,7 +44,8 @@ def _units():
              ("optim", "optim.cu", []), ("abi", "abi.cu", []),
              ("mlp_fwd_tc", "mlp_fwd_tc.cu", []), ("mlp_bwd_tc", "mlp_bwd_tc.cu", []),
              ("loss_terms", "loss_terms.cu", []), ("mlp_obs_tc", "mlp_obs_tc.cu", []),
-             ("obs_frames", "obs_frames.cu", []), ("batch_compose", "batch_compose.cu", [])]
+             ("obs_frames", "obs_frames.cu", []), ("batch_compose", "batch_compose.cu", []),
+             ("obs_norm", "obs_norm.cu", [])]
     for op in MLP_WIDTHS:
         for bwd in (0, 1):
             units.append((f"mlp_inst_op{op}_{'bwd' if bwd else 'fwd'}", "mlp_inst.cu",

@@ -397,18 +397,17 @@ extern "C" int impala_mlp_backward_pair_push_supported(int M_pi, int M_vf, int O
     return push_plans(M_pi, M_vf, O, H_pi, H_vf, A, true, true, true, &pi, &vf);
 }
 
-extern "C" int impala_mlp_backward_pair_push(const float* x, const float* params_pi, const float* params_vf,
-                                             const float* dlogits, const float* dv, void* workspace_pi,
-                                             int64_t workspace_pi_bytes, void* workspace_vf,
-                                             int64_t workspace_vf_bytes, int M_pi, int M_vf, int O, int H_pi,
-                                             int H_vf, int A, const double* extra, int n_extra,
-                                             void* const* peer_gather, const long long* seq,
-                                             int64_t slot_stride, int64_t buf_stride, int rank, int world,
-                                             void* stream) {
+// The two push entry points: n_extra logged extras (at most 32), then n_obs observation sums (0, or 2 O + 1).
+static int pair_push(const float* x, const float* params_pi, const float* params_vf, const float* dlogits,
+                     const float* dv, void* workspace_pi, int64_t workspace_pi_bytes, void* workspace_vf,
+                     int64_t workspace_vf_bytes, int M_pi, int M_vf, int O, int H_pi, int H_vf, int A,
+                     const double* extra, int n_extra, int n_obs, void* const* peer_gather, const long long* seq,
+                     int64_t slot_stride, int64_t buf_stride, int rank, int world, void* stream) {
     if (!x || !params_pi || !params_vf || !dlogits || !dv || !workspace_pi || !workspace_vf || !peer_gather ||
-        !seq || (n_extra > 0 && !extra))
+        !seq || (n_extra + n_obs > 0 && !extra))
         return IMPALA_ERR_BAD_ARG;
     if (world < 1 || world > 8 || rank < 0 || rank >= world || n_extra < 0 || n_extra > 32) return IMPALA_ERR_BAD_ARG;
+    n_extra += n_obs;
     MlpPlan pi, vf;
     if (!push_plans(M_pi, M_vf, O, H_pi, H_vf, A, aligned(x, 16), aligned(dlogits, 16), aligned(dv, 16), &pi, &vf))
         return IMPALA_ERR_UNSUPPORTED_SHAPE;
@@ -422,6 +421,33 @@ extern "C" int impala_mlp_backward_pair_push(const float* x, const float* params
         reinterpret_cast<float*>(static_cast<char*>(workspace_vf) + kWsHeader), nullptr, nullptr,
         static_cast<unsigned int*>(workspace_pi), M_pi, M_vf, O, H_pi, H_vf, A, (cudaStream_t)stream, &push, extra,
         n_extra);
+}
+
+extern "C" int impala_mlp_backward_pair_push(const float* x, const float* params_pi, const float* params_vf,
+                                             const float* dlogits, const float* dv, void* workspace_pi,
+                                             int64_t workspace_pi_bytes, void* workspace_vf,
+                                             int64_t workspace_vf_bytes, int M_pi, int M_vf, int O, int H_pi,
+                                             int H_vf, int A, const double* extra, int n_extra,
+                                             void* const* peer_gather, const long long* seq,
+                                             int64_t slot_stride, int64_t buf_stride, int rank, int world,
+                                             void* stream) {
+    return pair_push(x, params_pi, params_vf, dlogits, dv, workspace_pi, workspace_pi_bytes, workspace_vf,
+                     workspace_vf_bytes, M_pi, M_vf, O, H_pi, H_vf, A, extra, n_extra, 0, peer_gather, seq, slot_stride,
+                     buf_stride, rank, world, stream);
+}
+
+extern "C" int impala_mlp_backward_pair_push_obs_norm(const float* x, const float* params_pi, const float* params_vf,
+                                                      const float* dlogits, const float* dv, void* workspace_pi,
+                                                      int64_t workspace_pi_bytes, void* workspace_vf,
+                                                      int64_t workspace_vf_bytes, int M_pi, int M_vf, int O, int H_pi,
+                                                      int H_vf, int A, const double* extra, int n_extra,
+                                                      void* const* peer_gather, const long long* seq,
+                                                      int64_t slot_stride, int64_t buf_stride, int rank, int world,
+                                                      void* stream) {
+    if (O > IMPALA_OBS_NORM_MAX_FEATURES) return IMPALA_ERR_BAD_ARG;
+    return pair_push(x, params_pi, params_vf, dlogits, dv, workspace_pi, workspace_pi_bytes, workspace_vf,
+                     workspace_vf_bytes, M_pi, M_vf, O, H_pi, H_vf, A, extra, n_extra, 2 * O + 1, peer_gather, seq,
+                     slot_stride, buf_stride, rank, world, stream);
 }
 
 // ---- shared-torso network: one MLP with N + 1 outputs [policy | value] over M = (T + 1) B rows, whose

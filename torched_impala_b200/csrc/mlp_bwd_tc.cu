@@ -994,12 +994,14 @@ mlp_bwd_tc_pair_kernel(const __grid_constant__ BwdTcArgs a_pi, const __grid_cons
     reduce_rows(a_pi, n_pi / (a_pi.H / 64), blockIdx.x, gridDim.x, reinterpret_cast<double*>(scratch), pp, 0);
     reduce_rows(a_vf, n_vf / (a_vf.H / 64), (int)gridDim.x - 1 - (int)blockIdx.x, gridDim.x,
                 reinterpret_cast<double*>(scratch), pp, a_pi.lay.total);
-    if (PUSH && blockIdx.x == gridDim.x / 2 && (int)threadIdx.x < n_extra) {
+    if (PUSH) {  // the extras, spread over the grid (observation normalization adds 2 O + 1 of them)
         const long long step = *push.seq + 1;
-        const int64_t off = (step & 1) * push.buf_stride + (int64_t)push.rank * push.slot_stride + a_pi.lay.total +
-                            a_vf.lay.total + threadIdx.x;
-        const double val = extra[threadIdx.x];
-        for (int r = 0; r < push.world; ++r) ll_store(push.gather[r] + off, val, (unsigned)step);
+        const int64_t base = (step & 1) * push.buf_stride + (int64_t)push.rank * push.slot_stride + a_pi.lay.total +
+                             a_vf.lay.total;
+        for (int j = (int)(blockIdx.x * blockDim.x + threadIdx.x); j < n_extra; j += (int)(gridDim.x * blockDim.x)) {
+            const double val = extra[j];
+            for (int r = 0; r < push.world; ++r) ll_store(push.gather[r] + base + j, val, (unsigned)step);
+        }
     }
     grid_depart(a_pi.ctl);
 }

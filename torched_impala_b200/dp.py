@@ -106,15 +106,19 @@ def _wait(pred, timeout: float, what: str, ctl: ShardControl | None = None):
 LR_TABLE_KEY = "optim/lr_table"  # init_state.npz entry of the learning-rate table (absent: the default)
 
 
-def write_init_state(path: str, init_state: dict, lr_table=None, popart=None) -> None:
+def write_init_state(path: str, init_state: dict, lr_table=None, popart=None, obs_norm=None) -> None:
     """The worker ranks' start: both networks' parameters and the learning-rate table (tabulated on rank 0: a
     lambda need not pickle, and a command-line argument is capped at 128 KiB on Linux).  popart = {"mu", "nu"}:
-    the PopArt statistics the (folded) value function goes with, read back as state["popart"]."""
+    the PopArt statistics the (folded) value function goes with, read back as state["popart"]; obs_norm =
+    {"count", "mean", "var"}: the observation statistics the (folded) first layers go with, as state["obs_norm"]."""
     arrays = {f"{g}/{k}": np.asarray(v) for g, d in init_state.items() for k, v in d.items()}
     if lr_table is not None:
         arrays[LR_TABLE_KEY] = np.asarray(lr_table, np.float32)
     if popart is not None:
         arrays["popart/mu"], arrays["popart/nu"] = np.float64(popart["mu"]), np.float64(popart["nu"])
+    if obs_norm is not None:
+        for k in ("count", "mean", "var"):
+            arrays[f"obs_norm/{k}"] = np.asarray(obs_norm[k], np.float64)
     np.savez(path, **arrays)
 
 
@@ -127,7 +131,7 @@ def read_init_state(path: str):
             table = z[key]
             continue
         g, k = key.split("/", 1)
-        state.setdefault(g, {})[k] = z[key]  # "popart": the statistics, when written
+        state.setdefault(g, {})[k] = z[key]  # "popart", "obs_norm": the statistics, when written
     return state, table
 
 
@@ -135,7 +139,7 @@ class DpLeader:
     """Rank 0's handle on the worker ranks (lives inside the learner process, post-fork)."""
 
     def __init__(self, devices, cfg: dict, init_state: dict, slab_shm_name: str, slab_bytes: int,
-                 n_slabs: int, timeout: float = 200.0, lr_table=None, popart=None):
+                 n_slabs: int, timeout: float = 200.0, lr_table=None, popart=None, obs_norm=None):
         self.world = len(devices)
         self.devices = list(devices)
         self.timeout = timeout
@@ -144,7 +148,7 @@ class DpLeader:
         self.step_no = 0
         self._tmp = tempfile.mkdtemp(prefix="impala_dp_")
         state_path = os.path.join(self._tmp, "init_state.npz")
-        write_init_state(state_path, init_state, lr_table, popart)
+        write_init_state(state_path, init_state, lr_table, popart, obs_norm)
         self.procs = []
         root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
         for r in range(1, self.world):

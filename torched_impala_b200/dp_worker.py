@@ -34,7 +34,8 @@ def main():
         state, lr_table = dp.read_init_state(spec["state"])
         eng = engine_from_cfg(c, world, dev, dist.group.WORLD, lr_table)
         popart = state.pop("popart", None)  # rank 0's statistics: every rank starts identical
-        eng.load_state(state, {k: float(v) for k, v in popart.items()} if popart else None)
+        obs_norm = state.pop("obs_norm", None)
+        eng.load_state(state, {k: float(v) for k, v in popart.items()} if popart else None, obs_norm)
         shm = dp.attach_untracked(spec["slab_shm"])
         base = np.ndarray((1,), dtype=np.uint8, buffer=shm.buf).ctypes.data
         eng.register_host(base, spec["slab_bytes"] * spec["n_slabs"])

@@ -53,6 +53,16 @@ include/impala_b200.h (PyTorch only provides device memory, streams and
       IMPALA_ACT_MASKED); impala_vtrace_loss_mask takes the V-trace slot with the same flags and workspace, pi and mu
       renormalised over the legal entries.  No launch is added.
 
+obs_norm=True (observation normalization): impala_obs_normalize is the step's first launch after any compose. It
+replaces the widening / unstacking launch below (one launch more for float32 dense slabs). It writes normalized
+float32 rows (T+1, B, O) that every later kernel reads, and the batch's per-feature sums into `comm` after the
+logged extras. One launch after the optimizer, impala_obs_norm_update, merges the (rank-summed) sums into float64
+running statistics and writes `folded`, the block with its first layers in raw-observation coordinates: what
+`state()` returns and the Learner publishes. Byte observations of O > 128 then run the float kernels. Data-parallel:
+the sums ride every all-reduce route (the paired backward's fused push, as impala_mlp_backward_pair_push_obs_norm,
+impala_peer_push, NCCL); on the peer routes the update kernel adds the ranks' sums in rank order out of the gather
+buffer.
+
 obs_dtype="uint8" (byte observations): the slabs hold obs as uint8 (impala_batch_layout_obs).  For
 O > 128 the two networks run impala_mlp_{forward,backward}_u8 on the bytes, one after the other as the
 pair entry points do at those widths.  For O <= 128 impala_obs_u8_to_f32 widens the obs into a float32
@@ -83,13 +93,15 @@ after the compose launch are unchanged; the logged `batch_mean_reward` scalar is
 all B columns' rewards / B), the mean over the fresh trajectories is the caller's (Learner logs that one).
 
 The keyword options above (obs_dtype, frames, diagnostics, replay_slabs, replay_columns, optimizer, optimizer_kwargs,
-popart, popart_beta, reward_clip, action_dist, action_heads, shared_torso, action_mask) are the fields of
-`LearnerOptions`.
+popart, popart_beta, reward_clip, action_dist, action_heads, shared_torso, action_mask, obs_norm, obs_norm_eps) are the
+fields of `LearnerOptions`.
 """
 from __future__ import annotations
 
 import ctypes as C
 import dataclasses
+import math
+import numbers
 from typing import NamedTuple
 
 import numpy as np
@@ -131,6 +143,23 @@ def diagnostic_values(sums, value_fn_loss: float, global_batch: int) -> dict:
 def popart_sigma(mu: float, nu: float) -> float:
     """sigma of the PopArt statistics (mu, nu), as the optimizer kernel forms it."""
     return min(max(max(nu - mu * mu, 0.0) ** 0.5, 1e-4), 1e6)
+
+
+def check_obs_norm_args(obs_norm, eps, O: int) -> None:
+    """The observation-normalization setting, checked before any device work: a bool, a finite eps > 0 and at most
+    IMPALA_OBS_NORM_MAX_FEATURES features."""
+    if not isinstance(obs_norm, bool):
+        raise ValueError(f"obs_norm must be a bool, got {obs_norm!r}")
+    if isinstance(eps, bool) or not isinstance(eps, numbers.Real) or not math.isfinite(eps) or not eps > 0:
+        raise ValueError(f"obs_norm_eps must be a finite number > 0, got {eps!r}")
+    if obs_norm and O > _cabi.OBS_NORM_MAX_FEATURES:
+        raise ValueError(f"obs_norm takes at most {_cabi.OBS_NORM_MAX_FEATURES} observation features, got {O}")
+
+
+def obs_norm_f32(mean, var, eps: float):
+    """(mu_f, r_f): the float32 statistics the kernels normalize with, mean and 1 / sqrt(var + eps) rounded."""
+    mean, var = np.asarray(mean, np.float64), np.asarray(var, np.float64)
+    return mean.astype(np.float32), (1.0 / np.sqrt(var + eps)).astype(np.float32)
 
 
 def check_shared_torso(shared_torso: bool, H_pi: int, H_v: int, n_policy: int) -> bool:
@@ -178,18 +207,26 @@ class LearnerOptions:
     # invalid-action masking (categorical and multi-discrete): every step carries a legal word in its actions.
     # Init-only like action_heads (Learner._cfg carries it, engine_from_cfg passes it when true).
     action_mask: dataclasses.InitVar[bool] = False
+    # observation normalization: running per-feature mean and variance of the raw observations, folded into the
+    # published weights (module docstring).  Init-only like action_mask (Learner._cfg carries both, engine_from_cfg
+    # passes them when obs_norm is true).
+    obs_norm: dataclasses.InitVar[bool] = False
+    obs_norm_eps: dataclasses.InitVar[float] = 1e-8
 
-    def __post_init__(self, action_heads, action_mask):
+    def __post_init__(self, action_heads, action_mask, obs_norm, obs_norm_eps):
         object.__setattr__(self, "optimizer_kwargs", dict(self.optimizer_kwargs or {}))
         # a tuple whatever sequence came in; check() refuses bad entries
         heads = tuple(action_heads) if isinstance(action_heads, (list, tuple)) else action_heads
         object.__setattr__(self, "action_heads", heads)
         object.__setattr__(self, "action_mask", action_mask)
+        object.__setattr__(self, "obs_norm", obs_norm)
+        object.__setattr__(self, "obs_norm_eps", obs_norm_eps)
 
     def __eq__(self, other):
         if other.__class__ is not self.__class__:
             return NotImplemented
-        return self.action_heads == other.action_heads and self.action_mask is other.action_mask and all(
+        return self.action_heads == other.action_heads and self.action_mask is other.action_mask and \
+            self.obs_norm is other.obs_norm and self.obs_norm_eps == other.obs_norm_eps and all(
             getattr(self, f.name) == getattr(other, f.name) for f in dataclasses.fields(self))
 
     def check(self, B: int, O: int, A: int, H_pi: int, H_v: int, world: int = 1) -> CheckedOptions:
@@ -219,6 +256,7 @@ class LearnerOptions:
         check_shared_torso(self.shared_torso, H_pi, H_v, N_pi)
         reward_clip_code = _cabi.reward_clip_code(self.reward_clip)
         check_popart_args(self.popart, self.popart_beta)
+        check_obs_norm_args(self.obs_norm, self.obs_norm_eps, O)
         B_fresh = check_replay_args(B, self.replay_slabs, self.replay_columns)
         if self.replay_slabs and world > 1:
             raise ValueError(f"experience replay runs on one device, not {world}: the store is not sharded")
@@ -237,7 +275,8 @@ def engine_from_cfg(cfg: dict, world: int, device, process_group=None, lr_table=
                          process_group=process_group, lr_table=lr_table,
                          **{f.name: cfg[f.name] for f in dataclasses.fields(LearnerOptions)},
                          **({"action_heads": tuple(cfg["action_heads"])} if cfg.get("action_heads") else {}),
-                         **({"action_mask": True} if cfg.get("action_mask") else {}))
+                         **({"action_mask": True} if cfg.get("action_mask") else {}),
+                         **({"obs_norm": True, "obs_norm_eps": cfg["obs_norm_eps"]} if cfg.get("obs_norm") else {}))
 
 
 def _ptr(t: torch.Tensor) -> C.c_void_p:
@@ -286,6 +325,7 @@ class LearnerEngine:
         self.shared_torso, self.popart, self.diagnostics = bool(o.shared_torso), bool(o.popart), bool(o.diagnostics)
         self.popart_beta, self.replay_slabs = float(o.popart_beta), int(o.replay_slabs)
         self.frames, self.F = o.frames, O // o.frames
+        self.obs_norm, self.obs_norm_eps = bool(o.obs_norm), float(o.obs_norm_eps)
         self.dev = torch.device(device)
         torch.cuda.set_device(self.dev)
         self.T, self.B, self.O, self.A, self.H_pi, self.H_v = T, B_local, O, A, H_pi, H_v
@@ -317,8 +357,10 @@ class LearnerEngine:
         self.adam_m = torch.zeros(self.n_total, **f32)
         self.adam_v = torch.zeros(self.n_total, **f32)
         self.adam_step = torch.zeros(3, dtype=torch.int64, device=self.dev)  # step, beta1^t, beta2^t bits
-        # float64 [gradient | 4 loss scalars | (diagnostics: 8 off-policy sums |) pad]: the all-reduce payload
-        self.n_comm = self.n_total + self.n_extra + 4
+        # float64 [gradient | 4 loss scalars | (diagnostics: 8 off-policy sums |) (obs_norm: the batch's observation
+        # sums, 2 O + 1 |) pad]: the all-reduce payload
+        self.obs_sums_at = self.n_total + self.n_extra
+        self.n_comm = self.obs_sums_at + (2 * O + 1 if self.obs_norm else 0) + 4
         self.comm = torch.zeros(self.n_comm, dtype=torch.float64, device=self.dev)
         self.norms = torch.zeros(2, dtype=torch.float64, device=self.dev)
         # the schedule (rmsprop or an lr_lambda): update n reads entry min(n - 1, len - 1); the state buffers
@@ -396,14 +438,31 @@ class LearnerEngine:
         self.ws_vf = torch.zeros(self.ws_vf_bytes, dtype=torch.uint8, device=self.dev)
         # byte observations: O > 128 runs the networks on the bytes (impala_mlp_{forward,backward}_u8); narrower
         # observations are widened once per step into this float32 copy for the float kernels
-        self.obs_u8_native = o.obs_dtype == "uint8" and O > 128
-        self.obs_f32 = (torch.zeros((T + 1) * B_local * O, **f32) if o.obs_dtype == "uint8" and not self.obs_u8_native
-                        else None)
+        self.obs_u8_native = o.obs_dtype == "uint8" and O > 128 and not self.obs_norm
+        self.obs_f32 = (torch.zeros((T + 1) * B_local * O, **f32)
+                        if o.obs_dtype == "uint8" and not self.obs_u8_native and not self.obs_norm else None)
         # frames > 1: the dense rows the kernels read, rebuilt from the slab's frames once per step
         self.obs_dense = None
-        if o.frames > 1:
+        if o.frames > 1 and not self.obs_norm:
             self.obs_dense = self.obs_f32 if self.obs_f32 is not None else torch.zeros(
                 (T + 1) * B_local * O, dtype=torch.uint8 if self.obs_u8_native else torch.float32, device=self.dev)
+        # obs_norm: impala_obs_normalize writes the normalized float32 rows every later kernel reads (in place of the
+        # widening / unstacking launch), impala_obs_norm_update the statistics and the folded block after the optimizer
+        self.obs_normed = self.folded = None
+        # (W1 offset, b1 offset, H) of each network in `params`
+        self.w1_nets = ((self.pi_off[0], self.pi_off[1], H_pi),) if self.shared_torso else (
+            (self.pi_off[0], self.pi_off[1], H_pi), (self.n_pi + self.vf_off[0], self.n_pi + self.vf_off[1], H_v))
+        if self.obs_norm:
+            self.obs_normed = torch.zeros((T + 1) * B_local * O, **f32)
+            self.folded = torch.zeros(self.n_total, **f32)
+            # [count | mean (O) | var (O)] float64 and the kernels' float32 [mu_f (O) | r_f (O)]; fresh: 0, 0, 1
+            self.obs_stats = torch.zeros(1 + 2 * O, dtype=torch.float64, device=self.dev)
+            self.obs_norm_dev = torch.zeros(2 * O, **f32)
+            self._set_obs_stats(0.0, np.zeros(O), np.ones(O))
+            n = int(self.lib.impala_obs_normalize_workspace(T, B_local, O))
+            _cabi.check(min(n, 0), "impala_obs_normalize_workspace")
+            self.obs_norm_ws = torch.zeros(n, dtype=torch.uint8, device=self.dev)  # counters zeroed once
+            self.obs_norm_ctl = torch.zeros(2, dtype=torch.int32, device=self.dev)
         ws_fn = (self.lib.impala_vtrace_loss_diag_workspace if self.n_extra == 12
                  else self.lib.impala_vtrace_loss_workspace)
         self.ws_vt_bytes = int(ws_fn(T, B_local, A))
@@ -519,7 +578,7 @@ class LearnerEngine:
         for key, off, shp in zip(PKEYS, self.vf_off, shp_vf):
             yield "value_fn", key, self.n_pi + off, shp
 
-    def load_state(self, state: dict, popart: dict | None = None) -> None:
+    def load_state(self, state: dict, popart: dict | None = None, obs_norm: dict | None = None) -> None:
         """state = {"policy": state_dict, "value_fn": state_dict} (any float dtype, CPU).
 
         With PopArt the value function is taken FOLDED, in reward units (what `state()` returns): popart =
@@ -528,9 +587,16 @@ class LearnerEngine:
 
         Shared torso: the torso (W1, b1) and the policy head come from "policy", the value head (W2 of one row,
         b2 of one entry) from "value_fn"; the value function's first layer is ignored, so a two-network state
-        loads with the policy's torso.  load_state(state()) restores the block exactly."""
+        loads with the policy's torso.  load_state(state()) restores the block exactly.
+
+        With obs_norm the first layers are taken FOLDED into raw-observation coordinates too (what `state()` returns):
+        obs_norm = {"count", "mean", "var"} sets the statistics, and W1 = W1' / r_f, b1 = b1' + W1' mu_f (float64, with
+        the float32 mu_f, r_f the kernels use, obs_norm_f32) unfolds each network's first layer; obs_norm=None starts
+        from count 0, mean 0, var 1."""
         if popart is not None and not self.popart:
             raise ValueError("PopArt statistics given to an engine built with popart=False")
+        if obs_norm is not None and not self.obs_norm:
+            raise ValueError("observation statistics given to an engine built with obs_norm=False")
         mu, nu = (0.0, 1.0) if popart is None else (float(popart["mu"]), float(popart["nu"]))
         sigma = popart_sigma(mu, nu)
         flat = torch.zeros(self.n_total, dtype=torch.float32)
@@ -545,10 +611,37 @@ class LearnerEngine:
                 t = t.to(torch.float64)
                 t = t / sigma if key == PKEYS[2] else (t - mu) / sigma
             flat[off:off + t.numel()] = t.reshape(-1).to(torch.float32)
+        if self.obs_norm:
+            self.folded.copy_(flat)
+            O = self.O
+            count, mean, var = ((0.0, np.zeros(O), np.ones(O)) if obs_norm is None else
+                                (float(obs_norm["count"]), np.asarray(obs_norm["mean"], np.float64).reshape(-1),
+                                 np.asarray(obs_norm["var"], np.float64).reshape(-1)))
+            if mean.shape != (O,) or var.shape != (O,) or not count >= 0 or not (var >= 0).all():
+                raise ValueError(f"obs_norm statistics need a count >= 0 and mean, var of {O} features (var >= 0)")
+            mu_f, r_f = (x.astype(np.float64) for x in obs_norm_f32(mean, var, self.obs_norm_eps))
+            for grp, (w1, b1, H) in zip(("policy", "value_fn"), self.w1_nets):
+                W = np.asarray(torch.as_tensor(state[grp][PKEYS[0]]).detach().cpu().to(torch.float64))
+                b = np.asarray(torch.as_tensor(state[grp][PKEYS[1]]).detach().cpu().to(torch.float64))
+                flat[w1:w1 + H * O] = torch.from_numpy((W / r_f).reshape(-1))
+                flat[b1:b1 + H] = torch.from_numpy(b + W @ mu_f)
+            self._set_obs_stats(count, mean, var)
         self.params.copy_(flat)
         if self.popart:
             self.popart_buf.copy_(torch.tensor([mu, nu, sigma, mu, sigma], dtype=torch.float64))
         torch.cuda.synchronize(self.dev)
+
+    def _set_obs_stats(self, count: float, mean, var) -> None:
+        mu_f, r_f = obs_norm_f32(mean, var, self.obs_norm_eps)
+        self.obs_stats.copy_(torch.from_numpy(np.concatenate([[count], mean, var]).astype(np.float64)))
+        self.obs_norm_dev.copy_(torch.from_numpy(np.concatenate([mu_f, r_f])))
+
+    def obs_norm_stats(self) -> dict:
+        """The current observation statistics {"count": float, "mean", "var": float64 arrays of O} (waits for the
+        stream); var is 1 where nothing has been counted."""
+        self.stream.synchronize()
+        st = self.obs_stats.cpu().numpy()
+        return {"count": float(st[0]), "mean": st[1:1 + self.O].copy(), "var": st[1 + self.O:].copy()}
 
     def popart_stats(self) -> dict:
         """The current PopArt statistics {"mu", "nu", "sigma"} (float; waits for the stream)."""
@@ -557,9 +650,10 @@ class LearnerEngine:
         return {"mu": mu, "nu": nu, "sigma": sigma}
 
     def state(self, dtype=torch.float64) -> dict:
-        """Reference-format state_dicts (CPU, float64 like reference models.py:6)."""
+        """Reference-format state_dicts (CPU, float64 like reference models.py:6).  obs_norm: the first layers folded
+        into raw-observation coordinates (the block impala_obs_norm_update wrote), which is what actors run."""
         self.stream.synchronize()
-        flat = self.params.detach().cpu()
+        flat = (self.folded if self.obs_norm else self.params).detach().cpu()
         out = {"policy": {}, "value_fn": {}}
         mu, _, sigma = self.popart_buf[:3].tolist() if self.popart else (0.0, 1.0, 1.0)
         for grp, key, off, shp in self._segments():
@@ -571,7 +665,8 @@ class LearnerEngine:
         return out
 
     def normalized_state(self, dtype=torch.float64) -> dict:
-        """Like `state()`, but the value function as the engine holds it (normalized under PopArt)."""
+        """Like `state()`, but the networks as the engine holds them (the value function normalized under PopArt, the
+        first layers reading normalized observations under obs_norm)."""
         self.stream.synchronize()
         flat = self.params.detach().cpu()
         out = {"policy": {}, "value_fn": {}}
@@ -698,7 +793,13 @@ class LearnerEngine:
         g_vf = C.c_void_p(gbase + 8 * self.n_pi)
         scal = C.c_void_p(gbase + 8 * self.n_total)
         obs = _ptr(d["obs"])
-        if self.obs_dense is not None:  # frames: one unstacking launch (widening bytes for O <= 128)
+        if self.obs_norm:  # normalized float32 rows (any slab form) and the batch's sums into `comm`
+            _cabi.check(lib.impala_obs_normalize(obs, self.obs_code, T, B, self.F, self.frames, _ptr(d["lens"]),
+                                                 _ptr(self.obs_norm_dev), _ptr(self.obs_normed),
+                                                 C.c_void_p(gbase + 8 * self.obs_sums_at), _ptr(self.obs_norm_ws),
+                                                 self.obs_norm_ws.numel(), st), "impala_obs_normalize")
+            obs = _ptr(self.obs_normed)
+        elif self.obs_dense is not None:  # frames: one unstacking launch (widening bytes for O <= 128)
             out_code = _cabi.OBS_U8 if self.obs_dense.dtype == torch.uint8 else _cabi.OBS_F32
             _cabi.check(lib.impala_obs_unstack(obs, self.obs_code, _ptr(self.obs_dense), out_code, T + 1, B, self.F,
                                                self.frames, st), "impala_obs_unstack")
@@ -760,8 +861,9 @@ class LearnerEngine:
             _cabi.check(lib.impala_vtrace_loss(*vt_in, _ptr(self.ws_vt), self.ws_vt_bytes, *vt_hp),
                         "impala_vtrace_loss")
         pr = self.peer
-        if pr and pr["fused"]:
-            _cabi.check(lib.impala_mlp_backward_pair_push(
+        if pr and pr["fused"]:  # obs_norm: the observation sums follow the logged extras in `comm` and are pushed too
+            push = lib.impala_mlp_backward_pair_push_obs_norm if self.obs_norm else lib.impala_mlp_backward_pair_push
+            _cabi.check(push(
                 obs, p_pi, p_vf, _ptr(self.dlogits), _ptr(self.dv), _ptr(self.ws_pi), self.ws_pi_bytes,
                 _ptr(self.ws_vf), self.ws_vf_bytes, self.M_pi, self.M_vf, O, self.H_pi, self.H_v, A, scal, self.n_extra,
                 _ptr(pr["gather_ptrs"]), _ptr(pr["seq"]), pr["slot"], pr["buf"], pr["rank"], self.world, st),
@@ -793,6 +895,25 @@ class LearnerEngine:
         return self.optim.lr_of(n)
 
     def _enqueue_opt(self) -> int:
+        n = self._enqueue_rule()
+        if self.obs_norm:
+            n += self._enqueue_obs_norm_update()
+        return n
+
+    def _enqueue_obs_norm_update(self) -> int:
+        """The statistics merge and the folded block, one launch behind the optimizer."""
+        st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        nets = [x for net in self.w1_nets for x in net] + [0, 0, 0] * (2 - len(self.w1_nets))
+        pr = self.peer
+        peer = ((C.c_void_p(pr["gather"]), _ptr(pr["seq"]), pr["slot"], pr["buf"], self.world, self.obs_sums_at,
+                 _ptr(pr["err"]), pr["timeout_s"]) if pr else (None, None, 0, 0, 1, 0, None, 0.0))
+        _cabi.check(self.lib.impala_obs_norm_update(
+            _ptr(self.obs_stats), _ptr(self.obs_norm_dev), C.c_void_p(self.comm.data_ptr() + 8 * self.obs_sums_at),
+            self.obs_norm_eps, _ptr(self.params), _ptr(self.folded), self.n_total, self.O, *nets,
+            _ptr(self.obs_norm_ctl), *peer, st), "impala_obs_norm_update")
+        return 1
+
+    def _enqueue_rule(self) -> int:
         hp, st = self.hp, C.c_void_p(torch.cuda.current_stream().cuda_stream)
         if self.lr_table is not None:
             return self._enqueue_optim(st)
@@ -907,10 +1028,10 @@ class LearnerEngine:
 
                 dist.all_reduce(self.comm, op=dist.ReduceOp.SUM, group=self.pg)
             if fused_opt:
-                n += 1
+                n += 1 + self.obs_norm
             elif self.use_graph and self._graph_opt is not None:
                 self._graph_opt.replay()
-                n += 1
+                n += 1 + self.obs_norm
             else:
                 n += self._enqueue_opt()
         self.launches_per_step = n

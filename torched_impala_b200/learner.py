@@ -44,7 +44,11 @@ path of the device (SURVEY 8f-2, 8f-4):
   * `reward_clip="abs_one"` (clip(r, -1, 1), the paper's Atari setting) or `"soft_asymmetric"` (DMLab's
     5 tanh(r / 5), 1.5 tanh(r / 5) below 0): the V-trace kernel transforms the rewards it reads, so actors, the
     transport and replay keep raw rewards and `rewards/batch_mean_reward` stays the raw game score.  A
-    hyperparameter, not state: checkpoints are unchanged.
+    hyperparameter, not state: checkpoints are unchanged;
+  * `obs_norm=True`, `obs_norm_eps` (observation normalization, off by default): the networks train on observations
+    normalized by running per-feature statistics kept on the device (engine.py).  `policy`, `value_fn` and
+    checkpoints hold the networks FOLDED into raw-observation coordinates, plus the statistics under the key
+    "obs_norm", so actors keep feeding raw observations.
 
 CUDA is initialised inside the learner process only (`train.py:42` forces the fork start method,
 so the parent must never touch the device); a policy / value_fn that already lives on a CUDA
@@ -394,7 +398,8 @@ class _Publisher:
         eng = self.eng
         frozen, landed = self.ev_frozen[s], self.ev_landed[s]
         with eng._on_stream():
-            self.stage[s].copy_(eng.params[:eng.n_pi], non_blocking=True)
+            # obs_norm: the policy folded into raw-observation coordinates, which the actors feed it
+            self.stage[s].copy_((eng.folded if eng.obs_norm else eng.params)[:eng.n_pi], non_blocking=True)
             frozen.record(eng.stream)
         self.stream.wait_event(frozen)
         with torch.cuda.stream(self.stream):
@@ -453,6 +458,7 @@ class Learner:
         self.B_fresh = o.check(hparams.batch_size, *_dims(policy, value_fn, o.action_dist), len(self.devices)).B_fresh
         _check_ring(q, o, self.B_fresh)
         self.popart_init = None  # {"mu", "nu"} of the folded value_fn (load() of a PopArt checkpoint sets it)
+        self.obs_norm_init = None  # {"count", "mean", "var"} the folded first layers go with (obs_norm checkpoints)
         self.hp = hparams
         self.policy = policy
         self.value_fn = value_fn
@@ -514,15 +520,22 @@ class Learner:
         O, A, H_pi, H_v = _dims(self.policy, self.value_fn, self.options.action_dist)
         hp = self.hp._asdict() if hasattr(self.hp, "_asdict") else dict(self.hp)
         hp["log_path"] = None if hp.get("log_path") is None else str(hp["log_path"])
-        # action_heads and action_mask are init-only options (engine.LearnerOptions), so they ride next to the fields
+        # action_heads, action_mask, obs_norm and obs_norm_eps are init-only options (engine.LearnerOptions), so they
+        # ride next to the fields
+        o = self.options
         return dict(T=self.hp.max_timesteps, B=self.hp.batch_size, O=O, A=A, H_pi=H_pi, H_v=H_v, mode=self.mode, hp=hp,
-                    action_heads=list(self.options.action_heads), action_mask=self.options.action_mask,
+                    action_heads=list(o.action_heads), action_mask=o.action_mask, obs_norm=o.obs_norm,
+                    obs_norm_eps=o.obs_norm_eps,
                     **dataclasses.asdict(self.options))
 
     def _make_engine(self, process_group=None, world=1):
         eng = engine_from_cfg(self._cfg(), world, self.device, process_group, self.optim.lr_table)
-        eng.load_state(self._init_state(), self._popart_init())
+        eng.load_state(self._init_state(), self._popart_init(), self._obs_norm_init())
         return eng
+
+    def _obs_norm_init(self):
+        """The observation statistics the folded modules go with: those of a loaded checkpoint, else None (fresh)."""
+        return dict(self.obs_norm_init) if self.options.obs_norm and self.obs_norm_init is not None else None
 
     def _popart_init(self):
         """The statistics the folded value_fn goes with: those of a loaded checkpoint, else None (mu 0, nu 1)."""
@@ -540,6 +553,8 @@ class Learner:
         if self.options.popart:
             s = eng.popart_stats()
             self.popart_init = {"mu": s["mu"], "nu": s["nu"]}  # what save() writes next to the folded value_fn
+        if self.options.obs_norm:
+            self.obs_norm_init = eng.obs_norm_stats()  # what save() writes next to the folded first layers
         with torch.no_grad():
             self._version.value += 1
             for mod, grp in ((self.policy, "policy"), (self.value_fn, "value_fn")):
@@ -704,7 +719,8 @@ class Learner:
                 slabs = ring if ring is not None else stage
                 leader = dp.DpLeader(self.devices, self._cfg(), self._init_state(), slabs.shm.name,
                                      slabs.slab_bytes, slabs.K, timeout=max(60.0, float(self.timeout)),
-                                     lr_table=self.optim.lr_table, popart=self._popart_init())
+                                     lr_table=self.optim.lr_table, popart=self._popart_init(),
+                                     obs_norm=self._obs_norm_init())
                 torch.cuda.set_device(torch.device(self.device))
                 pg = leader.init_process_group(self.device)
             eng = self._make_engine(pg, world)  # first CUDA call of this process (post-fork)
@@ -847,6 +863,11 @@ class Learner:
             ckpt["shared_torso"] = True
         if self.options.popart:  # value_fn is folded (reward units); the statistics that unfold it
             ckpt["popart"] = dict(self.popart_init or {"mu": 0.0, "nu": 1.0})
+        if self.options.obs_norm:  # the first layers are folded (raw observations); the statistics that unfold them
+            O = _dims(self.policy, self.value_fn, self.options.action_dist)[0]
+            st = self.obs_norm_init or {"count": 0.0, "mean": np.zeros(O), "var": np.ones(O)}
+            ckpt["obs_norm"] = {"count": float(st["count"]), "mean": torch.tensor(np.asarray(st["mean"], np.float64)),
+                                "var": torch.tensor(np.asarray(st["var"], np.float64))}
         torch.save(ckpt, path)
 
     def load(self, path):
@@ -858,6 +879,10 @@ class Learner:
         self.value_fn.load_state_dict(checkpoint["value_fn_state_dict"])
         if "popart" in checkpoint:
             self.popart_init = {k: float(checkpoint["popart"][k]) for k in ("mu", "nu")}
+        if "obs_norm" in checkpoint:
+            st = checkpoint["obs_norm"]
+            self.obs_norm_init = {"count": float(st["count"]),
+                                  **{k: np.asarray(torch.as_tensor(st[k]), np.float64) for k in ("mean", "var")}}
 
     @property
     def policy_weights(self):
