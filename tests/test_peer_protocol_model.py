@@ -7,8 +7,10 @@ argument - parity-double-buffered slots need no acknowledgement round trip - is 
 property, independent of CUDA: rank threads with random delays run it here, writing element by
 element with pauses (so readers do see half-written slots), and check that every value a reader
 accepts is exactly the one the writer sent for that step (never a value a fast peer has already
-overwritten).  The same model with ONE buffer per rank must fail, which shows the test can see the
-hazard the second buffer removes."""
+overwritten).  Every rank reads the slots of a step twice, as the optimizer and then the observation-statistics
+update (impala_obs_norm_update, csrc/obs_norm.cu) do, the second pass after the first and before the rank's next
+push.  The same model with ONE buffer per rank must fail, which shows the test can see the hazard the second
+buffer removes.  A reader that waits too long is a failure too (a deadlock, not a pass)."""
 import random
 import threading
 import time
@@ -34,28 +36,30 @@ def run_ranks(world: int, steps: int, buffers: int, seed: int):
                     gather[p][s % buffers][me][e] = (s, (me, s, e))
                 if rng.random() < 0.2:
                     time.sleep(0)                        # a reader may observe a half-written slot
-            t0 = time.time()
-            got = []
-            for r in range(world):                       # optimizer: poll the LOCAL slots element by element
-                for e in range(ELEMS):
-                    while True:
-                        tag, val = gather[me][s % buffers][r][e]
-                        if tag == s:
-                            break
-                        if stop.is_set() or time.time() - t0 > 20:
-                            return
-                        if tag > s:                      # overwritten before it was read: the hazard
-                            errors.append((me, s, r, e, tag))
-                            stop.set()
-                            return
-                        time.sleep(0)
-                    got.append(val)
-                if rng.random() < 0.1:
-                    time.sleep(rng.random() * 3e-4)      # a slow reader
-            if got != [(r, s, e) for r in range(world) for e in range(ELEMS)]:
-                errors.append((me, s, got))
-                stop.set()
-                return
+            # the optimizer, then the statistics update: each polls the LOCAL slots of step s element by element
+            for reader in ("optimizer", "statistics"):
+                t0 = time.time()
+                got = []
+                for r in range(world):
+                    for e in range(ELEMS):
+                        while True:
+                            tag, val = gather[me][s % buffers][r][e]
+                            if tag == s:
+                                break
+                            if stop.is_set():
+                                return
+                            if tag > s or time.time() - t0 > 20:  # overwritten before it was read, or never written
+                                errors.append((reader, me, s, r, e, tag))
+                                stop.set()
+                                return
+                            time.sleep(0)
+                        got.append(val)
+                    if rng.random() < 0.1:
+                        time.sleep(rng.random() * 3e-4)  # a slow reader
+                if got != [(r, s, e) for r in range(world) for e in range(ELEMS)]:
+                    errors.append((reader, me, s, got))
+                    stop.set()
+                    return
 
     ts = [threading.Thread(target=rank, args=(r,)) for r in range(world)]
     for t in ts:

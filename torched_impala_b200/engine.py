@@ -497,11 +497,9 @@ class LearnerEngine:
         rank, world = dist.get_rank(self.pg), self.world
         ok, err, mine = os.environ.get("IMPALA_ALLREDUCE", "peer") != "nccl" and world <= 8, "", {}
         lib = self.lib
-        slot = self.n_comm                              # LL elements per rank slot: [gradient | scalars | pad]
-        buf = world * slot                              # LL elements per parity buffer
         if ok:
             try:
-                for name, nbytes in (("gather", 2 * 16 * buf),):
+                for name, nbytes in (("gather", self.gather_bytes(world)),):
                     ptr, handle = C.c_void_p(), (C.c_char * 64)()
                     _cabi.check(lib.impala_peer_alloc(nbytes, C.byref(ptr), handle), "impala_peer_alloc")
                     mine[name] = (ptr.value, bytes(handle.raw))
@@ -532,18 +530,42 @@ class LearnerEngine:
                 warnings.warn(f"peer-memory all-reduce unavailable ({err or 'a rank could not map its peers'}); "
                               "using the NCCL all-reduce between backward and optimizer")
             return
+        self._use_peers(mine["gather"][0], ptrs["gather"], rank, world, opened=opened)
+        torch.cuda.synchronize(self.dev)
+        dist.barrier(group=self.pg)
+
+    def gather_bytes(self, world: int) -> int:
+        """Bytes of one rank's gather buffer for `world` ranks: 2 parities x `world` slots of n_comm LL elements
+        (16 bytes per float64)."""
+        return 2 * 16 * world * self.n_comm
+
+    def _use_peers(self, gather_ptr: int, gather_ptrs, rank: int, world: int, timeout_s: float | None = None,
+                   opened=()) -> None:
+        """Make the step exchange `comm` by the push over peer memory as rank `rank` of `world`: gather_ptr is this
+        rank's zero-filled gather buffer (gather_bytes(world) bytes, 16-byte aligned), gather_ptrs every rank's as
+        this process addresses it.  _setup_peer_allreduce calls it with the mapped IPC buffers; any device addresses
+        serve (several simulated ranks on one device, each with its own buffer).  timeout_s=None: the
+        IMPALA_PEER_TIMEOUT_S environment variable, 600 s by default."""
+        import os
+
+        if not 1 <= world <= 8 or not 0 <= rank < world or len(gather_ptrs) != world:
+            raise ValueError(f"rank {rank} of {world} with {len(gather_ptrs)} gather buffers (1 to 8 ranks)")
+        if self.replay_slabs and world > 1:
+            raise ValueError(f"experience replay runs on one device, not {world}: the store is not sharded")
         i64 = dict(dtype=torch.int64, device=self.dev)
         # the fused push is the paired backward's; a shared torso pushes `comm` after its backward
-        fused = not self.shared_torso and bool(lib.impala_mlp_backward_pair_push_supported(
+        fused = not self.shared_torso and bool(self.lib.impala_mlp_backward_pair_push_supported(
             self.M_pi, self.M_vf, self.O, self.H_pi, self.H_v, self.N_pi))
         if os.environ.get("IMPALA_PUSH_FUSED", "1") == "0":
             fused = False
-        self.peer = dict(gather=mine["gather"][0], opened=opened, gather_ptrs=torch.tensor(ptrs["gather"], **i64),
-                         seq=torch.zeros(1, **i64), rank=rank, slot=slot, buf=buf, fused=fused,
-                         err=torch.zeros(1, dtype=torch.int32, device=self.dev),
-                         timeout_s=float(os.environ.get("IMPALA_PEER_TIMEOUT_S", "600")))
-        torch.cuda.synchronize(self.dev)
-        dist.barrier(group=self.pg)
+        if timeout_s is None:
+            timeout_s = float(os.environ.get("IMPALA_PEER_TIMEOUT_S", "600"))
+        slot = self.n_comm                              # LL elements per rank slot: [gradient | scalars | pad]
+        self.world = world
+        self.peer = dict(gather=int(gather_ptr), opened=list(opened),
+                         gather_ptrs=torch.tensor([int(p) for p in gather_ptrs], **i64),
+                         seq=torch.zeros(1, **i64), rank=rank, slot=slot, buf=world * slot, fused=fused,
+                         err=torch.zeros(1, dtype=torch.int32, device=self.dev), timeout_s=float(timeout_s))
 
     def _shapes(self, B: int) -> dict:
         """Shapes of the six batch tensors in a slab of B columns."""
